@@ -84,6 +84,7 @@ _SIGNATURES = {
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_colour_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
+    "dss_camera_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp, vp, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -66,6 +66,7 @@ enum BufId {
     BUF_KNN_COUNTS,   // 3-D grid of the K-NN search: points per cell
     BUF_KNN_OFFSETS,  //   exclusive scan of the counts
     BUF_KNN_SORTED,   //   points in cell order {x, y, z, index}
+    BUF_CAMERA,       // per-block fp64 partial sums of the camera gradients
     NUM_BUFS
 };
 
@@ -74,7 +75,8 @@ enum BufId {
 namespace dss {
 enum Stage {
     ST_PACK = 0, ST_PREPROCESS, ST_BIN_COUNT, ST_SCAN, ST_BIN_SCATTER, ST_RASTER_FWD, ST_VISIBILITY,
-    ST_SEARCH_RADIUS, ST_OCC_BWD, ST_COLOUR_BWD, ST_ZBUF_BWD, ST_CHAIN, ST_GRID, ST_OCC_BIN, ST_KNN, NUM_STAGES
+    ST_SEARCH_RADIUS, ST_OCC_BWD, ST_COLOUR_BWD, ST_ZBUF_BWD, ST_CHAIN, ST_GRID, ST_OCC_BIN, ST_KNN,
+    ST_CAMERA_BWD, NUM_STAGES
 };
 struct ProfPending {
     cudaEvent_t a, b;

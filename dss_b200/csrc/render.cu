@@ -78,10 +78,12 @@ __device__ __forceinline__ V3 normalize3_bwd(V3 y, float len, V3 gy) {
 
 // forward (and, with gc != nullptr, backward) of the shading of one (view, point).  sL: lights in shared memory.
 //   colour = albedo * (ambient + diffuse) + specular
-// backward: accumulates d albedo, d normal (un-normalised input normal), d position into g_alb / g_nrm / g_pos.
-template <bool BACKWARD>
+// backward: accumulates d albedo, d normal (un-normalised input normal), d position into g_alb / g_nrm / g_pos, and
+// with CAM_GRAD the camera-centre gradient (the view-direction half of d position, opposite sign) into *g_cam.
+template <bool BACKWARD, bool CAM_GRAD = false>
 __device__ __forceinline__ V3 shade_point(const float *sL, int n_lights, int light_type, float shininess, V3 amb, V3 p,
-                                          V3 nrm, V3 alb, V3 cam, V3 gc, V3 &g_alb, V3 &g_nrm, V3 &g_pos) {
+                                          V3 nrm, V3 alb, V3 cam, V3 gc, V3 &g_alb, V3 &g_nrm, V3 &g_pos,
+                                          V3 *g_cam = nullptr) {
     float nlen, vlen;
     const V3 nh = normalize3(nrm, nlen);
     const V3 v = normalize3(sub3(cam, p), vlen);
@@ -123,7 +125,9 @@ __device__ __forceinline__ V3 shade_point(const float *sL, int n_lights, int lig
     if (BACKWARD) {
         g_alb = add3(g_alb, v3(gc.x * (amb.x + diff.x), gc.y * (amb.y + diff.y), gc.z * (amb.z + diff.z)));
         g_nrm = add3(g_nrm, normalize3_bwd(nh, nlen, g_nh));
-        g_pos = sub3(g_pos, normalize3_bwd(v, vlen, g_v));                // v = normalize(cam - p)
+        const V3 g_cam_v = normalize3_bwd(v, vlen, g_v);                 // v = normalize(cam - p)
+        g_pos = sub3(g_pos, g_cam_v);
+        if (CAM_GRAD) *g_cam = add3(*g_cam, g_cam_v);
     }
     return v3(alb.x * (amb.x + diff.x) + spec.x, alb.y * (amb.y + diff.y) + spec.y, alb.z * (amb.z + diff.z) + spec.z);
 }
@@ -558,6 +562,146 @@ __global__ void __launch_bounds__(256) chain_kernel(const __grid_constant__ Chai
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Camera gradients (the reference differentiates through pytorch3d's transform, rasterizer.py:614, and the shading
+// reads cameras.get_camera_center()).  Per (view, point) slot with the clipped NDC gradient g = (gx, gy, gz) and
+// p_h = [p 1], clip = p_h M, w = clip3, (x, y) = clip01 / w:
+//   d L / d clip = (gx / w, gy / w, 0, -(gx x + gy y) / w)
+//   grad_proj[n][r][c] = sum_p p_h[r] dclip[c]        (column 2 stays zero: screen z is the view depth)
+//   grad_view[n][r][2] = sum_p p_h[r] gz
+// and with fused shading grad_cam[n] = sum_p normalize_bwd(v, g_v), v = normalize(cam - p).
+// Pass 1: grid (point blocks, views), every block writes its CAM_SUMS sums (fp64) to a partials array.  Pass 2: one
+// block per view adds its partials in block order.  Fixed grid and fixed reduction order: bit-reproducible.
+// ---------------------------------------------------------------------------------------------
+constexpr int CAM_SUMS = 19;   // 12 proj (rows 0..3 x columns 0, 1, 3), 4 view (rows 0..3, column 2), 3 camera centre
+
+struct CamArgs {
+    const float *pts, *proj, *gndc;
+    const int64_t *first_idx, *num_points;
+    int64_t P0;
+    int shared_cloud;
+    const float *nrm, *gsh;   // shading only: normals and d L / d shaded (N*P0,3)
+    ShadeArgs sh;
+    double *partials;         // (N, gridDim.x, CAM_SUMS)
+};
+
+// sum of acc[k] over the block (blockDim.x a multiple of 32, at most 256) in a fixed order; thread k < CAM_SUMS
+// returns sum k, the others 0
+__device__ __forceinline__ double block_sum(const double (&acc)[CAM_SUMS], double (*sPart)[CAM_SUMS]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < CAM_SUMS; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) sPart[warp][k] = v;
+    }
+    __syncthreads();
+    double v = 0.0;
+    if (threadIdx.x < CAM_SUMS)
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += sPart[w][threadIdx.x];
+    return v;
+}
+
+constexpr int CAM_BATCH = 4;   // slots per thread whose loads are issued together
+
+template <bool SHADE>
+__global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_constant__ CamArgs a) {
+    __shared__ float sM[16];
+    __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
+    __shared__ double sPart[8][CAM_SUMS];
+    const int n = blockIdx.y;
+    if (threadIdx.x < 16) sM[threadIdx.x] = a.proj[n * 16 + threadIdx.x];
+    if (SHADE) {
+        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = a.sh.lights[threadIdx.x];
+        if (threadIdx.x < 3) {
+            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = a.sh.ambient[threadIdx.x];
+            sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
+        }
+    }
+    __syncthreads();
+    double acc[CAM_SUMS];
+#pragma unroll
+    for (int k = 0; k < CAM_SUMS; ++k) acc[k] = 0.0;
+    const ViewRange vr = view_range(a.shared_cloud ? nullptr : a.first_idx, a.num_points, n, a.P0);
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < vr.count; i0 += CAM_BATCH * stride) {
+        float g[CAM_BATCH][3], gs[CAM_BATCH][3];
+#pragma unroll
+        for (int j = 0; j < CAM_BATCH; ++j) {
+            const int64_t i = i0 + j * stride, s = vr.first + i;
+            const bool in = i < vr.count;
+#pragma unroll
+            for (int e = 0; e < 3; ++e) {
+                g[j][e] = in ? a.gndc[s * 3 + e] : 0.0f;
+                gs[j][e] = (SHADE && in) ? a.gsh[s * 3 + e] : 0.0f;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < CAM_BATCH; ++j) {
+            const int64_t i = i0 + j * stride, s = vr.first + i;
+            const int64_t src = a.shared_cloud ? i : s;
+            const float gx = g[j][0], gy = g[j][1], gz = g[j][2];
+            if (gx != 0.0f || gy != 0.0f || gz != 0.0f) {
+                const float ph[4] = {a.pts[src * 3], a.pts[src * 3 + 1], a.pts[src * 3 + 2], 1.0f};
+                const float x = fmaf(ph[0], sM[0], fmaf(ph[1], sM[4], fmaf(ph[2], sM[8], sM[12])));
+                const float y = fmaf(ph[0], sM[1], fmaf(ph[1], sM[5], fmaf(ph[2], sM[9], sM[13])));
+                const float t = fmaf(ph[0], sM[3], fmaf(ph[1], sM[7], fmaf(ph[2], sM[11], sM[15])));
+                const float it = 1.0f / t;
+                const float d0 = gx * it, d1 = gy * it, d3 = -(gx * (x * it) + gy * (y * it)) * it;
+#pragma unroll
+                for (int r = 0; r < 4; ++r) {
+                    const double pr = (double)ph[r];
+                    acc[3 * r + 0] = fma(pr, (double)d0, acc[3 * r + 0]);
+                    acc[3 * r + 1] = fma(pr, (double)d1, acc[3 * r + 1]);
+                    acc[3 * r + 2] = fma(pr, (double)d3, acc[3 * r + 2]);
+                    acc[12 + r] = fma(pr, (double)gz, acc[12 + r]);
+                }
+            }
+            const V3 gc = v3(gs[j][0], gs[j][1], gs[j][2]);
+            if (SHADE && (gc.x != 0.0f || gc.y != 0.0f || gc.z != 0.0f)) {   // shared cloud: world point i
+                const float *amb = sL + DSS_MAX_LIGHTS * 9;
+                V3 ga = v3(0.f, 0.f, 0.f), gn = v3(0.f, 0.f, 0.f), gp = v3(0.f, 0.f, 0.f), gcam = v3(0.f, 0.f, 0.f);
+                shade_point<true, true>(sL, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(amb[0], amb[1], amb[2]),
+                                        v3(a.pts[i * 3], a.pts[i * 3 + 1], a.pts[i * 3 + 2]),
+                                        v3(a.nrm[i * 3], a.nrm[i * 3 + 1], a.nrm[i * 3 + 2]),
+                                        v3(a.sh.albedo[i * 3], a.sh.albedo[i * 3 + 1], a.sh.albedo[i * 3 + 2]),
+                                        v3(amb[3], amb[4], amb[5]), gc, ga, gn, gp, &gcam);
+                acc[16] += (double)gcam.x;
+                acc[17] += (double)gcam.y;
+                acc[18] += (double)gcam.z;
+            }
+        }
+    }
+    const double v = block_sum(acc, sPart);
+    if (threadIdx.x < CAM_SUMS) a.partials[((int64_t)n * gridDim.x + blockIdx.x) * CAM_SUMS + threadIdx.x] = v;
+}
+
+// one block per view: sums the view's partials in a fixed order and writes the (4,4) / (4,4) / (3,) rows
+__global__ void __launch_bounds__(256) camera_finish_kernel(const double *partials, int blocks, float *grad_proj,
+                                                            float *grad_view, float *grad_cam) {
+    __shared__ double sPart[8][CAM_SUMS];
+    __shared__ double sTot[CAM_SUMS];
+    const int n = blockIdx.x, k = threadIdx.x;
+    double acc[CAM_SUMS];
+#pragma unroll
+    for (int j = 0; j < CAM_SUMS; ++j) acc[j] = 0.0;
+    for (int b = threadIdx.x; b < blocks; b += blockDim.x) {
+        const double *p = partials + ((int64_t)n * blocks + b) * CAM_SUMS;
+#pragma unroll
+        for (int j = 0; j < CAM_SUMS; ++j) acc[j] += p[j];
+    }
+    const double v = block_sum(acc, sPart);
+    if (k < CAM_SUMS) sTot[k] = v;
+    __syncthreads();
+    if (k < 16) {
+        const int r = k >> 2, c = k & 3;
+        grad_proj[n * 16 + k] = c == 2 ? 0.0f : (float)sTot[3 * r + (c == 3 ? 2 : c)];
+        grad_view[n * 16 + k] = c == 2 ? (float)sTot[12 + r] : 0.0f;
+    }
+    if (grad_cam && k < 3) grad_cam[n * 3 + k] = (float)sTot[16 + k];
+}
+
 }  // namespace dss
 
 extern "C" {
@@ -694,6 +838,62 @@ int dss_render_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
         dim3 grid(nblocks(g->P0, 256, ctx->sm_count, 8), N);
         chain_kernel<<<grid, 256, 32 * sizeof(float), st>>>(c);
     }
+    DSS_LAUNCH_CHECK(ctx);
+    return DSS_OK;
+}
+
+int dss_camera_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_proj, float *grad_view,
+                        float *grad_cam_centres, void *stream) {
+    using namespace dss;
+    cudaStream_t st = (cudaStream_t)stream;
+    // every argument check comes before the first use of the context
+    int rc = check_common(g);
+    if (rc) return rc;
+    DSS_REQUIRE(grad_proj && grad_view, "camera backward needs grad_proj and grad_view");
+    DSS_REQUIRE(g->grad_ndc, "camera backward reads the grad_ndc that dss_render_backward wrote");
+    DSS_REQUIRE(g->points_world && g->proj, "camera backward needs points_world and proj");
+    if (grad_cam_centres) {
+        DSS_REQUIRE(g->shade, "grad_cam_centres needs the fused shading inputs (shade != 0)");
+        DSS_REQUIRE(g->grad_colours, "grad_cam_centres reads d L / d shaded from grad_colours");
+    }
+    DSS_REQUIRE(ctx != nullptr, "ctx is null");
+    const int N = g->n_views;
+    const bool shade = grad_cam_centres != nullptr;
+    if (g->P == 0 || g->P0 == 0) {
+        DSS_CUDA_TRY(cudaMemsetAsync(grad_proj, 0, (size_t)N * 16 * sizeof(float), st));
+        DSS_CUDA_TRY(cudaMemsetAsync(grad_view, 0, (size_t)N * 16 * sizeof(float), st));
+        if (shade) DSS_CUDA_TRY(cudaMemsetAsync(grad_cam_centres, 0, (size_t)N * 3 * sizeof(float), st));
+        return DSS_OK;
+    }
+    // one wave over all views: two blocks per SM fit (~110-130 registers per thread)
+    int64_t want = ((int64_t)ctx->sm_count * 2 + N - 1) / N, need = (g->P0 + 255) / 256;
+    const unsigned int blocks = (unsigned int)(want < need ? want : need);
+    CamArgs c;
+    memset(&c, 0, sizeof(c));
+    c.pts = g->points_world;
+    c.proj = g->proj;
+    c.gndc = g->grad_ndc;
+    c.first_idx = g->first_idx;
+    c.num_points = g->num_points;
+    c.P0 = g->P0;
+    c.shared_cloud = g->shared_cloud;
+    if (shade) {
+        c.nrm = g->normals_world;
+        c.gsh = g->grad_colours;
+        c.sh.albedo = g->albedo;
+        c.sh.lights = g->lights;
+        c.sh.ambient = g->ambient;
+        c.sh.cam = g->cam_centres;
+        c.sh.n_lights = g->n_lights;
+        c.sh.light_type = g->light_type;
+        c.sh.shininess = g->shininess;
+    }
+    if ((rc = ctx_get(ctx, BUF_CAMERA, (size_t)N * blocks * CAM_SUMS, &c.partials))) return rc;
+    StageScope prof(ctx, ST_CAMERA_BWD, st);
+    if (shade) camera_partials_kernel<true><<<dim3(blocks, N), 256, 0, st>>>(c);
+    else camera_partials_kernel<false><<<dim3(blocks, N), 256, 0, st>>>(c);
+    DSS_LAUNCH_CHECK(ctx);
+    camera_finish_kernel<<<N, 256, 0, st>>>(c.partials, (int)blocks, grad_proj, grad_view, grad_cam_centres);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }

@@ -4,10 +4,12 @@ forward  = dss_render_forward : per-(point,view) EWA preprocess -> tile binning 
            per-tile top-K rasterization + normalised blend              (rasterizer.py:584-664, renderer.py:36-82)
 backward = dss_render_backward: visibility / median radius -> occupancy gather -> colour scatter ->
            z scatter -> per-point clip -> chain to world space           (rasterizer.py:788-977, 667-673)
+           [+ dss_camera_backward when proj, view or the shading's camera centres require grad]
 
 Gradients follow the reference exactly: positions receive the occupancy surrogate gradient (and the
-z-buffer gradient when one is supplied), colours receive the compositor gradient, the per-point ellipse
-parameters are constants (computed under no_grad and detached: rasterizer.py:606-608, 562-565).
+z-buffer gradient when one is supplied), colours receive the compositor gradient, the cameras (proj, view,
+shading camera centres) receive what the reference's differentiable transform and shading give them, the
+per-point ellipse parameters are constants (computed under no_grad and detached: rasterizer.py:606-608, 562-565).
 """
 import ctypes as C
 from typing import NamedTuple, Optional
@@ -121,7 +123,8 @@ def _layout(points, proj, first_idx, num_points, shared):
 class _RenderFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, normals, colours, proj, view, h, first_idx, num_points, shared, prm, want_frags,
-                grad_sync=None, shading=None):
+                grad_sync=None, shading=None, cam_centres=None):
+        # cam_centres is shading.cam_centres, passed on its own so that autograd tracks it
         dev = _lib.require_cuda(points, normals, colours, proj, view, h, first_idx, num_points)
         points_c = _lib.as_f32(points.detach(), "points")
         normals_c = _lib.as_f32(normals.detach(), "normals")
@@ -221,11 +224,30 @@ class _RenderFunction(torch.autograd.Function):
             a.normals_world = _lib.ptr(normals_c)
             a.grad_albedo, a.grad_normals_world = _lib.ptr(grad_albedo), _lib.ptr(grad_normals)
             a.grad_points_shading = _lib.ptr(grad_pshade)
+        # camera gradients: only when asked for (the (P,3) NDC gradient is 96 MB at 1M points x 8 views)
+        want_cam = ctx.needs_input_grad[3] or ctx.needs_input_grad[4] or ctx.needs_input_grad[13]
+        grad_proj = grad_view = grad_cam = None
+        if want_cam:
+            grad_ndc = torch.empty((P, 3), dtype=torch.float32, device=dev)
+            a.grad_ndc = _lib.ptr(grad_ndc)
+            grad_proj, grad_view = (torch.empty((N, 4, 4), dtype=torch.float32, device=dev) for _ in range(2))
+            if shade is not None and ctx.needs_input_grad[13]:
+                grad_cam = torch.empty((N, 3), dtype=torch.float32, device=dev)
         lib = _lib.load()
+
+        def camera_backward():
+            # reads grad_ndc and (shading) the d L / d shaded scratch in grad_colours
+            a.grad_colours = _lib.ptr(grad_colours)
+            rc = lib.dss_camera_backward(_lib.ctx(dev), C.byref(a), _lib.ptr(grad_proj), _lib.ptr(grad_view),
+                                         _lib.ptr(grad_cam), _lib.stream_ptr(dev))
+            _lib.check(rc, "dss_camera_backward")
+
         with torch.cuda.device(dev):
             if grad_sync is None:
                 rc = lib.dss_render_backward(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
                 _lib.check(rc, "dss_render_backward")
+                if want_cam:
+                    camera_backward()
             else:
                 # data-parallel step (dss_b200/parallel.py): the colour gradients are final after the colour scatter --
                 # reduce them over the ranks on a side stream while the occupancy path runs here
@@ -246,11 +268,15 @@ class _RenderFunction(torch.autograd.Function):
                 if shade is not None:
                     main.wait_event(shade_done)
                     grad_points += grad_pshade           # position gradient through the shading
+                if want_cam:
+                    # the rank's own views: no collective (shared camera parameters are the caller's to reduce)
+                    camera_backward()
                 grad_sync.reduce_late(grad_points)
                 grad_sync.join(dev)
+        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam,)
         if shade is not None:
-            return (grad_points, grad_normals, grad_albedo) + (None,) * 10
-        return (grad_points, None, grad_colours) + (None,) * 10
+            return (grad_points, grad_normals, grad_albedo) + cams
+        return (grad_points, None, grad_colours) + cams
 
 
 def render_points(points, normals, colours, proj, view, h, params: SplatParams, first_idx=None, num_points=None,
@@ -260,16 +286,19 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     points, normals : (P0,3) when ``shared_cloud`` (one cloud seen from N cameras) else packed (P,3)
     colours         : (N*P0,3) / (P,3) per-(view,point) features (e.g. shaded rgb), or (P0,3) per-point
                       features used by every view of a shared cloud (gradient then summed over the views)
-    proj, view      : (N,4,4) full-projection and world-to-view matrices, row-vector convention
+    proj, view      : (N,4,4) full-projection and world-to-view matrices, row-vector convention; when they require
+                      grad they receive the gradient of the screen positions (proj: x, y; view: the depth)
     h               : (N,) per-view or (P,) per-splat variance scale (rasterizer.py:293-402)
     shading         : optional Shading -- `colours` is then the per-point albedo (P0,3) and the colour of every
                       (view, point) is computed in the preprocess kernel: albedo * (ambient + diffuse) + specular
-                      (DSS/core/texture.py:74-127); gradients flow to the albedo, the NORMALS and the positions
+                      (DSS/core/texture.py:74-127); gradients flow to the albedo, the NORMALS, the positions and,
+                      when it requires grad, shading.cam_centres (not to the lights)
     grad_sync       : optional dss_b200.parallel.GradSync -- the backward then returns gradients already summed over the
                       ranks of a view-sharded step, the collectives overlapped with the backward kernels
     """
     outs = _RenderFunction.apply(points, normals, colours, proj, view, h, first_idx, num_points,
-                                 bool(shared_cloud), params, bool(return_fragments), grad_sync, shading)
+                                 bool(shared_cloud), params, bool(return_fragments), grad_sync, shading,
+                                 shading.cam_centres if shading is not None else None)
     image, idx, weights, visible, records, scaler = outs[:6]
     zbuf, qvalue = (outs[6], outs[7]) if return_fragments else (None, None)
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
@@ -277,7 +306,8 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
 
 def make_shading(lights, view_matrices, shininess=64.0) -> Shading:
     """Shading record for the fused route from a DirectionalLights / PointLights object (dss_b200.core.lighting) and the
-    (N,4,4) world-to-view matrices of the step's cameras."""
+    (N,4,4) world-to-view matrices of the step's cameras.  The camera centres stay differentiable functions of
+    `view_matrices`, so learnable cameras receive the shading's gradient too."""
     from .core.lighting import pack_lights
     from .core.texture import camera_centres
     rows, ambient, kind = pack_lights(lights)

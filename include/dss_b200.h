@@ -290,6 +290,17 @@ DSS_API int dss_render_backward(dss_ctx *ctx, const dss_render_args *args, void 
  * Lets a data-parallel caller start the all-reduce of the colour gradients while dss_render_backward (called with
  * grad_colours == NULL on another stream) is still busy with the occupancy path (dss_b200/parallel.py). */
 DSS_API int dss_colour_backward(dss_ctx *ctx, const dss_render_args *args, void *stream);
+/* Camera gradients, after dss_render_backward has written args->grad_ndc (the clipped NDC gradient of every slot; the
+ * reference differentiates the screen positions through pytorch3d's transform, rasterizer.py:614).  With
+ * p_h = [p 1], clip = p_h proj[n], w = clip3, (x, y) = clip01 / w, summed over the slots of view n:
+ *   grad_proj[n][r][c] = sum p_h[r] (gx / w, gy / w, 0, -(gx x + gy y) / w)[c]      (N,4,4), column 2 zero
+ *   grad_view[n][r][c] = c == 2 ? sum p_h[r] gz : 0                                 (N,4,4)
+ * grad_cam_centres (N,3) or NULL: with fused shading (shade != 0) the gradient w.r.t. cam_centres through the view
+ * direction v = normalize(cam - p); reads the d L / d shaded scratch that the colour backward left in
+ * args->grad_colours and the shading inputs.  The splat shapes (ellipse, radii, scaler) are constants, as in the
+ * reference.  Deterministic: fixed-order fp64 sums, no atomics. */
+DSS_API int dss_camera_backward(dss_ctx *ctx, const dss_render_args *args, float *grad_proj, float *grad_view,
+                                float *grad_cam_centres, void *stream);
 /* per-(point,view) preprocess only (rasterizer.py:443-565 fused): writes ndc, ellipse, radii, scaler. */
 DSS_API int dss_preprocess(dss_ctx *ctx, const dss_render_args *args, void *stream);
 
