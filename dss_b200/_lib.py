@@ -42,7 +42,7 @@ class RenderArgs(C.Structure):
         ("grad_points_world", vp), ("search_radius", vp),
         ("shared_colours", C.c_int32),
         ("shade", C.c_int32), ("n_lights", C.c_int32), ("light_type", C.c_int32), ("shininess", C.c_float),
-        ("reserved0", C.c_int32),
+        ("lights_per_view", C.c_int32),
         ("albedo", vp), ("lights", vp), ("ambient", vp), ("cam_centres", vp), ("shaded", vp),
         ("grad_albedo", vp), ("grad_normals_world", vp), ("grad_points_shading", vp),
         ("cell_counts", vp),
@@ -85,6 +85,7 @@ _SIGNATURES = {
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_colour_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_camera_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp, vp, vp, vp]),
+    "dss_light_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp, vp, vp]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -114,12 +114,21 @@ class PointLights(_Lights):
 
 
 def pack_lights(lights):
-    """-> (rows (L,9) {direction|location, diffuse rgb, specular rgb}, ambient (3,), light_type) for the fused path.
-    The fused path shares one set of lights between the views ("Currently only supports the same lights for all
-    batches", config.py:105)."""
-    for t in (lights.diffuse_color, lights.specular_color, lights._vec, lights.ambient_color):
-        if t.shape[0] != 1:
-            raise ValueError("the fused shading takes one set of lights for all views ((1,L,3) tensors)")
-    rows = torch.cat([lights._vec[0], lights.diffuse_color[0], lights.specular_color[0]], dim=1).contiguous().float()
-    ambient = lights.ambient_color[0].sum(0).contiguous().float()          # texture.py:52-55: ambient colours are summed
-    return rows, ambient, int(lights.kind)
+    """-> (rows, ambient, light_type) for the fused path: rows {direction|location, diffuse rgb, specular rgb}.
+
+    Lights whose properties all have batch 1 (one set for every view) give rows (L,9) and ambient (3,).  Otherwise the
+    set is per view, as the reference's data gives every image its own light: properties of batch 1 broadcast against
+    those of batch N (as pytorch3d's TensorProperties do) and the result is rows (N,L,9), ambient (N,3).  The ambient
+    colours are summed over the lights (texture.py:52-55).  The result is differentiable w.r.t. the light tensors."""
+    props = (lights._vec, lights.diffuse_color, lights.specular_color, lights.ambient_color)
+    batches = sorted({int(t.shape[0]) for t in props})
+    if batches == [1]:
+        rows = torch.cat([lights._vec[0], lights.diffuse_color[0], lights.specular_color[0]], dim=1).contiguous().float()
+        ambient = lights.ambient_color[0].sum(0).contiguous().float()
+        return rows, ambient, int(lights.kind)
+    N = batches[-1]
+    if len(batches) > 2 or (len(batches) == 2 and batches[0] != 1):
+        raise ValueError("light properties must have batch 1 or N, got batches %s" % batches)
+    vec, dif, spe, amb = (t.expand(N, -1, -1) for t in props)
+    rows = torch.cat([vec, dif, spe], dim=2).contiguous().float()
+    return rows, amb.sum(1).contiguous().float(), int(lights.kind)

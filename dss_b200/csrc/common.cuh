@@ -67,6 +67,7 @@ enum BufId {
     BUF_KNN_OFFSETS,  //   exclusive scan of the counts
     BUF_KNN_SORTED,   //   points in cell order {x, y, z, index}
     BUF_CAMERA,       // per-block fp64 partial sums of the camera gradients
+    BUF_LIGHT,        // per-block fp64 partial sums of the light gradients
     NUM_BUFS
 };
 
@@ -76,7 +77,7 @@ namespace dss {
 enum Stage {
     ST_PACK = 0, ST_PREPROCESS, ST_BIN_COUNT, ST_SCAN, ST_BIN_SCATTER, ST_RASTER_FWD, ST_VISIBILITY,
     ST_SEARCH_RADIUS, ST_OCC_BWD, ST_COLOUR_BWD, ST_ZBUF_BWD, ST_CHAIN, ST_GRID, ST_OCC_BIN, ST_KNN,
-    ST_CAMERA_BWD, NUM_STAGES
+    ST_CAMERA_BWD, ST_LIGHT_BWD, NUM_STAGES
 };
 struct ProfPending {
     cudaEvent_t a, b;

@@ -18,8 +18,31 @@ static inline unsigned int nblocks(int64_t items, int threads, int sm_count, int
 struct ShadeArgs {
     const float *albedo, *lights, *ambient, *cam;
     int n_lights, light_type;
+    int per_view;   // lights (N,L,9) and ambient (N,3): one block of rows per view
     float shininess;
 };
+
+// the shading inputs of dss_render_args
+static ShadeArgs shade_args(const dss_render_args *g) {
+    ShadeArgs s;
+    s.albedo = g->albedo;
+    s.lights = g->lights;
+    s.ambient = g->ambient;
+    s.cam = g->cam_centres;
+    s.n_lights = g->n_lights;
+    s.light_type = g->light_type;
+    s.per_view = g->lights_per_view;
+    s.shininess = g->shininess;
+    return s;
+}
+
+// light rows and ambient of view n
+__device__ __forceinline__ const float *view_lights(const ShadeArgs &s, int n) {
+    return s.per_view ? s.lights + (int64_t)n * s.n_lights * 9 : s.lights;
+}
+__device__ __forceinline__ const float *view_ambient(const ShadeArgs &s, int n) {
+    return s.per_view ? s.ambient + (int64_t)n * 3 : s.ambient;
+}
 
 struct PreArgs {
     const float *pts, *nrm, *proj, *view, *h;
@@ -76,7 +99,56 @@ __device__ __forceinline__ V3 normalize3_bwd(V3 y, float len, V3 gy) {
     return mul3(sub3(gy, mul3(y, dot3(y, gy))), 1.0f / len);
 }
 
-// forward (and, with gc != nullptr, backward) of the shading of one (view, point).  sL: lights in shared memory.
+// One light's share of the shading of one (view, point): L is the light's row of 9 floats, nh / v the normalised
+// normal and view direction.  Adds the light's diffuse and specular terms to diff / spec; with BACKWARD (gc = d L / d
+// colour) also its share of d nh and d v to g_nh / g_v, and returns in g_d the gradient w.r.t. the normalised light
+// direction d.  Every user of the shading (forward, shading backward, camera and light gradients) goes through here.
+struct LightTerm {
+    V3 d;          // normalised light direction (direction, or location - p)
+    float dlen;    // clamped norm of the un-normalised one
+    float lam;     // relu(n.d): factor of the diffuse colour
+    float pw;      // (relu(v.r) [n.d > 0])^shininess: factor of the specular colour
+    V3 g_d;        // BACKWARD: d L / d d
+};
+template <bool BACKWARD>
+__device__ __forceinline__ LightTerm shade_light(const float *L, int light_type, float shininess, V3 p, V3 nh, V3 v,
+                                                 V3 alb, V3 gc, V3 &diff, V3 &spec, V3 &g_nh, V3 &g_v) {
+    LightTerm t;
+    const V3 draw = light_type ? sub3(v3(L[0], L[1], L[2]), p) : v3(L[0], L[1], L[2]);
+    t.d = normalize3(draw, t.dlen);
+    const V3 d = t.d;
+    const V3 cd = v3(L[3], L[4], L[5]), cs = v3(L[6], L[7], L[8]);
+    const float cosang = dot3(nh, d);
+    const float lam = fmaxf(cosang, 0.0f);                           // lighting.py:65
+    diff = add3(diff, mul3(cd, lam));
+    const float mask = cosang > 0.0f ? 1.0f : 0.0f;                   // :158
+    const V3 r = add3(mul3(d, -1.0f), mul3(nh, 2.0f * cosang));       // :163
+    const float vr = dot3(v, r);
+    const float alpha = fmaxf(vr, 0.0f) * mask;                       // :166-167
+    const float pw = alpha > 0.0f ? powf(alpha, shininess) : 0.0f;    // :169
+    spec = add3(spec, mul3(cs, pw));
+    t.lam = lam;
+    t.pw = pw;
+    if (BACKWARD) {
+        // diffuse: d/d cos = sum_c (gc*alb)_c cd_c  where cos > 0
+        float g_cos = (cosang > 0.0f) ? (gc.x * alb.x * cd.x + gc.y * alb.y * cd.y + gc.z * alb.z * cd.z) : 0.0f;
+        V3 g_d = v3(0.f, 0.f, 0.f);
+        if (alpha > 0.0f) {
+            const float g_alpha = dot3(gc, cs) * shininess * powf(alpha, shininess - 1.0f);
+            const float g_vr = g_alpha;                                // alpha = vr where vr > 0 and mask = 1
+            const V3 g_r = mul3(v, g_vr);
+            g_v = add3(g_v, mul3(r, g_vr));
+            g_cos += 2.0f * dot3(g_r, nh);
+            g_nh = add3(g_nh, mul3(g_r, 2.0f * cosang));
+            g_d = sub3(g_d, g_r);
+        }
+        g_nh = add3(g_nh, mul3(d, g_cos));
+        t.g_d = add3(g_d, mul3(nh, g_cos));
+    }
+    return t;
+}
+
+// forward (and, with gc != nullptr, backward) of the shading of one (view, point).  sL: the view's lights.
 //   colour = albedo * (ambient + diffuse) + specular
 // backward: accumulates d albedo, d normal (un-normalised input normal), d position into g_alb / g_nrm / g_pos, and
 // with CAM_GRAD the camera-centre gradient (the view-direction half of d position, opposite sign) into *g_cam.
@@ -90,37 +162,9 @@ __device__ __forceinline__ V3 shade_point(const float *sL, int n_lights, int lig
     V3 diff = v3(0.f, 0.f, 0.f), spec = v3(0.f, 0.f, 0.f);
     V3 g_nh = v3(0.f, 0.f, 0.f), g_v = v3(0.f, 0.f, 0.f);
     for (int l = 0; l < n_lights; ++l) {
-        const float *L = sL + l * 9;
-        float dlen;
-        const V3 draw = light_type ? sub3(v3(L[0], L[1], L[2]), p) : v3(L[0], L[1], L[2]);
-        const V3 d = normalize3(draw, dlen);
-        const V3 cd = v3(L[3], L[4], L[5]), cs = v3(L[6], L[7], L[8]);
-        const float cosang = dot3(nh, d);
-        const float lam = fmaxf(cosang, 0.0f);                           // lighting.py:65
-        diff = add3(diff, mul3(cd, lam));
-        const float mask = cosang > 0.0f ? 1.0f : 0.0f;                   // :158
-        const V3 r = add3(mul3(d, -1.0f), mul3(nh, 2.0f * cosang));       // :163
-        const float vr = dot3(v, r);
-        const float alpha = fmaxf(vr, 0.0f) * mask;                       // :166-167
-        const float pw = alpha > 0.0f ? powf(alpha, shininess) : 0.0f;    // :169
-        spec = add3(spec, mul3(cs, pw));
-        if (BACKWARD) {
-            // diffuse: d/d cos = sum_c (gc*alb)_c cd_c  where cos > 0
-            float g_cos = (cosang > 0.0f) ? (gc.x * alb.x * cd.x + gc.y * alb.y * cd.y + gc.z * alb.z * cd.z) : 0.0f;
-            V3 g_d = v3(0.f, 0.f, 0.f);
-            if (alpha > 0.0f) {
-                const float g_alpha = dot3(gc, cs) * shininess * powf(alpha, shininess - 1.0f);
-                const float g_vr = g_alpha;                                // alpha = vr where vr > 0 and mask = 1
-                const V3 g_r = mul3(v, g_vr);
-                g_v = add3(g_v, mul3(r, g_vr));
-                g_cos += 2.0f * dot3(g_r, nh);
-                g_nh = add3(g_nh, mul3(g_r, 2.0f * cosang));
-                g_d = sub3(g_d, g_r);
-            }
-            g_nh = add3(g_nh, mul3(d, g_cos));
-            g_d = add3(g_d, mul3(nh, g_cos));
-            if (light_type) g_pos = sub3(g_pos, normalize3_bwd(d, dlen, g_d));   // d = normalize(loc - p)
-        }
+        const LightTerm t = shade_light<BACKWARD>(sL + l * 9, light_type, shininess, p, nh, v, alb, gc, diff, spec, g_nh,
+                                                  g_v);
+        if (BACKWARD && light_type) g_pos = sub3(g_pos, normalize3_bwd(t.d, t.dlen, t.g_d));   // d = normalize(loc - p)
     }
     if (BACKWARD) {
         g_alb = add3(g_alb, v3(gc.x * (amb.x + diff.x), gc.y * (amb.y + diff.y), gc.z * (amb.z + diff.z)));
@@ -151,9 +195,9 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
     }
     constexpr bool shade = SHADE;
     if (shade) {
-        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = a.sh.lights[threadIdx.x];
+        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = view_lights(a.sh, n)[threadIdx.x];
         if (threadIdx.x < 3) {
-            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = a.sh.ambient[threadIdx.x];
+            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(a.sh, n)[threadIdx.x];
             sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
         }
     }
@@ -276,13 +320,14 @@ struct ShadeBwdArgs {
 };
 
 __global__ void __launch_bounds__(256) shade_backward_kernel(const __grid_constant__ ShadeBwdArgs a) {
-    extern __shared__ float sS[];   // lights (L*9), ambient (3), camera centres (N*3)
-    const int nl9 = a.sh.n_lights * 9;
-    for (int i = threadIdx.x; i < nl9; i += blockDim.x) sS[i] = a.sh.lights[i];
-    for (int i = threadIdx.x; i < 3; i += blockDim.x) sS[nl9 + i] = a.sh.ambient[i];
-    for (int i = threadIdx.x; i < a.N * 3; i += blockDim.x) sS[nl9 + 3 + i] = a.sh.cam[i];
+    // lights (L*9) and ambient (3), once or (per_view) for every view, then the camera centres (N*3)
+    extern __shared__ float sS[];
+    const int nl9 = a.sh.n_lights * 9, stride = nl9 + 3, rows = a.sh.per_view ? a.N : 1;
+    for (int i = threadIdx.x; i < rows * nl9; i += blockDim.x) sS[(i / nl9) * stride + i % nl9] = a.sh.lights[i];
+    for (int i = threadIdx.x; i < rows * 3; i += blockDim.x) sS[(i / 3) * stride + nl9 + i % 3] = a.sh.ambient[i];
+    float *sC = sS + rows * stride;
+    for (int i = threadIdx.x; i < a.N * 3; i += blockDim.x) sC[i] = a.sh.cam[i];
     __syncthreads();
-    const V3 amb = v3(sS[nl9], sS[nl9 + 1], sS[nl9 + 2]);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.P0; i += (int64_t)gridDim.x * blockDim.x) {
         const V3 p = v3(a.pts[i * 3], a.pts[i * 3 + 1], a.pts[i * 3 + 2]);
         const V3 nrm = v3(a.nrm[i * 3], a.nrm[i * 3 + 1], a.nrm[i * 3 + 2]);
@@ -292,9 +337,9 @@ __global__ void __launch_bounds__(256) shade_backward_kernel(const __grid_consta
             const float *g = a.gsh + ((int64_t)n * a.P0 + i) * 3;
             const V3 gc = v3(g[0], g[1], g[2]);
             if (gc.x == 0.0f && gc.y == 0.0f && gc.z == 0.0f) continue;
-            const float *c = sS + nl9 + 3 + n * 3;
-            shade_point<true>(sS, a.sh.n_lights, a.sh.light_type, a.sh.shininess, amb, p, nrm, alb, v3(c[0], c[1], c[2]), gc,
-                              ga, gn, gp);
+            const float *c = sC + n * 3, *L = sS + (a.sh.per_view ? n * stride : 0);
+            shade_point<true>(L, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(L[nl9], L[nl9 + 1], L[nl9 + 2]), p, nrm,
+                              alb, v3(c[0], c[1], c[2]), gc, ga, gn, gp);
         }
         a.g_alb[i * 3] = ga.x, a.g_alb[i * 3 + 1] = ga.y, a.g_alb[i * 3 + 2] = ga.z;
         a.g_nrm[i * 3] = gn.x, a.g_nrm[i * 3 + 1] = gn.y, a.g_nrm[i * 3 + 2] = gn.z;
@@ -344,20 +389,17 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     b.pts = g->points_world;
     b.nrm = g->normals_world;
     b.gsh = g->grad_colours;
-    b.sh.albedo = g->albedo;
-    b.sh.lights = g->lights;
-    b.sh.ambient = g->ambient;
-    b.sh.cam = g->cam_centres;
-    b.sh.n_lights = g->n_lights;
-    b.sh.light_type = g->light_type;
-    b.sh.shininess = g->shininess;
+    b.sh = shade_args(g);
     b.P0 = g->P0;
     b.N = N;
     b.g_alb = g->grad_albedo;
     b.g_nrm = g->grad_normals_world;
     b.g_pos = g->grad_points_shading;
+    // per-view lights at the limits (256 views x 8 lights) take 78 KB: more than the default 48 KB of dynamic shared memory
+    const size_t smem = (size_t)((g->n_lights * 9 + 3) * (g->lights_per_view ? N : 1) + N * 3) * sizeof(float);
+    if (smem > 48 * 1024)
+        DSS_CUDA_TRY(cudaFuncSetAttribute(shade_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     StageScope prof(ctx, ST_COLOUR_BWD, on);
-    const size_t smem = (size_t)(g->n_lights * 9 + 3 + N * 3) * sizeof(float);
     shade_backward_kernel<<<nblocks(g->P0, 256, ctx->sm_count, 8), 256, smem, on>>>(b);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
@@ -380,6 +422,8 @@ static int check_common(const dss_render_args *g) {
         DSS_REQUIRE(g->albedo && g->lights && g->ambient && g->cam_centres && g->normals_world, "shading needs albedo, lights, ambient, cam_centres, normals");
         DSS_REQUIRE(g->light_type == 0 || g->light_type == 1, "light_type must be 0 (directional) or 1 (point)");
     }
+    DSS_REQUIRE(g->lights_per_view == 0 || g->lights_per_view == 1, "lights_per_view must be 0 or 1");
+    DSS_REQUIRE(!g->lights_per_view || g->shade, "lights_per_view needs the fused shading (shade != 0)");
     return DSS_OK;
 }
 
@@ -416,13 +460,7 @@ static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, c
     memset(&a.sh, 0, sizeof(a.sh));
     a.shaded = nullptr;
     if (g->shade && g->shaded) {
-        a.sh.albedo = g->albedo;
-        a.sh.lights = g->lights;
-        a.sh.ambient = g->ambient;
-        a.sh.cam = g->cam_centres;
-        a.sh.n_lights = g->n_lights;
-        a.sh.light_type = g->light_type;
-        a.sh.shininess = g->shininess;
+        a.sh = shade_args(g);
         a.shaded = g->shaded;
     }
     dim3 grid(nblocks(g->P0, 256, ctx->sm_count, 8), g->n_views);
@@ -585,12 +623,13 @@ struct CamArgs {
     double *partials;         // (N, gridDim.x, CAM_SUMS)
 };
 
-// sum of acc[k] over the block (blockDim.x a multiple of 32, at most 256) in a fixed order; thread k < CAM_SUMS
+// sum of acc[k] over the block (blockDim.x a multiple of 32, at most 256) in a fixed order; thread k < K
 // returns sum k, the others 0
-__device__ __forceinline__ double block_sum(const double (&acc)[CAM_SUMS], double (*sPart)[CAM_SUMS]) {
+template <int K>
+__device__ __forceinline__ double block_sum(const double (&acc)[K], double (*sPart)[K]) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-    for (int k = 0; k < CAM_SUMS; ++k) {
+    for (int k = 0; k < K; ++k) {
         double v = acc[k];
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -598,7 +637,7 @@ __device__ __forceinline__ double block_sum(const double (&acc)[CAM_SUMS], doubl
     }
     __syncthreads();
     double v = 0.0;
-    if (threadIdx.x < CAM_SUMS)
+    if (threadIdx.x < K)
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += sPart[w][threadIdx.x];
     return v;
 }
@@ -613,9 +652,9 @@ __global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_const
     const int n = blockIdx.y;
     if (threadIdx.x < 16) sM[threadIdx.x] = a.proj[n * 16 + threadIdx.x];
     if (SHADE) {
-        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = a.sh.lights[threadIdx.x];
+        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = view_lights(a.sh, n)[threadIdx.x];
         if (threadIdx.x < 3) {
-            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = a.sh.ambient[threadIdx.x];
+            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(a.sh, n)[threadIdx.x];
             sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
         }
     }
@@ -700,6 +739,107 @@ __global__ void __launch_bounds__(256) camera_finish_kernel(const double *partia
         grad_view[n * 16 + k] = c == 2 ? (float)sTot[12 + r] : 0.0f;
     }
     if (grad_cam && k < 3) grad_cam[n * 3 + k] = (float)sTot[16 + k];
+}
+
+// ---------------------------------------------------------------------------------------------
+// Light gradients (the reference's lights are tensors that autograd reaches through lighting.py:10-172).  Light l's
+// share of the gradient depends only on its own terms and the normalised normal and view direction of the
+// (view, point); with gc = d L / d shaded:
+//   g_vec = normalize_bwd(d, g_d)   (direction; for point lights the location: d = normalize(loc - p))
+//   g_cd = gc * alb * relu(n.d),   g_cs = gc * pw,   g_amb = gc * alb   (ambient: summed over the lights' terms)
+// Pass 1: grid (point blocks, views, lights), every block writes its LIGHT_SUMS sums (fp64) to a partials array, the
+// ambient ones from the l = 0 slice.  Pass 2: one block per (light, output row) adds the partials in a fixed order.
+// ---------------------------------------------------------------------------------------------
+constexpr int LIGHT_SUMS = 12;   // direction or location (3), diffuse rgb (3), specular rgb (3), ambient rgb (3)
+
+struct LightArgs {
+    const float *pts, *nrm, *gsh;
+    ShadeArgs sh;
+    int64_t P0;
+    double *partials;   // (N, gridDim.z, gridDim.x, LIGHT_SUMS)
+};
+
+__global__ void __launch_bounds__(256) light_partials_kernel(const __grid_constant__ LightArgs a) {
+    __shared__ float sL[9 + 3];   // the light's row, camera centre
+    __shared__ double sPart[8][LIGHT_SUMS];
+    const int n = blockIdx.y, l = blockIdx.z;
+    if (threadIdx.x < 9) sL[threadIdx.x] = view_lights(a.sh, n)[l * 9 + threadIdx.x];
+    if (threadIdx.x < 3) sL[9 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
+    __syncthreads();
+    const V3 cam = v3(sL[9], sL[10], sL[11]);
+    double acc[LIGHT_SUMS];
+#pragma unroll
+    for (int k = 0; k < LIGHT_SUMS; ++k) acc[k] = 0.0;
+    const float *gsh = a.gsh + (int64_t)n * a.P0 * 3;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < a.P0; i0 += CAM_BATCH * stride) {
+        float g[CAM_BATCH][3];
+#pragma unroll
+        for (int j = 0; j < CAM_BATCH; ++j) {
+            const int64_t i = i0 + j * stride;
+#pragma unroll
+            for (int e = 0; e < 3; ++e) g[j][e] = i < a.P0 ? gsh[i * 3 + e] : 0.0f;
+        }
+#pragma unroll
+        for (int j = 0; j < CAM_BATCH; ++j) {
+            const V3 gc = v3(g[j][0], g[j][1], g[j][2]);
+            if (gc.x == 0.0f && gc.y == 0.0f && gc.z == 0.0f) continue;
+            const int64_t i = i0 + j * stride;
+            const V3 p = v3(a.pts[i * 3], a.pts[i * 3 + 1], a.pts[i * 3 + 2]);
+            const V3 alb = v3(a.sh.albedo[i * 3], a.sh.albedo[i * 3 + 1], a.sh.albedo[i * 3 + 2]);
+            float nlen, vlen;
+            const V3 nh = normalize3(v3(a.nrm[i * 3], a.nrm[i * 3 + 1], a.nrm[i * 3 + 2]), nlen);
+            const V3 v = normalize3(sub3(cam, p), vlen);
+            V3 diff = v3(0.f, 0.f, 0.f), spec = v3(0.f, 0.f, 0.f), g_nh = v3(0.f, 0.f, 0.f), g_v = v3(0.f, 0.f, 0.f);
+            const LightTerm t = shade_light<true>(sL, a.sh.light_type, a.sh.shininess, p, nh, v, alb, gc, diff, spec, g_nh,
+                                                  g_v);
+            const V3 gvec = normalize3_bwd(t.d, t.dlen, t.g_d);
+            const V3 ga = v3(gc.x * alb.x, gc.y * alb.y, gc.z * alb.z);
+            acc[0] += (double)gvec.x;
+            acc[1] += (double)gvec.y;
+            acc[2] += (double)gvec.z;
+            acc[3] += (double)(ga.x * t.lam);
+            acc[4] += (double)(ga.y * t.lam);
+            acc[5] += (double)(ga.z * t.lam);
+            acc[6] += (double)(gc.x * t.pw);
+            acc[7] += (double)(gc.y * t.pw);
+            acc[8] += (double)(gc.z * t.pw);
+            if (l == 0) {
+                acc[9] += (double)ga.x;
+                acc[10] += (double)ga.y;
+                acc[11] += (double)ga.z;
+            }
+        }
+    }
+    const double v = block_sum(acc, sPart);
+    if (threadIdx.x < LIGHT_SUMS)
+        a.partials[(((int64_t)n * gridDim.z + l) * gridDim.x + blockIdx.x) * LIGHT_SUMS + threadIdx.x] = v;
+}
+
+// block (l, m): light l of output row m -- view m with per-view lights (its partials in block order), the only row with
+// shared lights (the partials of view 0 in block order, then view 1, ...).  Each thread adds a fixed, strided subset,
+// block_sum combines them in a fixed order.
+__global__ void __launch_bounds__(256) light_finish_kernel(const double *partials, int blocks, int n_views, int per_view,
+                                                           float *grad_lights, float *grad_ambient) {
+    __shared__ double sPart[8][LIGHT_SUMS];
+    __shared__ double sTot[LIGHT_SUMS];
+    const int l = blockIdx.x, m = blockIdx.y, nl = gridDim.x, k = threadIdx.x;
+    const int n0 = per_view ? m : 0;
+    const int64_t count = (int64_t)(per_view ? 1 : n_views) * blocks;
+    double acc[LIGHT_SUMS];
+#pragma unroll
+    for (int j = 0; j < LIGHT_SUMS; ++j) acc[j] = 0.0;
+    for (int64_t e = threadIdx.x; e < count; e += blockDim.x) {
+        const int64_t n = n0 + e / blocks, b = e % blocks;
+        const double *p = partials + ((n * nl + l) * blocks + b) * LIGHT_SUMS;
+#pragma unroll
+        for (int j = 0; j < LIGHT_SUMS; ++j) acc[j] += p[j];
+    }
+    const double v = block_sum(acc, sPart);
+    if (k < LIGHT_SUMS) sTot[k] = v;
+    __syncthreads();
+    if (grad_lights && k < 9) grad_lights[((int64_t)m * nl + l) * 9 + k] = (float)sTot[k];
+    if (grad_ambient && l == 0 && k < 3) grad_ambient[m * 3 + k] = (float)sTot[9 + k];
 }
 
 }  // namespace dss
@@ -880,13 +1020,7 @@ int dss_camera_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_proj
     if (shade) {
         c.nrm = g->normals_world;
         c.gsh = g->grad_colours;
-        c.sh.albedo = g->albedo;
-        c.sh.lights = g->lights;
-        c.sh.ambient = g->ambient;
-        c.sh.cam = g->cam_centres;
-        c.sh.n_lights = g->n_lights;
-        c.sh.light_type = g->light_type;
-        c.sh.shininess = g->shininess;
+        c.sh = shade_args(g);
     }
     if ((rc = ctx_get(ctx, BUF_CAMERA, (size_t)N * blocks * CAM_SUMS, &c.partials))) return rc;
     StageScope prof(ctx, ST_CAMERA_BWD, st);
@@ -894,6 +1028,44 @@ int dss_camera_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_proj
     else camera_partials_kernel<false><<<dim3(blocks, N), 256, 0, st>>>(c);
     DSS_LAUNCH_CHECK(ctx);
     camera_finish_kernel<<<N, 256, 0, st>>>(c.partials, (int)blocks, grad_proj, grad_view, grad_cam_centres);
+    DSS_LAUNCH_CHECK(ctx);
+    return DSS_OK;
+}
+
+int dss_light_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_lights, float *grad_ambient, void *stream) {
+    using namespace dss;
+    cudaStream_t st = (cudaStream_t)stream;
+    // every argument check comes before the first use of the context
+    int rc = check_common(g);
+    if (rc) return rc;
+    DSS_REQUIRE(g->shade, "light backward needs the fused shading inputs (shade != 0)");
+    DSS_REQUIRE(g->grad_colours, "light backward reads d L / d shaded from grad_colours");
+    DSS_REQUIRE(g->points_world, "light backward needs points_world");
+    DSS_REQUIRE(ctx != nullptr, "ctx is null");
+    const int N = g->n_views, L = g->n_lights, rows = g->lights_per_view ? N : 1;
+    if (!grad_lights && !grad_ambient) return DSS_OK;
+    if (g->P0 == 0) {
+        if (grad_lights) DSS_CUDA_TRY(cudaMemsetAsync(grad_lights, 0, (size_t)rows * L * 9 * sizeof(float), st));
+        if (grad_ambient) DSS_CUDA_TRY(cudaMemsetAsync(grad_ambient, 0, (size_t)rows * 3 * sizeof(float), st));
+        return DSS_OK;
+    }
+    // the ambient sums live in the l = 0 slice: without grad_lights that slice is all that is needed
+    const int nl = grad_lights ? L : 1;
+    // one wave over all (view, light) slices, two blocks per SM, as the camera kernels
+    int64_t want = ((int64_t)ctx->sm_count * 2 + (int64_t)N * nl - 1) / ((int64_t)N * nl), need = (g->P0 + 255) / 256;
+    const unsigned int blocks = (unsigned int)(want < need ? want : need);
+    LightArgs c;
+    c.pts = g->points_world;
+    c.nrm = g->normals_world;
+    c.gsh = g->grad_colours;
+    c.sh = shade_args(g);
+    c.P0 = g->P0;
+    if ((rc = ctx_get(ctx, BUF_LIGHT, (size_t)N * nl * blocks * LIGHT_SUMS, &c.partials))) return rc;
+    StageScope prof(ctx, ST_LIGHT_BWD, st);
+    light_partials_kernel<<<dim3(blocks, N, nl), 256, 0, st>>>(c);
+    DSS_LAUNCH_CHECK(ctx);
+    light_finish_kernel<<<dim3(nl, rows), 256, 0, st>>>(c.partials, (int)blocks, N, g->lights_per_view, grad_lights,
+                                                          grad_ambient);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }

@@ -33,9 +33,10 @@ class GraphedRenderStep:
         leaf = lambda t: t.detach().clone().requires_grad_(True)
         self.points, self.colours = leaf(points), leaf(colours)
         self.normals = leaf(normals) if shading is not None else normals.detach().clone()
-        # the cameras are constants of the captured step (no camera gradients)
+        # the cameras and the lights (shared or per view) are constants of the captured step (no gradients to them)
         self._args = (self.points, self.normals, self.colours, proj.detach(), view.detach(), h, params)
-        self._shading = shading._replace(cam_centres=shading.cam_centres.detach()) if shading is not None else None
+        self._shading = shading._replace(cam_centres=shading.cam_centres.detach(), lights=shading.lights.detach(),
+                                         ambient=shading.ambient.detach()) if shading is not None else None
         if grad_sync is not None and grad_sync.world_size > 1:
             # capturing the two overlapped NCCL all-reduces (issued from two streams inside the
             # backward) deadlocks at replay -- a view-sharded step is launched eagerly

@@ -5,11 +5,13 @@ forward  = dss_render_forward : per-(point,view) EWA preprocess -> tile binning 
 backward = dss_render_backward: visibility / median radius -> occupancy gather -> colour scatter ->
            z scatter -> per-point clip -> chain to world space           (rasterizer.py:788-977, 667-673)
            [+ dss_camera_backward when proj, view or the shading's camera centres require grad]
+           [+ dss_light_backward when the shading's lights or ambient colour require grad]
 
 Gradients follow the reference exactly: positions receive the occupancy surrogate gradient (and the
 z-buffer gradient when one is supplied), colours receive the compositor gradient, the cameras (proj, view,
-shading camera centres) receive what the reference's differentiable transform and shading give them, the
-per-point ellipse parameters are constants (computed under no_grad and detached: rasterizer.py:606-608, 562-565).
+shading camera centres) and the shading's lights receive what the reference's differentiable transform and shading
+give them, the shininess and the per-point ellipse parameters are constants (computed under no_grad and detached:
+rasterizer.py:606-608, 562-565).
 """
 import ctypes as C
 from typing import NamedTuple, Optional
@@ -37,8 +39,8 @@ class SplatParams(NamedTuple):
 class Shading(NamedTuple):
     """Fused per-point shading (SURVEY.md 8(f)3): pass as ``shading=`` with the per-point albedo as ``colours``.
     Build it from the light objects with :func:`make_shading`."""
-    lights: torch.Tensor         # (L,9) {direction | location, diffuse rgb, specular rgb}
-    ambient: torch.Tensor        # (3,)
+    lights: torch.Tensor         # (L,9) {direction | location, diffuse rgb, specular rgb}, or (N,L,9): a set per view
+    ambient: torch.Tensor        # (3,), or (N,3) with per-view lights
     cam_centres: torch.Tensor    # (N,3) camera centres in world space
     light_type: int = 0          # 0 directional, 1 point
     shininess: float = 64.0
@@ -57,7 +59,8 @@ class RenderOutput(NamedTuple):
 
 def _fill_shading(a, sh, albedo):
     a.shade = 1
-    a.n_lights = int(sh.lights.shape[0])
+    a.n_lights = int(sh.lights.shape[-2])
+    a.lights_per_view = int(sh.lights.dim() == 3)
     a.light_type = int(sh.light_type)
     a.shininess = float(sh.shininess)
     a.albedo, a.lights, a.ambient, a.cam_centres = _lib.ptr(albedo), _lib.ptr(sh.lights), _lib.ptr(sh.ambient), \
@@ -65,10 +68,13 @@ def _fill_shading(a, sh, albedo):
 
 
 def _check_shading(sh, N, dev):
-    if sh.lights.dim() != 2 or sh.lights.shape[1] != 9 or not (1 <= sh.lights.shape[0] <= _lib.MAX_LIGHTS):
-        raise RuntimeError("shading.lights must be (L,9) with 1 <= L <= %d" % _lib.MAX_LIGHTS)
-    if tuple(sh.ambient.shape) != (3,) or tuple(sh.cam_centres.shape) != (N, 3):
-        raise RuntimeError("shading.ambient must be (3,) and shading.cam_centres (N,3)")
+    per_view = sh.lights.dim() == 3
+    if (sh.lights.dim() not in (2, 3) or sh.lights.shape[-1] != 9 or not (1 <= sh.lights.shape[-2] <= _lib.MAX_LIGHTS)
+            or (per_view and sh.lights.shape[0] != N)):
+        raise RuntimeError("shading.lights must be (L,9) or, per view, (%d,L,9) with 1 <= L <= %d, got %s"
+                           % (N, _lib.MAX_LIGHTS, tuple(sh.lights.shape)))
+    if tuple(sh.ambient.shape) != ((N, 3) if per_view else (3,)) or tuple(sh.cam_centres.shape) != (N, 3):
+        raise RuntimeError("shading.ambient must be (3,), or (N,3) with per-view lights, and shading.cam_centres (N,3)")
     _lib.require_cuda(sh.lights, sh.ambient, sh.cam_centres)
     return Shading(_lib.as_f32(sh.lights.detach(), "lights"), _lib.as_f32(sh.ambient.detach(), "ambient"),
                    _lib.as_f32(sh.cam_centres.detach(), "cam_centres"), int(sh.light_type), float(sh.shininess))
@@ -123,8 +129,8 @@ def _layout(points, proj, first_idx, num_points, shared):
 class _RenderFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, normals, colours, proj, view, h, first_idx, num_points, shared, prm, want_frags,
-                grad_sync=None, shading=None, cam_centres=None):
-        # cam_centres is shading.cam_centres, passed on its own so that autograd tracks it
+                grad_sync=None, shading=None, cam_centres=None, lights=None, ambient=None):
+        # cam_centres, lights and ambient are the shading's tensors, passed on their own so that autograd tracks them
         dev = _lib.require_cuda(points, normals, colours, proj, view, h, first_idx, num_points)
         points_c = _lib.as_f32(points.detach(), "points")
         normals_c = _lib.as_f32(normals.detach(), "normals")
@@ -233,7 +239,21 @@ class _RenderFunction(torch.autograd.Function):
             grad_proj, grad_view = (torch.empty((N, 4, 4), dtype=torch.float32, device=dev) for _ in range(2))
             if shade is not None and ctx.needs_input_grad[13]:
                 grad_cam = torch.empty((N, 3), dtype=torch.float32, device=dev)
+        # light gradients: only when asked for, in the shape of the shading's tensors
+        grad_lights = grad_amb = None
+        if shade is not None:
+            sh = shade[0]
+            grad_lights = torch.empty_like(sh.lights) if ctx.needs_input_grad[14] else None
+            grad_amb = torch.empty_like(sh.ambient) if ctx.needs_input_grad[15] else None
+        want_light = grad_lights is not None or grad_amb is not None
         lib = _lib.load()
+
+        def light_backward():
+            # reads the d L / d shaded scratch in grad_colours
+            a.grad_colours = _lib.ptr(grad_colours)
+            rc = lib.dss_light_backward(_lib.ctx(dev), C.byref(a), _lib.ptr(grad_lights), _lib.ptr(grad_amb),
+                                        _lib.stream_ptr(dev))
+            _lib.check(rc, "dss_light_backward")
 
         def camera_backward():
             # reads grad_ndc and (shading) the d L / d shaded scratch in grad_colours
@@ -248,6 +268,8 @@ class _RenderFunction(torch.autograd.Function):
                 _lib.check(rc, "dss_render_backward")
                 if want_cam:
                     camera_backward()
+                if want_light:
+                    light_backward()
             else:
                 # data-parallel step (dss_b200/parallel.py): the colour gradients are final after the colour scatter --
                 # reduce them over the ranks on a side stream while the occupancy path runs here
@@ -271,9 +293,12 @@ class _RenderFunction(torch.autograd.Function):
                 if want_cam:
                     # the rank's own views: no collective (shared camera parameters are the caller's to reduce)
                     camera_backward()
+                if want_light:
+                    # after the shading work of the side stream (waited for above); no collective either
+                    light_backward()
                 grad_sync.reduce_late(grad_points)
                 grad_sync.join(dev)
-        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam,)
+        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb)
         if shade is not None:
             return (grad_points, grad_normals, grad_albedo) + cams
         return (grad_points, None, grad_colours) + cams
@@ -292,13 +317,15 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     shading         : optional Shading -- `colours` is then the per-point albedo (P0,3) and the colour of every
                       (view, point) is computed in the preprocess kernel: albedo * (ambient + diffuse) + specular
                       (DSS/core/texture.py:74-127); gradients flow to the albedo, the NORMALS, the positions and,
-                      when it requires grad, shading.cam_centres (not to the lights)
+                      when they require grad, shading.cam_centres, shading.lights and shading.ambient (hence to the
+                      light objects' tensors through make_shading); the shininess stays a constant
     grad_sync       : optional dss_b200.parallel.GradSync -- the backward then returns gradients already summed over the
                       ranks of a view-sharded step, the collectives overlapped with the backward kernels
     """
     outs = _RenderFunction.apply(points, normals, colours, proj, view, h, first_idx, num_points,
                                  bool(shared_cloud), params, bool(return_fragments), grad_sync, shading,
-                                 shading.cam_centres if shading is not None else None)
+                                 *((shading.cam_centres, shading.lights, shading.ambient) if shading is not None
+                                   else (None, None, None)))
     image, idx, weights, visible, records, scaler = outs[:6]
     zbuf, qvalue = (outs[6], outs[7]) if return_fragments else (None, None)
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
@@ -306,11 +333,16 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
 
 def make_shading(lights, view_matrices, shininess=64.0) -> Shading:
     """Shading record for the fused route from a DirectionalLights / PointLights object (dss_b200.core.lighting) and the
-    (N,4,4) world-to-view matrices of the step's cameras.  The camera centres stay differentiable functions of
-    `view_matrices`, so learnable cameras receive the shading's gradient too."""
+    (N,4,4) world-to-view matrices of the step's cameras.  Lights of batch 1 are shared by the views, lights of batch N
+    give every view its own set (see pack_lights).  The camera centres and the light rows stay differentiable functions
+    of `view_matrices` and of the light tensors, so learnable cameras and lights receive the shading's gradient too."""
     from .core.lighting import pack_lights
     from .core.texture import camera_centres
     rows, ambient, kind = pack_lights(lights)
+    N = view_matrices.shape[0]
+    if rows.dim() == 3 and rows.shape[0] != N:
+        raise ValueError("the lights have batch %d: the fused shading takes lights of batch 1 or N = %d"
+                         % (rows.shape[0], N))
     dev = view_matrices.device
     return Shading(rows.to(dev), ambient.to(dev), camera_centres(view_matrices).contiguous().float(), kind, float(shininess))
 

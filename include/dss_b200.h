@@ -260,10 +260,13 @@ typedef struct dss_render_args {
     int32_t n_lights;              /* L, 1 .. DSS_MAX_LIGHTS                                       */
     int32_t light_type;            /* 0: directional (rows of `lights` start with a direction), 1: point (a location) */
     float shininess;               /* specular exponent (texture.py:76: 64)                        */
-    int32_t reserved0;
+    /* 0: one set of lights for every view, `lights` (L,9) and `ambient` (3,).  1 (shade only): a set per view, as the
+     * reference's data gives every image its own light (texture.py:113-114 gathers the light properties per view):
+     * `lights` (N,L,9) and `ambient` (N,3), view n's rows at lights + n*L*9 and ambient + n*3. */
+    int32_t lights_per_view;
     const float *albedo;           /* (P0,3) per-point rgb                                         */
-    const float *lights;           /* (L,9) {direction | location, diffuse rgb, specular rgb}      */
-    const float *ambient;          /* (3,) ambient colour (summed over the lights' ambient terms)  */
+    const float *lights;           /* (L,9) {direction | location, diffuse rgb, specular rgb}, or (N,L,9) per view */
+    const float *ambient;          /* (3,) ambient colour (summed over the lights' ambient terms), or (N,3) per view */
     const float *cam_centres;      /* (N,3) camera centres in world space                          */
     float *shaded;                 /* (P,3) shaded colours: written by the forward, the blend reads them */
     /* backward (shade): `grad_colours` is then a (P,3) SCRATCH that receives d L / d shaded; outputs: */
@@ -301,6 +304,14 @@ DSS_API int dss_colour_backward(dss_ctx *ctx, const dss_render_args *args, void 
  * reference.  Deterministic: fixed-order fp64 sums, no atomics. */
 DSS_API int dss_camera_backward(dss_ctx *ctx, const dss_render_args *args, float *grad_proj, float *grad_view,
                                 float *grad_cam_centres, void *stream);
+/* Light gradients of the fused shading (shade != 0), after the colour backward has left d L / d shaded in
+ * args->grad_colours (as for grad_cam_centres above).  Outputs have the shape of the inputs: grad_lights (L,9) and
+ * grad_ambient (3,), summed over the views, or (N,L,9) and (N,3) with lights_per_view.  Row l holds the gradient w.r.t.
+ * light l's direction (directional) or location (point), diffuse rgb and specular rgb; the ambient gradient is that of
+ * the summed ambient colour.  `shininess` gets no gradient.  Either output may be NULL.  Deterministic: fixed-order fp64
+ * sums, no atomics. */
+DSS_API int dss_light_backward(dss_ctx *ctx, const dss_render_args *args, float *grad_lights, float *grad_ambient,
+                               void *stream);
 /* per-(point,view) preprocess only (rasterizer.py:443-565 fused): writes ndc, ellipse, radii, scaler. */
 DSS_API int dss_preprocess(dss_ctx *ctx, const dss_render_args *args, void *stream);
 
