@@ -6,7 +6,7 @@ import torch
 
 import oracle
 from dss_b200.ops import SplatParams, preprocess_points, render_points
-from tests.util import packed_offsets, scene
+from tests.util import packed_offsets, render_backward_f64_of, scene
 
 pytestmark = pytest.mark.gpu
 
@@ -105,24 +105,11 @@ def test_render_backward_matches_oracle(cuda_device, P0, N, S):
     g = torch.Generator().manual_seed(9)
     grad_image = (torch.randn(N, S, S, 4, generator=g) * 1e-3)
     out.image.backward(grad_image.to(d))
-    # ---- oracle on the CUDA forward's own fragments ----
-    first, num = packed_offsets(N, P0)
-    rec = _np(out.records)
-    ndc, radii = rec[:, :3].copy(), rec[:, 3:5].copy()
-    idx, q = _np(out.idx), _np(out.qvalue)
-    vis = oracle.visibility(idx, N * P0)
-    rs = oracle.search_radius(radii, vis, _np(first), _np(num), prm.radii_backward_scaler)
-    _, g64 = oracle.occ_backward_fast(ndc, radii, vis, rs, _np(grad_image[..., 3]), _np(first), _np(num))
-    # colours
-    wcol = oracle.blend_backward_colours(idx, q, _np(out.scaler), _np(grad_image), N * P0)
-    np.testing.assert_allclose(_np(c.grad), wcol, rtol=2e-4, atol=1e-7)
-    # clip (rasterizer.py:667-673) and chain through ndc = (X/T, Y/T, z_view) in float64
-    gn = np.concatenate([g64, np.zeros((N * P0, 1))], 1)
-    nrm_g = np.linalg.norm(gn, axis=1, keepdims=True)
-    gn = gn / np.maximum(nrm_g, 1e-12) * np.minimum(nrm_g, prm.clip_pts_grad)
-    pre = oracle.preprocess_f64(_np(proj), _np(view), _np(pts), _np(nrm), _np(h), 1.0, 1.0, S)
-    J = pre["jac"].reshape(N, P0, 3, 2)
-    want = np.einsum("npkj,npj->pk", J, gn[:, :2].reshape(N, P0, 2))
+    # ---- float64 reference on the CUDA forward's own fragments ----
+    ref = render_backward_f64_of(out, pts, proj, view, prm, grad_image)
+    assert np.array_equal(_np(out.visible), ref["vis"])
+    np.testing.assert_allclose(_np(c.grad), ref["colours"], rtol=2e-4, atol=1e-7)
+    want = ref["world"]
     got = _np(p.grad)
     scale = np.abs(want).max()
     assert scale > 0
@@ -130,7 +117,8 @@ def test_render_backward_matches_oracle(cuda_device, P0, N, S):
 
 
 def test_backward_is_deterministic_and_linear_in_grad(cuda_device):
-    """size-independent properties: position gradients are bit-reproducible (gather, no atomics) and,
+    """size-independent properties: position gradients are bit-reproducible (gather, no atomics; the same shape, so the
+    same staged-window hint) and,
     with clipping off and a single-signed grad image, linear in the upstream gradient."""
     P0, N, S = 20000, 2, 128
     pts, nrm, col, proj, view, cams = scene(P0, N, seed=5)
