@@ -6,14 +6,6 @@
 
 namespace dss {
 
-static inline unsigned int nblocks(int64_t items, int threads, int sm_count, int per_sm) {
-    int64_t b = (items + threads - 1) / threads;
-    const int64_t cap = (int64_t)sm_count * per_sm;
-    if (b > cap) b = cap;
-    if (b < 1) b = 1;
-    return (unsigned int)b;
-}
-
 // ---------------------------------------------------------------------------------------------
 // visibility (rasterizer.py:854-860): any slot of a pixel whose first slot is occupied.
 // ---------------------------------------------------------------------------------------------
@@ -36,7 +28,7 @@ int visibility_from_idx(dss_ctx *ctx, const int32_t *idx, int64_t num_pixels, in
     DSS_CUDA_TRY(cudaMemsetAsync(visible, 0, (size_t)(P > 0 ? P : 0), st));
     if (num_pixels == 0 || P == 0) return DSS_OK;
     StageScope prof(ctx, ST_VISIBILITY, st);
-    visibility_kernel<<<nblocks(num_pixels, 256, ctx->sm_count, 16), 256, 0, st>>>(idx, num_pixels, K, P, visible);
+    visibility_kernel<<<grid_blocks(num_pixels, 256, ctx->sm_count, 16), 256, 0, st>>>(idx, num_pixels, K, P, visible);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
@@ -64,7 +56,7 @@ int zbuf_backward(dss_ctx *ctx, const int32_t *idx, const float *grad_zbuf, int6
                   float *z_grad, int z_stride, cudaStream_t st) {
     if (num_pixels == 0) return DSS_OK;
     StageScope prof(ctx, ST_ZBUF_BWD, st);
-    zbuf_backward_kernel<<<nblocks(num_pixels, 256, ctx->sm_count, 16), 256, 0, st>>>(idx, grad_zbuf, num_pixels,
+    zbuf_backward_kernel<<<grid_blocks(num_pixels, 256, ctx->sm_count, 16), 256, 0, st>>>(idx, grad_zbuf, num_pixels,
                                                                                       K, z_grad, z_stride);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
@@ -100,7 +92,7 @@ int colour_backward(dss_ctx *ctx, const int32_t *idx, const float *weights, cons
                     cudaStream_t st) {
     if (num_pixels == 0) return DSS_OK;
     StageScope prof(ctx, ST_COLOUR_BWD, st);
-    colour_backward_kernel<<<nblocks(num_pixels, 256, ctx->sm_count, 16), 256, 0, st>>>(
+    colour_backward_kernel<<<grid_blocks(num_pixels, 256, ctx->sm_count, 16), 256, 0, st>>>(
         idx, weights, reinterpret_cast<const float4 *>(grad_image), num_pixels, K, grad_colours, colour_P0, pixels_per_view);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;

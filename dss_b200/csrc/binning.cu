@@ -322,14 +322,6 @@ bin_scatter_kernel(const float4 *__restrict__ rec, const int64_t *__restrict__ f
     }
 }
 
-static inline unsigned int blocks_for(int64_t work_items, int threads, int sm_count, int per_sm) {
-    int64_t b = (work_items + threads - 1) / threads;
-    const int64_t cap = (int64_t)sm_count * per_sm;
-    if (b > cap) b = cap;
-    if (b < 1) b = 1;
-    return (unsigned int)b;
-}
-
 template <typename Kern>
 static int prepare_smem(Kern kern, size_t bytes) {
     if (bytes > 48 * 1024)
@@ -457,7 +449,7 @@ int dss_grid_insert_points_2d(dss_ctx *ctx, const float *points, const int64_t *
     DSS_REQUIRE(ctx && points && lengths && params && grid_cnt && grid_cell && grid_idx, "null pointer");
     DSS_REQUIRE(N >= 0 && Pmax >= 0 && G >= 0, "negative size");
     if (N == 0 || Pmax == 0) return DSS_OK;
-    dim3 grid(dss::blocks_for(Pmax, 256, ctx->sm_count, 8), N);
+    dim3 grid(dss::grid_blocks(Pmax, 256, ctx->sm_count, 8), N);
     dss::grid_insert_2d_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(points, lengths, params, grid_cnt,
                                                                        grid_cell, grid_idx, Pmax, G);
     DSS_LAUNCH_CHECK(ctx);
@@ -471,7 +463,7 @@ int dss_grid_counting_sort_2d(dss_ctx *ctx, const float *points, const int64_t *
                 "null pointer");
     DSS_REQUIRE(N >= 0 && Pmax >= 0 && G >= 0, "negative size");
     if (N == 0 || Pmax == 0) return DSS_OK;
-    dim3 grid(dss::blocks_for(Pmax, 256, ctx->sm_count, 8), N);
+    dim3 grid(dss::grid_blocks(Pmax, 256, ctx->sm_count, 8), N);
     dss::grid_counting_sort_2d_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
         points, lengths, grid_cell, grid_idx, grid_off, sorted_points, sorted_idx, Pmax, G);
     DSS_LAUNCH_CHECK(ctx);

@@ -142,7 +142,23 @@ inline int ctx_get(dss_ctx *ctx, BufId id, size_t count, T **out) {
     return rc;
 }
 
+// Grid size of a grid-stride launch: one thread per item, at most per_sm blocks per SM, at least one block.
+inline unsigned int grid_blocks(int64_t items, int threads, int sm_count, int per_sm) {
+    int64_t b = (items + threads - 1) / threads;
+    const int64_t cap = (int64_t)sm_count * per_sm;
+    if (b > cap) b = cap;
+    if (b < 1) b = 1;
+    return (unsigned int)b;
+}
+
 // ---- device helpers -------------------------------------------------------------------------
+
+// MUFU reciprocal (rcp.approx, denormals flushed to zero): never contracted or rewritten by the compiler.
+__device__ __forceinline__ float rcp_approx(float x) {
+    float y;
+    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
 
 // Pixel index -> NDC centre, the reference's expression (DSS/csrc/rasterization_utils.cuh:8-11).
 // No multiply-add pair, so immune to FMA contraction: int->float, add, IEEE divide, add.

@@ -162,14 +162,6 @@ occ_cellbin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ v
     }
 }
 
-static inline unsigned int occ_nblocks(int64_t items, int threads, int sm_count, int per_sm) {
-    int64_t b = (items + threads - 1) / threads;
-    const int64_t cap = (int64_t)sm_count * per_sm;
-    if (b > cap) b = cap;
-    if (b < 1) b = 1;
-    return (unsigned int)b;
-}
-
 // ---------------------------------------------------------------------------------------------
 // Search radius: radii_s * lower median of the flattened (rx, ry) of the view's visible points
 // (rasterizer.py:888, torch.median = element (m-1)/2 of the ascending sort of m = 2 n_vis values).
@@ -239,14 +231,62 @@ __device__ void select_resolve(const unsigned int *hist_n, int upto, unsigned in
     }
 }
 
-__global__ void __launch_bounds__(256)
-select_hist_kernel(const float4 *__restrict__ rec, const float *__restrict__ radii,
-                   const uint8_t *__restrict__ visible, const int64_t *__restrict__ first_idx,
-                   const int64_t *__restrict__ num_points, int64_t P0_shared, int pass,
-                   unsigned int *__restrict__ hist) {
+// Record sources of one histogram pass (`pass` travels with the source, so that every instantiation keeps the parameter
+// layout of the kernel it replaced).  range(n, ...) gives view n's record indices [beg, end); load(i, rx, ry) reads
+// record i's radii and returns false for a record that does not count.
+// Packed records (or, rec == null, the (P,2) radii) of the view's slots, filtered by the visibility bytes.
+struct SelectPacked {
+    using Index = int64_t;
+    const float4 *rec;
+    const float *radii;
+    const uint8_t *visible;
+    const int64_t *first_idx, *num_points;
+    int64_t P0_shared;
+    int pass;
+    __device__ __forceinline__ void range(int n, int64_t &beg, int64_t &end) const {
+        const ViewRange vr = view_range(first_idx, num_points, n, P0_shared);
+        beg = vr.first;
+        end = vr.first + vr.count;
+    }
+    __device__ __forceinline__ bool load(int64_t p, float &rx, float &ry) const {
+        if (!visible[p]) return false;
+        if (rec) {
+            rx = __ldg(&rec[2 * p]).w;
+            ry = __ldg(&rec[2 * p + 1]).x;
+        } else {
+            rx = radii[p * 2];
+            ry = radii[p * 2 + 1];
+        }
+        return true;
+    }
+};
+// The compact records {px, py, rx, ry} of the visible splats, contiguous per view:
+// [tile_offsets[n*nt], tile_offsets[(n+1)*nt]).
+struct SelectCompact {
+    using Index = int;
+    const float4 *crec;
+    const int32_t *tile_offsets;
+    int nt;
+    int pass;
+    __device__ __forceinline__ void range(int n, int &beg, int &end) const {
+        beg = __ldg(&tile_offsets[(int64_t)n * nt]);
+        end = __ldg(&tile_offsets[(int64_t)(n + 1) * nt]);
+    }
+    __device__ __forceinline__ bool load(int i, float &rx, float &ry) const {
+        const float4 c = __ldg(&crec[i]);
+        rx = c.z;
+        ry = c.w;
+        return true;
+    }
+};
+
+// One radix-select pass over the radii of view blockIdx.y: the keys that match the prefix chosen by the earlier passes
+// are counted by their next 8 bits in shared memory, then added to the view's histogram of this pass.
+template <class Src>
+__global__ void __launch_bounds__(256) select_hist_kernel(const __grid_constant__ Src src, unsigned int *__restrict__ hist) {
     __shared__ unsigned int s_hist[256];
     __shared__ unsigned int s_prefix;
-    const int n = blockIdx.y;
+    const int n = blockIdx.y, pass = src.pass;
     unsigned int *hist_n = hist + (int64_t)n * 4 * 256;
     s_hist[threadIdx.x] = 0;
     if (threadIdx.x < 32) {
@@ -258,19 +298,11 @@ select_hist_kernel(const float4 *__restrict__ rec, const float *__restrict__ rad
     __syncthreads();
     const unsigned int prefix = s_prefix;
     const int shift = 24 - 8 * pass;
-    const ViewRange vr = view_range(first_idx, num_points, n, P0_shared);
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < vr.count;
-         i += (int64_t)gridDim.x * blockDim.x) {
-        const int64_t p = vr.first + i;
-        if (!visible[p]) continue;
+    typename Src::Index beg, end;
+    src.range(n, beg, end);
+    for (typename Src::Index i = beg + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
         float rx, ry;
-        if (rec) {
-            rx = __ldg(&rec[2 * p]).w;
-            ry = __ldg(&rec[2 * p + 1]).x;
-        } else {
-            rx = radii[p * 2];
-            ry = radii[p * 2 + 1];
-        }
+        if (!src.load(i, rx, ry)) continue;
         const unsigned int kx = float_key(rx), ky = float_key(ry);
         if (pass == 0 || (kx >> (shift + 8)) == prefix) atomicAdd(&s_hist[(kx >> shift) & 255u], 1u);
         if (pass == 0 || (ky >> (shift + 8)) == prefix) atomicAdd(&s_hist[(ky >> shift) & 255u], 1u);
@@ -298,50 +330,15 @@ int search_radius(dss_ctx *ctx, const float4 *rec, const float *radii, const uin
     StageScope prof(ctx, ST_SEARCH_RADIUS, st);
     DSS_CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)N * 4 * 256 * sizeof(unsigned int), st));
     if (P0 > 0) {
-        dim3 grid(occ_nblocks(P0, 256, ctx->sm_count, 4), N);
+        dim3 grid(grid_blocks(P0, 256, ctx->sm_count, 4), N);
         for (int pass = 0; pass < 4; ++pass) {
-            select_hist_kernel<<<grid, 256, 0, st>>>(rec, radii, visible, first_idx, num_points, P0, pass, hist);
+            select_hist_kernel<<<grid, 256, 0, st>>>(SelectPacked{rec, radii, visible, first_idx, num_points, P0, pass}, hist);
             DSS_LAUNCH_CHECK(ctx);
         }
     }
     select_final_kernel<<<N, 32, 0, st>>>(hist, radii_s, rs);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Search radius: radii_s * lower median of the flattened (rx, ry) of the view's visible points
-// (rasterizer.py:888; torch.median = element (m-1)/2 of the ascending sort of m = 2 n_vis values).
-// Exact 4-pass radix select (8 bits per pass, MSB first) over the compact records of the view, which are
-// contiguous: [tile_offsets[n*nt], tile_offsets[(n+1)*nt]).
-// ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256)
-select_hist_compact_kernel(const float4 *__restrict__ crec, const int32_t *__restrict__ tile_offsets, int nt, int pass,
-                           unsigned int *__restrict__ hist) {
-    __shared__ unsigned int s_hist[256];
-    __shared__ unsigned int s_prefix;
-    const int n = blockIdx.y;
-    unsigned int *hist_n = hist + (int64_t)n * 4 * 256;
-    s_hist[threadIdx.x] = 0;
-    if (threadIdx.x < 32) {
-        unsigned int prefix;
-        unsigned long long rank, total;
-        select_resolve(hist_n, pass, prefix, rank, total);
-        if (threadIdx.x == 0) s_prefix = prefix;
-    }
-    __syncthreads();
-    const unsigned int prefix = s_prefix;
-    const int shift = 24 - 8 * pass;
-    const int beg = tile_offsets[(int64_t)n * nt], end = tile_offsets[(int64_t)(n + 1) * nt];
-    for (int i = beg + blockIdx.x * blockDim.x + threadIdx.x; i < end; i += gridDim.x * blockDim.x) {
-        const float4 c = __ldg(&crec[i]);
-        const unsigned int kx = float_key(c.z), ky = float_key(c.w);
-        if (pass == 0 || (kx >> (shift + 8)) == prefix) atomicAdd(&s_hist[(kx >> shift) & 255u], 1u);
-        if (pass == 0 || (ky >> (shift + 8)) == prefix) atomicAdd(&s_hist[(ky >> shift) & 255u], 1u);
-    }
-    __syncthreads();
-    const unsigned int v = s_hist[threadIdx.x];
-    if (v) atomicAdd(&hist_n[pass * 256 + threadIdx.x], v);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -379,12 +376,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {
         if (++spins > (1u << 24)) __trap();
     }
-}
-
-__device__ __forceinline__ float rcp_approx(float x) {
-    float y;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
 }
 
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
@@ -744,12 +735,59 @@ occ_tile_kernel(const __grid_constant__ OccTileArgs a) {
 
 
 // ---------------------------------------------------------------------------------------------
-// Generic gather for views whose window does not fit the staged box (very large search radius): one warp per
-// visible splat, lanes stride over the (2R+1)^2 pixel window in global memory, the reference's per-pair rule
-// (rasterize_points_backward.cu:141-178), warp reduction.
+// Direct gathers from the gradient image in global memory, one warp per point (no staging, no atomics).
+// warp_window_gather: the lanes stride over the pixels of the window |x - px| <= ex, |y - py| <= ey (conservative, in
+// NDC-index space, clamped to the image); for every pixel with a non-zero gradient g, rule(dx, dy, g, gx, gy) adds that
+// pixel's share.  Returns the warp's sums (gx, gy) in every lane.  Each caller keeps its own expression text for d2,
+// the test and eps_denom, so their FMA contraction is the caller's own.
 // ---------------------------------------------------------------------------------------------
 constexpr int OCC_WARPS = 8;
 
+template <class Rule>
+__device__ __forceinline__ float2 warp_window_gather(const float *__restrict__ gview, int pix_stride, int S, float inv_S,
+                                                     bool pow2, float px, float py, float ex, float ey, Rule rule) {
+    constexpr unsigned FULL = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    const float half_S = 0.5f * (float)S;
+    // pixel i has centre -1 + (2i+1)/S (clamped in float first: saturating conversions of huge extents must not wrap)
+    const float top = (float)(S - 1);
+    const int xi_lo = (int)fminf(fmaxf(floorf((px - ex + 1.0f) * half_S - 0.5f) - 1.0f, 0.0f), top + 1.0f);
+    const int xi_hi = (int)fmaxf(fminf(ceilf((px + ex + 1.0f) * half_S - 0.5f) + 1.0f, top), -1.0f);
+    const int yi_lo = (int)fminf(fmaxf(floorf((py - ey + 1.0f) * half_S - 0.5f) - 1.0f, 0.0f), top + 1.0f);
+    const int yi_hi = (int)fmaxf(fminf(ceilf((py + ey + 1.0f) * half_S - 0.5f) + 1.0f, top), -1.0f);
+    const int W = xi_hi - xi_lo + 1, H = yi_hi - yi_lo + 1;
+    float gx = 0.f, gy = 0.f;
+    if (W > 0 && H > 0) {
+        const int total = W * H;
+        int wy = lane / W, wx = lane - wy * W;
+        const int step_y = 32 / W, step_x = 32 - step_y * W;
+        for (int w = lane; w < total; w += 32) {
+            const int xi = xi_lo + wx, yi = yi_lo + wy;
+            const float g = __ldg(gview + ((int64_t)(S - 1 - yi) * S + (S - 1 - xi)) * pix_stride);
+            if (g != 0.0f) {
+                const float xf = pix_to_ndc_fast(xi, S, inv_S, pow2);
+                const float yf = pix_to_ndc_fast(yi, S, inv_S, pow2);
+                rule(xf - px, yf - py, g, gx, gy);
+            }
+            wx += step_x;
+            wy += step_y;
+            if (wx >= W) {
+                wx -= W;
+                wy += 1;
+            }
+        }
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        gx += __shfl_xor_sync(FULL, gx, d);
+        gy += __shfl_xor_sync(FULL, gy, d);
+    }
+    return make_float2(gx, gy);
+}
+
+// Generic gather for views whose window does not fit the staged box (very large search radius): the disc of radius r
+// around every visible splat, the reference's per-pair rule (rasterize_points_backward.cu:141-178); a warp takes the
+// visible splats of its 32 slots in turn.
 __global__ void __launch_bounds__(OCC_WARPS * 32)
 occ_generic_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ visible,
                    const float *__restrict__ rs, const float *__restrict__ grad, int pix_stride,
@@ -764,7 +802,6 @@ occ_generic_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ v
     const float r2 = r * r;
     const bool pow2 = (S & (S - 1)) == 0;
     const float inv_S = 1.0f / (float)S;
-    const float half_S = 0.5f * (float)S;
     const float *gview = grad + ((int64_t)n * S * S) * pix_stride + pix_offset;
     constexpr unsigned FULL = 0xffffffffu;
 
@@ -794,50 +831,19 @@ occ_generic_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ v
             const float py = __shfl_sync(FULL, A.y, src);
             const float rx = __shfl_sync(FULL, A.w, src);
             const float ryb = __shfl_sync(FULL, ry, src);
-            // conservative window in NDC-index space: pixel i has centre -1 + (2i+1)/S
-            // (clamped in float first: saturating conversions of huge radii must not wrap)
-            const float top = (float)(S - 1);
-            const int xi_lo = (int)fminf(fmaxf(floorf((px - r + 1.0f) * half_S - 0.5f) - 1.0f, 0.0f), top + 1.0f);
-            const int xi_hi = (int)fmaxf(fminf(ceilf((px + r + 1.0f) * half_S - 0.5f) + 1.0f, top), -1.0f);
-            const int yi_lo = (int)fminf(fmaxf(floorf((py - r + 1.0f) * half_S - 0.5f) - 1.0f, 0.0f), top + 1.0f);
-            const int yi_hi = (int)fmaxf(fminf(ceilf((py + r + 1.0f) * half_S - 0.5f) + 1.0f, top), -1.0f);
-            const int W = xi_hi - xi_lo + 1, H = yi_hi - yi_lo + 1;
-            float gx = 0.f, gy = 0.f;
-            if (W > 0 && H > 0) {
-                const int total = W * H;
-                int wy = lane / W, wx = lane - wy * W;
-                const int step_y = 32 / W, step_x = 32 - step_y * W;
-                for (int w = lane; w < total; w += 32) {
-                    const int xi = xi_lo + wx, yi = yi_lo + wy;
-                    const float g = __ldg(gview + ((int64_t)(S - 1 - yi) * S + (S - 1 - xi)) * pix_stride);
-                    if (g != 0.0f) {
-                        const float xf = pix_to_ndc_fast(xi, S, inv_S, pow2);
-                        const float yf = pix_to_ndc_fast(yi, S, inv_S, pow2);
-                        const float dx = xf - px, dy = yf - py;
-                        const float d2 = dx * dx + dy * dy;
-                        const bool outside = (fabsf(dx) > rx) || (fabsf(dy) > ryb);
-                        if (!(d2 > r2) && !(g > 0.0f && outside)) {
-                            const float den = eps_denom(d2, 1e-10f);
-                            gx += dx / den * g;
-                            gy += dy / den * g;
-                        }
-                    }
-                    wx += step_x;
-                    wy += step_y;
-                    if (wx >= W) {
-                        wx -= W;
-                        wy += 1;
-                    }
+            const float2 g2 = warp_window_gather(gview, pix_stride, S, inv_S, pow2, px, py, r, r,
+                                                 [&](float dx, float dy, float g, float &gx, float &gy) {
+                const float d2 = dx * dx + dy * dy;
+                const bool outside = (fabsf(dx) > rx) || (fabsf(dy) > ryb);
+                if (!(d2 > r2) && !(g > 0.0f && outside)) {
+                    const float den = eps_denom(d2, 1e-10f);
+                    gx += dx / den * g;
+                    gy += dy / den * g;
                 }
-            }
-#pragma unroll
-            for (int d = 16; d > 0; d >>= 1) {
-                gx += __shfl_xor_sync(FULL, gx, d);
-                gy += __shfl_xor_sync(FULL, gy, d);
-            }
+            });
             if (lane == src) {
-                out_x = gx;
-                out_y = gy;
+                out_x = g2.x;
+                out_y = g2.y;
             }
         }
         if (in_range) grad_xy[p] = make_float2(out_x, out_y);
@@ -849,7 +855,7 @@ occ_generic_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ v
 // the reference by backward_occ_fast = True, rasterizer.py:816, kept for completeness): EVERY renderable point of the view
 // (z >= 0, |x|,|y| <= 1 -- not only the visible ones) gathers over the RECTANGLE |dx| <= rx*s, |dy| <= ry*s instead of
 // the disc; positive gradients only count inside the splat's own bbox ((rx*s)/s, (ry*s)/s as the reference writes it).
-// Same gather formulation as occ_generic_kernel: one warp per point, lanes stride over the window, no atomics.
+// One warp per point on warp_window_gather, like occ_generic_kernel.
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(OCC_WARPS * 32)
 occ_slow_kernel(const float *__restrict__ points, const float *__restrict__ radii, float radii_s,
@@ -859,54 +865,27 @@ occ_slow_kernel(const float *__restrict__ points, const float *__restrict__ radi
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const ViewRange vr = view_range(first_idx, num_points, n, 0);
     const bool pow2 = (S & (S - 1)) == 0;
-    const float inv_S = 1.0f / (float)S, half_S = 0.5f * (float)S;
+    const float inv_S = 1.0f / (float)S;
     const float *gview = grad + ((int64_t)n * S * S) * pix_stride + pix_offset;
-    constexpr unsigned FULL = 0xffffffffu;
     for (int64_t i = (int64_t)blockIdx.x * OCC_WARPS + warp; i < vr.count; i += (int64_t)gridDim.x * OCC_WARPS) {
         const int64_t p = vr.first + i;
         const float px = points[p * 3], py = points[p * 3 + 1], pz = points[p * 3 + 2];
-        float gx = 0.f, gy = 0.f;
+        float2 g2 = make_float2(0.f, 0.f);
         if (!(pz < 0.0f || fabsf(py) > 1.0f || fabsf(px) > 1.0f)) {            // rasterize_points.cu:719
             const float rxs = radii[p * 2] * radii_s, rys = radii[p * 2 + 1] * radii_s;   // :725-726
             const float rxb = rxs / radii_s, ryb = rys / radii_s;                            // :744
-            const float top = (float)(S - 1);
-            const int xi_lo = (int)fminf(fmaxf(floorf((px - rxs + 1.0f) * half_S - 0.5f) - 1.0f, 0.0f), top + 1.0f);
-            const int xi_hi = (int)fmaxf(fminf(ceilf((px + rxs + 1.0f) * half_S - 0.5f) + 1.0f, top), -1.0f);
-            const int yi_lo = (int)fminf(fmaxf(floorf((py - rys + 1.0f) * half_S - 0.5f) - 1.0f, 0.0f), top + 1.0f);
-            const int yi_hi = (int)fmaxf(fminf(ceilf((py + rys + 1.0f) * half_S - 0.5f) + 1.0f, top), -1.0f);
-            const int W = xi_hi - xi_lo + 1, H = yi_hi - yi_lo + 1;
-            if (W > 0 && H > 0) {
-                const int total = W * H;
-                int wy = lane / W, wx = lane - wy * W;
-                const int step_y = 32 / W, step_x = 32 - step_y * W;
-                for (int w = lane; w < total; w += 32) {
-                    const int xi = xi_lo + wx, yi = yi_lo + wy;
-                    const float g = __ldg(gview + ((int64_t)(S - 1 - yi) * S + (S - 1 - xi)) * pix_stride);
-                    if (g != 0.0f) {
-                        const float dx = pix_to_ndc_fast(xi, S, inv_S, pow2) - px, dy = pix_to_ndc_fast(yi, S, inv_S, pow2) - py;
-                        const bool in_rect = !(fabsf(dx) > rxs || fabsf(dy) > rys);                       // :728
-                        const bool outside_splat = (fabsf(dx) > rxb) || (fabsf(dy) > ryb);               // :744
-                        if (in_rect && !(g > 0.0f && outside_splat)) {
-                            const float den = eps_denom(dx * dx + dy * dy, 1e-10f);                       // :752-753
-                            gx += dx / den * g;
-                            gy += dy / den * g;
-                        }
-                    }
-                    wx += step_x;
-                    wy += step_y;
-                    if (wx >= W) {
-                        wx -= W;
-                        wy += 1;
-                    }
+            g2 = warp_window_gather(gview, pix_stride, S, inv_S, pow2, px, py, rxs, rys,
+                                    [&](float dx, float dy, float g, float &gx, float &gy) {
+                const bool in_rect = !(fabsf(dx) > rxs || fabsf(dy) > rys);                       // :728
+                const bool outside_splat = (fabsf(dx) > rxb) || (fabsf(dy) > ryb);               // :744
+                if (in_rect && !(g > 0.0f && outside_splat)) {
+                    const float den = eps_denom(dx * dx + dy * dy, 1e-10f);                       // :752-753
+                    gx += dx / den * g;
+                    gy += dy / den * g;
                 }
-            }
+            });
         }
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) {
-            gx += __shfl_xor_sync(FULL, gx, d);
-            gy += __shfl_xor_sync(FULL, gy, d);
-        }
-        if (lane == 0) grad_xy[p] = make_float2(gx, gy);
+        if (lane == 0) grad_xy[p] = g2;
     }
 }
 
@@ -973,7 +952,7 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
                                                             crec, cids);
                 DSS_LAUNCH_CHECK(ctx);
             } else {
-                dim3 bgrid(occ_nblocks(P0, 256 * 4, ctx->sm_count, 8), N);
+                dim3 bgrid(grid_blocks(P0, 256 * 4, ctx->sm_count, 8), N);
                 if (cell_counts) {
                     // the forward's blend epilogue has counted already (one count per visible splat, same cells): take a
                     // copy -- pass 1 counts the working copy back down to zero, the caller's tensor stays intact
@@ -996,9 +975,9 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
             if ((rc = ctx_get(ctx, BUF_SELECT, (size_t)N * 4 * 256, &hist))) return rc;
             StageScope prof(ctx, ST_SEARCH_RADIUS, st);
             DSS_CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)N * 4 * 256 * sizeof(unsigned int), st));
-            dim3 grid(occ_nblocks(P0 / 4 + 1, 256, ctx->sm_count, 1), N);
+            dim3 grid(grid_blocks(P0 / 4 + 1, 256, ctx->sm_count, 1), N);
             for (int pass = 0; pass < 4; ++pass) {
-                select_hist_compact_kernel<<<grid, 256, 0, st>>>(crec, offsets, OB * OB * cs, pass, hist);
+                select_hist_kernel<<<grid, 256, 0, st>>>(SelectCompact{crec, offsets, OB * OB * cs, pass}, hist);
                 DSS_LAUNCH_CHECK(ctx);
             }
             select_final_kernel<<<N, 32, 0, st>>>(hist, radii_s, rs);
@@ -1063,7 +1042,7 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
     {
         // views whose window does not fit (very large search radius) take the direct global-memory gather
         StageScope prof(ctx, ST_OCC_BWD, st);
-        dim3 grid(occ_nblocks(P0, OCC_WARPS * 32, ctx->sm_count, 4), N);   // grid-stride; usually every block returns at once
+        dim3 grid(grid_blocks(P0, OCC_WARPS * 32, ctx->sm_count, 4), N);   // grid-stride; usually every block returns at once
         occ_generic_kernel<<<grid, OCC_WARPS * 32, 0, st>>>(rec, visible, rs, grad_occ, pix_stride, pix_offset, first_idx,
                                                             num_points, P0, S, R_box,
                                                             reinterpret_cast<float2 *>(grad_xy));
@@ -1100,7 +1079,7 @@ int dss_occ_backward_slow(dss_ctx *ctx, const float *points, const float *radii,
     cudaStream_t st = (cudaStream_t)stream;
     DSS_CUDA_TRY(cudaMemsetAsync(grad_xy, 0, (size_t)P * 2 * sizeof(float), st));   // rows outside every view range
     StageScope prof(ctx, ST_OCC_BWD, st);
-    dim3 grid(occ_nblocks(P, OCC_WARPS, ctx->sm_count, 16), N);
+    dim3 grid(grid_blocks(P, OCC_WARPS, ctx->sm_count, 16), N);
     occ_slow_kernel<<<grid, OCC_WARPS * 32, 0, st>>>(points, radii, radii_s, grad_occ, pix_stride, pix_offset, first_idx,
                                                      num_points, image_size, reinterpret_cast<float2 *>(grad_xy));
     DSS_LAUNCH_CHECK(ctx);

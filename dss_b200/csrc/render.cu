@@ -7,14 +7,6 @@
 
 namespace dss {
 
-static inline unsigned int nblocks(int64_t items, int threads, int sm_count, int per_sm) {
-    int64_t b = (items + threads - 1) / threads;
-    const int64_t cap = (int64_t)sm_count * per_sm;
-    if (b > cap) b = cap;
-    if (b < 1) b = 1;
-    return (unsigned int)b;
-}
-
 struct ShadeArgs {
     const float *albedo, *lights, *ambient, *cam;
     int n_lights, light_type;
@@ -43,6 +35,15 @@ __device__ __forceinline__ const float *view_lights(const ShadeArgs &s, int n) {
 __device__ __forceinline__ const float *view_ambient(const ShadeArgs &s, int n) {
     return s.per_view ? s.ambient + (int64_t)n * 3 : s.ambient;
 }
+// stages view n's shading rows into sL[DSS_MAX_LIGHTS * 9 + 6]: lights, then ambient (3) and camera centre (3) at
+// DSS_MAX_LIGHTS * 9 (the caller synchronises)
+__device__ __forceinline__ void stage_view_shading(float *sL, const ShadeArgs &s, int n) {
+    if (threadIdx.x < s.n_lights * 9) sL[threadIdx.x] = view_lights(s, n)[threadIdx.x];
+    if (threadIdx.x < 3) {
+        sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(s, n)[threadIdx.x];
+        sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = s.cam[n * 3 + threadIdx.x];
+    }
+}
 
 struct PreArgs {
     const float *pts, *nrm, *proj, *view, *h;
@@ -57,13 +58,8 @@ struct PreArgs {
     float *shaded;
 };
 
-// Fast reciprocal / division / square root (MUFU based, <= 2 ulp): the per-splat quantities are compared with the
-// float64 oracle at 2e-5 .. 2e-3 relative, IEEE-exact division and sqrt were a third of this kernel's instructions.
-__device__ __forceinline__ float fast_rcp(float x) {
-    float y;
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
+// Fast reciprocal (rcp_approx, common.cuh) and square root (MUFU based, <= 2 ulp): the per-splat quantities are compared
+// with the float64 oracle at 2e-5 .. 2e-3 relative, IEEE-exact division and sqrt were a third of this kernel's instructions.
 __device__ __forceinline__ float fast_sqrt(float x) {
     float y;
     asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -194,13 +190,7 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         sV[threadIdx.x] = a.view[n * 16 + threadIdx.x];
     }
     constexpr bool shade = SHADE;
-    if (shade) {
-        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = view_lights(a.sh, n)[threadIdx.x];
-        if (threadIdx.x < 3) {
-            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(a.sh, n)[threadIdx.x];
-            sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
-        }
-    }
+    if (shade) stage_view_shading(sL, a.sh, n);
     __syncthreads();
     const ViewRange vr = view_range(a.shared_cloud ? nullptr : a.first_idx, a.num_points, n, a.P0);
     const float pix = 2.0f / (float)a.S;
@@ -219,7 +209,7 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         float zv = fmaf(p0, sV[2], fmaf(p1, sV[6], fmaf(p2, sV[10], sV[14])));
         const float te = py_eps_denom(t);
         const float t2 = py_eps_denom(t * t);
-        const float it = fast_rcp(te), it2 = fast_rcp(t2);
+        const float it = rcp_approx(te), it2 = rcp_approx(t2);
         // J = d(ndc xy)/d(world xyz), 3x2 (Mk = W @ Jk, rasterizer.py:483-494)
         float J0[3], J1[3];
 #pragma unroll
@@ -236,15 +226,15 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         const float hh = a.h_per_splat ? a.h[s] : a.h[n];
         const float G00 = fmaf(hh, T00, aa), G01 = hh * T01, G11 = fmaf(hh, T11, aa);
         const float detG = G00 * G11 - G01 * G01;
-        const float idet = fast_rcp(detG);
+        const float idet = rcp_approx(detG);
         const float ea = G11 * idet, eb = -2.0f * G01 * idet, ec = G00 * idet;   // rasterizer.py:543-551
         const float den = py_eps_denom(4.0f * ea * ec - eb * eb);                 // :509-519
-        const float iden = fast_rcp(den);
+        const float iden = rcp_approx(den);
         const float ry = fast_sqrt(py_eps_sqrt(4.0f * ea * a.cutoffC * iden));
         const float rx = fast_sqrt(py_eps_sqrt(4.0f * ec * a.cutoffC * iden));
         const float detT = fmaxf(T00 * T11 - T01 * T01, 0.0f);
         const float sc = fast_sqrt(detT) *
-                         fast_rcp(py_eps_denom(fast_sqrt(py_eps_sqrt(detG * (4.0f * CUDART_PI_F * CUDART_PI_F)))));  // :558-559
+                         rcp_approx(py_eps_denom(fast_sqrt(py_eps_sqrt(detG * (4.0f * CUDART_PI_F * CUDART_PI_F)))));  // :558-559
         // filters (rasterizer.py:187-192, :152): view-space depth range, optional backface
         bool keep = (zv >= a.znear) && (zv <= a.zfar);
         if (a.backface) {
@@ -257,7 +247,7 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
             zlo = min(zlo, zb);
             zhi = max(zhi, zb);
         }
-        const float irt = fast_rcp(t);
+        const float irt = rcp_approx(t);
         const float xn = x * irt, yn = y * irt;
         a.rec[2 * s] = make_float4(xn, yn, zv, rx);
         a.rec[2 * s + 1] = make_float4(ry, ea, eb, ec);
@@ -400,7 +390,7 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     if (smem > 48 * 1024)
         DSS_CUDA_TRY(cudaFuncSetAttribute(shade_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     StageScope prof(ctx, ST_COLOUR_BWD, on);
-    shade_backward_kernel<<<nblocks(g->P0, 256, ctx->sm_count, 8), 256, smem, on>>>(b);
+    shade_backward_kernel<<<grid_blocks(g->P0, 256, ctx->sm_count, 8), 256, smem, on>>>(b);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
@@ -463,7 +453,7 @@ static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, c
         a.sh = shade_args(g);
         a.shaded = g->shaded;
     }
-    dim3 grid(nblocks(g->P0, 256, ctx->sm_count, 8), g->n_views);
+    dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 8), g->n_views);
     StageScope prof(ctx, ST_PREPROCESS, st);
     if (a.shaded) preprocess_kernel<true><<<grid, 256, 0, st>>>(a);
     else preprocess_kernel<false><<<grid, 256, 0, st>>>(a);
@@ -651,13 +641,7 @@ __global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_const
     __shared__ double sPart[8][CAM_SUMS];
     const int n = blockIdx.y;
     if (threadIdx.x < 16) sM[threadIdx.x] = a.proj[n * 16 + threadIdx.x];
-    if (SHADE) {
-        if (threadIdx.x < a.sh.n_lights * 9) sL[threadIdx.x] = view_lights(a.sh, n)[threadIdx.x];
-        if (threadIdx.x < 3) {
-            sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(a.sh, n)[threadIdx.x];
-            sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
-        }
-    }
+    if (SHADE) stage_view_shading(sL, a.sh, n);
     __syncthreads();
     double acc[CAM_SUMS];
 #pragma unroll
@@ -716,30 +700,18 @@ __global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_const
     if (threadIdx.x < CAM_SUMS) a.partials[((int64_t)n * gridDim.x + blockIdx.x) * CAM_SUMS + threadIdx.x] = v;
 }
 
-// one block per view: sums the view's partials in a fixed order and writes the (4,4) / (4,4) / (3,) rows
-__global__ void __launch_bounds__(256) camera_finish_kernel(const double *partials, int blocks, float *grad_proj,
-                                                            float *grad_view, float *grad_cam) {
-    __shared__ double sPart[8][CAM_SUMS];
-    __shared__ double sTot[CAM_SUMS];
-    const int n = blockIdx.x, k = threadIdx.x;
-    double acc[CAM_SUMS];
-#pragma unroll
-    for (int j = 0; j < CAM_SUMS; ++j) acc[j] = 0.0;
-    for (int b = threadIdx.x; b < blocks; b += blockDim.x) {
-        const double *p = partials + ((int64_t)n * blocks + b) * CAM_SUMS;
-#pragma unroll
-        for (int j = 0; j < CAM_SUMS; ++j) acc[j] += p[j];
+// output rows of the camera gradients: view m's (4,4) / (4,4) / (3,) rows from its CAM_SUMS totals
+struct CamRows {
+    float *grad_proj, *grad_view, *grad_cam;
+    __device__ __forceinline__ void operator()(const double *tot, int l, int m, int k) const {
+        if (k < 16) {
+            const int r = k >> 2, c = k & 3;
+            grad_proj[m * 16 + k] = c == 2 ? 0.0f : (float)tot[3 * r + (c == 3 ? 2 : c)];
+            grad_view[m * 16 + k] = c == 2 ? (float)tot[12 + r] : 0.0f;
+        }
+        if (grad_cam && k < 3) grad_cam[m * 3 + k] = (float)tot[16 + k];
     }
-    const double v = block_sum(acc, sPart);
-    if (k < CAM_SUMS) sTot[k] = v;
-    __syncthreads();
-    if (k < 16) {
-        const int r = k >> 2, c = k & 3;
-        grad_proj[n * 16 + k] = c == 2 ? 0.0f : (float)sTot[3 * r + (c == 3 ? 2 : c)];
-        grad_view[n * 16 + k] = c == 2 ? (float)sTot[12 + r] : 0.0f;
-    }
-    if (grad_cam && k < 3) grad_cam[n * 3 + k] = (float)sTot[16 + k];
-}
+};
 
 // ---------------------------------------------------------------------------------------------
 // Light gradients (the reference's lights are tensors that autograd reaches through lighting.py:10-172).  Light l's
@@ -816,30 +788,47 @@ __global__ void __launch_bounds__(256) light_partials_kernel(const __grid_consta
         a.partials[(((int64_t)n * gridDim.z + l) * gridDim.x + blockIdx.x) * LIGHT_SUMS + threadIdx.x] = v;
 }
 
-// block (l, m): light l of output row m -- view m with per-view lights (its partials in block order), the only row with
-// shared lights (the partials of view 0 in block order, then view 1, ...).  Each thread adds a fixed, strided subset,
-// block_sum combines them in a fixed order.
-__global__ void __launch_bounds__(256) light_finish_kernel(const double *partials, int blocks, int n_views, int per_view,
-                                                           float *grad_lights, float *grad_ambient) {
-    __shared__ double sPart[8][LIGHT_SUMS];
-    __shared__ double sTot[LIGHT_SUMS];
+// output rows of the light gradients: light l's row of output row m, and the ambient row from the l = 0 slice
+struct LightRows {
+    float *grad_lights, *grad_ambient;
+    __device__ __forceinline__ void operator()(const double *tot, int l, int m, int k) const {
+        if (grad_lights && k < 9) grad_lights[((int64_t)m * gridDim.x + l) * 9 + k] = (float)tot[k];
+        if (grad_ambient && l == 0 && k < 3) grad_ambient[m * 3 + k] = (float)tot[9 + k];
+    }
+};
+
+// Pass 2 of the camera and light gradients over partials (N, nl, blocks, SUMS).  Block (l, m) sums slice l of output row
+// m -- view m (per_view: cameras, per-view lights; its partials in block order), or, for the only row of shared lights,
+// the partials of view 0 in block order, then view 1, ....  Each thread adds a fixed, strided subset, block_sum combines
+// them in a fixed order, rows(totals, l, m, k) writes the outputs.
+template <int SUMS, class Rows>
+__global__ void __launch_bounds__(256) grad_finish_kernel(const double *partials, int blocks, int n_views, int per_view,
+                                                          const Rows rows) {
+    __shared__ double sPart[8][SUMS];
+    __shared__ double sTot[SUMS];
     const int l = blockIdx.x, m = blockIdx.y, nl = gridDim.x, k = threadIdx.x;
     const int n0 = per_view ? m : 0;
     const int64_t count = (int64_t)(per_view ? 1 : n_views) * blocks;
-    double acc[LIGHT_SUMS];
+    double acc[SUMS];
 #pragma unroll
-    for (int j = 0; j < LIGHT_SUMS; ++j) acc[j] = 0.0;
+    for (int j = 0; j < SUMS; ++j) acc[j] = 0.0;
     for (int64_t e = threadIdx.x; e < count; e += blockDim.x) {
         const int64_t n = n0 + e / blocks, b = e % blocks;
-        const double *p = partials + ((n * nl + l) * blocks + b) * LIGHT_SUMS;
+        const double *p = partials + ((n * nl + l) * blocks + b) * SUMS;
 #pragma unroll
-        for (int j = 0; j < LIGHT_SUMS; ++j) acc[j] += p[j];
+        for (int j = 0; j < SUMS; ++j) acc[j] += p[j];
     }
     const double v = block_sum(acc, sPart);
-    if (k < LIGHT_SUMS) sTot[k] = v;
+    if (k < SUMS) sTot[k] = v;
     __syncthreads();
-    if (grad_lights && k < 9) grad_lights[((int64_t)m * nl + l) * 9 + k] = (float)sTot[k];
-    if (grad_ambient && l == 0 && k < 3) grad_ambient[m * 3 + k] = (float)sTot[9 + k];
+    rows(sTot, l, m, k);
+}
+
+// point blocks per slice of the partials kernels: one wave over all slices at two blocks per SM (95-122 registers per
+// thread), and no more blocks than the points need
+static unsigned int wave_blocks(const dss_ctx *ctx, int64_t slices, int64_t P0) {
+    const int64_t want = ((int64_t)ctx->sm_count * 2 + slices - 1) / slices, need = (P0 + 255) / 256;
+    return (unsigned int)(want < need ? want : need);
 }
 
 }  // namespace dss
@@ -973,9 +962,9 @@ int dss_render_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     c.grad_world = g->grad_points_world;
     StageScope prof(ctx, ST_CHAIN, st);
     if (g->shared_cloud) {
-        chain_kernel<<<nblocks(g->P0, 256, ctx->sm_count, 8), 256, (size_t)N * 32 * sizeof(float), st>>>(c);
+        chain_kernel<<<grid_blocks(g->P0, 256, ctx->sm_count, 8), 256, (size_t)N * 32 * sizeof(float), st>>>(c);
     } else {
-        dim3 grid(nblocks(g->P0, 256, ctx->sm_count, 8), N);
+        dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 8), N);
         chain_kernel<<<grid, 256, 32 * sizeof(float), st>>>(c);
     }
     DSS_LAUNCH_CHECK(ctx);
@@ -1005,9 +994,7 @@ int dss_camera_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_proj
         if (shade) DSS_CUDA_TRY(cudaMemsetAsync(grad_cam_centres, 0, (size_t)N * 3 * sizeof(float), st));
         return DSS_OK;
     }
-    // one wave over all views: two blocks per SM fit (~110-130 registers per thread)
-    int64_t want = ((int64_t)ctx->sm_count * 2 + N - 1) / N, need = (g->P0 + 255) / 256;
-    const unsigned int blocks = (unsigned int)(want < need ? want : need);
+    const unsigned int blocks = wave_blocks(ctx, N, g->P0);
     CamArgs c;
     memset(&c, 0, sizeof(c));
     c.pts = g->points_world;
@@ -1027,7 +1014,8 @@ int dss_camera_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_proj
     if (shade) camera_partials_kernel<true><<<dim3(blocks, N), 256, 0, st>>>(c);
     else camera_partials_kernel<false><<<dim3(blocks, N), 256, 0, st>>>(c);
     DSS_LAUNCH_CHECK(ctx);
-    camera_finish_kernel<<<N, 256, 0, st>>>(c.partials, (int)blocks, grad_proj, grad_view, grad_cam_centres);
+    grad_finish_kernel<CAM_SUMS><<<dim3(1, N), 256, 0, st>>>(c.partials, (int)blocks, N, 1,
+                                                             CamRows{grad_proj, grad_view, grad_cam_centres});
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
@@ -1051,9 +1039,7 @@ int dss_light_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_light
     }
     // the ambient sums live in the l = 0 slice: without grad_lights that slice is all that is needed
     const int nl = grad_lights ? L : 1;
-    // one wave over all (view, light) slices, two blocks per SM, as the camera kernels
-    int64_t want = ((int64_t)ctx->sm_count * 2 + (int64_t)N * nl - 1) / ((int64_t)N * nl), need = (g->P0 + 255) / 256;
-    const unsigned int blocks = (unsigned int)(want < need ? want : need);
+    const unsigned int blocks = wave_blocks(ctx, (int64_t)N * nl, g->P0);
     LightArgs c;
     c.pts = g->points_world;
     c.nrm = g->normals_world;
@@ -1064,8 +1050,8 @@ int dss_light_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_light
     StageScope prof(ctx, ST_LIGHT_BWD, st);
     light_partials_kernel<<<dim3(blocks, N, nl), 256, 0, st>>>(c);
     DSS_LAUNCH_CHECK(ctx);
-    light_finish_kernel<<<dim3(nl, rows), 256, 0, st>>>(c.partials, (int)blocks, N, g->lights_per_view, grad_lights,
-                                                          grad_ambient);
+    grad_finish_kernel<LIGHT_SUMS><<<dim3(nl, rows), 256, 0, st>>>(c.partials, (int)blocks, N, g->lights_per_view,
+                                                                    LightRows{grad_lights, grad_ambient});
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
