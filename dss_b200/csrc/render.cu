@@ -337,6 +337,34 @@ __global__ void __launch_bounds__(256) shade_backward_kernel(const __grid_consta
     }
 }
 
+// Packed clouds: every packed row is its own (view, point), so d albedo / d normal / d position are per row.  Grid
+// (point blocks, views), one thread per row of view n's range (as the packed branch of chain_kernel); each row is
+// written once, by its view (deterministic, no atomics).  Rows outside every range are left to the caller.
+__global__ void __launch_bounds__(256) shade_backward_packed_kernel(const __grid_constant__ ShadeBwdArgs a,
+                                                                    const int64_t *first_idx,
+                                                                    const int64_t *num_points) {
+    __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
+    const int n = blockIdx.y;
+    stage_view_shading(sL, a.sh, n);
+    __syncthreads();
+    const float *amb = sL + DSS_MAX_LIGHTS * 9;
+    const ViewRange vr = view_range(first_idx, num_points, n, a.P0);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < vr.count; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t s = vr.first + i;
+        const V3 gc = v3(a.gsh[s * 3], a.gsh[s * 3 + 1], a.gsh[s * 3 + 2]);
+        V3 ga = v3(0.f, 0.f, 0.f), gn = v3(0.f, 0.f, 0.f), gp = v3(0.f, 0.f, 0.f);
+        if (gc.x != 0.0f || gc.y != 0.0f || gc.z != 0.0f)
+            shade_point<true>(sL, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(amb[0], amb[1], amb[2]),
+                              v3(a.pts[s * 3], a.pts[s * 3 + 1], a.pts[s * 3 + 2]),
+                              v3(a.nrm[s * 3], a.nrm[s * 3 + 1], a.nrm[s * 3 + 2]),
+                              v3(a.sh.albedo[s * 3], a.sh.albedo[s * 3 + 1], a.sh.albedo[s * 3 + 2]),
+                              v3(amb[3], amb[4], amb[5]), gc, ga, gn, gp);
+        a.g_alb[s * 3] = ga.x, a.g_alb[s * 3 + 1] = ga.y, a.g_alb[s * 3 + 2] = ga.z;
+        a.g_nrm[s * 3] = gn.x, a.g_nrm[s * 3 + 1] = gn.y, a.g_nrm[s * 3 + 2] = gn.z;
+        a.g_pos[s * 3] = gp.x, a.g_pos[s * 3 + 1] = gp.y, a.g_pos[s * 3 + 2] = gp.z;
+    }
+}
+
 // Fork/join of the context's side stream: once work has been forked, EVERY return path makes the caller's stream wait
 // for it (an error return that skipped the join would let the caller free tensors the side stream still writes).
 struct SideJoin {
@@ -372,7 +400,7 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     DSS_CUDA_TRY(cudaMemsetAsync(g->grad_colours, 0, (size_t)(cP0 > 0 ? cP0 : g->P) * 3 * sizeof(float), on));
     int rc = colour_backward(ctx, g->idx, g->weights, g->grad_image, npix, K, g->grad_colours, cP0, (int64_t)S * S, on);
     if (rc || !g->shade) return rc;
-    // shading backward: d shaded (N*P0,3) -> d albedo, d normal, d position, per world point
+    // shading backward: d shaded (P,3) -> d albedo, d normal, d position, per world point (shared cloud) or packed row
     DSS_REQUIRE(g->grad_albedo && g->grad_normals_world && g->grad_points_shading && g->points_world,
                 "shading backward needs grad_albedo, grad_normals_world, grad_points_shading");
     ShadeBwdArgs b;
@@ -385,6 +413,13 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     b.g_alb = g->grad_albedo;
     b.g_nrm = g->grad_normals_world;
     b.g_pos = g->grad_points_shading;
+    if (!g->shared_cloud) {
+        StageScope prof(ctx, ST_COLOUR_BWD, on);
+        shade_backward_packed_kernel<<<dim3(grid_blocks(g->P0, 256, ctx->sm_count, 8), N), 256, 0, on>>>(
+            b, g->first_idx, g->num_points);
+        DSS_LAUNCH_CHECK(ctx);
+        return DSS_OK;
+    }
     // per-view lights at the limits (256 views x 8 lights) take 78 KB: more than the default 48 KB of dynamic shared memory
     const size_t smem = (size_t)((g->n_lights * 9 + 3) * (g->lights_per_view ? N : 1) + N * 3) * sizeof(float);
     if (smem > 48 * 1024)
@@ -407,7 +442,6 @@ static int check_common(const dss_render_args *g) {
     DSS_REQUIRE(!g->shared_cloud || g->P == (int64_t)g->n_views * g->P0, "P != n_views * P0");
     DSS_REQUIRE(!g->shared_cloud || g->n_views <= DSS_MAX_SHARED_VIEWS, "a shared cloud takes at most 256 views per call");
     if (g->shade) {
-        DSS_REQUIRE(g->shared_cloud, "fused shading needs a shared cloud");
         DSS_REQUIRE(g->n_lights >= 1 && g->n_lights <= DSS_MAX_LIGHTS, "n_lights must be in [1, 8]");
         DSS_REQUIRE(g->albedo && g->lights && g->ambient && g->cam_centres && g->normals_world, "shading needs albedo, lights, ambient, cam_centres, normals");
         DSS_REQUIRE(g->light_type == 0 || g->light_type == 1, "light_type must be 0 (directional) or 1 (point)");
@@ -468,7 +502,7 @@ static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, c
 // and writes the sum (deterministic, no atomics); otherwise one thread per packed splat.
 // ---------------------------------------------------------------------------------------------
 struct ChainArgs {
-    const float *gshade;   // (P0,3) position gradient through the shading, added to the result (shared cloud), or null
+    const float *gshade;   // position gradient through the shading, (P0,3) or (P,3) like grad_world, added to it, or null
     const float *pts, *proj, *view;
     const float2 *gxy;     // (P,2) occupancy gradient
     const float *gz;       // (P,) z gradient or null
@@ -583,6 +617,11 @@ __global__ void __launch_bounds__(256) chain_kernel(const __grid_constant__ Chai
             float w0 = 0.f, w1 = 0.f, w2 = 0.f;
             if (gx != 0.0f || gy != 0.0f || gz != 0.0f)
                 chain_one(sMat, sMat + 16, a.pts[s * 3], a.pts[s * 3 + 1], a.pts[s * 3 + 2], gx, gy, gz, w0, w1, w2);
+            if (a.gshade) {
+                w0 += a.gshade[s * 3 + 0];
+                w1 += a.gshade[s * 3 + 1];
+                w2 += a.gshade[s * 3 + 2];
+            }
             a.grad_world[s * 3 + 0] = w0;
             a.grad_world[s * 3 + 1] = w1;
             a.grad_world[s * 3 + 2] = w2;
@@ -608,7 +647,7 @@ struct CamArgs {
     const int64_t *first_idx, *num_points;
     int64_t P0;
     int shared_cloud;
-    const float *nrm, *gsh;   // shading only: normals and d L / d shaded (N*P0,3)
+    const float *nrm, *gsh;   // shading only: normals and d L / d shaded (P,3)
     ShadeArgs sh;
     double *partials;         // (N, gridDim.x, CAM_SUMS)
 };
@@ -682,13 +721,13 @@ __global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_const
                 }
             }
             const V3 gc = v3(gs[j][0], gs[j][1], gs[j][2]);
-            if (SHADE && (gc.x != 0.0f || gc.y != 0.0f || gc.z != 0.0f)) {   // shared cloud: world point i
+            if (SHADE && (gc.x != 0.0f || gc.y != 0.0f || gc.z != 0.0f)) {
                 const float *amb = sL + DSS_MAX_LIGHTS * 9;
                 V3 ga = v3(0.f, 0.f, 0.f), gn = v3(0.f, 0.f, 0.f), gp = v3(0.f, 0.f, 0.f), gcam = v3(0.f, 0.f, 0.f);
                 shade_point<true, true>(sL, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(amb[0], amb[1], amb[2]),
-                                        v3(a.pts[i * 3], a.pts[i * 3 + 1], a.pts[i * 3 + 2]),
-                                        v3(a.nrm[i * 3], a.nrm[i * 3 + 1], a.nrm[i * 3 + 2]),
-                                        v3(a.sh.albedo[i * 3], a.sh.albedo[i * 3 + 1], a.sh.albedo[i * 3 + 2]),
+                                        v3(a.pts[src * 3], a.pts[src * 3 + 1], a.pts[src * 3 + 2]),
+                                        v3(a.nrm[src * 3], a.nrm[src * 3 + 1], a.nrm[src * 3 + 2]),
+                                        v3(a.sh.albedo[src * 3], a.sh.albedo[src * 3 + 1], a.sh.albedo[src * 3 + 2]),
                                         v3(amb[3], amb[4], amb[5]), gc, ga, gn, gp, &gcam);
                 acc[16] += (double)gcam.x;
                 acc[17] += (double)gcam.y;
@@ -727,7 +766,9 @@ constexpr int LIGHT_SUMS = 12;   // direction or location (3), diffuse rgb (3), 
 struct LightArgs {
     const float *pts, *nrm, *gsh;
     ShadeArgs sh;
+    const int64_t *first_idx, *num_points;
     int64_t P0;
+    int shared_cloud;
     double *partials;   // (N, gridDim.z, gridDim.x, LIGHT_SUMS)
 };
 
@@ -742,25 +783,27 @@ __global__ void __launch_bounds__(256) light_partials_kernel(const __grid_consta
     double acc[LIGHT_SUMS];
 #pragma unroll
     for (int k = 0; k < LIGHT_SUMS; ++k) acc[k] = 0.0;
-    const float *gsh = a.gsh + (int64_t)n * a.P0 * 3;
+    // view n's rows of d L / d shaded: n*P0 .. n*P0+P0 (shared cloud, world point i) or its packed range (row s)
+    const ViewRange vr = view_range(a.shared_cloud ? nullptr : a.first_idx, a.num_points, n, a.P0);
+    const float *gsh = a.gsh + vr.first * 3;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < a.P0; i0 += CAM_BATCH * stride) {
+    for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < vr.count; i0 += CAM_BATCH * stride) {
         float g[CAM_BATCH][3];
 #pragma unroll
         for (int j = 0; j < CAM_BATCH; ++j) {
             const int64_t i = i0 + j * stride;
 #pragma unroll
-            for (int e = 0; e < 3; ++e) g[j][e] = i < a.P0 ? gsh[i * 3 + e] : 0.0f;
+            for (int e = 0; e < 3; ++e) g[j][e] = i < vr.count ? gsh[i * 3 + e] : 0.0f;
         }
 #pragma unroll
         for (int j = 0; j < CAM_BATCH; ++j) {
             const V3 gc = v3(g[j][0], g[j][1], g[j][2]);
             if (gc.x == 0.0f && gc.y == 0.0f && gc.z == 0.0f) continue;
-            const int64_t i = i0 + j * stride;
-            const V3 p = v3(a.pts[i * 3], a.pts[i * 3 + 1], a.pts[i * 3 + 2]);
-            const V3 alb = v3(a.sh.albedo[i * 3], a.sh.albedo[i * 3 + 1], a.sh.albedo[i * 3 + 2]);
+            const int64_t i = i0 + j * stride, src = a.shared_cloud ? i : vr.first + i;
+            const V3 p = v3(a.pts[src * 3], a.pts[src * 3 + 1], a.pts[src * 3 + 2]);
+            const V3 alb = v3(a.sh.albedo[src * 3], a.sh.albedo[src * 3 + 1], a.sh.albedo[src * 3 + 2]);
             float nlen, vlen;
-            const V3 nh = normalize3(v3(a.nrm[i * 3], a.nrm[i * 3 + 1], a.nrm[i * 3 + 2]), nlen);
+            const V3 nh = normalize3(v3(a.nrm[src * 3], a.nrm[src * 3 + 1], a.nrm[src * 3 + 2]), nlen);
             const V3 v = normalize3(sub3(cam, p), vlen);
             V3 diff = v3(0.f, 0.f, 0.f), spec = v3(0.f, 0.f, 0.f), g_nh = v3(0.f, 0.f, 0.f), g_v = v3(0.f, 0.f, 0.f);
             const LightTerm t = shade_light<true>(sL, a.sh.light_type, a.sh.shininess, p, nh, v, alb, gc, diff, spec, g_nh,
@@ -1045,7 +1088,10 @@ int dss_light_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_light
     c.nrm = g->normals_world;
     c.gsh = g->grad_colours;
     c.sh = shade_args(g);
+    c.first_idx = g->first_idx;
+    c.num_points = g->num_points;
     c.P0 = g->P0;
+    c.shared_cloud = g->shared_cloud;
     if ((rc = ctx_get(ctx, BUF_LIGHT, (size_t)N * nl * blocks * LIGHT_SUMS, &c.partials))) return rc;
     StageScope prof(ctx, ST_LIGHT_BWD, st);
     light_partials_kernel<<<dim3(blocks, N, nl), 256, 0, st>>>(c);

@@ -37,8 +37,8 @@ class SplatParams(NamedTuple):
 
 
 class Shading(NamedTuple):
-    """Fused per-point shading (SURVEY.md 8(f)3): pass as ``shading=`` with the per-point albedo as ``colours``.
-    Build it from the light objects with :func:`make_shading`."""
+    """Fused per-point shading (SURVEY.md 8(f)3): pass as ``shading=`` with the per-point albedo as ``colours`` (per
+    world point of a shared cloud, or per packed row).  Build it from the light objects with :func:`make_shading`."""
     lights: torch.Tensor         # (L,9) {direction | location, diffuse rgb, specular rgb}, or (N,L,9): a set per view
     ambient: torch.Tensor        # (3,), or (N,3) with per-view lights
     cam_centres: torch.Tensor    # (N,3) camera centres in world space
@@ -140,8 +140,12 @@ class _RenderFunction(torch.autograd.Function):
         h_c = _lib.as_f32(h.detach().reshape(-1), "h")
         N, P0, P = _layout(points_c, proj_c, first_idx, num_points, shared)
         if shading is not None:
-            if not shared or tuple(colours_c.shape) != (P0, 3):
-                raise RuntimeError("fused shading takes a shared cloud and the per-point albedo (P0,3) as colours")
+            if tuple(colours_c.shape) != (P0, 3):
+                raise RuntimeError("fused shading takes the per-point albedo as colours: (%d, 3) for a %s, got %s"
+                                   % (P0, "shared cloud" if shared else "packed cloud, one row per packed point",
+                                      tuple(colours_c.shape)))
+            if not shared and grad_sync is not None:
+                raise RuntimeError("grad_sync does not take packed clouds with fused shading")
             shading = _check_shading(shading, N, dev)
         shared_col = bool(shared) and (N > 1 or shading is not None) and tuple(colours_c.shape) == (P0, 3)
         if tuple(colours_c.shape) != (P, 3) and not shared_col:
@@ -225,7 +229,9 @@ class _RenderFunction(torch.autograd.Function):
         grad_albedo = grad_pshade = None
         if shade is not None:
             sh, normals_c, albedo_c = shade
-            grad_albedo, grad_normals, grad_pshade = (torch.empty((P0, 3), dtype=torch.float32, device=dev) for _ in range(3))
+            # per world point (shared cloud) or per packed row, whose uncovered rows the kernels never write
+            alloc = torch.empty if shared else torch.zeros
+            grad_albedo, grad_normals, grad_pshade = (alloc((P0, 3), dtype=torch.float32, device=dev) for _ in range(3))
             _fill_shading(a, sh, albedo_c)
             a.normals_world = _lib.ptr(normals_c)
             a.grad_albedo, a.grad_normals_world = _lib.ptr(grad_albedo), _lib.ptr(grad_normals)
@@ -314,13 +320,16 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     proj, view      : (N,4,4) full-projection and world-to-view matrices, row-vector convention; when they require
                       grad they receive the gradient of the screen positions (proj: x, y; view: the depth)
     h               : (N,) per-view or (P,) per-splat variance scale (rasterizer.py:293-402)
-    shading         : optional Shading -- `colours` is then the per-point albedo (P0,3) and the colour of every
-                      (view, point) is computed in the preprocess kernel: albedo * (ambient + diffuse) + specular
-                      (DSS/core/texture.py:74-127); gradients flow to the albedo, the NORMALS, the positions and,
-                      when they require grad, shading.cam_centres, shading.lights and shading.ambient (hence to the
-                      light objects' tensors through make_shading); the shininess stays a constant
+    shading         : optional Shading -- `colours` is then the per-point albedo, (P0,3) for a shared cloud or (P,3),
+                      one row per packed point, for packed clouds, and the colour of every (view, point) is computed in
+                      the preprocess kernel: albedo * (ambient + diffuse) + specular (DSS/core/texture.py:74-127), with
+                      view n's lights and camera centre for the rows of view n; gradients flow to the albedo, the
+                      NORMALS, the positions and, when they require grad, shading.cam_centres, shading.lights and
+                      shading.ambient (hence to the light objects' tensors through make_shading); the shininess stays
+                      a constant.  Packed rows that no view range covers get zero gradients.
     grad_sync       : optional dss_b200.parallel.GradSync -- the backward then returns gradients already summed over the
-                      ranks of a view-sharded step, the collectives overlapped with the backward kernels
+                      ranks of a view-sharded step, the collectives overlapped with the backward kernels (not with
+                      fused shading of packed clouds)
     """
     outs = _RenderFunction.apply(points, normals, colours, proj, view, h, first_idx, num_points,
                                  bool(shared_cloud), params, bool(return_fragments), grad_sync, shading,

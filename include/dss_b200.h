@@ -249,13 +249,16 @@ typedef struct dss_render_args {
      * shading) and `grad_colours` is (P0,3), summed over the views. */
     int32_t shared_colours;
     /* ---- per-point shading fused into the path (SURVEY.md 8(f)3; DSS/core/texture.py:74-127, lighting.py:10-172) ----
-     * shade != 0 (shared_cloud only): the per-(view,point) colours are COMPUTED instead of read from `colours`:
+     * shade != 0 (shared or packed clouds): the per-(view,point) colours are COMPUTED instead of read from `colours`:
      *   shaded = albedo * (ambient + sum_l Cd_l relu(n.d_l)) + sum_l Cs_l (relu(v.r_l) [n.d_l > 0])^shininess,
      *   n = normalize(normal), d_l = normalize(direction_l) or normalize(location_l - p), v = normalize(cam - p),
      *   r_l = -d_l + 2 (n.d_l) n          (all normalisations as F.normalize(eps = 1e-6))
      * in the preprocess kernel (forward), and the backward turns the colour gradient into gradients w.r.t. the albedo,
      * the NORMALS and (view direction, point lights) the positions -- what torch autograd does in the reference after
-     * ~40 ATen kernels on (N*P0,3) tensors. */
+     * ~40 ATen kernels on (N*P0,3) tensors.  Packed clouds (shared_cloud == 0) shade every packed row with the lights
+     * and camera centre of the view whose range holds it; albedo and the three gradients below are then (P,3), one row
+     * per packed row, and rows that no view range covers are not written (the caller zero-fills them, as for
+     * grad_points_world). */
     int32_t shade;
     int32_t n_lights;              /* L, 1 .. DSS_MAX_LIGHTS                                       */
     int32_t light_type;            /* 0: directional (rows of `lights` start with a direction), 1: point (a location) */
@@ -264,16 +267,16 @@ typedef struct dss_render_args {
      * reference's data gives every image its own light (texture.py:113-114 gathers the light properties per view):
      * `lights` (N,L,9) and `ambient` (N,3), view n's rows at lights + n*L*9 and ambient + n*3. */
     int32_t lights_per_view;
-    const float *albedo;           /* (P0,3) per-point rgb                                         */
+    const float *albedo;           /* (P0,3) per-point rgb, or (P,3) per packed row                */
     const float *lights;           /* (L,9) {direction | location, diffuse rgb, specular rgb}, or (N,L,9) per view */
     const float *ambient;          /* (3,) ambient colour (summed over the lights' ambient terms), or (N,3) per view */
     const float *cam_centres;      /* (N,3) camera centres in world space                          */
     float *shaded;                 /* (P,3) shaded colours: written by the forward, the blend reads them */
     /* backward (shade): `grad_colours` is then a (P,3) SCRATCH that receives d L / d shaded; outputs: */
-    float *grad_albedo;            /* (P0,3) summed over views                                     */
-    float *grad_normals_world;     /* (P0,3) summed over views                                     */
-    float *grad_points_shading;    /* (P0,3) position gradient through the shading; dss_render_backward adds it to
-                                      grad_points_world when it ran the colour half itself (grad_colours != NULL) */
+    float *grad_albedo;            /* (P0,3) summed over views, or (P,3) per packed row             */
+    float *grad_normals_world;     /* (P0,3) summed over views, or (P,3) per packed row             */
+    float *grad_points_shading;    /* (P0,3) or (P,3) position gradient through the shading; dss_render_backward adds it
+                                      to grad_points_world when it ran the colour half itself (grad_colours != NULL) */
     /* optional (n_views * OB * OB * 1024,) int32, OB = ceil(S / 32): written by the forward (one count per visible splat in
      * the cell -- pixel of a 32x32 tile -- of its centre; `visible` must then be 4-byte aligned with its capacity rounded
      * up to a multiple of 4), read by the backward, whose binning then skips its counting pass over all P splats.  Give
