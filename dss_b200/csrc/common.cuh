@@ -49,10 +49,8 @@ enum BufId {
     BUF_TILE_IDS,     // CSR id lists
     BUF_SELECT,       // radix-select histograms
     BUF_MISC,
-    BUF_VIS,
     BUF_RS,
     BUF_GRADXY,
-    BUF_CUTOFF,
     BUF_ZRANGE,
     BUF_STATS,
     BUF_OCC_REC,      // compact tile-ordered {px,py,rx,ry} of the visible splats (occupancy backward)

@@ -6,6 +6,31 @@ namespace dss {
 
 constexpr int RASTER_TILE = 16;  // pixels per side of a raster tile (one 256-thread CTA)
 
+// Cells of the occupancy backward's binning: the pixels of 32x32-pixel tiles, a view's tiles row-major (OB = occ_tiles(S)
+// per side), 1024 cells per tile, row-major inside the tile.  A splat belongs to the cell of its centre pixel.  The
+// forward's blend epilogue counts the visible splats per cell (RasterArgs::cell_counts) and the backward's binning claims
+// its slots by counting those counts back down: both must put a splat in the same cell, so both use these functions.
+constexpr int OCC_TILE_SHIFT = 5;
+constexpr int OCC_TILE = 1 << OCC_TILE_SHIFT;      // pixels per side of a backward tile
+constexpr int OCC_CELLS = OCC_TILE * OCC_TILE;     // cells per tile
+
+__host__ __device__ __forceinline__ int occ_tiles(int S) { return (S + OCC_TILE - 1) >> OCC_TILE_SHIFT; }
+// counters of the cell-level binning (and length of dss_render_args::cell_counts) for N views of S x S pixels
+inline int64_t occ_cell_count(int N, int S) { return (int64_t)N * occ_tiles(S) * occ_tiles(S) * OCC_CELLS; }
+
+// centre pixel of NDC coordinate p, clamped to the image
+__device__ __forceinline__ int centre_pixel(float p, int S) {
+    return min(max((int)floorf((p + 1.0f) * (0.5f * (float)S)), 0), S - 1);
+}
+// view-local tile and global cell of pixel (cx, cy) of view n (cx, cy >= 0, as centre_pixel returns them)
+__device__ __forceinline__ int occ_tile_of(int cx, int cy, int OB) {
+    return (cy >> OCC_TILE_SHIFT) * OB + (cx >> OCC_TILE_SHIFT);
+}
+__device__ __forceinline__ int64_t occ_cell(int n, int OB, int cx, int cy) {
+    return (((int64_t)n * OB + (cy >> OCC_TILE_SHIFT)) * OB + (cx >> OCC_TILE_SHIFT)) * OCC_CELLS +
+           (cy & (OCC_TILE - 1)) * OCC_TILE + (cx & (OCC_TILE - 1));
+}
+
 // Small device -> host read-back WITHOUT the copy engine: a one-block kernel stores the words straight into pinned,
 // device-mapped host memory.  A cudaMemcpyAsync would queue behind whatever large D2H copy another stream has in
 // flight (copies of one direction are served in order) and, being in stream order, stall every kernel enqueued
@@ -91,12 +116,10 @@ struct RasterArgs {
     int64_t colour_P0;     // > 0: colour row of packed splat id in view n is id - n * colour_P0
     float *image;          // (N,S,S,4)
     float *weights;        // (N,S,S,K)
-    int32_t *cell_counts;  // optional (N*OB*OB*1024,), zeroed by the caller, OB = ceil(S/32): the blend epilogue counts every
-                           // visible splat once in the 32x32-tile / pixel cell of its centre (the count pass of the occupancy
-                           // backward's binning, fused); needs `visible` 4-byte aligned with capacity rounded up to 4
+    int32_t *cell_counts;  // optional (occ_cell_count(N, S),), zeroed by the caller: the blend epilogue counts every visible
+                           // splat once in its cell (occ_cell; the count pass of the occupancy backward's binning, fused);
+                           // needs `visible` 4-byte aligned with capacity rounded up to 4
     uint8_t *visible;      // (P,) must be zeroed by the caller
-    int64_t visible_count; // P (to re-zero `visible` when a pass has to be repeated)
-    int force_pixel_parallel;  // testing: use the pixel-parallel kernel even for K <= 8
     unsigned long long *stats; // optional debug counters (dss_debug_raster_stats) or nullptr
 };
 

@@ -24,15 +24,10 @@
 
 namespace dss {
 
-constexpr int OCC_TILE = 32;            // pixels per side of a backward tile
 constexpr int OCC_ITEM = 128;           // splats per work item (= records staged per TMA copy)
 constexpr int OCC_GROUP = 4;            // consecutive items handed to one CTA
 constexpr int OCC_SLACK = 64;           // floats of slack behind each staged plane / the column table
 constexpr int OCC_RBOX_MAX = 40;        // largest window halo the tile kernel stages (2 x 2 planes <= ~200 KB)
-
-__device__ __forceinline__ int centre_pixel(float p, int S) {
-    return min(max((int)floorf((p + 1.0f) * (0.5f * (float)S)), 0), S - 1);
-}
 
 // ---------------------------------------------------------------------------------------------
 // planes: (N, 2, Hp, W) floats, plane 0 = min(g, 0), plane 1 = max(g, 0); element (y, x) holds NDC-index pixel
@@ -80,7 +75,7 @@ occ_bin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ visib
         const int64_t i = chunk0 + j * 256 + threadIdx.x;
         if (i < vr.count && visible[vr.first + i]) {
             const float4 A = __ldg(&rec[2 * (vr.first + i)]);
-            tile[j] = (centre_pixel(A.y, S) / OCC_TILE) * OB + centre_pixel(A.x, S) / OCC_TILE;
+            tile[j] = occ_tile_of(centre_pixel(A.x, S), centre_pixel(A.y, S), OB);
             atomicAdd(&s_hist[tile[j]], 1);
         }
     }
@@ -110,8 +105,8 @@ occ_bin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ visib
         }
 }
 
-// Cell-level variant: the bins are the PIXELS (32 x 32 cells per tile, cell = tile * 1024 + local pixel), so a tile's
-// compact list comes out ordered by pixel row, then column.  Consecutive splats of a list then sit in the same or the
+// Cell-level variant: the bins are the PIXELS (occ_cell, kernels.cuh), so a tile's compact list comes out ordered by pixel
+// row, then column.  Consecutive splats of a list then sit in the same or the
 // next pixel -- the splats a warp of the tile kernel works on together read (nearly) the same shared-memory rows and
 // columns, which turns its 4-way bank conflicts into broadcasts.  Two million bins per 8 views do not fit a block
 // histogram: plain global atomics (1.5M visible splats over 0.5M occupied cells -- no hot spots).
@@ -148,9 +143,7 @@ occ_cellbin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ v
         for (int j = 0; j < U; ++j) {
             if (!vis[j]) continue;
             const int64_t p = vr.first + i0 + j * stride;
-            const int cx = centre_pixel(A[j].x, S), cy = centre_pixel(A[j].y, S);
-            const int64_t tile = (int64_t)n * OB * OB + (cy / OCC_TILE) * OB + cx / OCC_TILE;
-            const int64_t cell = tile * (OCC_TILE * OCC_TILE) + (cy % OCC_TILE) * OCC_TILE + (cx % OCC_TILE);
+            const int64_t cell = occ_cell(n, OB, centre_pixel(A[j].x, S), centre_pixel(A[j].y, S));
             if (PASS == 0) {
                 atomicAdd(&counters[cell], 1);
             } else {
@@ -433,7 +426,7 @@ struct OccTileArgs {
     const float4 *crec;          // compact tile-ordered records {px, py, rx, ry}
     const int32_t *cids;         // packed splat id of every compact record
     const int32_t *tile_offsets; // (N*OB*OB*cs + 1): list of tile t = [tile_offsets[t*cs], tile_offsets[(t+1)*cs])
-    int cs;                      // bins per tile: 1 (tile-level binning) or 1024 (cell-level, lists ordered by pixel)
+    int cs;                      // bins per tile: 1 (tile-level binning) or OCC_CELLS (cell-level, lists ordered by pixel)
     const int32_t *part_off;     // (N*OB*OB + 1) exclusive scan of the items per tile; last = number of items
     const int32_t *item_tile;    // tile (n*OB*OB + tile) of every item
     int *group_counter;          // next group of items to hand out (zero at launch)
@@ -896,7 +889,7 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
                  const int64_t *num_points, int N, int64_t P0, int S, float *grad_xy, const int32_t *cell_counts,
                  cudaStream_t st) {
     if (N <= 0 || P0 <= 0) return DSS_OK;
-    const int OB = (S + OCC_TILE - 1) / OCC_TILE;
+    const int OB = occ_tiles(S);
     const int64_t nt = (int64_t)N * OB * OB;
     const int64_t Ptot = (first_idx == nullptr) ? (int64_t)N * P0 : P0;   // packed mode passes P0 = P
     const bool compute_rs = radii_s >= 0.0f;
@@ -924,7 +917,7 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
         float *planes = nullptr;
         const int PAD = R_box, W = OB * OCC_TILE + 2 * PAD, Hp = W;
         // bins: pixels (lists ordered by pixel inside a tile) unless that needs more than 32M counters
-        const int cs = (!ctx->occ_tilebin && nt * (OCC_TILE * OCC_TILE) <= ((int64_t)32 << 20)) ? OCC_TILE * OCC_TILE : 1;
+        const int cs = (!ctx->occ_tilebin && nt * OCC_CELLS <= ((int64_t)32 << 20)) ? OCC_CELLS : 1;
         const int64_t nc = nt * cs;
         if ((rc = ctx_get(ctx, BUF_OCC_COUNTS, (size_t)(nc + 1), &counts))) return rc;
         if ((rc = ctx_get(ctx, BUF_TILE_OFFSETS, (size_t)(nc + 1), &offsets))) return rc;

@@ -26,6 +26,67 @@ __device__ __forceinline__ bool frag_less(float za, int ia, float zb, int ib) {
     return (za < zb) || (za == zb && ia < ib);
 }
 
+// The output of pixel (xi, yi) of view n, shared by both raster kernels, which must agree to the bit.  fz / fq / fid: the
+// pixel's nearest fragments in (z, id) order; emit[k]: fragment k is output (k < K and the depth merge has not stopped the
+// list before it); any: the pixel has a fragment at all; centre(k): the NDC centre (x, y) of emitted fragment k's splat,
+// asked for only when the epilogue counts cells.  Writes idx / zbuf / qvalue (-1 past the emitted fragments), the
+// occupancy and, when blending, the image, the weights, the visibility bytes and the cell counts.
+template <int KMAX, bool BLEND, class Centre>
+__device__ __forceinline__ void pixel_epilogue(const RasterArgs &a, int n, int xi, int yi, const float (&fz)[KMAX],
+                                               const float (&fq)[KMAX], const int (&fid)[KMAX], const bool (&emit)[KMAX],
+                                               bool any, Centre centre) {
+    const int S = a.S, K = a.K;
+    // image row S-1-yi, col S-1-xi: rasterize_points.cu:577-580
+    const int64_t pix = ((int64_t)n * S + (S - 1 - yi)) * S + (S - 1 - xi);
+#pragma unroll
+    for (int k = 0; k < KMAX; ++k) {
+        if (k < K) {
+            a.idx[pix * K + k] = emit[k] ? fid[k] : -1;
+            if (a.zbuf) a.zbuf[pix * K + k] = emit[k] ? fz[k] : -1.0f;
+            if (a.qvalue) a.qvalue[pix * K + k] = emit[k] ? fq[k] : -1.0f;
+        }
+    }
+    const float occ = any ? 1.0f : 0.0f;
+    if (a.occ) a.occ[pix] = occ;
+    if (BLEND) {
+        // renderer.py:53 w = exp(-0.5 q) * scaler ; norm_weighted_sum [ext]: sum w f / max(sum w, 1e-4)
+        float w[KMAX];
+        float wsum = 0.f, r = 0.f, g = 0.f, b = 0.f;
+#pragma unroll
+        for (int k = 0; k < KMAX; ++k) {
+            w[k] = 0.f;
+            if (emit[k]) {
+                const int id = fid[k];
+                w[k] = expf(-0.5f * fq[k]) * __ldg(&a.scaler[id]);
+                const float *c = a.colours + ((int64_t)id - (int64_t)n * a.colour_P0) * 3;
+                r += w[k] * __ldg(c + 0);
+                g += w[k] * __ldg(c + 1);
+                b += w[k] * __ldg(c + 2);
+                wsum += w[k];
+                if (a.cell_counts) {
+                    // visibility byte + (first setter only) one count in the backward binning's cell of the splat's
+                    // centre pixel: the backward's counting pass over all P splats disappears
+                    unsigned int *word = reinterpret_cast<unsigned int *>(a.visible) + (id >> 2);
+                    const unsigned int bit = 1u << ((id & 3) * 8);
+                    if (!(*reinterpret_cast<volatile unsigned int *>(word) & bit) && !(atomicOr(word, bit) & bit)) {
+                        const float2 p = centre(k);
+                        atomicAdd(&a.cell_counts[occ_cell(n, occ_tiles(S), centre_pixel(p.x, S), centre_pixel(p.y, S))], 1);
+                    }
+                } else if (a.visible) {
+                    a.visible[id] = 1;
+                }
+            }
+        }
+        const float inv = 1.0f / fmaxf(wsum, 1e-4f);
+        reinterpret_cast<float4 *>(a.image)[pix] = make_float4(r * inv, g * inv, b * inv, occ);
+        if (a.weights) {
+#pragma unroll
+            for (int k = 0; k < KMAX; ++k)
+                if (k < K) a.weights[pix * K + k] = w[k] * inv;
+        }
+    }
+}
+
 template <int KMAX, bool PER_POINT_CUTOFF, bool BLEND>
 __global__ void __launch_bounds__(RASTER_THREADS)
 raster_fwd_kernel(const __grid_constant__ RasterArgs a) {
@@ -131,8 +192,6 @@ raster_fwd_kernel(const __grid_constant__ RasterArgs a) {
     }
 
     if (!valid) return;
-    // ---- epilogue: depth merge, outputs (image row S-1-yi, col S-1-xi: rasterize_points.cu:577-580) ----
-    const int64_t pix = ((int64_t)n * S + (S - 1 - yi)) * S + (S - 1 - xi);
     const bool any = fid[0] != INT32_MAX;
     const float z0 = fz[0];
     bool emit[KMAX];
@@ -143,42 +202,9 @@ raster_fwd_kernel(const __grid_constant__ RasterArgs a) {
         open = open && (k < K) && (fid[k] != INT32_MAX) && !(fz[k] - z0 > a.depth_merge);
         emit[k] = open;
     }
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-        if (k < K) {
-            a.idx[pix * K + k] = emit[k] ? fid[k] : -1;
-            if (a.zbuf) a.zbuf[pix * K + k] = emit[k] ? fz[k] : -1.0f;
-            if (a.qvalue) a.qvalue[pix * K + k] = emit[k] ? fq[k] : -1.0f;
-        }
-    }
-    const float occ = any ? 1.0f : 0.0f;
-    if (a.occ) a.occ[pix] = occ;
-    if (BLEND) {
-        // renderer.py:53 w = exp(-0.5 q) * scaler ; norm_weighted_sum [ext]: sum w f / max(sum w, 1e-4)
-        float w[KMAX];
-        float wsum = 0.f, r = 0.f, g = 0.f, b = 0.f;
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            w[k] = 0.f;
-            if (emit[k]) {
-                const int id = fid[k];
-                w[k] = expf(-0.5f * fq[k]) * __ldg(&a.scaler[id]);
-                const float *c = a.colours + ((int64_t)id - (int64_t)n * a.colour_P0) * 3;
-                r += w[k] * __ldg(c + 0);
-                g += w[k] * __ldg(c + 1);
-                b += w[k] * __ldg(c + 2);
-                wsum += w[k];
-                if (a.visible) a.visible[id] = 1;
-            }
-        }
-        const float inv = 1.0f / fmaxf(wsum, 1e-4f);
-        reinterpret_cast<float4 *>(a.image)[pix] = make_float4(r * inv, g * inv, b * inv, occ);
-        if (a.weights) {
-#pragma unroll
-            for (int k = 0; k < KMAX; ++k)
-                if (k < K) a.weights[pix * K + k] = w[k] * inv;
-        }
-    }
+    pixel_epilogue<KMAX, BLEND>(a, n, xi, yi, fz, fq, fid, emit, any, [&](int k) {
+        return __ldg(reinterpret_cast<const float2 *>(&a.rec[2 * (int64_t)fid[k]]));
+    });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -201,23 +227,23 @@ __device__ __forceinline__ unsigned long long make_key(float z, int id) {
     return ((unsigned long long)__float_as_uint(z) << 32) | (unsigned int)id;
 }
 
+// The fragments of the tile's pixel `tid`: keys from the K-lists in shared memory, records gathered up to the depth merge's
+// stop, q recomputed for them with the accept test's expression text.  Then the common epilogue.
 template <int KMAX, bool BLEND>
-__device__ __forceinline__ void raster_epilogue(const RasterArgs &a, const unsigned long long *s_keys, bool tile_has_entries,
+__device__ __forceinline__ void sliced_epilogue(const RasterArgs &a, const unsigned long long *s_keys, bool tile_has_entries,
                                                 int n, int tx0, int ty0, bool pow2, float inv_S) {
     const int S = a.S, K = a.K;
     const int tid = threadIdx.x;
-    const int beg = 0, end = tile_has_entries ? 1 : 0;
     // one thread per pixel
     const int xi = tx0 + (tid & (RASTER_TILE - 1));
     const int yi = ty0 + (tid >> 4);
     if (xi >= S || yi >= S) return;
-    const int64_t pix = ((int64_t)n * S + (S - 1 - yi)) * S + (S - 1 - xi);
     const float xf = pix_to_ndc_fast(xi, S, inv_S, pow2);
     const float yf = pix_to_ndc_fast(yi, S, inv_S, pow2);
     float fz[KMAX], fq[KMAX], fcx[KMAX], fcy[KMAX];
     int fid[KMAX];
     bool emit[KMAX];
-    bool open = beg < end;
+    bool open = tile_has_entries;
     float z0 = 0.f;
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) {
@@ -250,56 +276,8 @@ __device__ __forceinline__ void raster_epilogue(const RasterArgs &a, const unsig
             }
         }
     }
-    const bool any = (beg < end) && (s_keys[tid * KMAX] != KEY_EMPTY);
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-        if (k < K) {
-            a.idx[pix * K + k] = fid[k];
-            if (a.zbuf) a.zbuf[pix * K + k] = fz[k];
-            if (a.qvalue) a.qvalue[pix * K + k] = fq[k];
-        }
-    }
-    const float occ = any ? 1.0f : 0.0f;
-    if (a.occ) a.occ[pix] = occ;
-    if (BLEND) {
-        float w[KMAX];
-        float wsum = 0.f, r = 0.f, g = 0.f, b = 0.f;
-#pragma unroll
-        for (int k = 0; k < KMAX; ++k) {
-            w[k] = 0.f;
-            if (emit[k]) {
-                const int id = fid[k];
-                w[k] = expf(-0.5f * fq[k]) * __ldg(&a.scaler[id]);
-                const float *c = a.colours + ((int64_t)id - (int64_t)n * a.colour_P0) * 3;
-                r += w[k] * __ldg(c + 0);
-                g += w[k] * __ldg(c + 1);
-                b += w[k] * __ldg(c + 2);
-                wsum += w[k];
-                if (a.cell_counts) {
-                    // visibility byte + (first setter only) one count in the backward binning's cell of the splat's
-                    // centre pixel: the backward's counting pass over all P splats disappears
-                    unsigned int *word = reinterpret_cast<unsigned int *>(a.visible) + (id >> 2);
-                    const unsigned int bit = 1u << ((id & 3) * 8);
-                    if (!(*reinterpret_cast<volatile unsigned int *>(word) & bit) && !(atomicOr(word, bit) & bit)) {
-                        const int cx = min(max((int)floorf((fcx[k] + 1.0f) * (0.5f * (float)S)), 0), S - 1);
-                        const int cy = min(max((int)floorf((fcy[k] + 1.0f) * (0.5f * (float)S)), 0), S - 1);
-                        const int OB = (S + 31) >> 5;
-                        const int64_t cell = (((int64_t)n * OB + (cy >> 5)) * OB + (cx >> 5)) * 1024 + (cy & 31) * 32 + (cx & 31);
-                        atomicAdd(&a.cell_counts[cell], 1);
-                    }
-                } else if (a.visible) {
-                    a.visible[id] = 1;
-                }
-            }
-        }
-        const float inv = 1.0f / fmaxf(wsum, 1e-4f);
-        reinterpret_cast<float4 *>(a.image)[pix] = make_float4(r * inv, g * inv, b * inv, occ);
-        if (a.weights) {
-#pragma unroll
-            for (int k = 0; k < KMAX; ++k)
-                if (k < K) a.weights[pix * K + k] = w[k] * inv;
-        }
-    }
+    const bool any = tile_has_entries && (s_keys[tid * KMAX] != KEY_EMPTY);
+    pixel_epilogue<KMAX, BLEND>(a, n, xi, yi, fz, fq, fid, emit, any, [&](int k) { return make_float2(fcx[k], fcy[k]); });
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -657,7 +635,7 @@ raster_sliced_kernel(const __grid_constant__ RasterArgs a) {
             if (overflow) atomicAdd(&a.stats[6], 1ull);
         }
     }
-    raster_epilogue<KMAX, BLEND>(a, s_keys, beg < end, n, tx0, ty0, pow2, inv_S);
+    sliced_epilogue<KMAX, BLEND>(a, s_keys, beg < end, n, tx0, ty0, pow2, inv_S);
 }
 
 
@@ -719,12 +697,8 @@ static int launch_raster(dss_ctx *ctx, const RasterArgs &a, cudaStream_t st) {
 
 int raster_forward(dss_ctx *ctx, const RasterArgs &a, cudaStream_t st) {
     if (a.N <= 0 || a.S <= 0) return DSS_OK;
-    if (!a.force_pixel_parallel) {
-        if (a.K <= 5) return launch_scatter<5>(ctx, a, st);
-        if (a.K <= 8) return launch_scatter<8>(ctx, a, st);
-    }
-    if (a.K <= 5) return launch_raster<5>(ctx, a, st);
-    if (a.K <= 8) return launch_raster<8>(ctx, a, st);
+    if (a.K <= 5) return launch_scatter<5>(ctx, a, st);
+    if (a.K <= 8) return launch_scatter<8>(ctx, a, st);
     if (a.K <= 16) return launch_raster<16>(ctx, a, st);
     return launch_raster<DSS_MAX_POINTS_PER_PIXEL>(ctx, a, st);
 }
@@ -732,7 +706,7 @@ int raster_forward(dss_ctx *ctx, const RasterArgs &a, cudaStream_t st) {
 int bin_and_raster(dss_ctx *ctx, RasterArgs a, const int64_t *first_idx, const int64_t *num_points,
                    int64_t P0, cudaStream_t st) {
     const int S = a.S;
-    const bool scatter_path = a.K <= 8 && !a.force_pixel_parallel;
+    const bool scatter_path = a.K <= 8;
     a.B = (S + RASTER_TILE - 1) / RASTER_TILE;
     a.NS = scatter_path ? choose_depth_slices(a.B) : 1;
     if (a.NS > 1 && ctx->ns_override > 0 && ctx->ns_override < a.NS) a.NS = ctx->ns_override;

@@ -903,12 +903,11 @@ int dss_render_forward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     if ((rc = ctx_get(ctx, BUF_ZRANGE, (size_t)(2 * g->n_views), &zrange))) return rc;
     if ((rc = run_preprocess(ctx, g, rec, st, zrange))) return rc;
     if (g->visible) DSS_CUDA_TRY(cudaMemsetAsync(g->visible, 0, (size_t)g->P, st));
-    // fused count pass of the backward's binning (see RasterArgs::cell_counts): cells = pixels of 32x32 tiles
+    // fused count pass of the backward's binning (see RasterArgs::cell_counts)
     int32_t *cell_counts = nullptr;
-    if (g->cell_counts && g->visible && g->points_per_pixel <= 8 && (reinterpret_cast<uintptr_t>(g->visible) & 3) == 0) {
-        const int64_t OB = (g->image_size + 31) / 32;
+    if (g->cell_counts && g->visible && (reinterpret_cast<uintptr_t>(g->visible) & 3) == 0) {
         cell_counts = g->cell_counts;
-        DSS_CUDA_TRY(cudaMemsetAsync(cell_counts, 0, (size_t)g->n_views * OB * OB * 1024 * sizeof(int32_t), st));
+        DSS_CUDA_TRY(cudaMemsetAsync(cell_counts, 0, (size_t)occ_cell_count(g->n_views, g->image_size) * sizeof(int32_t), st));
     }
     RasterArgs a;
     memset(&a, 0, sizeof(a));
@@ -930,7 +929,6 @@ int dss_render_forward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     a.weights = g->weights;
     a.visible = g->visible;
     a.cell_counts = cell_counts;
-    a.visible_count = g->P;
     a.zrange = zrange;   // already filled by the preprocess kernel
     return bin_and_raster(ctx, a, g->shared_cloud ? nullptr : g->first_idx, g->num_points, g->P0, st);
 }
@@ -976,7 +974,7 @@ int dss_render_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     }
     if ((rc = occ_backward(ctx, rec, g->visible, rs, g->radii_backward_scaler, g->grad_image, 4, 3, fi, g->num_points, N,
                            g->P0, S, gxy,
-                           (g->cell_counts && K <= 8 && (reinterpret_cast<uintptr_t>(g->visible) & 3) == 0) ? g->cell_counts : nullptr,
+                           (g->cell_counts && (reinterpret_cast<uintptr_t>(g->visible) & 3) == 0) ? g->cell_counts : nullptr,
                            st)))
         return rc;
     if (g->search_radius)

@@ -167,8 +167,9 @@ class _RenderFunction(torch.autograd.Function):
         # (capacity rounded up to 4 bytes: the blend epilogue sets the bytes with word atomics when it also counts the
         #  visible splats per backward-binning cell, see dss_render_args.cell_counts)
         visible = torch.empty(((P + 3) // 4 * 4,), dtype=torch.uint8, device=dev)[:P]
+        # one counter per backward-binning cell: the size dss_render_args.cell_counts states (include/dss_b200.h)
         OB = (S + 31) // 32
-        cell_counts = torch.empty((N * OB * OB * 1024,), dtype=torch.int32, device=dev) if K <= 8 else None
+        cell_counts = torch.empty((N * OB * OB * 1024,), dtype=torch.int32, device=dev)
         zbuf = torch.empty((N, S, S, K), **f32) if want_frags else None
         qvalue = torch.empty((N, S, S, K), **f32) if want_frags else None
         fi = first_idx.contiguous() if first_idx is not None else None

@@ -1,7 +1,8 @@
 """The whole fused backward (dss_render_backward) against its float64 reference (tests/util.py render_backward_f64) on
 the forward's own fragments, in the configurations the operator tests do not reach: packed clouds with ragged and empty
-views and rows no view covers, per-splat h (the Vrk_isotropic layout), a z-buffer loss, K > 8, the tile-level backward
-binning with more than 96 views, filtered slots, and a staged-window hint left by a different call.
+views and rows no view covers, per-splat h (the Vrk_isotropic layout), a z-buffer loss, K > 8 (the pixel-parallel
+forward, whose blend epilogue counts the backward's binning cells too), the tile-level backward binning with more than 96
+views, filtered slots, and a staged-window hint left by a different call.
 
 Each case checks the clipped NDC gradient the library writes (grad_ndc), the position gradient per packed row and the
 point / colour gradients autograd returns."""
@@ -9,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+from dss_b200 import _lib
 from dss_b200.core.camera import camera_matrices
 from dss_b200.ops import SplatParams, render_points
 from tests.util import (backward_via_lib, preprocess_f64_slots, random_cameras, render_backward_f64_of, scene,
@@ -166,21 +168,44 @@ def test_zbuffer_loss_matches_float64(cuda_device, layout, clip):
                       zloss=True, seed=44, world_rows=np.arange(P0), pts_leaf=leaf)
 
 
-# ---- K > 8: the pixel-parallel forward allocates no cell counts, the backward counts on its own -----------------
+def _backward_launches(d, pts, nrm, col, proj, view, h, prm, first=None, num=None):
+    """kernel launches of one autograd backward (image loss) through render_points"""
+    shared = first is None
+    fi = None if shared else torch.as_tensor(first).to(d)
+    nm = None if shared else torch.as_tensor(num).to(d)
+    out = render_points(pts.detach().requires_grad_(True), nrm, col, proj, view, h, prm, first_idx=fi, num_points=nm,
+                        shared_cloud=shared)
+    torch.cuda.synchronize(d)
+    n0 = _lib.launch_count(d)
+    out.image.backward(torch.ones_like(out.image))
+    torch.cuda.synchronize(d)
+    return _lib.launch_count(d) - n0
+
+
+# ---- K > 8: the pixel-parallel forward counts the backward's binning cells like the sliced one (autograd's backward
+#      takes those counts; dss_render_backward without them counts on its own), so its backward launches no more
+#      kernels than at K = 5 --------------------------------------------------------------------------------------
 @pytest.mark.parametrize("layout", ["packed", "shared"])
-def test_k12_backward_counts_its_own_cells(cuda_device, layout):
+def test_k12_backward_takes_the_forward_cell_counts(cuda_device, layout):
     d = cuda_device
     if layout == "packed":
         args, kw = _packed_case(d, K=12, per_splat_h=True, clip=0.05, zloss=True, seed=47)
         _render_and_check(*args, **kw)
-        return
-    P0, N = 8000, 2
-    pts, nrm, col, proj, view, _ = scene(P0, N, seed=47)
-    prm = SplatParams(image_size=96, points_per_pixel=12, znear=0.1, clip_pts_grad=0.05)
-    leaf = pts.to(d).requires_grad_(True)
-    _render_and_check(leaf, nrm.to(d), col.to(d).repeat(N, 1), proj.to(d), view.to(d),
-                      torch.full((N,), 3e-4, device=d), prm, zloss=True, seed=48, world_rows=np.arange(P0),
-                      pts_leaf=leaf)
+        launch_args, ranges = args[:6], dict(first=kw["first"], num=kw["num"])
+    else:
+        P0, N = 8000, 2
+        pts, nrm, col, proj, view, _ = scene(P0, N, seed=47)
+        prm = SplatParams(image_size=96, points_per_pixel=12, znear=0.1, clip_pts_grad=0.05)
+        leaf = pts.to(d).requires_grad_(True)
+        h = torch.full((N,), 3e-4, device=d)
+        args = (leaf, nrm.to(d), col.to(d).repeat(N, 1), proj.to(d), view.to(d), h, prm)
+        _render_and_check(*args, zloss=True, seed=48, world_rows=np.arange(P0), pts_leaf=leaf)
+        launch_args, ranges = args[:6], {}
+    prm = args[6]
+    assert prm.points_per_pixel == 12
+    k12 = _backward_launches(d, *launch_args, prm, **ranges)
+    k5 = _backward_launches(d, *launch_args, prm._replace(points_per_pixel=5), **ranges)
+    assert k12 == k5, (k12, k5)
 
 
 # ---- 129 shared views at S = 512: tile-level backward binning (N * 16^2 * 1024 > 32M cells), and views past the
