@@ -30,7 +30,7 @@ constexpr int OCC_SLACK = 64;           // floats of slack behind each staged pl
 constexpr int OCC_RBOX_MAX = 40;        // largest window halo the tile kernel stages (2 x 2 planes <= ~200 KB)
 
 // ---------------------------------------------------------------------------------------------
-// planes: (N, 2, Hp, W) floats, plane 0 = min(g, 0), plane 1 = max(g, 0); element (y, x) holds NDC-index pixel
+// planes: (N, 2, Hp, W) floats, plane 0 = min(g, 0) (and NaN), plane 1 = max(g, 0); element (y, x) holds NDC-index pixel
 // (yi, xi) = (y - PAD, x - PAD), i.e. image row S-1-yi, col S-1-xi (rasterize_points_backward.cu:100-104);
 // zero outside the image so that border windows need no bounds tests.
 // ---------------------------------------------------------------------------------------------
@@ -45,9 +45,14 @@ occ_planes_kernel(const float *__restrict__ grad, int pix_stride, int pix_offset
     if (yi >= 0 && yi < S && xi >= 0 && xi < S)
         g = __ldg(grad + (((int64_t)n * S + (S - 1 - yi)) * S + (S - 1 - xi)) * pix_stride + pix_offset);
     float *p = planes + (((int64_t)n * 2) * Hp + y) * W + x;
-    p[0] = fminf(g, 0.0f);
+    // a NaN goes to g- (fminf would drop it): the reference adds it to every point whose disc holds the pixel
+    p[0] = isnan(g) ? g : fminf(g, 0.0f);
     p[(int64_t)Hp * W] = fmaxf(g, 0.0f);
 }
+
+// The id a compact record carries to the tile kernel's store: the packed id, or -1 for a splat behind the camera,
+// which gets no gradient (rasterize_points_backward.cu:145) but stays binned, so that the bins match the counts.
+__device__ __forceinline__ int32_t occ_store_id(int64_t p, float z) { return z < 0.0f ? -1 : (int32_t)p; }
 
 // ---------------------------------------------------------------------------------------------
 // Bin the visible splats by the tile that contains their (clamped) centre: one entry per splat, so the
@@ -101,7 +106,7 @@ occ_bin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ visib
             const float ry = __ldg(&rec[2 * p + 1]).x;
             const int slot = atomicAdd(&s_hist[tile[j]], 1);
             crec[slot] = make_float4(A.x, A.y, A.w, ry);
-            cids[slot] = (int32_t)p;
+            cids[slot] = occ_store_id(p, A.z);
         }
 }
 
@@ -149,7 +154,7 @@ occ_cellbin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ v
             } else {
                 const int slot = offsets[cell] + atomicSub(&counters[cell], 1) - 1;
                 crec[slot] = make_float4(A[j].x, A[j].y, A[j].w, ry[j]);
-                cids[slot] = (int32_t)p;
+                cids[slot] = occ_store_id(p, A[j].z);
             }
         }
     }
@@ -424,7 +429,7 @@ occ_items_kernel(const int32_t *__restrict__ part_off, int64_t nt, int32_t *__re
 
 struct OccTileArgs {
     const float4 *crec;          // compact tile-ordered records {px, py, rx, ry}
-    const int32_t *cids;         // packed splat id of every compact record
+    const int32_t *cids;         // packed splat id of every compact record (occ_store_id: -1 behind the camera)
     const int32_t *tile_offsets; // (N*OB*OB*cs + 1): list of tile t = [tile_offsets[t*cs], tile_offsets[(t+1)*cs])
     int cs;                      // bins per tile: 1 (tile-level binning) or OCC_CELLS (cell-level, lists ordered by pixel)
     const int32_t *part_off;     // (N*OB*OB + 1) exclusive scan of the items per tile; last = number of items
@@ -566,8 +571,9 @@ __device__ __forceinline__ void occ_item(const OccTileArgs &a, const OccItem &it
             gx += __shfl_xor_sync(FULL, gx, d);
             gy += __shfl_xor_sync(FULL, gy, d);
         }
-        // rasterize_points_backward.cu:145 -- points outside the renderable area get no gradient
-        if (have && gl == 0 && !(fabsf(py) > 1.0f || fabsf(px) > 1.0f)) a.grad_xy[id] = make_float2(gx, gy);
+        // rasterize_points_backward.cu:145 -- points outside the renderable area or behind the camera (id < 0) get no
+        // gradient
+        if (have && gl == 0 && id >= 0 && !(fabsf(py) > 1.0f || fabsf(px) > 1.0f)) a.grad_xy[id] = make_float2(gx, gy);
     }
 }
 

@@ -141,21 +141,34 @@ def search_radius(radii, vis, first_idx, num_pts, radii_s):
     return rs
 
 
-def occ_backward_fast(points, radii, vis, rs, grad_occ, first_idx, num_pts, bruteforce=False):
-    """-> (grad_f32 (P,2), grad_f64 (P,2)).  rasterize_points_backward.cu:85-178."""
+def occ_backward_fast(points, radii, vis, rs, grad_occ, first_idx, num_pts, bruteforce=False, fma_mode=0,
+                      stats=False):
+    """-> (grad_f32 (P,2), grad_f64 (P,2)).  rasterize_points_backward.cu:85-178.
+
+    fma_mode: the rounding of d2 = dx*dx + dy*dy in the disc test -- 0: two products and a sum (the reference's x86
+    build), 1: fmaf(dx, dx, dy*dy) (the reference's CUDA build and our kernels).  stats=True appends a dict with
+    "abs" (P,2), the per-point float64 sums of |dx/den*g| and |dy/den*g| over the contributing pairs, and "pairs"
+    (P,) int32, their number.  bruteforce=True visits every pixel for every point; grad_f32 is then None."""
     points, radii, rs, grad_occ = _f32(points), _f32(radii), _f32(rs), _f32(grad_occ)
     first_idx, num_pts = _i64(first_idx), _i64(num_pts)
     vis = np.ascontiguousarray(vis, np.uint8)
     N, S = grad_occ.shape[0], grad_occ.shape[1]
     P = points.shape[0]
     g64 = np.zeros((P, 2), np.float64)
+    a64 = np.zeros((P, 2), np.float64) if stats else None
+    npairs = np.zeros(P, np.int32) if stats else None
+    g32 = None
     if bruteforce:
         lib().oracle_occ_backward_fast_bruteforce(_p(points), _p(radii), _p(vis), _p(rs), _p(grad_occ),
-                                                  _p(first_idx), _p(num_pts), C.c_int(N), C.c_int(S), _p(g64))
-        return None, g64
-    g32 = np.zeros((P, 2), np.float32)
-    lib().oracle_occ_backward_fast(_p(points), _p(radii), _p(vis), _p(rs), _p(grad_occ), _p(first_idx),
-                                   _p(num_pts), C.c_int(N), C.c_int(S), _p(g32), _p(g64))
+                                                  _p(first_idx), _p(num_pts), C.c_int(N), C.c_int(S),
+                                                  C.c_int(int(fma_mode)), _p(g64), _p(a64), _p(npairs))
+    else:
+        g32 = np.zeros((P, 2), np.float32)
+        lib().oracle_occ_backward_fast(_p(points), _p(radii), _p(vis), _p(rs), _p(grad_occ), _p(first_idx),
+                                       _p(num_pts), C.c_int(N), C.c_int(S), C.c_int(int(fma_mode)), _p(g32), _p(g64),
+                                       _p(a64), _p(npairs))
+    if stats:
+        return g32, g64, dict(abs=a64, pairs=npairs)
     return g32, g64
 
 

@@ -353,21 +353,35 @@ ORACLE_API void oracle_search_radius(const float *radii, const uint8_t *vis, con
  *   skip p if pz<0 or |px|>1 or |py|>1;  d2 = dx*dx+dy*dy; skip if d2 > r_n^2;
  *   skip if g>0 and (|dx|>rx or |dy|>ry);
  *   grad_x += dx / eps_denom(d2,1e-10) * g  (same for y).
+ * fma_mode selects the rounding of d2 in the disc test (and in the fp32 denominator):
+ *   0: dx*dx + dy*dy, two products and a sum rounded apart (the x86 build of the reference);
+ *   1: fmaf(dx, dx, dy*dy), what nvcc makes of the same expression (SASS of rasterize_points_backward.cu:150:
+ *      FMUL dy*dy, FFMA dx*dx + that) and what both of our gathers compute.
+ * Pairs within an ulp of r^2 can fall on different sides in the two modes.
  * grad_f32: fp32 accumulation in ascending pixel order (row-major over the output image);
  * grad_f64: double accumulation of the same fp32 terms' exact values (arbiter).
- * Either output pointer may be NULL.  Output (P,2), zero for invisible points.
+ * abs_f64 (P,2): per point sum |dx/den*g| and sum |dy/den*g| of those terms, in double -- the scale of a rounding
+ * bound for any fp32 summation of them; npairs (P,): the number of contributing (point, pixel) pairs.
+ * Every output pointer may be NULL; without abs_f64 and npairs the loop does no extra work.
+ * Output (P,2), zero for invisible points.
  * ---------------------------------------------------------------------------------------- */
+static inline float occ_d2(float dx, float dy, int fma_mode) {
+    return fma_mode ? fmaf(dx, dx, dy * dy) : dx * dx + dy * dy;
+}
+
 ORACLE_API void oracle_occ_backward_fast(
     const float *points, const float *radii, const uint8_t *vis, const float *rs,
     const float *grad_occ, const int64_t *first_idx, const int64_t *num_pts, int N, int S,
-    float *grad_f32, double *grad_f64) {
+    int fma_mode, float *grad_f32, double *grad_f64, double *abs_f64, int32_t *npairs) {
+    const int stats = abs_f64 != NULL || npairs != NULL;
     for (int n = 0; n < N; ++n) {
         const float r = rs[n], r2 = r * r;
         const int64_t p0 = first_idx[n], p1 = first_idx[n] + num_pts[n];
 #pragma omp parallel for schedule(dynamic, 64)
         for (int64_t p = p0; p < p1; ++p) {
             float gx = 0.0f, gy = 0.0f;
-            double gxd = 0.0, gyd = 0.0;
+            double gxd = 0.0, gyd = 0.0, axd = 0.0, ayd = 0.0;
+            int32_t pairs = 0;
             const float px = points[p * 3 + 0], py = points[p * 3 + 1], pz = points[p * 3 + 2];
             const float rx = radii[p * 2 + 0], ry = radii[p * 2 + 1];
             if (vis[p] && !(pz < 0 || fabsf(py) > 1.0f || fabsf(px) > 1.0f)) {
@@ -385,7 +399,7 @@ ORACLE_API void oracle_occ_backward_fast(
                         if (g == 0.0f) continue;
                         const float xf = pix_to_ndc(S - 1 - col, S);
                         const float dx = xf - px, dy = yf - py;
-                        const float d2 = dx * dx + dy * dy;
+                        const float d2 = occ_d2(dx, dy, fma_mode);
                         if (d2 > r2) continue;
                         const int outside = (fabsf(dx) > rx) || (fabsf(dy) > ry);
                         if (g > 0.0f && outside) continue;
@@ -393,28 +407,37 @@ ORACLE_API void oracle_occ_backward_fast(
                         gx += dx / den * g;
                         gy += dy / den * g;
                         const double dend = eps_denom_d((double)dx * dx + (double)dy * dy, 1e-10);
-                        gxd += (double)dx / dend * g;
-                        gyd += (double)dy / dend * g;
+                        const double tx = (double)dx / dend * g, ty = (double)dy / dend * g;
+                        gxd += tx;
+                        gyd += ty;
+                        if (stats) {
+                            axd += fabs(tx);
+                            ayd += fabs(ty);
+                            ++pairs;
+                        }
                     }
                 }
             }
             if (grad_f32) { grad_f32[p * 2] = gx; grad_f32[p * 2 + 1] = gy; }
             if (grad_f64) { grad_f64[p * 2] = gxd; grad_f64[p * 2 + 1] = gyd; }
+            if (abs_f64) { abs_f64[p * 2] = axd; abs_f64[p * 2 + 1] = ayd; }
+            if (npairs) npairs[p] = pairs;
         }
     }
 }
 
 /* Brute-force variant with no pixel window at all: every pixel x every visible point.
- * Validates the window logic above on small inputs. */
+ * Validates the window logic above on small inputs (same fma_mode and optional outputs). */
 ORACLE_API void oracle_occ_backward_fast_bruteforce(
     const float *points, const float *radii, const uint8_t *vis, const float *rs,
     const float *grad_occ, const int64_t *first_idx, const int64_t *num_pts, int N, int S,
-    double *grad_f64) {
+    int fma_mode, double *grad_f64, double *abs_f64, int32_t *npairs) {
     for (int n = 0; n < N; ++n) {
         const float r = rs[n], r2 = r * r;
 #pragma omp parallel for schedule(dynamic, 64)
         for (int64_t p = first_idx[n]; p < first_idx[n] + num_pts[n]; ++p) {
-            double gxd = 0.0, gyd = 0.0;
+            double gxd = 0.0, gyd = 0.0, axd = 0.0, ayd = 0.0;
+            int32_t pairs = 0;
             const float px = points[p * 3 + 0], py = points[p * 3 + 1], pz = points[p * 3 + 2];
             const float rx = radii[p * 2 + 0], ry = radii[p * 2 + 1];
             if (vis[p] && !(pz < 0 || fabsf(py) > 1.0f || fabsf(px) > 1.0f)) {
@@ -424,16 +447,22 @@ ORACLE_API void oracle_occ_backward_fast_bruteforce(
                         if (g == 0.0f) continue;
                         const float xf = pix_to_ndc(S - 1 - col, S), yf = pix_to_ndc(S - 1 - row, S);
                         const float dx = xf - px, dy = yf - py;
-                        const float d2 = dx * dx + dy * dy;
+                        const float d2 = occ_d2(dx, dy, fma_mode);
                         if (d2 > r2) continue;
                         if (g > 0.0f && ((fabsf(dx) > rx) || (fabsf(dy) > ry))) continue;
                         const double dend = eps_denom_d((double)dx * dx + (double)dy * dy, 1e-10);
-                        gxd += (double)dx / dend * g;
-                        gyd += (double)dy / dend * g;
+                        const double tx = (double)dx / dend * g, ty = (double)dy / dend * g;
+                        gxd += tx;
+                        gyd += ty;
+                        axd += fabs(tx);
+                        ayd += fabs(ty);
+                        ++pairs;
                     }
             }
             grad_f64[p * 2] = gxd;
             grad_f64[p * 2 + 1] = gyd;
+            if (abs_f64) { abs_f64[p * 2] = axd; abs_f64[p * 2 + 1] = ayd; }
+            if (npairs) npairs[p] = pairs;
         }
     }
 }

@@ -9,7 +9,7 @@ import pytest
 import torch
 
 import oracle
-from tests.util import golden_case, random_screen_splats, scene
+from tests.util import OCC_FAMILIES, golden_case, occ_edge_splats, pix_ndc, random_screen_splats, scene
 
 GOLDEN = sorted(p for p in glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.npz"))
                 if not os.path.basename(p).startswith(("knn_", "ref_")))
@@ -111,10 +111,92 @@ def test_occ_backward_window_equals_bruteforce():
     rs = oracle.search_radius(rad, vis, first, num, 4.0)
     g = (np.random.default_rng(0).standard_normal((N, S, S)) * 1e-3).astype(np.float32)
     g[np.random.default_rng(1).random((N, S, S)) < 0.5] = 0
-    _, a = oracle.occ_backward_fast(pts, rad, vis, rs, g, first, num)
-    _, b = oracle.occ_backward_fast(pts, rad, vis, rs, g, first, num, bruteforce=True)
-    np.testing.assert_allclose(a, b, rtol=1e-12, atol=1e-15)
-    assert (a[vis == 0] == 0).all() and np.abs(a).sum() > 0
+    for mode in (0, 1):
+        _, a, sa = oracle.occ_backward_fast(pts, rad, vis, rs, g, first, num, fma_mode=mode, stats=True)
+        _, b, sb = oracle.occ_backward_fast(pts, rad, vis, rs, g, first, num, bruteforce=True, fma_mode=mode,
+                                            stats=True)
+        np.testing.assert_allclose(a, b, rtol=1e-12, atol=1e-15)
+        np.testing.assert_allclose(sa["abs"], sb["abs"], rtol=1e-12, atol=1e-15)
+        assert np.array_equal(sa["pairs"], sb["pairs"])
+        assert (a[vis == 0] == 0).all() and np.abs(a).sum() > 0 and (np.abs(a) <= sa["abs"] * (1 + 1e-12)).all()
+        # without the optional outputs: the same gradients
+        _, c = oracle.occ_backward_fast(pts, rad, vis, rs, g, first, num, fma_mode=mode)
+        assert np.array_equal(a, c)
+
+
+@pytest.mark.parametrize("family,S,r_px", [("disc_edge", 64, 5), ("disc_edge", 256, 13), ("disc_near", 128, None),
+                                           ("disc_near", 200, None), ("disc_near", 256, 9.6), ("box_edge", 128, None),
+                                           ("centre", 64, None), ("border", 17, None), ("ragged", 64, None)])
+def test_occ_backward_families_window_equals_bruteforce(family, S, r_px):
+    """the pixel window of the gather oracle loses no pair at the disc, box and image edges, in either rounding"""
+    d = occ_edge_splats(family, S, seed=1, r_px=r_px)
+    args = [d[k] for k in ("pts", "rad", "vis", "rs", "g", "first", "num")]
+    for mode in (0, 1):
+        _, a, sa = oracle.occ_backward_fast(*args, fma_mode=mode, stats=True)
+        _, b, sb = oracle.occ_backward_fast(*args, bruteforce=True, fma_mode=mode, stats=True)
+        np.testing.assert_allclose(a, b, rtol=1e-12, atol=1e-15)
+        assert np.array_equal(sa["pairs"], sb["pairs"])
+
+
+def _round_f32(q):
+    """Fraction -> the nearest fp32 value (ties to even) as a Fraction; normal range only"""
+    from fractions import Fraction
+    if q == 0:
+        return q
+    s, q = (-1 if q < 0 else 1), abs(q)
+    e = q.numerator.bit_length() - q.denominator.bit_length()
+    while Fraction(2) ** e > q:
+        e -= 1
+    while Fraction(2) ** (e + 1) <= q:
+        e += 1
+    m = q * Fraction(2) ** (23 - e)
+    fl = m.numerator // m.denominator
+    rem = m - fl
+    if rem > Fraction(1, 2) or (rem == Fraction(1, 2) and fl % 2):
+        fl += 1
+    return s * Fraction(fl) / Fraction(2) ** (23 - e)
+
+
+def _disc_member(dx, dy, r2, mode):
+    """exact model of the fp32 disc test: fma_mode 0 rounds dx*dx, dy*dy and their sum; 1 rounds dy*dy and the sum"""
+    from fractions import Fraction
+    X, Y = Fraction(float(dx)) ** 2, Fraction(float(dy)) ** 2
+    d2 = _round_f32(_round_f32(X) + _round_f32(Y)) if mode == 0 else _round_f32(X + _round_f32(Y))
+    return d2 <= Fraction(float(r2))
+
+
+@pytest.mark.parametrize("S,r_px", [(128, None), (200, None), (256, 9.6)])
+def test_occ_fma_mode_decides_near_boundary_pairs(S, r_px):
+    """near the disc edge the two roundings of d2 decide pairs differently: the fixture finds at least 20 such pairs,
+    an exact rational model agrees with the fixture on every one of them, and the oracle's pair counts move by exactly
+    those pairs between fma_mode 0 and 1"""
+    d = occ_edge_splats("disc_near", S, seed=1, r_px=r_px)
+    flips = d["flips"]
+    assert len(flips) >= 20
+    r2 = np.float32(d["rs"][0] * d["rs"][0])
+    want = np.zeros(len(d["pts"]), np.int64)
+    for n, p, xi, yi in flips:
+        dx = np.float32(pix_ndc(xi, S) - d["pts"][p, 0])
+        dy = np.float32(pix_ndc(yi, S) - d["pts"][p, 1])
+        m0, m1 = _disc_member(dx, dy, r2, 0), _disc_member(dx, dy, r2, 1)
+        assert m0 != m1
+        want[p] += 1 if m1 else -1
+    args = [d[k] for k in ("pts", "rad", "vis", "rs", "g", "first", "num")]
+    s0 = oracle.occ_backward_fast(*args, fma_mode=0, stats=True)[2]
+    s1 = oracle.occ_backward_fast(*args, fma_mode=1, stats=True)[2]
+    assert np.array_equal(s1["pairs"].astype(np.int64) - s0["pairs"], want)
+    print("pairs decided differently by the two roundings: %d" % len(flips))
+
+
+def test_occ_exact_disc_edge_is_inside():
+    """centres on pixel centres, r = 5 px at a power-of-two size: the (3, 4, 5) offsets have d2 == r^2 exactly and
+    count in both roundings; with r one ulp smaller they do not (12 pairs per point)"""
+    d = occ_edge_splats("disc_edge", 64, seed=2)
+    args = [d[k] for k in ("pts", "rad", "vis", "rs", "g", "first", "num")]
+    f, m = d["first"], d["num"]
+    for mode in (0, 1):
+        pairs = oracle.occ_backward_fast(*args, fma_mode=mode, stats=True)[2]["pairs"]
+        assert (pairs[f[0]:f[0] + m[0]] - pairs[f[1]:f[1] + m[1]] == 12).all()
 
 
 def test_search_radius_is_torch_lower_median():

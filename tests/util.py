@@ -243,6 +243,217 @@ def edge_screen_splats(family, S, seed=0, P=1200):
     return pts, ell, cutoff, rad, first, num
 
 
+def pix_ndc(i, S):
+    """fp32 NDC centre of pixel index i (NDC-index orientation), as pix_to_ndc computes it: -1 + (2i + 1) / S"""
+    return np.float32(-1) + np.float32(2 * np.asarray(i) + 1) / np.float32(S)
+
+
+def occ_d2_modes(dx, dy):
+    """fp32 d2 of the occupancy gather's disc test in both roundings -> (dx*dx + dy*dy, fmaf(dx, dx, dy*dy)), exact.
+    dx*dx is exact in float64 and, while dx*dx and dy*dy lie within a factor 16 of each other, so is its sum with the
+    rounded dy*dy; the caller keeps only such pairs (`ok`).  -> (d2_mode0, d2_mode1, ok)"""
+    dx, dy = np.asarray(dx, np.float32), np.asarray(dy, np.float32)
+    xx, yy = dx.astype(np.float64) ** 2, dy.astype(np.float64) ** 2
+    yyf = yy.astype(np.float32)
+    d0 = (xx.astype(np.float32) + yyf).astype(np.float32)
+    d1 = (xx + yyf.astype(np.float64)).astype(np.float32)
+    ok = (xx <= 16 * yy) & (yy <= 16 * xx)
+    return d0, d1, ok
+
+
+OCC_FAMILIES = ("disc_edge", "disc_near", "box_edge", "centre", "border", "dense", "many_tiles", "ragged")
+
+
+def occ_edge_splats(family, S, seed=0, r_px=None):
+    """Seeded inputs of the occupancy gather (_C.occ_backward) at the places where it goes wrong -> dict of
+    pts (P,3), rad (P,2), vis (P,) uint8, first, num (N,), g (N,S,S) alpha gradient in image orientation (row r, col c
+    is NDC-index pixel (S-1-c, S-1-r)), rs (N,) search radii, and `flips` (disc_near: the (view, point, xi, yi) pairs
+    whose disc membership differs between fma_mode 0 and 1).  Radii in pixels below are multiples of 2/S in NDC.
+
+    disc_edge : S a power of two, centres on pixel centres, r = 5 px, g != 0 at the (3,4,5) offsets, where
+                d2 == r^2 exactly (view 0: included); view 1 is the same with r one ulp smaller (excluded)
+    disc_near : sub-pixel centres placed so that d2 lies within an ulp of r^2 at one pixel each, kept where the two
+                roundings of d2 decide the pair differently (at least 20 such pairs)
+    box_edge  : positive gradients at |dx| == rx and |dy| == ry exactly (and the same box one ulp smaller), ry > r
+                (the centre-row band capped at the window), ry below half a pixel, rx >> r
+    centre    : points on pixel centres with g != 0 there (d2 = 0), and a few ulp off them (d2 < 1e-10)
+    border    : |x| or |y| exactly 1 (gradient), nextafter(1, 2) (none), centres within a window of the edges and
+                corners
+    dense     : 129 and ~5000 splats over one tile, 257 in one pixel: several work items per tile
+    many_tiles: S = 1024, two views, a few splats in nearly every tile: more item groups than persistent CTAs
+    ragged    : views with 0, 1 and 2 visible splats (and invisible ones), an empty range, and visible splats behind
+                the camera or outside the image
+    """
+    rng = np.random.default_rng(3000 + seed + 13 * OCC_FAMILIES.index(family))
+    pix = 2.0 / S
+    f32 = np.float32
+    views = []            # per view: (x, y, z, rx, ry, vis, g, rs)
+
+    def grad(lo=0.5, hi=1.5, zero=0.5, neg=0.5):
+        g = rng.uniform(lo, hi, (S, S)) * 1e-3
+        g[rng.random((S, S)) < neg] *= -1
+        g[rng.random((S, S)) < zero] = 0
+        return g.astype(f32)
+
+    def put(g, xi, yi, v):
+        g[S - 1 - np.asarray(yi), S - 1 - np.asarray(xi)] = v
+
+    def view(x, y, rx, ry, g, rs, z=None, vis=None):
+        n = len(x)
+        views.append((np.asarray(x, f32), np.asarray(y, f32), f32(1) if z is None else np.asarray(z, f32),
+                      np.asarray(rx, f32) * np.ones(n, f32), np.asarray(ry, f32) * np.ones(n, f32),
+                      np.ones(n, np.uint8) if vis is None else np.asarray(vis, np.uint8), g, f32(rs)))
+
+    flips = []
+    if family == "disc_edge":
+        assert S & (S - 1) == 0
+        r_px = r_px or 5
+        a_, b_ = {5: (3, 4), 10: (6, 8), 13: (5, 12)}[r_px]           # a^2 + b^2 = r^2
+        r = f32(r_px * pix)
+        c = np.arange(r_px + 1, S - r_px - 1, 2 * r_px + 3)
+        xi, yi = (a.ravel() for a in np.meshgrid(c, c))
+        g = grad(zero=0.3)
+        for kx, ky in ((a_, b_), (b_, a_), (r_px, 0), (0, r_px)):
+            for sx in (-1, 1):
+                for sy in (-1, 1):
+                    put(g, xi + sx * kx, yi + sy * ky, (rng.uniform(0.5, 1.5, len(xi)) * 1e-3 *
+                                                        rng.choice([-1, 1], len(xi))).astype(f32))
+        for rv in (r, np.nextafter(r, f32(0))):
+            view(pix_ndc(xi, S), pix_ndc(yi, S), (r_px + 1) * pix, (r_px + 1) * pix, g, rv)
+    elif family == "disc_near":
+        r_px = r_px or 4.6
+        r = f32(r_px * pix)
+        r2 = f32(r * r)
+        g = grad(zero=0.5)
+        xs, ys, used = [], [], set()
+        for _ in range(200):
+            m = 4096
+            e = int(r_px) + 2
+            xi = rng.integers(e, S - e, m)
+            yi = rng.integers(e, S - e, m)
+            kx = np.rint(r_px * rng.choice([0.5, 0.6, 0.7, 0.8], m)).astype(np.int64)
+            ky = np.rint(np.sqrt(r_px ** 2 - kx ** 2)).astype(np.int64) * rng.choice([-1, 1], m)
+            kx = kx * rng.choice([-1, 1], m)
+            px = (pix_ndc(xi, S) + f32(pix) * rng.uniform(-0.45, 0.45, m).astype(f32)).astype(f32)
+            dx = (pix_ndc(xi + kx, S) - px).astype(f32)
+            dyt = np.sqrt(np.maximum(float(r2) - dx.astype(np.float64) ** 2, 0.0))
+            py = (pix_ndc(yi + ky, S).astype(np.float64) - np.sign(ky) * dyt).astype(f32)
+            dy = (pix_ndc(yi + ky, S) - py).astype(f32)
+            d0, d1, ok = occ_d2_modes(dx, dy)
+            sel = np.nonzero(ok & ((d0 <= r2) != (d1 <= r2)) & (np.abs(py) < 1) & (np.abs(px) < 1))[0]
+            for i in sel:
+                key = (int(xi[i] + kx[i]), int(yi[i] + ky[i]))
+                if key in used:
+                    continue
+                used.add(key)
+                xs.append(px[i])
+                ys.append(py[i])
+                flips.append((0, len(xs) - 1, key[0], key[1]))
+            if len(flips) >= 40:
+                break
+        assert len(flips) >= 20, len(flips)
+        for _, _, fx, fy in flips:    # a negative gradient acts on the whole disc
+            put(g, fx, fy, f32(-rng.uniform(0.5, 1.5) * 1e-3))
+        m = 100
+        xs += list(rng.uniform(-1, 1, m).astype(f32))
+        ys += list(rng.uniform(-1, 1, m).astype(f32))
+        view(xs, ys, (r_px + 1) * pix, (r_px + 1) * pix, g, r)
+    elif family == "box_edge":
+        assert S & (S - 1) == 0
+        r_px = r_px or 6
+        c = np.arange(r_px + 2, S - r_px - 2, 2 * r_px + 3)
+        xi, yi = (a.ravel() for a in np.meshgrid(c, c))
+        n = len(xi)
+        kind = np.arange(n) % 6
+        kx = rng.integers(2, 5, n).astype(f32)
+        ky = rng.integers(2, 5, n).astype(f32)
+        rx = np.select([kind == 0, kind == 1, kind == 2, kind == 3, kind == 4],
+                       [kx * f32(pix), np.nextafter(kx * f32(pix), f32(0)), f32(1.5 * r_px * pix), f32(3 * pix),
+                        f32(3 * r_px * pix)], f32(4 * pix)).astype(f32)
+        ry = np.select([kind == 0, kind == 1, kind == 2, kind == 3, kind == 4],
+                       [ky * f32(pix), np.nextafter(ky * f32(pix), f32(0)), f32(1.5 * r_px * pix), f32(0.3 * pix),
+                        f32(2 * pix)], f32(4 * pix)).astype(f32)
+        x = pix_ndc(xi, S)
+        y = pix_ndc(yi, S)
+        y = np.where(kind == 3, y + f32(0.2 * pix), y).astype(f32)    # off the row centre, within ry of it
+        g = grad(zero=0.1, neg=0.2)
+        view(x, y, rx, ry, g, f32(r_px * pix))
+    elif family == "centre":
+        assert S & (S - 1) == 0
+        c = np.arange(4, S - 4, 9)
+        xi, yi = (a.ravel() for a in np.meshgrid(c, c))
+        x, y = pix_ndc(xi, S), pix_ndc(yi, S)
+        n = len(x)
+        k = np.arange(n) % 4            # 0: on the centre; 1..3: that many ulp off it (x, y or both)
+        for _ in range(3):
+            step = k > _
+            x = np.where(step & (np.arange(n) % 3 != 1), np.nextafter(x, f32(2)), x).astype(f32)
+            y = np.where(step & (np.arange(n) % 3 != 0), np.nextafter(y, f32(-2)), y).astype(f32)
+        g = grad(zero=0.2)
+        put(g, xi, yi, (rng.uniform(0.5, 1.5, n) * 1e-3 * rng.choice([-1, 1], n)).astype(f32))
+        view(x, y, 3 * pix, 3 * pix, g, f32(3.4 * pix))
+    elif family == "border":
+        m = 60
+        one, past = f32(1), np.nextafter(f32(1), f32(2))
+        side = rng.choice([-1, 1], (m, 2)).astype(f32)
+        t = rng.uniform(-1, 1, m).astype(f32)
+        axis = np.arange(m) % 2
+        edge = np.where(np.arange(m) % 3 == 2, past, one)
+        x = np.where(axis == 0, side[:, 0] * edge, t).astype(f32)
+        y = np.where(axis == 1, side[:, 1] * edge, t).astype(f32)
+        corners = np.array([[a * b, c * d] for a in (1, -1) for c in (1, -1) for b, d in ((one, one), (past, one))],
+                           f32)
+        near = rng.uniform(-1, 1, (200, 2)).astype(f32)
+        near = np.sign(near) * (1 - np.abs(near) * f32(6 * pix))          # within 6 px of an edge or a corner
+        pts = np.concatenate([np.stack([x, y], 1), corners, near.astype(f32)])
+        view(pts[:, 0], pts[:, 1], 2 * pix, 2 * pix, grad(zero=0.2), f32(3.7 * pix))
+    elif family == "dense":
+        def in_tile(tx, ty, n):
+            lo = lambda t: pix_ndc(32 * t, S) - f32(0.5 * pix)
+            hi = lambda t: pix_ndc(min(32 * t + 31, S - 1), S) + f32(0.45 * pix)
+            return rng.uniform(lo(tx), hi(tx), n), rng.uniform(lo(ty), hi(ty), n)
+        parts = [in_tile(0, 0, 129), in_tile(1, 1, 5000)]
+        px_, py_ = pix_ndc(45, S), pix_ndc(12, S)
+        parts.append((px_ + rng.uniform(-0.45, 0.45, 257) * pix, py_ + rng.uniform(-0.45, 0.45, 257) * pix))
+        x = np.concatenate([p[0] for p in parts])
+        y = np.concatenate([p[1] for p in parts])
+        n = len(x)
+        view(x, y, rng.uniform(0.5, 4, n) * pix, rng.uniform(0.5, 4, n) * pix, grad(zero=0.3), f32(3.3 * pix))
+    elif family == "many_tiles":
+        for _ in range(2):
+            n = 3000
+            view(rng.uniform(-1, 1, n), rng.uniform(-1, 1, n), rng.uniform(0.5, 4, n) * pix,
+                 rng.uniform(0.5, 4, n) * pix, grad(zero=0.9), f32(3.2 * pix))
+    elif family == "ragged":
+        def some(n, nvis):
+            vis = np.zeros(n, np.uint8)
+            vis[rng.choice(n, nvis, replace=False)] = 1
+            return rng.uniform(-0.9, 0.9, n), rng.uniform(-0.9, 0.9, n), vis
+        for n, nvis in ((3, 0), (3, 1), (4, 2), (0, 0)):
+            x, y, vis = some(n, nvis)
+            view(x, y, 3 * pix, 3 * pix, grad(zero=0.2), f32(4.2 * pix), vis=vis)
+        n = 30       # visible, but behind the camera / outside the image / ordinary
+        x, y = rng.uniform(-0.9, 0.9, n), rng.uniform(-0.9, 0.9, n)
+        z = np.where(np.arange(n) % 3 == 0, -rng.uniform(0.5, 2, n), rng.uniform(0.5, 2, n))
+        x = np.where(np.arange(n) % 3 == 1, rng.choice([-1.01, 1.01], n), x)
+        view(x, y, 3 * pix, 3 * pix, grad(zero=0.2), f32(4.2 * pix), z=z)
+    else:
+        raise ValueError(family)
+    num = np.array([len(v[0]) for v in views], np.int64)
+    first = (np.cumsum(num) - num).astype(np.int64)
+    P = int(num.sum())
+    pts = np.zeros((P, 3), np.float32)
+    rad = np.zeros((P, 2), np.float32)
+    vis = np.zeros(P, np.uint8)
+    for (x, y, z, rx, ry, v, _, _), f, m in zip(views, first, num):
+        pts[f:f + m] = np.stack([x, y, np.broadcast_to(z, x.shape)], 1)
+        rad[f:f + m] = np.stack([rx, ry], 1)
+        vis[f:f + m] = v
+    g = np.ascontiguousarray(np.stack([v[6] for v in views]))
+    rs = np.array([v[7] for v in views], np.float32)
+    return dict(pts=pts, rad=rad, vis=vis, first=first, num=num, g=g, rs=rs, flips=flips)
+
+
 def rim_mask(q, cutoff_at_idx):
     """pixels whose fragments sit within a few ulp of the cutoff (FMA contraction can flip them)."""
     return np.abs(q - cutoff_at_idx) <= 8 * np.spacing(np.abs(cutoff_at_idx).astype(np.float32))
@@ -405,7 +616,7 @@ def render_backward_f64(ndc, radii, idx, qvalue, scaler, pts, proj, view, prm, g
     first, num = view_ranges(N, pts.shape[0], first, num)
     vis = oracle.visibility(idx, P)
     rs = oracle.search_radius(radii, vis, first, num, prm.radii_backward_scaler)
-    g32, g64 = oracle.occ_backward_fast(ndc, radii, vis, rs, np.ascontiguousarray(gi[..., 3]), first, num)
+    g32, g64 = oracle.occ_backward_fast(ndc, radii, vis, rs, np.ascontiguousarray(gi[..., 3]), first, num, fma_mode=1)
     raw = np.concatenate([g64, np.zeros((P, 1))], 1)
     raw32 = np.concatenate([g32.astype(np.float64), np.zeros((P, 1))], 1)
     if grad_zbuf is not None:
