@@ -80,6 +80,8 @@ _SIGNATURES = {
     "dss_zbuf_backward": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int, vp, vp]),
     "dss_knn_points": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_float,
                                  vp, vp, vp]),
+    "dss_surface_regulariser": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int64, vp, vp, C.c_int, C.c_int,
+                                          vp, vp, vp, vp, C.c_float, C.c_float, vp, vp, vp]),
     "dss_preprocess": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),

@@ -66,6 +66,7 @@ enum BufId {
     BUF_KNN_SORTED,   //   points in cell order {x, y, z, index}
     BUF_CAMERA,       // per-block fp64 partial sums of the camera gradients
     BUF_LIGHT,        // per-block fp64 partial sums of the light gradients
+    BUF_REGULARISER,  // denoised normals (P,3) and per-cloud bounding boxes of the surface regularisers
     NUM_BUFS
 };
 
@@ -174,6 +175,13 @@ __device__ __forceinline__ float eps_denom(float d, float eps) {
     const float a = fmaxf(fabsf(d), eps);
     return d < 0.0f ? -a : a;
 }
+
+// Order-preserving float <-> int map: integer atomicMin / atomicMax then give float extremes in any order.
+__device__ __forceinline__ int f2ord(float f) {
+    const int i = __float_as_int(f);
+    return i >= 0 ? i : i ^ 0x7fffffff;
+}
+__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 
 struct ViewRange {
     int64_t first;

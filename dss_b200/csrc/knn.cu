@@ -29,12 +29,6 @@ struct KnnGrid {          // per cloud, lives on the device
     int res[3];
 };
 
-__device__ __forceinline__ int f2ord(float f) {            // order-preserving float -> int (for atomicMin/Max)
-    const int i = __float_as_int(f);
-    return i >= 0 ? i : i ^ 0x7fffffff;
-}
-__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
 __global__ void knn_bbox_init_kernel(int *bbox, int N) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < N * 6) bbox[i] = (i % 6 < 3) ? INT32_MAX : INT32_MIN;

@@ -194,6 +194,29 @@ DSS_API int dss_knn_points(dss_ctx *ctx, const float *queries, const int64_t *qu
                            const int64_t *num_points, int N, int64_t Pq, int64_t P, int K, float radius,
                            float *sq_dists, int32_t *idxs, void *stream);
 
+/* ---- surface regularisers of the training step (SURVEY.md section 8(f) row 2) -----------------------------------
+ * Replaces the torch bodies of ProjectionLoss (kind 0) and RepulsionLoss (kind 1) (DSS/training/losses.py:282-497) on
+ * packed clouds (points, normals (P,3); first_idx, num_points as for dss_knn_points).  knn_dists (P, K-1+self_col) f32
+ * and knn_idx (same shape) i32 hold each row's K-NN as dss_knn_points writes it (local indices, ascending, -1 padded;
+ * a missing entry is taken as pytorch3d's padding: distance 0, index 0); self_col = 1: column 0 is the query itself and
+ * is dropped, self_col = 0: the rows hold the K-1 neighbours only.  2 <= K <= 32.  The neighbour positions: knn_pos
+ * (P, K-1+self_col, 3) f32, one per column, used as given (a caller's pytorch3d `knn`), or, when knn_pos is NULL, read
+ * at the neighbour's index from neighbour_points (P,3) f32 -- the positions the rows were built on, which the loss keeps
+ * when it reuses its rows after the points moved -- or from `points` when that is NULL too; read by index they are zero
+ * from column num_points[n] of the given row on, as knn_gather(..., lengths) gives them.  reliable (P,) bytes or NULL: rows
+ * marked keep their own normal in the denoise (visibility & inmask); visible (P,) bytes or NULL (kind 0 only): the
+ * neighbour weight 1 / 0.1 (losses.py:335-337).  Outputs:
+ *   kind 0: loss (P,) = sum w_j sdf_j^2 / eps_denom(sum w_j), grad_coef (P,3) = d loss_i / d p_i;
+ *   kind 1: loss (P,3) = exp(-|r_i|), grad_coef (P,9) = row-major M_i with d L / d p_i = M_i (d L / d loss_i).
+ * The neighbours, the weights and the denoised normals are constants, as in the reference: row i's loss depends on p_i
+ * only.  Deterministic (no float atomics); no host synchronisation; scratch from the context. */
+DSS_API int dss_surface_regulariser(dss_ctx *ctx, int kind, const float *points, const float *normals,
+                                    const int64_t *first_idx, const int64_t *num_points, int N, int64_t P,
+                                    const float *knn_dists, const int32_t *knn_idx, int K, int self_col,
+                                    const float *knn_pos, const float *neighbour_points, const uint8_t *reliable,
+                                    const uint8_t *visible, float sharpness_sigma, float filter_scale, float *loss,
+                                    float *grad_coef, void *stream);
+
 /* ---- fused renderer path (what bench.py times) ----------------------------------------------
  * One call per direction for SurfaceSplattingRenderer.forward / its autograd backward
  * (DSS/core/renderer.py:36-82, DSS/core/rasterizer.py:584-664,749-977).  All pointers device. */
