@@ -67,6 +67,7 @@ enum BufId {
     BUF_CAMERA,       // per-block fp64 partial sums of the camera gradients
     BUF_LIGHT,        // per-block fp64 partial sums of the light gradients
     BUF_REGULARISER,  // denoised normals (P,3) and per-cloud bounding boxes of the surface regularisers
+    BUF_IMAGE_LOSS,   // per-block fp64 partial sums of the image loss, and the finish's block counter
     NUM_BUFS
 };
 
@@ -182,6 +183,53 @@ __device__ __forceinline__ int f2ord(float f) {
     return i >= 0 ? i : i ^ 0x7fffffff;
 }
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
+
+// sum of acc[k] over the block (blockDim.x a multiple of 32, at most 256) in a fixed order; thread k < K
+// returns sum k, the others 0
+template <int K>
+__device__ __forceinline__ double block_sum(const double (&acc)[K], double (*sPart)[K]) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) sPart[warp][k] = v;
+    }
+    __syncthreads();
+    double v = 0.0;
+    if (threadIdx.x < K)
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += sPart[w][threadIdx.x];
+    return v;
+}
+
+// Pass 2 of the fixed-order fp64 sums (camera and light gradients, image loss) over partials (N, nl, blocks, SUMS).
+// Block (l, m) sums slice l of output row m -- view m (per_view: cameras, per-view lights, image loss; its partials in
+// block order), or, for the only row of shared lights, the partials of view 0 in block order, then view 1, ....  Each
+// thread adds a fixed, strided subset, block_sum combines them in a fixed order, rows(totals, l, m, k) writes the
+// outputs.
+template <int SUMS, class Rows>
+__global__ void __launch_bounds__(256) grad_finish_kernel(const double *partials, int blocks, int n_views, int per_view,
+                                                          const Rows rows) {
+    __shared__ double sPart[8][SUMS];
+    __shared__ double sTot[SUMS];
+    const int l = blockIdx.x, m = blockIdx.y, nl = gridDim.x, k = threadIdx.x;
+    const int n0 = per_view ? m : 0;
+    const int64_t count = (int64_t)(per_view ? 1 : n_views) * blocks;
+    double acc[SUMS];
+#pragma unroll
+    for (int j = 0; j < SUMS; ++j) acc[j] = 0.0;
+    for (int64_t e = threadIdx.x; e < count; e += blockDim.x) {
+        const int64_t n = n0 + e / blocks, b = e % blocks;
+        const double *p = partials + ((n * nl + l) * blocks + b) * SUMS;
+#pragma unroll
+        for (int j = 0; j < SUMS; ++j) acc[j] += p[j];
+    }
+    const double v = block_sum(acc, sPart);
+    if (k < SUMS) sTot[k] = v;
+    __syncthreads();
+    rows(sTot, l, m, k);
+}
 
 struct ViewRange {
     int64_t first;

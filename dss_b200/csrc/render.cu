@@ -652,25 +652,6 @@ struct CamArgs {
     double *partials;         // (N, gridDim.x, CAM_SUMS)
 };
 
-// sum of acc[k] over the block (blockDim.x a multiple of 32, at most 256) in a fixed order; thread k < K
-// returns sum k, the others 0
-template <int K>
-__device__ __forceinline__ double block_sum(const double (&acc)[K], double (*sPart)[K]) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < K; ++k) {
-        double v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) sPart[warp][k] = v;
-    }
-    __syncthreads();
-    double v = 0.0;
-    if (threadIdx.x < K)
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += sPart[w][threadIdx.x];
-    return v;
-}
-
 constexpr int CAM_BATCH = 4;   // slots per thread whose loads are issued together
 
 template <bool SHADE>
@@ -839,33 +820,6 @@ struct LightRows {
         if (grad_ambient && l == 0 && k < 3) grad_ambient[m * 3 + k] = (float)tot[9 + k];
     }
 };
-
-// Pass 2 of the camera and light gradients over partials (N, nl, blocks, SUMS).  Block (l, m) sums slice l of output row
-// m -- view m (per_view: cameras, per-view lights; its partials in block order), or, for the only row of shared lights,
-// the partials of view 0 in block order, then view 1, ....  Each thread adds a fixed, strided subset, block_sum combines
-// them in a fixed order, rows(totals, l, m, k) writes the outputs.
-template <int SUMS, class Rows>
-__global__ void __launch_bounds__(256) grad_finish_kernel(const double *partials, int blocks, int n_views, int per_view,
-                                                          const Rows rows) {
-    __shared__ double sPart[8][SUMS];
-    __shared__ double sTot[SUMS];
-    const int l = blockIdx.x, m = blockIdx.y, nl = gridDim.x, k = threadIdx.x;
-    const int n0 = per_view ? m : 0;
-    const int64_t count = (int64_t)(per_view ? 1 : n_views) * blocks;
-    double acc[SUMS];
-#pragma unroll
-    for (int j = 0; j < SUMS; ++j) acc[j] = 0.0;
-    for (int64_t e = threadIdx.x; e < count; e += blockDim.x) {
-        const int64_t n = n0 + e / blocks, b = e % blocks;
-        const double *p = partials + ((n * nl + l) * blocks + b) * SUMS;
-#pragma unroll
-        for (int j = 0; j < SUMS; ++j) acc[j] += p[j];
-    }
-    const double v = block_sum(acc, sPart);
-    if (k < SUMS) sTot[k] = v;
-    __syncthreads();
-    rows(sTot, l, m, k);
-}
 
 // point blocks per slice of the partials kernels: one wave over all slices at two blocks per SM (95-122 registers per
 // thread), and no more blocks than the points need

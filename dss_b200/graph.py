@@ -8,6 +8,11 @@ allocates in steady state (DESIGN.md "Host side"), so the whole step can be capt
     step.replay()                    # image in step.image, gradients in step.grad_points / step.grad_colours
     step.points.data.add_(...)       # update the step's OWN static leaves in place (optimizer step), replay again
 
+With ``targets=(img, mask_img, lambda_rgb, lambda_silhouette)`` instead of ``grad_image`` the captured step is render
+forward -> ``image_loss`` (dss_b200.training.losses, its fused route) -> backward of ``loss``: the step owns static copies
+``step.img`` / ``step.mask_img`` that the caller updates in place between replays (the next batch), and ``step.loss``
+holds the loss dict's device scalars of the last replay.
+
 The step owns its differentiated inputs (`step.points`, `step.colours`, `step.normals`: fresh leaf copies of what was passed
 in): a leaf that has already been through an eager backward on the default stream carries an AccumulateGrad node bound
 to that stream, and synchronising with the legacy default stream is not capturable.
@@ -21,13 +26,28 @@ import torch
 
 from . import _lib
 from .ops import render_points
+from .training.losses import fused_image_loss_targets, image_loss
 
 __all__ = ["GraphedRenderStep"]
 
 
 class GraphedRenderStep:
-    def __init__(self, points, normals, colours, proj, view, h, params, grad_image, shading=None, warmup=3,
-                 grad_sync=None):
+    def __init__(self, points, normals, colours, proj, view, h, params, grad_image=None, shading=None, warmup=3,
+                 grad_sync=None, targets=None):
+        if (grad_image is None) == (targets is None):
+            raise ValueError("pass exactly one of grad_image and targets=(img, mask_img, lambda_rgb, lambda_silhouette)")
+        if targets is not None:
+            img, mask_img, lambda_rgb, lambda_sil = targets
+            _lib.require_cuda(points, img, mask_img)
+            # the step differentiates its own detached copies; the torch body would wait for the device, which a
+            # capture cannot do
+            if not fused_image_loss_targets(img.detach(), mask_img.detach()):
+                raise TypeError("targets must be a float32 img and a float32, uint8 or bool mask_img (the fused image "
+                                "loss); got %s and %s" % (img.dtype, mask_img.dtype))
+            # static copies the caller refills in place between replays (clone keeps a permuted view's strides)
+            self.img, self.mask_img = img.detach().clone(), mask_img.detach().clone()
+            self._lambdas = (float(lambda_rgb), float(lambda_sil))
+        self.loss = None
         dev = _lib.require_cuda(points, normals, colours, proj, view, h, grad_image)
         self.device = dev
         leaf = lambda t: t.detach().clone().requires_grad_(True)
@@ -77,7 +97,11 @@ class GraphedRenderStep:
         self._clear_grads()
         points, normals, colours, proj, view, h, params = self._args
         out = render_points(points, normals, colours, proj, view, h, params, shading=self._shading, grad_sync=self._sync)
-        out.image.backward(self.grad_image)
+        if self.grad_image is not None:
+            out.image.backward(self.grad_image)
+        else:
+            self.loss = image_loss(out.image, self.img, self.mask_img, *self._lambdas)
+            self.loss["loss"].backward()
         return out
 
     def _tile_total(self):

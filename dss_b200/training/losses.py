@@ -18,6 +18,7 @@ Two routes compute the same formulas, chosen by device and dtype:
 CUDA tensors take the CUDA K-NN; a caller on another device passes ``knn_tree=(dists, idx, knn)`` (the reference has
 the same keyword) -- there is no CPU search in this package.
 """
+import ctypes as C
 from typing import NamedTuple, Optional
 
 import torch
@@ -26,7 +27,7 @@ import torch.nn as nn
 from .. import _lib
 
 __all__ = ["BaseLoss", "L1Loss", "L2Loss", "SurfaceLoss", "ProjectionLoss", "RepulsionLoss", "KNN",
-           "surface_regulariser"]
+           "surface_regulariser", "IouLoss", "image_loss", "image_loss_torch", "fused_image_loss_targets"]
 
 
 class KNN(NamedTuple):
@@ -447,3 +448,121 @@ class RepulsionLoss(SurfaceLoss):
         repel = torch.sum(proj * weights.unsqueeze(-1), dim=1) / eps_denom(torch.sum(weights, dim=1).unsqueeze(-1))
         repel = repel * density_w                                                                      # :482-485
         return torch.exp(-repel.abs())                                                                 # :487
+
+
+# -- image loss --------------------------------------------------------------------------------------------------------
+class IouLoss(BaseLoss):
+    """losses.py:498-513: 1 - intersection / union over every dimension but the first (the trainer builds it with
+    ``channel_dim=None``)."""
+
+    def compute(self, predict, target, **kwargs):
+        dims = tuple(range(predict.ndimension())[1:])
+        intersect = (predict * target).sum(dims)
+        union = (predict + target - predict * target).sum(dims)
+        return 1.0 - intersect / eps_denom(union)
+
+
+def _image_loss_inputs(rgba, img, mask_img):
+    """shape and device checks shared by both routes; returns the mask as (N,H,W)"""
+    if rgba.dim() != 4 or rgba.shape[-1] != 4:
+        raise RuntimeError("rgba must have shape (N, H, W, 4), got %s" % (tuple(rgba.shape),))
+    N, H, W = rgba.shape[:3]
+    if N < 1 or H < 1 or W < 1:
+        raise RuntimeError("rgba must hold at least one pixel, got %s" % (tuple(rgba.shape),))
+    if tuple(img.shape) != (N, H, W, 3):
+        raise RuntimeError("img must have shape (N, H, W, 3) = %s, got %s" % ((N, H, W, 3), tuple(img.shape)))
+    if tuple(mask_img.shape) not in ((N, H, W), (N, 1, H, W)):
+        raise RuntimeError("mask_img must have shape (N, H, W) or (N, 1, H, W), got %s" % (tuple(mask_img.shape),))
+    if not (rgba.device == img.device == mask_img.device):
+        raise RuntimeError("rgba, img and mask_img must be on one device")
+    return mask_img.reshape(N, H, W)
+
+
+def image_loss_torch(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0):
+    """Trainer.calc_dr_loss (trainer.py:332-376) in torch ops, line for line, its host synchronisations included (the
+    ``mask_pred.sum() > 0`` branch and the boolean index); any dtype and device.  The float64 reference of the tests."""
+    mask_img = _image_loss_inputs(rgba, img, mask_img)
+    img_pred, mask_img_pred = rgba[..., :3], rgba[..., 3]
+    zero = rgba.new_zeros(())
+    loss_dr_silhouette = zero
+    loss_dr_rgb = zero
+    if lambda_rgb > 0:
+        mask_pred = mask_img.bool() & mask_img_pred.bool()
+        if mask_pred.sum() > 0:
+            loss_dr_rgb = L1Loss(reduction="mean")(img, img_pred, mask=mask_pred) * lambda_rgb
+    if lambda_silhouette > 0:
+        loss_mask = (mask_img.float() - mask_img_pred).abs()
+        loss_mask = loss_mask.mean()
+        loss_iou = IouLoss(reduction="mean", channel_dim=None)(mask_img.float(), mask_img_pred)
+        loss_dr_silhouette = (0.01 * loss_iou + loss_mask) * lambda_silhouette
+    return {"loss": loss_dr_rgb + loss_dr_silhouette + zero, "loss_dr_rgb": loss_dr_rgb,
+            "loss_dr_silhouette": loss_dr_silhouette, "loss_image_gradients": zero}
+
+
+def _image_loss_call(name, rgba, img, mask, lambda_rgb, lambda_sil, *tail):
+    N, H, W = rgba.shape[:3]
+    dev = rgba.device
+    strides = (C.c_int64 * 4)(*img.stride())
+    with torch.cuda.device(dev):
+        rc = getattr(_lib.load(), name)(
+            _lib.ctx(dev), _lib.ptr(rgba), _lib.ptr(img), strides, _lib.ptr(mask), int(mask.dtype != torch.float32),
+            N, H, W, float(lambda_rgb), float(lambda_sil), *[_lib.ptr(t) for t in tail], _lib.stream_ptr(dev))
+    _lib.check(rc, name)
+
+
+class _ImageLoss(torch.autograd.Function):
+    """dss_image_loss_forward (the three loss scalars and the per-view totals) and dss_image_loss_backward (the RGBA
+    gradient, from the upstream gradients of the three scalars on the device)."""
+
+    @staticmethod
+    def forward(ctx, rgba, img, mask, lambda_rgb, lambda_sil):
+        N, dev = rgba.shape[0], rgba.device
+        totals = torch.empty((N + 1, 5), dtype=torch.float64, device=dev)
+        loss, loss_rgb, loss_sil = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(3))
+        _image_loss_call("dss_image_loss_forward", rgba, img, mask, lambda_rgb, lambda_sil, totals, loss, loss_rgb,
+                         loss_sil)
+        ctx.lambdas = (lambda_rgb, lambda_sil)
+        ctx.save_for_backward(rgba, img, mask, totals)
+        return loss, loss_rgb, loss_sil
+
+    @staticmethod
+    def backward(ctx, g_loss, g_rgb, g_sil):
+        rgba, img, mask, totals = ctx.saved_tensors
+        grad = torch.empty_like(rgba, memory_format=torch.contiguous_format)
+        ups = [g.to(torch.float32).contiguous() for g in (g_loss, g_rgb, g_sil)]
+        _image_loss_call("dss_image_loss_backward", rgba, img, mask, *ctx.lambdas, totals, *ups, grad)
+        return grad, None, None, None, None
+
+
+def fused_image_loss_targets(img, mask_img):
+    """True when the targets take image_loss's fused route (with a float32 CUDA rgba): float32 GT RGB, a float32, uint8
+    or bool mask, neither requiring grad (the fused route differentiates the RGBA only; the torch body gives the
+    targets their gradient)"""
+    return img.is_cuda and img.dtype == torch.float32 and mask_img.dtype in (torch.float32, torch.uint8, torch.bool) \
+        and not img.requires_grad and not mask_img.requires_grad
+
+
+def image_loss(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0):
+    """The image loss of the training step, ``Trainer.calc_dr_loss`` (trainer.py:332-376) on the renderer's RGBA:
+    the masked RGB L1 (``L1Loss``, mean over the pixels where both masks are non-zero) times ``lambda_rgb`` and the
+    silhouette L1 plus 0.01 x ``IouLoss`` times ``lambda_silhouette``; a term whose lambda is not > 0 is absent.
+
+    ``rgba`` (N,H,W,4): the rendered image, its last channel the predicted mask; ``img`` (N,H,W,3) ground-truth RGB,
+    any strides (``img.permute(0, 2, 3, 1)`` of an (N,3,H,W) batch reads in place); ``mask_img`` (N,H,W) or (N,1,H,W)
+    float, uint8 or bool, its value used in the silhouette terms.  Returns the reference's loss dict (``loss``,
+    ``loss_dr_rgb``, ``loss_dr_silhouette``, ``loss_image_gradients`` = 0) as device scalars.
+
+    float32 CUDA inputs take the fused route (csrc/image_loss.cu: two launches forward, one backward, no host
+    synchronisation, bit-reproducible), which differentiates ``rgba``; every other dtype or device, and targets that
+    require grad, run :func:`image_loss_torch`."""
+    mask = _image_loss_inputs(rgba, img, mask_img)
+    if not (rgba.is_cuda and rgba.dtype == torch.float32 and fused_image_loss_targets(img, mask)):
+        return image_loss_torch(rgba, img, mask_img, lambda_rgb, lambda_silhouette)
+    lambda_rgb, lambda_silhouette = float(lambda_rgb), float(lambda_silhouette)
+    rgba_c = rgba.contiguous()
+    if rgba_c.data_ptr() % 16:
+        rgba_c = rgba_c.clone()
+    mask = mask.contiguous()
+    loss, loss_rgb, loss_sil = _ImageLoss.apply(rgba_c, img, mask, lambda_rgb, lambda_silhouette)
+    zero = torch.zeros((), dtype=torch.float32, device=rgba.device)
+    return {"loss": loss, "loss_dr_rgb": loss_rgb, "loss_dr_silhouette": loss_sil, "loss_image_gradients": zero}

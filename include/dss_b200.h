@@ -217,6 +217,34 @@ DSS_API int dss_surface_regulariser(dss_ctx *ctx, int kind, const float *points,
                                     const uint8_t *visible, float sharpness_sigma, float filter_scale, float *loss,
                                     float *grad_coef, void *stream);
 
+/* ---- image loss of the training step ----------------------------------------------------------------------------
+ * Trainer.calc_dr_loss (DSS/training/trainer.py:332-376) on the renderer's RGBA: with mask_pred = m != 0 && alpha != 0
+ * (NaN counts as non-zero, as torch's .bool()),
+ *   loss_rgb = lambda_rgb * sum_{mask_pred} sum_c |gt - pred| / M, M = |mask_pred| (0 when M == 0),
+ *   loss_sil = lambda_sil * (sum |m - alpha| / (N H W) + 0.01 * mean_n (1 - I_n / eps_denom(U_n))),
+ *   I_n = sum_view n m alpha, U_n = sum_view n (m + alpha - m alpha), loss = loss_rgb + loss_sil.
+ * A term whose lambda is not > 0 is absent (0, no gradient; without the RGB term gt is not read).  pred (N,H,W,4) f32 contiguous,
+ * 16-byte aligned; gt rgb f32 at gt[n*s0 + y*s1 + x*s2 + c*s3] with gt_strides = {s0, s1, s2, s3} (host array, in
+ * elements); mask (N,H,W) contiguous, f32 (mask_kind 0) or bytes (mask_kind 1: bool / uint8), its value used in the
+ * silhouette terms.  H*W <= 2^31-1, N <= 65535.
+ * Forward (2 launches): totals (N+1, 5) f64, caller-owned and kept for the backward -- row n: M_n, sum |d rgb|,
+ * sum |m - alpha|, I_n, U_n of view n; row N: the sums of the first three, sum_n (1 - I_n / eps_denom(U_n)), 0 -- and
+ * the three f32 scalars loss, loss_rgb, loss_sil, all on the device.
+ * Backward (1 launch): grad_pred (N,H,W,4) f32, 16-byte aligned, every element written, from the upstream gradients of
+ * the three scalars (device f32 scalars): rgb sign(pred - gt) lambda_rgb (g_loss + g_rgb) / M inside mask_pred, else 0;
+ * alpha lambda_sil (g_loss + g_sil) (sign(alpha - m) / (N H W) - 0.01 (m E_n - I_n (1 - m) dE_n) / (N E_n^2)) with
+ * E_n = eps_denom(U_n) and dE_n = [|U_n| >= 1e-17]; sign(0) = sign(NaN) = 0, as torch's abs backward.
+ * Deterministic: fixed-order fp64 sums, no float atomics; no host synchronisation; partial sums in context scratch. */
+DSS_API int dss_image_loss_forward(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
+                                   const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb,
+                                   double lambda_sil, double *totals, float *loss, float *loss_rgb, float *loss_sil,
+                                   void *stream);
+DSS_API int dss_image_loss_backward(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
+                                    const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb,
+                                    double lambda_sil, const double *totals, const float *grad_loss,
+                                    const float *grad_loss_rgb, const float *grad_loss_sil, float *grad_pred,
+                                    void *stream);
+
 /* ---- fused renderer path (what bench.py times) ----------------------------------------------
  * One call per direction for SurfaceSplattingRenderer.forward / its autograd backward
  * (DSS/core/renderer.py:36-82, DSS/core/rasterizer.py:584-664,749-977).  All pointers device. */
