@@ -15,6 +15,8 @@
 // Everything (bounding box, grid parameters, counting sort) is computed on the device; no host round trip.
 #include <math_constants.h>
 
+#include <cfloat>
+
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -44,7 +46,7 @@ knn_bbox_kernel(const float *__restrict__ pts, const int64_t *__restrict__ first
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             const float v = pts[(f + i) * 3 + k];
-            if (v == v) {                           // NaN coordinates do not shape the grid
+            if (isfinite(v)) {                      // NaN and +-inf coordinates do not shape the grid
                 lo[k] = min(lo[k], f2ord(v));
                 hi[k] = max(hi[k], f2ord(v));
             }
@@ -66,6 +68,14 @@ knn_bbox_kernel(const float *__restrict__ pts, const int64_t *__restrict__ first
 
 // Cell size from the density: clouds on this path are surfaces, so aim at ~3 points per occupied cell of a surface
 // with the bounding box's face area; never more than KNN_GMAX cells; never finer than 1/1024 of the largest extent.
+//
+// The grid holds for every input, 1 <= res[k] and res[0] res[1] res[2] <= KNN_GMAX, so no cell index leaves the cloud's
+// counters.  The bounding box holds finite coordinates only, so each extent is finite once an overflowing difference
+// (+-3e38 in one cloud) is clamped to FLT_MAX; `cell` is finite and positive (an overflowing density cell is clamped to
+// FLT_MAX, a zero one replaced by 1).  Then e/cell is in [0, inf] and r = floor(e/cell) + 1 in [1, inf]; the growth test
+// compares integers below 2^24 exactly (a product of such r that rounds is larger than 2^21 before and after rounding),
+// so a loop exit means the grid fits.  If 64 steps of x1.26 do not suffice (far outliers, a radius far below the
+// extent), cell >= emax / 126 gives e/cell <= 126 (1 + 3u) < 127 on every axis: res <= 127 and 127^3 < 2^21.
 __global__ void knn_params_kernel(const int *__restrict__ bbox, const int64_t *__restrict__ num, float radius, int N,
                                   KnnGrid *__restrict__ grids) {
     const int n = blockIdx.x * blockDim.x + threadIdx.x;
@@ -75,7 +85,7 @@ __global__ void knn_params_kernel(const int *__restrict__ bbox, const int64_t *_
     for (int k = 0; k < 3; ++k) {
         const float lo = ord2f(bbox[n * 6 + k]), hi = ord2f(bbox[n * 6 + 3 + k]);
         g.gmin[k] = (num[n] > 0 && hi >= lo) ? lo : 0.0f;
-        e[k] = (num[n] > 0 && hi >= lo) ? fmaxf(hi - lo, 0.0f) : 0.0f;
+        e[k] = (num[n] > 0 && hi >= lo) ? fminf(fmaxf(hi - lo, 0.0f), FLT_MAX) : 0.0f;
     }
     const float emax = fmaxf(e[0], fmaxf(e[1], e[2]));
     const float P = (float)(num[n] > 0 ? num[n] : 1);
@@ -83,12 +93,15 @@ __global__ void knn_params_kernel(const int *__restrict__ bbox, const int64_t *_
     float cell = sqrtf(3.0f * area / P);
     cell = fmaxf(cell, emax * (1.0f / 1024.0f));
     if (radius > 0.0f) cell = fminf(cell, radius);
+    cell = fminf(cell, FLT_MAX);
     if (!(cell > 0.0f)) cell = 1.0f;                               // degenerate cloud (single point / all equal)
-    for (int it = 0; it < 64; ++it) {                              // grow until the grid fits
+    bool fits = false;
+    for (int it = 0; it < 64 && !fits; ++it) {                     // grow until the grid fits
         const float r0 = floorf(e[0] / cell) + 1.0f, r1 = floorf(e[1] / cell) + 1.0f, r2 = floorf(e[2] / cell) + 1.0f;
-        if (r0 * r1 * r2 <= (float)KNN_GMAX) break;
-        cell *= 1.26f;
+        fits = r0 * r1 * r2 <= (float)KNN_GMAX;
+        if (!fits) cell *= 1.26f;
     }
+    if (!fits) cell = fmaxf(cell, emax * (1.0f / 126.0f));
     g.cell = cell;
     g.inv_cell = 1.0f / cell;
     for (int k = 0; k < 3; ++k) g.res[k] = (int)(floorf(e[k] / cell) + 1.0f);
@@ -143,19 +156,34 @@ __device__ __forceinline__ void knn_insert(float (&bd)[KMAX], int (&bi)[KMAX], i
 
 // One thread per query.  self_mode: the queries are the data points themselves, visited in grid order so that
 // neighbouring threads read the same cells.
+//
+// The ring bound.  After ring R every cell within R of the query's cell (cx, cy, cz) has been visited, so an unseen
+// point lies R + 1 or more cells away along some axis.  The computed coordinate t = fl(fl(v - gmin) * inv_cell) differs
+// from (v - gmin) * inv_cell by at most err = 2.0001 u t (two roundings, u = 2^-24); clamping into a border cell only
+// moves t outward, and only t < res + 1 decides a cell, so err <= 2.0001 u (maxres + 1).  The unseen point is
+// therefore at least (R - 2 err) / inv_cell away along that axis, and 1 / inv_cell >= cell (1 - u).  Its computed
+// squared distance (one difference, one square, two sums of non-negative terms) is at least (1 - 5u) times the exact
+// one, and reach2 = fl(fl(fl(R - slack) * cell)^2) at most (1 + 5u) (R - slack)^2 cell^2.  Hence bd[K-1] < reach2
+// proves that no unseen point can enter the list once R - slack <= (R - 2 err)(1 - 6.1u), i.e. for
+// slack >= 2 err + 6.1 u R; with R <= maxres, slack = 16 u (maxres + 2) covers it.  That is ~1e-3 cells at the
+// density floor's res <= 1025, and ~2 cells at the res = 2^21 the radius clamp allows along one axis, where t itself
+// is only known to ~0.25 cells.
 template <int KMAX>
 __global__ void __launch_bounds__(128)
 knn_search_kernel(const float *__restrict__ queries, const int64_t *__restrict__ qfirst, const int64_t *__restrict__ qnum,
-                  const int64_t *__restrict__ dfirst, const KnnGrid *__restrict__ grids,
-                  const int32_t *__restrict__ offsets, const float4 *__restrict__ sorted, int self_mode, int K,
-                  float radius, float *__restrict__ out_d, int32_t *__restrict__ out_i) {
+                  const KnnGrid *__restrict__ grids, const int32_t *__restrict__ offsets,
+                  const float4 *__restrict__ sorted, int self_mode, int K, float radius, float *__restrict__ out_d,
+                  int32_t *__restrict__ out_i) {
     const int n = blockIdx.y;
     const int64_t qf = qfirst[n], qc = qnum[n];
     const KnnGrid g = grids[n];
     const int32_t *off = offsets + (int64_t)n * KNN_GMAX;
-    const int64_t dbase = dfirst[n];                 // == first slot of this cloud in `sorted`
+    // the scan runs over all clouds, so cloud n's first slot in `sorted` is the sum of the earlier clouds' sizes, whatever
+    // gaps the caller's first_idx leaves between them
+    const int64_t dbase = off[0];
     const float r2 = radius > 0.0f ? radius * radius : CUDART_INF_F;
     const int maxres = max(g.res[0], max(g.res[1], g.res[2]));
+    const float slack = (float)(maxres + 2) * 0x1p-20f;             // 16 u (maxres + 2), see above
     for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < qc; t += (int64_t)gridDim.x * blockDim.x) {
         float qx, qy, qz;
         int64_t row;
@@ -177,9 +205,12 @@ knn_search_kernel(const float *__restrict__ queries, const int64_t *__restrict__
         const int cx = knn_axis_cell(qx, g.gmin[0], g.inv_cell, g.res[0]);
         const int cy = knn_axis_cell(qy, g.gmin[1], g.inv_cell, g.res[1]);
         const int cz = knn_axis_cell(qz, g.gmin[2], g.inv_cell, g.res[2]);
+        // a non-finite query is at distance inf or NaN from every point, so it has no neighbour: skip the search
+        // (which no bound would cut short)
+        const bool finite = isfinite(qx) && isfinite(qy) && isfinite(qz);
         // distance from the query to the faces of its own cell along the grid: queries outside the box (general mode)
         // are clamped into a border cell, the ring bound below then starts from their distance to that cell's far side
-        for (int ring = 0; ring <= maxres; ++ring) {
+        for (int ring = 0; finite && ring <= maxres; ++ring) {
             const int x0 = max(cx - ring, 0), x1 = min(cx + ring, g.res[0] - 1);
             const int y0 = max(cy - ring, 0), y1 = min(cy + ring, g.res[1] - 1);
             for (int x = x0; x <= x1; ++x)
@@ -211,7 +242,7 @@ knn_search_kernel(const float *__restrict__ queries, const int64_t *__restrict__
                 }
             // every point not yet seen lies outside the cube of (2 ring + 1)^3 cells around the query's cell, i.e. at
             // least ring cells away (minus rounding slack): stop when that cannot beat the K-th best or the radius
-            const float reach = fmaxf((float)ring - 1e-3f, 0.0f) * g.cell;
+            const float reach = fmaxf((float)ring - slack, 0.0f) * g.cell;
             const float reach2 = reach * reach;
             if (reach2 >= r2 || bd[K - 1] < reach2) break;
             if (x0 == 0 && y0 == 0 && x1 == g.res[0] - 1 && y1 == g.res[1] - 1 && cz - ring <= 0 && cz + ring >= g.res[2] - 1)
@@ -284,17 +315,15 @@ int dss_knn_points(dss_ctx *ctx, const float *queries, const int64_t *query_firs
     {
         const unsigned qb = (unsigned)((Pq + 127) / 128 > 0 ? (Pq + 127) / 128 : 1);
         dim3 grid(qb < 65535u ? qb : 65535u, N);
-        // offsets index `sorted` globally (the scan runs over all clouds), so cloud n's first slot is offsets[n*GMAX];
-        // in self mode thread t of cloud n reads sorted[first_idx[n] + t] -- identical because every earlier cloud
-        // contributes exactly num_points entries
+        // offsets index `sorted` globally (the scan runs over all clouds), so cloud n's first slot is offsets[n*GMAX]
         if (K <= 8)
-            knn_search_kernel<8><<<grid, 128, 0, st>>>(queries, query_first_idx, query_num, first_idx, grids, offsets, sorted,
+            knn_search_kernel<8><<<grid, 128, 0, st>>>(queries, query_first_idx, query_num, grids, offsets, sorted,
                                                        self_mode ? 1 : 0, K, radius, sq_dists, idxs);
         else if (K <= 16)
-            knn_search_kernel<16><<<grid, 128, 0, st>>>(queries, query_first_idx, query_num, first_idx, grids, offsets, sorted,
+            knn_search_kernel<16><<<grid, 128, 0, st>>>(queries, query_first_idx, query_num, grids, offsets, sorted,
                                                         self_mode ? 1 : 0, K, radius, sq_dists, idxs);
         else
-            knn_search_kernel<32><<<grid, 128, 0, st>>>(queries, query_first_idx, query_num, first_idx, grids, offsets, sorted,
+            knn_search_kernel<32><<<grid, 128, 0, st>>>(queries, query_first_idx, query_num, grids, offsets, sorted,
                                                         self_mode ? 1 : 0, K, radius, sq_dists, idxs);
         DSS_LAUNCH_CHECK(ctx);
     }

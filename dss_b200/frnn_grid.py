@@ -49,8 +49,11 @@ def counting_sort_cuda(points, lengths, grid_cell, grid_idx, grid_off, sorted_po
 
 def knn_points_packed(points, first_idx, num_points, K, r=-1.0, queries=None, query_first_idx=None, query_num=None,
                       return_idx=True):
-    """Packed form: ``points`` (P,3) f32, cloud n owns rows [first_idx[n], first_idx[n] + num_points[n]) (contiguous).
-    Returns ``(sq_dists (Pq,K) f32 ascending, idxs (Pq,K) int32 local to the cloud or None)``, -1 padded."""
+    """Packed form: ``points`` (P,3) f32, cloud n owns rows [first_idx[n], first_idx[n] + num_points[n]).  The ranges
+    may leave gaps between them (padded storage passed as packed: first_idx = n * Pmax, num_points = lengths) but must
+    not overlap; rows outside every query range are left unwritten.  Returns ``(sq_dists (Pq,K) f32 ascending, idxs
+    (Pq,K) int32 local to the cloud or None)``, -1 padded.  Rows of points or queries with a NaN or infinite coordinate
+    are all -1, and such points are nobody's neighbour."""
     dev = _lib.require_cuda(points, first_idx, num_points, queries, query_first_idx, query_num)
     if points.dim() != 2 or points.shape[1] != 3:
         raise RuntimeError("points must have shape (P, 3)")

@@ -185,9 +185,11 @@ DSS_API int dss_zbuf_backward(dss_ctx *ctx, const int32_t *idx, const float *gra
  * splats (DSS/core/rasterizer.py:313-326, 369-388).  For every query of cloud n: the K points of cloud n with the
  * smallest (squared distance, index), squared distance < r^2 (r <= 0: no limit), ascending; missing entries are -1.
  * Semantics and tie rule of the reference's ground truth FRNNBruteForceCPU (bruteforce_cpu.cpp:8-64).
- * Packed layout: cloud n owns rows [first_idx[n], first_idx[n] + num_points[n]) and the clouds are contiguous
- * (first_idx[n] = sum of the earlier num_points); idxs are local to the cloud.  queries == NULL (or == points): the
- * cloud is searched against itself (the self match, distance 0, is returned first, as in the reference).
+ * Packed layout: cloud n owns rows [first_idx[n], first_idx[n] + num_points[n]); the ranges may leave gaps (padded
+ * storage passed as packed) but must not overlap, and rows outside every query range are not written.  idxs are local
+ * to the cloud.  queries == NULL (or == points): the cloud is searched against itself (the self match, distance 0, is
+ * returned first, as in the reference).  A point or query with a NaN or infinite coordinate is at distance inf or NaN
+ * from everything, so it is nobody's neighbour and its own row is all -1; it does not shape the grid.
  * sq_dists (Pq,K) f32, idxs (Pq,K) i32 or NULL.  1 <= K <= 32.  No host synchronisation. */
 DSS_API int dss_knn_points(dss_ctx *ctx, const float *queries, const int64_t *query_first_idx,
                            const int64_t *query_num, const float *points, const int64_t *first_idx,

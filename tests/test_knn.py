@@ -19,7 +19,7 @@ CASES = [("k7_r0.2", 7, 0.2), ("k12_r0.05", 12, 0.05)]
 
 
 def _clouds(d):
-    return sorted(k[:-len("__points")] for k in d.files if k.endswith("__points"))
+    return sorted(k[:-len("__points")] for k in d.files if k.endswith("__points") and not k.startswith("edge_"))
 
 
 def test_oracle_knn_reproduces_reference_bruteforce_golden_vectors():
@@ -35,6 +35,30 @@ def test_oracle_knn_reproduces_reference_bruteforce_golden_vectors():
     # the small radius leaves some lists short (-1 padding exercised), the self match is always first
     short = d["teapot_normal_dense__k12_r0.05__idxs"]
     assert (short[:, -1] == -1).any() and (short[:, 0] == np.arange(len(short))).all()
+    # the edge families, padded batches (tests/golden/make_golden_knn.py: edge_families)
+    names = [c[0] for c in edge_cases(d)]
+    assert {"edge_duplicates", "edge_r2_boundary", "edge_lattice_ties", "edge_nonfinite", "edge_long_line",
+            "edge_ragged"} <= set(names)
+    for name, pts, lens, K, r in edge_cases(d):
+        first = np.arange(len(lens), dtype=np.int64) * pts.shape[1]
+        dist, idx = oracle.knn_brute(pts.reshape(-1, 3), first, lens, pts.reshape(-1, 3), first, lens, K, r)
+        dist, idx = dist.reshape(pts.shape[:2] + (K,)), idx.reshape(pts.shape[:2] + (K,))
+        assert np.array_equal(dist.view(np.uint32), d[name + "__dists"].view(np.uint32)), name
+        assert np.array_equal(idx, d[name + "__idxs"]), name
+    # what the families are there for, in the reference's own output
+    nf = d["edge_nonfinite__points"][0]
+    bad = ~np.isfinite(nf).all(1)
+    assert bad.sum() == 6 and (d["edge_nonfinite__idxs"][0][bad] == -1).all()
+    on = d["edge_r2_boundary__idxs"][0]
+    assert (on[:20, 1] == -1).all() and (on[40:60, 1] == np.arange(60, 80)).all()    # at r: out; one ulp inside: in
+    z = (d["edge_duplicates__dists"][0] == 0).all(1)                          # 13 copies of 3 points, K = 8
+    assert z.sum() == 39 and (np.diff(d["edge_duplicates__idxs"][0][z], axis=1) > 0).all()
+
+
+def edge_cases(d):
+    """-> [(name, points (N,P,3), lengths (N,), K, r)] of the edge families stored in the K-NN golden file"""
+    names = sorted(k[:-len("__lengths")] for k in d.files if k.startswith("edge_") and k.endswith("__lengths"))
+    return [(n, d[n + "__points"], d[n + "__lengths"], int(d[n + "__K"]), float(d[n + "__r"])) for n in names]
 
 
 def _witness_clouds():
@@ -62,6 +86,58 @@ def test_oracle_knn_matches_compiled_reference_witness():
     dist, idx = oracle.knn_brute(q, np.array([0, 300]), l1, pts, np.array([0, 400]), l2, 5, 0.4)
     assert np.array_equal(dist[:300], dists[0, :300]) and np.array_equal(dist[300:], dists[1, :180])
     assert np.array_equal(idx[:300], idxs[0, :300]) and np.array_equal(idx[300:], idxs[1, :180])
+
+
+def test_cell_model_puts_a_close_pair_two_cells_apart():
+    """Why the ring bound's slack grows with the grid.  On a line longer than 1024 r the radius clamp sets the cell to
+    r and the grid to up to 2^21 cells along x; the computed cell coordinate t = fl(fl(x - gmin) * inv_cell) is then
+    known to ~0.1 cell only, so a fixed slack of 1e-3 cells is unsound.  This float32 model of the kernel's grid puts
+    x = 130105.83f and 130106.02f, 0.977 cells apart, two cells apart; tests/test_gpu_knn_edges.py runs the kernel on
+    a cloud of such pairs (tests.util.knn_long_line)."""
+    from tests.util import knn_cell_model, knn_long_line
+    f32 = np.float32
+    gmin = f32(-1234.567)
+    ends = np.array([[gmin, 0, 0], [f32(gmin + f32(419000)), 0, 0]], f32)
+    lo, cell, inv, res, cell_of = knn_cell_model(ends, 0.2)
+    assert cell == f32(0.2) and inv == f32(5) and res[0] == 2095001 and (1 << 20) < res[0] <= (1 << 21)
+    a, b = f32(130105.83), f32(130106.02)
+    ca, cb = cell_of(np.array([[a, 0, 0], [b, 0, 0]], f32))[:, 0]
+    assert cb - ca == 2
+    d = f32(b - a)
+    assert float(d) == 0.1953125 and float(d) / float(cell) < 0.999
+    reach2 = f32(f32(f32(f32(1) - f32(1e-3)) * cell) ** 2)       # the old stop test after ring 1
+    assert f32(d * d) < reach2
+    # the slack the kernel derives (16 u (maxres + 2)) covers the error of t at this size: 2 err < slack
+    t_exact = (np.float64(b) - np.float64(gmin)) * np.float64(inv)
+    t_comp = np.float64(f32(f32(b - gmin) * inv))
+    slack = (res.max() + 2) * 2.0 ** -20
+    assert abs(t_comp - t_exact) > 1e-3 and 2 * 2.0001 * 2.0 ** -24 * (res.max() + 1) < slack
+    # the generator of the GPU family: every triple as documented, on the grid of the whole cloud
+    pts, A, B, C = knn_long_line()
+    assert len(A) >= 60
+    _, cell2, _, res2, cell_of2 = knn_cell_model(pts, 0.2)
+    assert cell2 == cell and (res2 == [2095001, 1, 1]).all()
+    ca, cb, cc = cell_of2(pts[A]), cell_of2(pts[B]), cell_of2(pts[C])
+    assert (cb[:, 0] - ca[:, 0] == 2).all() and (cc == ca).all()
+    dab = ((pts[B] - pts[A]).astype(f32) ** 2).astype(f32).sum(1, dtype=f32)
+    dac = ((pts[C] - pts[A]).astype(f32) ** 2).astype(f32).sum(1, dtype=f32)
+    assert (dab < dac).all() and (dac < reach2).all()
+
+
+def test_cell_model_grid_fits_for_adversarial_extents():
+    """The argument in knn_params_kernel: for any finite extents and any radius, 1 <= res[k] and prod res <= 2^21
+    (on the float32 model; the GPU file runs the kernel on such clouds)."""
+    from tests.util import knn_cell_model
+    f32 = np.float32
+    big = f32(3e38)
+    cases = [([[-big, 0, 0], [big, 0, 0]], r) for r in (-1.0, 0.2, 1e-30)]
+    cases += [([[0, 0, 0], [1e8, 0, 0], [0, 1e8, 0], [0, 0, 1e8]], r) for r in (-1.0, 0.2, 1e-6)]
+    cases += [([[-big, -big, -big], [big, big, big]], r) for r in (-1.0, 0.2)]
+    cases += [([[0, 0, 0], [1e-30, 1e-30, 1e-30]], r) for r in (-1.0, 0.2)]
+    cases += [([[0, 0, 0]], 0.2), ([[-0.0, 0, 0], [0.0, 0, 0]], -1.0)]
+    for p, r in cases:
+        _, cell, inv, res, _ = knn_cell_model(np.array(p, f32), r)
+        assert np.isfinite(cell) and cell > 0 and (res >= 1).all() and int(np.prod(res)) <= (1 << 21), (p, r, res)
 
 
 # ------------------------------------------------------------------------------------------------------------

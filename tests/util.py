@@ -243,6 +243,92 @@ def edge_screen_splats(family, S, seed=0, P=1200):
     return pts, ell, cutoff, rad, first, num
 
 
+def knn_cell_model(points, radius):
+    """float32 model of the K-NN grid (knn_params_kernel, knn_axis_cell in dss_b200/csrc/knn.cu) for one cloud of
+    finite points -> (gmin (3,), cell, inv_cell, res (3,), cell_of) with cell_of(x) the (M,3) integer cells of (M,3)
+    points.  The same float32 operations in the same order (IEEE, no contraction); it documents why the ring bound
+    needs its slack and places test points, it does not stand in for the kernel."""
+    f32 = np.float32
+    p = np.asarray(points, f32)
+    lo, hi = p.min(0), p.max(0)
+    with np.errstate(over="ignore"):
+        return _knn_cell_model(p, lo, hi, radius)
+
+
+def _knn_cell_model(p, lo, hi, radius):
+    f32 = np.float32
+    e = np.minimum(np.maximum((hi - lo).astype(f32), f32(0)), f32(np.finfo(f32).max))
+    emax = e.max()
+    area = f32(2) * f32(f32(f32(e[0] * e[1]) + f32(e[1] * e[2])) + f32(e[0] * e[2]))
+    cell = np.sqrt(f32(f32(f32(3) * area) / f32(len(p))))
+    cell = max(cell, f32(emax * f32(1.0 / 1024.0)))
+    if radius > 0:
+        cell = min(cell, f32(radius))
+    cell = min(f32(cell), f32(np.finfo(f32).max))
+    if not cell > 0:
+        cell = f32(1)
+    fits = False
+    for _ in range(64):
+        r = np.floor((e / cell).astype(f32)) + f32(1)
+        fits = f32(f32(r[0] * r[1]) * r[2]) <= f32(1 << 21)
+        if fits:
+            break
+        cell = f32(cell * f32(1.26))
+    if not fits:
+        cell = max(cell, f32(emax * f32(1.0 / 126.0)))
+    inv = f32(f32(1) / cell)
+    res = (np.floor((e / cell).astype(f32)) + f32(1)).astype(np.int64)
+
+    def cell_of(x):
+        t = ((np.asarray(x, f32) - lo).astype(f32) * inv).astype(f32)
+        return np.clip(np.floor(t), 0, res - 1).astype(np.int64)
+    return lo, cell, inv, res, cell_of
+
+
+def knn_long_line(n_pairs=120, y_c=0.1985, seed=0):
+    """A line cloud along x at the largest grid the radius clamp allows for r = 0.2 (cell 0.2f, 2095001 cells along x,
+    gmin = -1234.567f), holding `n_pairs` triples (A, B, C) that knn_cell_model puts in the worst place for the ring
+    bound: B lies two cells right of A (computed) although |AB| < 0.977 cell, and C = (A_x, y_c, 0) sits in A's cell
+    with |AB| < |AC| < 0.999 cell.  A search that trusts the computed cells to 1e-3 stops after ring 1 with C as A's
+    nearest other point and misses B.  -> (points (P,3) f32, rows of A (n_pairs,), rows of B, rows of C)"""
+    f32 = np.float32
+    gmin, span, r = f32(-1234.567), f32(419000.0), f32(0.2)
+    reach2 = f32(f32(f32(f32(1) - f32(1e-3)) * r) ** 2)
+    dC = f32(f32(y_c) * f32(y_c))
+    ends = np.array([[gmin, 0, 0], [f32(gmin + span), 0, 0]], f32)
+    *_, cell_of = knn_cell_model(np.concatenate([ends, [[0, f32(y_c), 0]]]), float(r))
+    assert dC < reach2
+    rng = np.random.default_rng(seed)
+    pairs = []
+    # windows of consecutive floats at several magnitudes (float spacing 2^-7 .. 2^-5 along x); within a window the
+    # chosen pairs lie more than 2 apart, so no two triples are within r of each other
+    for x0 in (20000.0, 70000.0, 130000.0, 200000.0, 300000.0, 380000.0):
+        i0 = int(np.float32(x0).view(np.int32))
+        xi = np.arange(i0, i0 + 40000, dtype=np.int32).view(f32)
+        c = cell_of(np.stack([xi, np.zeros_like(xi), np.zeros_like(xi)], 1))[:, 0]
+        cand = {}
+        for k in range(1, 60):
+            d = (xi[k:] - xi[:-k]).astype(f32)
+            for i in np.nonzero((c[k:] - c[:-k] == 2) & ((d * d).astype(f32) < dC))[0]:
+                cand.setdefault(int(i), int(i + k))
+        last = -np.inf
+        for i in sorted(cand):
+            if xi[i] - last > 2.0:
+                pairs.append((xi[i], xi[cand[i]]))
+                last = xi[i]
+    pick = np.sort(rng.choice(len(pairs), min(n_pairs, len(pairs)), replace=False))
+    a = np.array([pairs[i][0] for i in pick], f32)
+    b = np.array([pairs[i][1] for i in pick], f32)
+    z = np.zeros_like(a)
+    pts = np.concatenate([ends, np.stack([a, z, z], 1), np.stack([b, z, z], 1), np.stack([a, np.full_like(a, y_c), z], 1)])
+    perm = rng.permutation(len(pts))
+    pts = np.ascontiguousarray(pts[perm])
+    rank = np.empty_like(perm)
+    rank[perm] = np.arange(len(perm))
+    m = len(a)
+    return pts, rank[2:2 + m], rank[2 + m:2 + 2 * m], rank[2 + 2 * m:]
+
+
 def pix_ndc(i, S):
     """fp32 NDC centre of pixel index i (NDC-index orientation), as pix_to_ndc computes it: -1 + (2i + 1) / S"""
     return np.float32(-1) + np.float32(2 * np.asarray(i) + 1) / np.float32(S)
