@@ -7,56 +7,25 @@
 
 namespace dss {
 
-struct ShadeArgs {
-    const float *albedo, *lights, *ambient, *cam;
-    int n_lights, light_type;
-    int per_view;   // lights (N,L,9) and ambient (N,3): one block of rows per view
-    float shininess;
-};
-
-// the shading inputs of dss_render_args
-static ShadeArgs shade_args(const dss_render_args *g) {
-    ShadeArgs s;
-    s.albedo = g->albedo;
-    s.lights = g->lights;
-    s.ambient = g->ambient;
-    s.cam = g->cam_centres;
-    s.n_lights = g->n_lights;
-    s.light_type = g->light_type;
-    s.per_view = g->lights_per_view;
-    s.shininess = g->shininess;
-    return s;
-}
+// Every kernel of this file takes the call's dss_render_args as it is (`g`, a __grid_constant__ parameter), plus only
+// what the call does not hold: context scratch and, for the chain, what the host decided from the call.
 
 // light rows and ambient of view n
-__device__ __forceinline__ const float *view_lights(const ShadeArgs &s, int n) {
-    return s.per_view ? s.lights + (int64_t)n * s.n_lights * 9 : s.lights;
+__device__ __forceinline__ const float *view_lights(const dss_render_args &g, int n) {
+    return g.lights_per_view ? g.lights + (int64_t)n * g.n_lights * 9 : g.lights;
 }
-__device__ __forceinline__ const float *view_ambient(const ShadeArgs &s, int n) {
-    return s.per_view ? s.ambient + (int64_t)n * 3 : s.ambient;
+__device__ __forceinline__ const float *view_ambient(const dss_render_args &g, int n) {
+    return g.lights_per_view ? g.ambient + (int64_t)n * 3 : g.ambient;
 }
 // stages view n's shading rows into sL[DSS_MAX_LIGHTS * 9 + 6]: lights, then ambient (3) and camera centre (3) at
 // DSS_MAX_LIGHTS * 9 (the caller synchronises)
-__device__ __forceinline__ void stage_view_shading(float *sL, const ShadeArgs &s, int n) {
-    if (threadIdx.x < s.n_lights * 9) sL[threadIdx.x] = view_lights(s, n)[threadIdx.x];
+__device__ __forceinline__ void stage_view_shading(float *sL, const dss_render_args &g, int n) {
+    if (threadIdx.x < g.n_lights * 9) sL[threadIdx.x] = view_lights(g, n)[threadIdx.x];
     if (threadIdx.x < 3) {
-        sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(s, n)[threadIdx.x];
-        sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = s.cam[n * 3 + threadIdx.x];
+        sL[DSS_MAX_LIGHTS * 9 + threadIdx.x] = view_ambient(g, n)[threadIdx.x];
+        sL[DSS_MAX_LIGHTS * 9 + 3 + threadIdx.x] = g.cam_centres[n * 3 + threadIdx.x];
     }
 }
-
-struct PreArgs {
-    const float *pts, *nrm, *proj, *view, *h;
-    const int64_t *first_idx, *num_points;
-    int64_t P0;
-    int shared_cloud, h_per_splat, S, backface;
-    float cutoffC, sigma, znear, zfar;
-    float4 *rec;
-    float *ndc, *ellipse, *radii, *scaler;
-    int32_t *zrange;   // (N,2) float bits: min / max view depth of the renderable splats, or null
-    ShadeArgs sh;      // sh.albedo != nullptr: write the shaded colour of every (view, point) to `shaded`
-    float *shaded;
-};
 
 // Fast reciprocal (rcp_approx, common.cuh) and square root (MUFU based, <= 2 ulp): the per-splat quantities are compared
 // with the float64 oracle at 2e-5 .. 2e-3 relative, IEEE-exact division and sqrt were a third of this kernel's instructions.
@@ -84,6 +53,7 @@ __device__ __forceinline__ float dot3(V3 a, V3 b) { return a.x * b.x + a.y * b.y
 __device__ __forceinline__ V3 add3(V3 a, V3 b) { return v3(a.x + b.x, a.y + b.y, a.z + b.z); }
 __device__ __forceinline__ V3 sub3(V3 a, V3 b) { return v3(a.x - b.x, a.y - b.y, a.z - b.z); }
 __device__ __forceinline__ V3 mul3(V3 a, float s) { return v3(a.x * s, a.y * s, a.z * s); }
+__device__ __forceinline__ void store3(float *p, V3 a) { p[0] = a.x, p[1] = a.y, p[2] = a.z; }
 // F.normalize(x, p=2, dim=-1, eps=1e-6): x / max(|x|, eps); returns the (clamped) norm through `len`
 __device__ __forceinline__ V3 normalize3(V3 a, float &len) {
     len = fmaxf(sqrtf(dot3(a, a)), 1e-6f);
@@ -179,29 +149,33 @@ __device__ __forceinline__ V3 shade_point(const float *sL, int n_lights, int lig
 // (x/t, y/t, view-space z) -- about 40 ATen launches incl. batched det/inverse in the reference.
 // Filtered points keep their slot but get z = -1, which every later stage treats as "not renderable"
 // exactly like the reference treats points behind the camera (rasterize_points.cu:87-88).
+// rec: the (P,2) records (g.records or context scratch); zrange: (N,2) float bits, min / max view depth of the
+// renderable splats, or null.  SHADE: write the shaded colour of every (view, point) to g.shaded.
 // ---------------------------------------------------------------------------------------------
 template <bool SHADE>
-__global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__ PreArgs a) {
+__global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__ dss_render_args g, float4 *rec,
+                                                         int32_t *zrange) {
     __shared__ float sM[16], sV[16];
     __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
     const int n = blockIdx.y;
     if (threadIdx.x < 16) {
-        sM[threadIdx.x] = a.proj[n * 16 + threadIdx.x];
-        sV[threadIdx.x] = a.view[n * 16 + threadIdx.x];
+        sM[threadIdx.x] = g.proj[n * 16 + threadIdx.x];
+        sV[threadIdx.x] = g.view[n * 16 + threadIdx.x];
     }
     constexpr bool shade = SHADE;
-    if (shade) stage_view_shading(sL, a.sh, n);
+    if (shade) stage_view_shading(sL, g, n);
     __syncthreads();
-    const ViewRange vr = view_range(a.shared_cloud ? nullptr : a.first_idx, a.num_points, n, a.P0);
-    const float pix = 2.0f / (float)a.S;
-    const float aa = a.sigma * pix * pix;
+    const ViewRange vr = view_range(g.shared_cloud ? nullptr : g.first_idx, g.num_points, n, g.P0);
+    const float pix = 2.0f / (float)g.image_size;
+    const float aa = g.antialiasing_sigma * pix * pix;
     int zlo = 0x7f7fffff, zhi = 0;   // depth range of this thread's renderable splats (float bits)
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < vr.count;
          i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t s = vr.first + i;                     // packed slot
-        const int64_t src = a.shared_cloud ? i : s;         // where the world-space point lives
-        const float p0 = a.pts[src * 3 + 0], p1 = a.pts[src * 3 + 1], p2 = a.pts[src * 3 + 2];
-        const float n0 = a.nrm[src * 3 + 0], n1 = a.nrm[src * 3 + 1], n2 = a.nrm[src * 3 + 2];
+        const int64_t src = g.shared_cloud ? i : s;         // where the world-space point lives
+        const float p0 = g.points_world[src * 3 + 0], p1 = g.points_world[src * 3 + 1], p2 = g.points_world[src * 3 + 2];
+        const float n0 = g.normals_world[src * 3 + 0], n1 = g.normals_world[src * 3 + 1],
+                    n2 = g.normals_world[src * 3 + 2];
         // [p 1] . M  (row-vector convention, rasterizer.py:465-476)
         const float x = fmaf(p0, sM[0], fmaf(p1, sM[4], fmaf(p2, sM[8], sM[12])));
         const float y = fmaf(p0, sM[1], fmaf(p1, sM[5], fmaf(p2, sM[9], sM[13])));
@@ -223,21 +197,21 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         const float T00 = (J0[0] * J0[0] + J0[1] * J0[1] + J0[2] * J0[2]) - nj0 * nj0;
         const float T01 = (J0[0] * J1[0] + J0[1] * J1[1] + J0[2] * J1[2]) - nj0 * nj1;
         const float T11 = (J1[0] * J1[0] + J1[1] * J1[1] + J1[2] * J1[2]) - nj1 * nj1;
-        const float hh = a.h_per_splat ? a.h[s] : a.h[n];
+        const float hh = g.h_per_splat ? g.h[s] : g.h[n];
         const float G00 = fmaf(hh, T00, aa), G01 = hh * T01, G11 = fmaf(hh, T11, aa);
         const float detG = G00 * G11 - G01 * G01;
         const float idet = rcp_approx(detG);
         const float ea = G11 * idet, eb = -2.0f * G01 * idet, ec = G00 * idet;   // rasterizer.py:543-551
         const float den = py_eps_denom(4.0f * ea * ec - eb * eb);                 // :509-519
         const float iden = rcp_approx(den);
-        const float ry = fast_sqrt(py_eps_sqrt(4.0f * ea * a.cutoffC * iden));
-        const float rx = fast_sqrt(py_eps_sqrt(4.0f * ec * a.cutoffC * iden));
+        const float ry = fast_sqrt(py_eps_sqrt(4.0f * ea * g.cutoff_threshold * iden));
+        const float rx = fast_sqrt(py_eps_sqrt(4.0f * ec * g.cutoff_threshold * iden));
         const float detT = fmaxf(T00 * T11 - T01 * T01, 0.0f);
         const float sc = fast_sqrt(detT) *
                          rcp_approx(py_eps_denom(fast_sqrt(py_eps_sqrt(detG * (4.0f * CUDART_PI_F * CUDART_PI_F)))));  // :558-559
         // filters (rasterizer.py:187-192, :152): view-space depth range, optional backface
-        bool keep = (zv >= a.znear) && (zv <= a.zfar);
-        if (a.backface) {
+        bool keep = (zv >= g.znear) && (zv <= g.zfar);
+        if (g.backface_culling) {
             const float nz = n0 * sV[2] + n1 * sV[6] + n2 * sV[10];
             keep = keep && (nz < 0.0f);
         }
@@ -249,36 +223,36 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         }
         const float irt = rcp_approx(t);
         const float xn = x * irt, yn = y * irt;
-        a.rec[2 * s] = make_float4(xn, yn, zv, rx);
-        a.rec[2 * s + 1] = make_float4(ry, ea, eb, ec);
-        if (a.scaler) a.scaler[s] = sc;
-        if (a.ndc) {
-            a.ndc[s * 3 + 0] = xn;
-            a.ndc[s * 3 + 1] = yn;
-            a.ndc[s * 3 + 2] = zv;
+        rec[2 * s] = make_float4(xn, yn, zv, rx);
+        rec[2 * s + 1] = make_float4(ry, ea, eb, ec);
+        if (g.scaler) g.scaler[s] = sc;
+        if (g.ndc) {
+            g.ndc[s * 3 + 0] = xn;
+            g.ndc[s * 3 + 1] = yn;
+            g.ndc[s * 3 + 2] = zv;
         }
-        if (a.ellipse) {
-            a.ellipse[s * 3 + 0] = ea;
-            a.ellipse[s * 3 + 1] = eb;
-            a.ellipse[s * 3 + 2] = ec;
+        if (g.ellipse) {
+            g.ellipse[s * 3 + 0] = ea;
+            g.ellipse[s * 3 + 1] = eb;
+            g.ellipse[s * 3 + 2] = ec;
         }
-        if (a.radii) {
-            a.radii[s * 2 + 0] = rx;
-            a.radii[s * 2 + 1] = ry;
+        if (g.radii) {
+            g.radii[s * 2 + 0] = rx;
+            g.radii[s * 2 + 1] = ry;
         }
         if (shade) {
             V3 ga, gn, gp;
             const float *amb = sL + DSS_MAX_LIGHTS * 9;
-            const V3 c = shade_point<false>(sL, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(amb[0], amb[1], amb[2]),
+            const V3 c = shade_point<false>(sL, g.n_lights, g.light_type, g.shininess, v3(amb[0], amb[1], amb[2]),
                                             v3(p0, p1, p2), v3(n0, n1, n2),
-                                            v3(a.sh.albedo[src * 3], a.sh.albedo[src * 3 + 1], a.sh.albedo[src * 3 + 2]),
+                                            v3(g.albedo[src * 3], g.albedo[src * 3 + 1], g.albedo[src * 3 + 2]),
                                             v3(amb[3], amb[4], amb[5]), v3(0.f, 0.f, 0.f), ga, gn, gp);
-            a.shaded[s * 3 + 0] = c.x;
-            a.shaded[s * 3 + 1] = c.y;
-            a.shaded[s * 3 + 2] = c.z;
+            g.shaded[s * 3 + 0] = c.x;
+            g.shaded[s * 3 + 1] = c.y;
+            g.shaded[s * 3 + 2] = c.z;
         }
     }
-    if (a.zrange) {   // one pair of atomics per block
+    if (zrange) {   // one pair of atomics per block
         __shared__ int s_lo[8], s_hi[8];
         zlo = __reduce_min_sync(0xffffffffu, zlo);
         zhi = __reduce_max_sync(0xffffffffu, zhi);
@@ -292,8 +266,8 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
                 zlo = min(zlo, s_lo[w]);
                 zhi = max(zhi, s_hi[w]);
             }
-            atomicMin(&a.zrange[2 * n], zlo);
-            atomicMax(&a.zrange[2 * n + 1], zhi);
+            atomicMin(&zrange[2 * n], zlo);
+            atomicMax(&zrange[2 * n + 1], zhi);
         }
     }
 }
@@ -301,67 +275,57 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
 // d L / d shaded (N*P0,3) -> d albedo, d normal, d position (through the shading) per world point, summed over the views:
 // one thread per point loops over the views (deterministic, no atomics) and re-evaluates the lighting of the
 // (view, point) pairs that received a colour gradient (the visible ones, ~18 %).
-struct ShadeBwdArgs {
-    const float *pts, *nrm, *gsh;
-    ShadeArgs sh;
-    int64_t P0;
-    int N;
-    float *g_alb, *g_nrm, *g_pos;
-};
-
-__global__ void __launch_bounds__(256) shade_backward_kernel(const __grid_constant__ ShadeBwdArgs a) {
+__global__ void __launch_bounds__(256) shade_backward_kernel(const __grid_constant__ dss_render_args g) {
     // lights (L*9) and ambient (3), once or (per_view) for every view, then the camera centres (N*3)
     extern __shared__ float sS[];
-    const int nl9 = a.sh.n_lights * 9, stride = nl9 + 3, rows = a.sh.per_view ? a.N : 1;
-    for (int i = threadIdx.x; i < rows * nl9; i += blockDim.x) sS[(i / nl9) * stride + i % nl9] = a.sh.lights[i];
-    for (int i = threadIdx.x; i < rows * 3; i += blockDim.x) sS[(i / 3) * stride + nl9 + i % 3] = a.sh.ambient[i];
+    const int nl9 = g.n_lights * 9, stride = nl9 + 3, rows = g.lights_per_view ? g.n_views : 1;
+    for (int i = threadIdx.x; i < rows * nl9; i += blockDim.x) sS[(i / nl9) * stride + i % nl9] = g.lights[i];
+    for (int i = threadIdx.x; i < rows * 3; i += blockDim.x) sS[(i / 3) * stride + nl9 + i % 3] = g.ambient[i];
     float *sC = sS + rows * stride;
-    for (int i = threadIdx.x; i < a.N * 3; i += blockDim.x) sC[i] = a.sh.cam[i];
+    for (int i = threadIdx.x; i < g.n_views * 3; i += blockDim.x) sC[i] = g.cam_centres[i];
     __syncthreads();
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.P0; i += (int64_t)gridDim.x * blockDim.x) {
-        const V3 p = v3(a.pts[i * 3], a.pts[i * 3 + 1], a.pts[i * 3 + 2]);
-        const V3 nrm = v3(a.nrm[i * 3], a.nrm[i * 3 + 1], a.nrm[i * 3 + 2]);
-        const V3 alb = v3(a.sh.albedo[i * 3], a.sh.albedo[i * 3 + 1], a.sh.albedo[i * 3 + 2]);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < g.P0; i += (int64_t)gridDim.x * blockDim.x) {
+        const V3 p = v3(g.points_world[i * 3], g.points_world[i * 3 + 1], g.points_world[i * 3 + 2]);
+        const V3 nrm = v3(g.normals_world[i * 3], g.normals_world[i * 3 + 1], g.normals_world[i * 3 + 2]);
+        const V3 alb = v3(g.albedo[i * 3], g.albedo[i * 3 + 1], g.albedo[i * 3 + 2]);
         V3 ga = v3(0.f, 0.f, 0.f), gn = v3(0.f, 0.f, 0.f), gp = v3(0.f, 0.f, 0.f);
-        for (int n = 0; n < a.N; ++n) {
-            const float *g = a.gsh + ((int64_t)n * a.P0 + i) * 3;
-            const V3 gc = v3(g[0], g[1], g[2]);
+        for (int n = 0; n < g.n_views; ++n) {
+            const float *gs = g.grad_colours + ((int64_t)n * g.P0 + i) * 3;
+            const V3 gc = v3(gs[0], gs[1], gs[2]);
             if (gc.x == 0.0f && gc.y == 0.0f && gc.z == 0.0f) continue;
-            const float *c = sC + n * 3, *L = sS + (a.sh.per_view ? n * stride : 0);
-            shade_point<true>(L, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(L[nl9], L[nl9 + 1], L[nl9 + 2]), p, nrm,
-                              alb, v3(c[0], c[1], c[2]), gc, ga, gn, gp);
+            const float *c = sC + n * 3, *L = sS + (g.lights_per_view ? n * stride : 0);
+            shade_point<true>(L, g.n_lights, g.light_type, g.shininess, v3(L[nl9], L[nl9 + 1], L[nl9 + 2]), p, nrm, alb,
+                              v3(c[0], c[1], c[2]), gc, ga, gn, gp);
         }
-        a.g_alb[i * 3] = ga.x, a.g_alb[i * 3 + 1] = ga.y, a.g_alb[i * 3 + 2] = ga.z;
-        a.g_nrm[i * 3] = gn.x, a.g_nrm[i * 3 + 1] = gn.y, a.g_nrm[i * 3 + 2] = gn.z;
-        a.g_pos[i * 3] = gp.x, a.g_pos[i * 3 + 1] = gp.y, a.g_pos[i * 3 + 2] = gp.z;
+        store3(g.grad_albedo + i * 3, ga);
+        store3(g.grad_normals_world + i * 3, gn);
+        store3(g.grad_points_shading + i * 3, gp);
     }
 }
 
 // Packed clouds: every packed row is its own (view, point), so d albedo / d normal / d position are per row.  Grid
 // (point blocks, views), one thread per row of view n's range (as the packed branch of chain_kernel); each row is
 // written once, by its view (deterministic, no atomics).  Rows outside every range are left to the caller.
-__global__ void __launch_bounds__(256) shade_backward_packed_kernel(const __grid_constant__ ShadeBwdArgs a,
-                                                                    const int64_t *first_idx,
-                                                                    const int64_t *num_points) {
+__global__ void __launch_bounds__(256) shade_backward_packed_kernel(const __grid_constant__ dss_render_args g) {
     __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
     const int n = blockIdx.y;
-    stage_view_shading(sL, a.sh, n);
+    stage_view_shading(sL, g, n);
     __syncthreads();
     const float *amb = sL + DSS_MAX_LIGHTS * 9;
-    const ViewRange vr = view_range(first_idx, num_points, n, a.P0);
+    const ViewRange vr = view_range(g.first_idx, g.num_points, n, g.P0);
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < vr.count; i += (int64_t)gridDim.x * blockDim.x) {
         const int64_t s = vr.first + i;
-        const V3 gc = v3(a.gsh[s * 3], a.gsh[s * 3 + 1], a.gsh[s * 3 + 2]);
+        const V3 gc = v3(g.grad_colours[s * 3], g.grad_colours[s * 3 + 1], g.grad_colours[s * 3 + 2]);
         V3 ga = v3(0.f, 0.f, 0.f), gn = v3(0.f, 0.f, 0.f), gp = v3(0.f, 0.f, 0.f);
         if (gc.x != 0.0f || gc.y != 0.0f || gc.z != 0.0f)
-            shade_point<true>(sL, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(amb[0], amb[1], amb[2]),
-                              v3(a.pts[s * 3], a.pts[s * 3 + 1], a.pts[s * 3 + 2]),
-                              v3(a.nrm[s * 3], a.nrm[s * 3 + 1], a.nrm[s * 3 + 2]),
-                              v3(a.sh.albedo[s * 3], a.sh.albedo[s * 3 + 1], a.sh.albedo[s * 3 + 2]),
+            shade_point<true>(sL, g.n_lights, g.light_type, g.shininess, v3(amb[0], amb[1], amb[2]),
+                              v3(g.points_world[s * 3], g.points_world[s * 3 + 1], g.points_world[s * 3 + 2]),
+                              v3(g.normals_world[s * 3], g.normals_world[s * 3 + 1], g.normals_world[s * 3 + 2]),
+                              v3(g.albedo[s * 3], g.albedo[s * 3 + 1], g.albedo[s * 3 + 2]),
                               v3(amb[3], amb[4], amb[5]), gc, ga, gn, gp);
-        a.g_alb[s * 3] = ga.x, a.g_alb[s * 3 + 1] = ga.y, a.g_alb[s * 3 + 2] = ga.z;
-        a.g_nrm[s * 3] = gn.x, a.g_nrm[s * 3 + 1] = gn.y, a.g_nrm[s * 3 + 2] = gn.z;
-        a.g_pos[s * 3] = gp.x, a.g_pos[s * 3 + 1] = gp.y, a.g_pos[s * 3 + 2] = gp.z;
+        store3(g.grad_albedo + s * 3, ga);
+        store3(g.grad_normals_world + s * 3, gn);
+        store3(g.grad_points_shading + s * 3, gp);
     }
 }
 
@@ -403,20 +367,9 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     // shading backward: d shaded (P,3) -> d albedo, d normal, d position, per world point (shared cloud) or packed row
     DSS_REQUIRE(g->grad_albedo && g->grad_normals_world && g->grad_points_shading && g->points_world,
                 "shading backward needs grad_albedo, grad_normals_world, grad_points_shading");
-    ShadeBwdArgs b;
-    b.pts = g->points_world;
-    b.nrm = g->normals_world;
-    b.gsh = g->grad_colours;
-    b.sh = shade_args(g);
-    b.P0 = g->P0;
-    b.N = N;
-    b.g_alb = g->grad_albedo;
-    b.g_nrm = g->grad_normals_world;
-    b.g_pos = g->grad_points_shading;
     if (!g->shared_cloud) {
         StageScope prof(ctx, ST_COLOUR_BWD, on);
-        shade_backward_packed_kernel<<<dim3(grid_blocks(g->P0, 256, ctx->sm_count, 8), N), 256, 0, on>>>(
-            b, g->first_idx, g->num_points);
+        shade_backward_packed_kernel<<<dim3(grid_blocks(g->P0, 256, ctx->sm_count, 8), N), 256, 0, on>>>(*g);
         DSS_LAUNCH_CHECK(ctx);
         return DSS_OK;
     }
@@ -425,7 +378,7 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     if (smem > 48 * 1024)
         DSS_CUDA_TRY(cudaFuncSetAttribute(shade_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     StageScope prof(ctx, ST_COLOUR_BWD, on);
-    shade_backward_kernel<<<grid_blocks(g->P0, 256, ctx->sm_count, 8), 256, smem, on>>>(b);
+    shade_backward_kernel<<<grid_blocks(g->P0, 256, ctx->sm_count, 8), 256, smem, on>>>(*g);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
@@ -458,39 +411,11 @@ static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, c
     }
     if (g->P == 0 || g->P0 == 0) return DSS_OK;
     DSS_REQUIRE(g->points_world && g->normals_world && g->proj && g->view && g->h, "null input array");
-    PreArgs a;
-    a.pts = g->points_world;
-    a.nrm = g->normals_world;
-    a.proj = g->proj;
-    a.view = g->view;
-    a.h = g->h;
-    a.first_idx = g->first_idx;
-    a.num_points = g->num_points;
-    a.P0 = g->P0;
-    a.shared_cloud = g->shared_cloud;
-    a.h_per_splat = g->h_per_splat;
-    a.S = g->image_size;
-    a.backface = g->backface_culling;
-    a.cutoffC = g->cutoff_threshold;
-    a.sigma = g->antialiasing_sigma;
-    a.znear = g->znear;
-    a.zfar = g->zfar;
-    a.rec = rec;
-    a.ndc = g->ndc;
-    a.ellipse = g->ellipse;
-    a.radii = g->radii;
-    a.scaler = g->scaler;
-    a.zrange = reinterpret_cast<int32_t *>(zrange);
-    memset(&a.sh, 0, sizeof(a.sh));
-    a.shaded = nullptr;
-    if (g->shade && g->shaded) {
-        a.sh = shade_args(g);
-        a.shaded = g->shaded;
-    }
+    int32_t *zr = reinterpret_cast<int32_t *>(zrange);
     dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 8), g->n_views);
     StageScope prof(ctx, ST_PREPROCESS, st);
-    if (a.shaded) preprocess_kernel<true><<<grid, 256, 0, st>>>(a);
-    else preprocess_kernel<false><<<grid, 256, 0, st>>>(a);
+    if (g->shade && g->shaded) preprocess_kernel<true><<<grid, 256, 0, st>>>(*g, rec, zr);
+    else preprocess_kernel<false><<<grid, 256, 0, st>>>(*g, rec, zr);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
@@ -500,19 +425,10 @@ static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, c
 // ndc = (X/T, Y/T, z_view) to world space: d ndc_xy / d p = J (the same Jacobian as the forward
 // pass), d z_view / d p = V[:3, 2].  shared_cloud: one thread per world point loops over the views
 // and writes the sum (deterministic, no atomics); otherwise one thread per packed splat.
+//   grad_xy:    (P,2) occupancy gradient
+//   grad_z:     (P,) z gradient or null
+//   grad_shade: position gradient through the shading, shaped like grad_points_world and added to it, or null
 // ---------------------------------------------------------------------------------------------
-struct ChainArgs {
-    const float *gshade;   // position gradient through the shading, (P0,3) or (P,3) like grad_world, added to it, or null
-    const float *pts, *proj, *view;
-    const float2 *gxy;     // (P,2) occupancy gradient
-    const float *gz;       // (P,) z gradient or null
-    const int64_t *first_idx, *num_points;
-    int64_t P0;
-    int N, shared_cloud;
-    float clip;
-    float *grad_ndc;       // (P,3) or null
-    float *grad_world;     // (P0,3) or (P,3)
-};
 
 __device__ __forceinline__ void chain_one(const float *M, const float *V, float p0, float p1, float p2,
                                           float gx, float gy, float gz, float &w0, float &w1, float &w2) {
@@ -543,39 +459,40 @@ __device__ __forceinline__ void clip_grad(float clip, float &gx, float &gy, floa
     }
 }
 
-__global__ void __launch_bounds__(256) chain_kernel(const __grid_constant__ ChainArgs a) {
+__global__ void __launch_bounds__(256) chain_kernel(const __grid_constant__ dss_render_args g, const float2 *grad_xy,
+                                                    const float *grad_z, const float *grad_shade) {
     extern __shared__ float sMat[];  // N * 32 floats: proj then view per view (shared_cloud) or 32 (packed)
-    if (a.shared_cloud) {
-        for (int i = threadIdx.x; i < a.N * 16; i += blockDim.x) {
-            sMat[(i / 16) * 32 + (i % 16)] = a.proj[i];
-            sMat[(i / 16) * 32 + 16 + (i % 16)] = a.view[i];
+    if (g.shared_cloud) {
+        for (int i = threadIdx.x; i < g.n_views * 16; i += blockDim.x) {
+            sMat[(i / 16) * 32 + (i % 16)] = g.proj[i];
+            sMat[(i / 16) * 32 + 16 + (i % 16)] = g.view[i];
         }
         __syncthreads();
-        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.P0;
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < g.P0;
              i += (int64_t)gridDim.x * blockDim.x) {
-            const float p0 = a.pts[i * 3], p1 = a.pts[i * 3 + 1], p2 = a.pts[i * 3 + 2];
+            const float p0 = g.points_world[i * 3], p1 = g.points_world[i * 3 + 1], p2 = g.points_world[i * 3 + 2];
             float acc0 = 0.f, acc1 = 0.f, acc2 = 0.f;
             // views in batches of four: the (independent) gradient loads of a batch are issued together
-            for (int n0 = 0; n0 < a.N; n0 += 4) {
+            for (int n0 = 0; n0 < g.n_views; n0 += 4) {
                 float2 g4[4];
                 float gz4[4];
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
-                    const int64_t s = (int64_t)(n0 + j) * a.P0 + i;
-                    g4[j] = (n0 + j < a.N) ? a.gxy[s] : make_float2(0.f, 0.f);
-                    gz4[j] = (a.gz && n0 + j < a.N) ? a.gz[s] : 0.0f;
+                    const int64_t s = (int64_t)(n0 + j) * g.P0 + i;
+                    g4[j] = (n0 + j < g.n_views) ? grad_xy[s] : make_float2(0.f, 0.f);
+                    gz4[j] = (grad_z && n0 + j < g.n_views) ? grad_z[s] : 0.0f;
                 }
 #pragma unroll
                 for (int j = 0; j < 4; ++j) {
                     const int n = n0 + j;
-                    if (n >= a.N) break;
-                    const int64_t s = (int64_t)n * a.P0 + i;
+                    if (n >= g.n_views) break;
+                    const int64_t s = (int64_t)n * g.P0 + i;
                     float gx = g4[j].x, gy = g4[j].y, gz = gz4[j];
-                    clip_grad(a.clip, gx, gy, gz);
-                    if (a.grad_ndc) {
-                        a.grad_ndc[s * 3 + 0] = gx;
-                        a.grad_ndc[s * 3 + 1] = gy;
-                        a.grad_ndc[s * 3 + 2] = gz;
+                    clip_grad(g.clip_pts_grad, gx, gy, gz);
+                    if (g.grad_ndc) {
+                        g.grad_ndc[s * 3 + 0] = gx;
+                        g.grad_ndc[s * 3 + 1] = gy;
+                        g.grad_ndc[s * 3 + 2] = gz;
                     }
                     if (gx != 0.0f || gy != 0.0f || gz != 0.0f) {
                         float w0, w1, w2;
@@ -586,45 +503,46 @@ __global__ void __launch_bounds__(256) chain_kernel(const __grid_constant__ Chai
                     }
                 }
             }
-            if (a.gshade) {
-                acc0 += a.gshade[i * 3 + 0];
-                acc1 += a.gshade[i * 3 + 1];
-                acc2 += a.gshade[i * 3 + 2];
+            if (grad_shade) {
+                acc0 += grad_shade[i * 3 + 0];
+                acc1 += grad_shade[i * 3 + 1];
+                acc2 += grad_shade[i * 3 + 2];
             }
-            a.grad_world[i * 3 + 0] = acc0;
-            a.grad_world[i * 3 + 1] = acc1;
-            a.grad_world[i * 3 + 2] = acc2;
+            g.grad_points_world[i * 3 + 0] = acc0;
+            g.grad_points_world[i * 3 + 1] = acc1;
+            g.grad_points_world[i * 3 + 2] = acc2;
         }
     } else {
         const int n = blockIdx.y;
         if (threadIdx.x < 16) {
-            sMat[threadIdx.x] = a.proj[n * 16 + threadIdx.x];
-            sMat[16 + threadIdx.x] = a.view[n * 16 + threadIdx.x];
+            sMat[threadIdx.x] = g.proj[n * 16 + threadIdx.x];
+            sMat[16 + threadIdx.x] = g.view[n * 16 + threadIdx.x];
         }
         __syncthreads();
-        const ViewRange vr = view_range(a.first_idx, a.num_points, n, a.P0);
+        const ViewRange vr = view_range(g.first_idx, g.num_points, n, g.P0);
         for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < vr.count;
              i += (int64_t)gridDim.x * blockDim.x) {
             const int64_t s = vr.first + i;
-            const float2 g = a.gxy[s];
-            float gx = g.x, gy = g.y, gz = a.gz ? a.gz[s] : 0.0f;
-            clip_grad(a.clip, gx, gy, gz);
-            if (a.grad_ndc) {
-                a.grad_ndc[s * 3 + 0] = gx;
-                a.grad_ndc[s * 3 + 1] = gy;
-                a.grad_ndc[s * 3 + 2] = gz;
+            const float2 gxy = grad_xy[s];
+            float gx = gxy.x, gy = gxy.y, gz = grad_z ? grad_z[s] : 0.0f;
+            clip_grad(g.clip_pts_grad, gx, gy, gz);
+            if (g.grad_ndc) {
+                g.grad_ndc[s * 3 + 0] = gx;
+                g.grad_ndc[s * 3 + 1] = gy;
+                g.grad_ndc[s * 3 + 2] = gz;
             }
             float w0 = 0.f, w1 = 0.f, w2 = 0.f;
             if (gx != 0.0f || gy != 0.0f || gz != 0.0f)
-                chain_one(sMat, sMat + 16, a.pts[s * 3], a.pts[s * 3 + 1], a.pts[s * 3 + 2], gx, gy, gz, w0, w1, w2);
-            if (a.gshade) {
-                w0 += a.gshade[s * 3 + 0];
-                w1 += a.gshade[s * 3 + 1];
-                w2 += a.gshade[s * 3 + 2];
+                chain_one(sMat, sMat + 16, g.points_world[s * 3], g.points_world[s * 3 + 1], g.points_world[s * 3 + 2],
+                          gx, gy, gz, w0, w1, w2);
+            if (grad_shade) {
+                w0 += grad_shade[s * 3 + 0];
+                w1 += grad_shade[s * 3 + 1];
+                w2 += grad_shade[s * 3 + 2];
             }
-            a.grad_world[s * 3 + 0] = w0;
-            a.grad_world[s * 3 + 1] = w1;
-            a.grad_world[s * 3 + 2] = w2;
+            g.grad_points_world[s * 3 + 0] = w0;
+            g.grad_points_world[s * 3 + 1] = w1;
+            g.grad_points_world[s * 3 + 2] = w2;
         }
     }
 }
@@ -642,51 +560,44 @@ __global__ void __launch_bounds__(256) chain_kernel(const __grid_constant__ Chai
 // ---------------------------------------------------------------------------------------------
 constexpr int CAM_SUMS = 19;   // 12 proj (rows 0..3 x columns 0, 1, 3), 4 view (rows 0..3, column 2), 3 camera centre
 
-struct CamArgs {
-    const float *pts, *proj, *gndc;
-    const int64_t *first_idx, *num_points;
-    int64_t P0;
-    int shared_cloud;
-    const float *nrm, *gsh;   // shading only: normals and d L / d shaded (P,3)
-    ShadeArgs sh;
-    double *partials;         // (N, gridDim.x, CAM_SUMS)
-};
-
 constexpr int CAM_BATCH = 4;   // slots per thread whose loads are issued together
 
+// partials: (N, gridDim.x, CAM_SUMS).  SHADE: also the camera-centre sums, from d L / d shaded in g.grad_colours.
 template <bool SHADE>
-__global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_constant__ CamArgs a) {
+__global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_constant__ dss_render_args g,
+                                                              double *partials) {
     __shared__ float sM[16];
     __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
     __shared__ double sPart[8][CAM_SUMS];
     const int n = blockIdx.y;
-    if (threadIdx.x < 16) sM[threadIdx.x] = a.proj[n * 16 + threadIdx.x];
-    if (SHADE) stage_view_shading(sL, a.sh, n);
+    if (threadIdx.x < 16) sM[threadIdx.x] = g.proj[n * 16 + threadIdx.x];
+    if (SHADE) stage_view_shading(sL, g, n);
     __syncthreads();
     double acc[CAM_SUMS];
 #pragma unroll
     for (int k = 0; k < CAM_SUMS; ++k) acc[k] = 0.0;
-    const ViewRange vr = view_range(a.shared_cloud ? nullptr : a.first_idx, a.num_points, n, a.P0);
+    const ViewRange vr = view_range(g.shared_cloud ? nullptr : g.first_idx, g.num_points, n, g.P0);
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < vr.count; i0 += CAM_BATCH * stride) {
-        float g[CAM_BATCH][3], gs[CAM_BATCH][3];
+        float gd[CAM_BATCH][3], gs[CAM_BATCH][3];
 #pragma unroll
         for (int j = 0; j < CAM_BATCH; ++j) {
             const int64_t i = i0 + j * stride, s = vr.first + i;
             const bool in = i < vr.count;
 #pragma unroll
             for (int e = 0; e < 3; ++e) {
-                g[j][e] = in ? a.gndc[s * 3 + e] : 0.0f;
-                gs[j][e] = (SHADE && in) ? a.gsh[s * 3 + e] : 0.0f;
+                gd[j][e] = in ? g.grad_ndc[s * 3 + e] : 0.0f;
+                gs[j][e] = (SHADE && in) ? g.grad_colours[s * 3 + e] : 0.0f;
             }
         }
 #pragma unroll
         for (int j = 0; j < CAM_BATCH; ++j) {
             const int64_t i = i0 + j * stride, s = vr.first + i;
-            const int64_t src = a.shared_cloud ? i : s;
-            const float gx = g[j][0], gy = g[j][1], gz = g[j][2];
+            const int64_t src = g.shared_cloud ? i : s;
+            const float gx = gd[j][0], gy = gd[j][1], gz = gd[j][2];
             if (gx != 0.0f || gy != 0.0f || gz != 0.0f) {
-                const float ph[4] = {a.pts[src * 3], a.pts[src * 3 + 1], a.pts[src * 3 + 2], 1.0f};
+                const float ph[4] = {g.points_world[src * 3], g.points_world[src * 3 + 1], g.points_world[src * 3 + 2],
+                                     1.0f};
                 const float x = fmaf(ph[0], sM[0], fmaf(ph[1], sM[4], fmaf(ph[2], sM[8], sM[12])));
                 const float y = fmaf(ph[0], sM[1], fmaf(ph[1], sM[5], fmaf(ph[2], sM[9], sM[13])));
                 const float t = fmaf(ph[0], sM[3], fmaf(ph[1], sM[7], fmaf(ph[2], sM[11], sM[15])));
@@ -705,11 +616,12 @@ __global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_const
             if (SHADE && (gc.x != 0.0f || gc.y != 0.0f || gc.z != 0.0f)) {
                 const float *amb = sL + DSS_MAX_LIGHTS * 9;
                 V3 ga = v3(0.f, 0.f, 0.f), gn = v3(0.f, 0.f, 0.f), gp = v3(0.f, 0.f, 0.f), gcam = v3(0.f, 0.f, 0.f);
-                shade_point<true, true>(sL, a.sh.n_lights, a.sh.light_type, a.sh.shininess, v3(amb[0], amb[1], amb[2]),
-                                        v3(a.pts[src * 3], a.pts[src * 3 + 1], a.pts[src * 3 + 2]),
-                                        v3(a.nrm[src * 3], a.nrm[src * 3 + 1], a.nrm[src * 3 + 2]),
-                                        v3(a.sh.albedo[src * 3], a.sh.albedo[src * 3 + 1], a.sh.albedo[src * 3 + 2]),
-                                        v3(amb[3], amb[4], amb[5]), gc, ga, gn, gp, &gcam);
+                shade_point<true, true>(
+                    sL, g.n_lights, g.light_type, g.shininess, v3(amb[0], amb[1], amb[2]),
+                    v3(g.points_world[src * 3], g.points_world[src * 3 + 1], g.points_world[src * 3 + 2]),
+                    v3(g.normals_world[src * 3], g.normals_world[src * 3 + 1], g.normals_world[src * 3 + 2]),
+                    v3(g.albedo[src * 3], g.albedo[src * 3 + 1], g.albedo[src * 3 + 2]), v3(amb[3], amb[4], amb[5]), gc,
+                    ga, gn, gp, &gcam);
                 acc[16] += (double)gcam.x;
                 acc[17] += (double)gcam.y;
                 acc[18] += (double)gcam.z;
@@ -717,7 +629,7 @@ __global__ void __launch_bounds__(256) camera_partials_kernel(const __grid_const
         }
     }
     const double v = block_sum(acc, sPart);
-    if (threadIdx.x < CAM_SUMS) a.partials[((int64_t)n * gridDim.x + blockIdx.x) * CAM_SUMS + threadIdx.x] = v;
+    if (threadIdx.x < CAM_SUMS) partials[((int64_t)n * gridDim.x + blockIdx.x) * CAM_SUMS + threadIdx.x] = v;
 }
 
 // output rows of the camera gradients: view m's (4,4) / (4,4) / (3,) rows from its CAM_SUMS totals
@@ -744,51 +656,44 @@ struct CamRows {
 // ---------------------------------------------------------------------------------------------
 constexpr int LIGHT_SUMS = 12;   // direction or location (3), diffuse rgb (3), specular rgb (3), ambient rgb (3)
 
-struct LightArgs {
-    const float *pts, *nrm, *gsh;
-    ShadeArgs sh;
-    const int64_t *first_idx, *num_points;
-    int64_t P0;
-    int shared_cloud;
-    double *partials;   // (N, gridDim.z, gridDim.x, LIGHT_SUMS)
-};
-
-__global__ void __launch_bounds__(256) light_partials_kernel(const __grid_constant__ LightArgs a) {
+// partials: (N, gridDim.z, gridDim.x, LIGHT_SUMS)
+__global__ void __launch_bounds__(256) light_partials_kernel(const __grid_constant__ dss_render_args g,
+                                                             double *partials) {
     __shared__ float sL[9 + 3];   // the light's row, camera centre
     __shared__ double sPart[8][LIGHT_SUMS];
     const int n = blockIdx.y, l = blockIdx.z;
-    if (threadIdx.x < 9) sL[threadIdx.x] = view_lights(a.sh, n)[l * 9 + threadIdx.x];
-    if (threadIdx.x < 3) sL[9 + threadIdx.x] = a.sh.cam[n * 3 + threadIdx.x];
+    if (threadIdx.x < 9) sL[threadIdx.x] = view_lights(g, n)[l * 9 + threadIdx.x];
+    if (threadIdx.x < 3) sL[9 + threadIdx.x] = g.cam_centres[n * 3 + threadIdx.x];
     __syncthreads();
     const V3 cam = v3(sL[9], sL[10], sL[11]);
     double acc[LIGHT_SUMS];
 #pragma unroll
     for (int k = 0; k < LIGHT_SUMS; ++k) acc[k] = 0.0;
     // view n's rows of d L / d shaded: n*P0 .. n*P0+P0 (shared cloud, world point i) or its packed range (row s)
-    const ViewRange vr = view_range(a.shared_cloud ? nullptr : a.first_idx, a.num_points, n, a.P0);
-    const float *gsh = a.gsh + vr.first * 3;
+    const ViewRange vr = view_range(g.shared_cloud ? nullptr : g.first_idx, g.num_points, n, g.P0);
+    const float *gsh = g.grad_colours + vr.first * 3;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t i0 = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i0 < vr.count; i0 += CAM_BATCH * stride) {
-        float g[CAM_BATCH][3];
+        float gs[CAM_BATCH][3];
 #pragma unroll
         for (int j = 0; j < CAM_BATCH; ++j) {
             const int64_t i = i0 + j * stride;
 #pragma unroll
-            for (int e = 0; e < 3; ++e) g[j][e] = i < vr.count ? gsh[i * 3 + e] : 0.0f;
+            for (int e = 0; e < 3; ++e) gs[j][e] = i < vr.count ? gsh[i * 3 + e] : 0.0f;
         }
 #pragma unroll
         for (int j = 0; j < CAM_BATCH; ++j) {
-            const V3 gc = v3(g[j][0], g[j][1], g[j][2]);
+            const V3 gc = v3(gs[j][0], gs[j][1], gs[j][2]);
             if (gc.x == 0.0f && gc.y == 0.0f && gc.z == 0.0f) continue;
-            const int64_t i = i0 + j * stride, src = a.shared_cloud ? i : vr.first + i;
-            const V3 p = v3(a.pts[src * 3], a.pts[src * 3 + 1], a.pts[src * 3 + 2]);
-            const V3 alb = v3(a.sh.albedo[src * 3], a.sh.albedo[src * 3 + 1], a.sh.albedo[src * 3 + 2]);
+            const int64_t i = i0 + j * stride, src = g.shared_cloud ? i : vr.first + i;
+            const V3 p = v3(g.points_world[src * 3], g.points_world[src * 3 + 1], g.points_world[src * 3 + 2]);
+            const V3 alb = v3(g.albedo[src * 3], g.albedo[src * 3 + 1], g.albedo[src * 3 + 2]);
             float nlen, vlen;
-            const V3 nh = normalize3(v3(a.nrm[src * 3], a.nrm[src * 3 + 1], a.nrm[src * 3 + 2]), nlen);
+            const V3 nh =
+                normalize3(v3(g.normals_world[src * 3], g.normals_world[src * 3 + 1], g.normals_world[src * 3 + 2]), nlen);
             const V3 v = normalize3(sub3(cam, p), vlen);
             V3 diff = v3(0.f, 0.f, 0.f), spec = v3(0.f, 0.f, 0.f), g_nh = v3(0.f, 0.f, 0.f), g_v = v3(0.f, 0.f, 0.f);
-            const LightTerm t = shade_light<true>(sL, a.sh.light_type, a.sh.shininess, p, nh, v, alb, gc, diff, spec, g_nh,
-                                                  g_v);
+            const LightTerm t = shade_light<true>(sL, g.light_type, g.shininess, p, nh, v, alb, gc, diff, spec, g_nh, g_v);
             const V3 gvec = normalize3_bwd(t.d, t.dlen, t.g_d);
             const V3 ga = v3(gc.x * alb.x, gc.y * alb.y, gc.z * alb.z);
             acc[0] += (double)gvec.x;
@@ -809,7 +714,7 @@ __global__ void __launch_bounds__(256) light_partials_kernel(const __grid_consta
     }
     const double v = block_sum(acc, sPart);
     if (threadIdx.x < LIGHT_SUMS)
-        a.partials[(((int64_t)n * gridDim.z + l) * gridDim.x + blockIdx.x) * LIGHT_SUMS + threadIdx.x] = v;
+        partials[(((int64_t)n * gridDim.z + l) * gridDim.x + blockIdx.x) * LIGHT_SUMS + threadIdx.x] = v;
 }
 
 // output rows of the light gradients: light l's row of output row m, and the ambient row from the l = 0 slice
@@ -940,27 +845,16 @@ int dss_render_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
         DSS_CUDA_TRY(cudaMemsetAsync(gz, 0, (size_t)P * sizeof(float), st));
         if ((rc = zbuf_backward(ctx, g->idx, g->grad_zbuf, npix, K, gz, 1, st))) return rc;
     }
-    ChainArgs c;
-    c.gshade = (g->shade && g->grad_colours != nullptr) ? g->grad_points_shading : nullptr;
-    c.pts = g->points_world;
-    c.proj = g->proj;
-    c.view = g->view;
-    c.gxy = reinterpret_cast<const float2 *>(gxy);
-    c.gz = gz;
-    c.first_idx = fi;
-    c.num_points = g->num_points;
-    c.P0 = g->P0;
-    c.N = N;
-    c.shared_cloud = g->shared_cloud;
-    c.clip = g->clip_pts_grad;
-    c.grad_ndc = g->grad_ndc;
-    c.grad_world = g->grad_points_world;
+    const float2 *grad_xy = reinterpret_cast<const float2 *>(gxy);
+    // the shading's position gradient exists only when this call ran the colour half
+    const float *grad_shade = (g->shade && g->grad_colours != nullptr) ? g->grad_points_shading : nullptr;
     StageScope prof(ctx, ST_CHAIN, st);
     if (g->shared_cloud) {
-        chain_kernel<<<grid_blocks(g->P0, 256, ctx->sm_count, 8), 256, (size_t)N * 32 * sizeof(float), st>>>(c);
+        chain_kernel<<<grid_blocks(g->P0, 256, ctx->sm_count, 8), 256, (size_t)N * 32 * sizeof(float), st>>>(
+            *g, grad_xy, gz, grad_shade);
     } else {
         dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 8), N);
-        chain_kernel<<<grid, 256, 32 * sizeof(float), st>>>(c);
+        chain_kernel<<<grid, 256, 32 * sizeof(float), st>>>(*g, grad_xy, gz, grad_shade);
     }
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
@@ -990,26 +884,13 @@ int dss_camera_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_proj
         return DSS_OK;
     }
     const unsigned int blocks = wave_blocks(ctx, N, g->P0);
-    CamArgs c;
-    memset(&c, 0, sizeof(c));
-    c.pts = g->points_world;
-    c.proj = g->proj;
-    c.gndc = g->grad_ndc;
-    c.first_idx = g->first_idx;
-    c.num_points = g->num_points;
-    c.P0 = g->P0;
-    c.shared_cloud = g->shared_cloud;
-    if (shade) {
-        c.nrm = g->normals_world;
-        c.gsh = g->grad_colours;
-        c.sh = shade_args(g);
-    }
-    if ((rc = ctx_get(ctx, BUF_CAMERA, (size_t)N * blocks * CAM_SUMS, &c.partials))) return rc;
+    double *partials = nullptr;
+    if ((rc = ctx_get(ctx, BUF_CAMERA, (size_t)N * blocks * CAM_SUMS, &partials))) return rc;
     StageScope prof(ctx, ST_CAMERA_BWD, st);
-    if (shade) camera_partials_kernel<true><<<dim3(blocks, N), 256, 0, st>>>(c);
-    else camera_partials_kernel<false><<<dim3(blocks, N), 256, 0, st>>>(c);
+    if (shade) camera_partials_kernel<true><<<dim3(blocks, N), 256, 0, st>>>(*g, partials);
+    else camera_partials_kernel<false><<<dim3(blocks, N), 256, 0, st>>>(*g, partials);
     DSS_LAUNCH_CHECK(ctx);
-    grad_finish_kernel<CAM_SUMS><<<dim3(1, N), 256, 0, st>>>(c.partials, (int)blocks, N, 1,
+    grad_finish_kernel<CAM_SUMS><<<dim3(1, N), 256, 0, st>>>(partials, (int)blocks, N, 1,
                                                              CamRows{grad_proj, grad_view, grad_cam_centres});
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
@@ -1035,20 +916,12 @@ int dss_light_backward(dss_ctx *ctx, const dss_render_args *g, float *grad_light
     // the ambient sums live in the l = 0 slice: without grad_lights that slice is all that is needed
     const int nl = grad_lights ? L : 1;
     const unsigned int blocks = wave_blocks(ctx, (int64_t)N * nl, g->P0);
-    LightArgs c;
-    c.pts = g->points_world;
-    c.nrm = g->normals_world;
-    c.gsh = g->grad_colours;
-    c.sh = shade_args(g);
-    c.first_idx = g->first_idx;
-    c.num_points = g->num_points;
-    c.P0 = g->P0;
-    c.shared_cloud = g->shared_cloud;
-    if ((rc = ctx_get(ctx, BUF_LIGHT, (size_t)N * nl * blocks * LIGHT_SUMS, &c.partials))) return rc;
+    double *partials = nullptr;
+    if ((rc = ctx_get(ctx, BUF_LIGHT, (size_t)N * nl * blocks * LIGHT_SUMS, &partials))) return rc;
     StageScope prof(ctx, ST_LIGHT_BWD, st);
-    light_partials_kernel<<<dim3(blocks, N, nl), 256, 0, st>>>(c);
+    light_partials_kernel<<<dim3(blocks, N, nl), 256, 0, st>>>(*g, partials);
     DSS_LAUNCH_CHECK(ctx);
-    grad_finish_kernel<LIGHT_SUMS><<<dim3(nl, rows), 256, 0, st>>>(c.partials, (int)blocks, N, g->lights_per_view,
+    grad_finish_kernel<LIGHT_SUMS><<<dim3(nl, rows), 256, 0, st>>>(partials, (int)blocks, N, g->lights_per_view,
                                                                     LightRows{grad_lights, grad_ambient});
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
