@@ -57,7 +57,7 @@ enum BufId {
     BUF_OCC_PLANES,   // zero-padded g-/g+ planes of the alpha gradient
     BUF_OCC_PARTS,    // work items per tile and their exclusive scan
     BUF_OCC_ITEMS,    // tile of every work item
-    BUF_OCC_COUNTS,   // per-tile counters of the occupancy binning (kept at zero between calls)
+    BUF_OCC_COUNTS,   // per-cell (pixel) counters of the occupancy binning (kept at zero between calls)
     BUF_OCC_IDS,      // packed splat id of every compact record
     BUF_TILE_ORDER,   // launch order of the forward tiles
     BUF_BIN_RECTS,    // packed tile rectangle + depth slice of every splat (count pass -> scatter pass)
@@ -109,7 +109,6 @@ struct dss_ctx {
     size_t occ_counts_elems;
     int ns_override;    // tuning (env DSS_NS): number of depth slices of the forward tile lists, 0 = automatic
     int no_tile_order;  // tuning (env DSS_NO_TILE_ORDER=1): launch the raster tiles in index order
-    int occ_tilebin;    // tuning (env DSS_OCC_TILEBIN=1): bin the backward's visible splats by tile only (unordered lists)
     int bin_no_rects;   // tuning (env DSS_BIN_NORECTS=1): the scatter pass derives the tile rectangles again
     int bin_direct;     // tuning (env DSS_BIN_DIRECT): tile binning with plain global atomics instead of per-block histograms
     double stage_ms[dss::NUM_STAGES];

@@ -290,8 +290,6 @@ int dss_create(dss_ctx **out) {
         c->sync_forward = (sf && sf[0] == '1') ? 1 : 0;
         const char *to = getenv("DSS_NO_TILE_ORDER");
         c->no_tile_order = (to && to[0] == '1') ? 1 : 0;
-        const char *tb = getenv("DSS_OCC_TILEBIN");
-        c->occ_tilebin = (tb && tb[0] == '1') ? 1 : 0;
         const char *ns = getenv("DSS_NS");
         c->ns_override = ns ? atoi(ns) : 0;
     }

@@ -15,17 +15,14 @@ constexpr int OCC_TILE = 1 << OCC_TILE_SHIFT;      // pixels per side of a backw
 constexpr int OCC_CELLS = OCC_TILE * OCC_TILE;     // cells per tile
 
 __host__ __device__ __forceinline__ int occ_tiles(int S) { return (S + OCC_TILE - 1) >> OCC_TILE_SHIFT; }
-// counters of the cell-level binning (and length of dss_render_args::cell_counts) for N views of S x S pixels
+// counters of the binning (and length of dss_render_args::cell_counts) for N views of S x S pixels
 inline int64_t occ_cell_count(int N, int S) { return (int64_t)N * occ_tiles(S) * occ_tiles(S) * OCC_CELLS; }
 
 // centre pixel of NDC coordinate p, clamped to the image
 __device__ __forceinline__ int centre_pixel(float p, int S) {
     return min(max((int)floorf((p + 1.0f) * (0.5f * (float)S)), 0), S - 1);
 }
-// view-local tile and global cell of pixel (cx, cy) of view n (cx, cy >= 0, as centre_pixel returns them)
-__device__ __forceinline__ int occ_tile_of(int cx, int cy, int OB) {
-    return (cy >> OCC_TILE_SHIFT) * OB + (cx >> OCC_TILE_SHIFT);
-}
+// global cell of pixel (cx, cy) of view n (cx, cy >= 0, as centre_pixel returns them)
 __device__ __forceinline__ int64_t occ_cell(int n, int OB, int cx, int cy) {
     return (((int64_t)n * OB + (cy >> OCC_TILE_SHIFT)) * OB + (cx >> OCC_TILE_SHIFT)) * OCC_CELLS +
            (cy & (OCC_TILE - 1)) * OCC_TILE + (cx & (OCC_TILE - 1));
@@ -136,7 +133,7 @@ int search_radius(dss_ctx *ctx, const float4 *rec, const float *radii, const uin
                   float *rs, cudaStream_t st);
 // rs is an input when radii_s < 0, otherwise rs[n] = radii_s * lower median of the visible radii is computed here
 // cell_counts (optional): per-cell counts of the visible splats produced by the forward (RasterArgs::cell_counts); when
-// given and the cell-level binning is in use, the counting pass is replaced by a copy of these counts
+// given and the staged gather runs, the counting pass is replaced by a copy of these counts
 int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float *rs, float radii_s,
                  const float *grad_occ, int pix_stride, int pix_offset, const int64_t *first_idx,
                  const int64_t *num_points, int N, int64_t P0, int S, float *grad_xy, const int32_t *cell_counts,

@@ -8,9 +8,9 @@
 //   occ_planes   alpha gradient -> two zero-padded planes per view in NDC-index orientation: g- = min(g, 0)
 //                (acts on the whole search disc) and g+ = max(g, 0) (acts inside the splat's bbox only,
 //                rasterize_points_backward.cu:161-168)
-//   occ_bin x2   visible splats -> 32x32-pixel tiles by centre (count / scan / scatter); the scatter writes
-//                COMPACT tile-ordered records {px, py, rx, ry} + ids, so everything downstream reads
-//                contiguous memory
+//   occ_bin      visible splats -> the pixel cells of 32x32-pixel tiles by centre (count / scan / scatter; the
+//                fused forward does the count); the scatter writes COMPACT records {px, py, rx, ry} + ids in
+//                tile order, pixel-ordered inside a tile, so everything downstream reads contiguous memory
 //   select x4    exact lower median of the visible radii per view (radix select) over the compact records
 //                (rasterizer.py:888) -> search radius r_n
 //   occ_tile     one CTA per (tile, chunk of its list): the (32 + 2R)^2 windows of both planes and the
@@ -32,7 +32,8 @@ constexpr int OCC_RBOX_MAX = 40;        // largest window halo the tile kernel s
 // ---------------------------------------------------------------------------------------------
 // planes: (N, 2, Hp, W) floats, plane 0 = min(g, 0) (and NaN), plane 1 = max(g, 0); element (y, x) holds NDC-index pixel
 // (yi, xi) = (y - PAD, x - PAD), i.e. image row S-1-yi, col S-1-xi (rasterize_points_backward.cu:100-104);
-// zero outside the image so that border windows need no bounds tests.
+// zero outside the image so that border windows need no bounds tests.  One block row per plane row: occ_backward
+// requires Hp <= 65535 (gridDim.y).
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 occ_planes_kernel(const float *__restrict__ grad, int pix_stride, int pix_offset, int S, int PAD, int W, int Hp,
@@ -55,66 +56,15 @@ occ_planes_kernel(const float *__restrict__ grad, int pix_stride, int pix_offset
 __device__ __forceinline__ int32_t occ_store_id(int64_t p, float z) { return z < 0.0f ? -1 : (int32_t)p; }
 
 // ---------------------------------------------------------------------------------------------
-// Bin the visible splats by the tile that contains their (clamped) centre: one entry per splat, so the
-// lists are bounded by P and no host round trip is needed.  PASS 0 counts, PASS 1 scatters compact records.
-// ---------------------------------------------------------------------------------------------
-template <int PASS>
-__global__ void __launch_bounds__(256)
-occ_bin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ visible,
-               const int64_t *__restrict__ first_idx, const int64_t *__restrict__ num_points, int64_t P0_shared,
-               int S, int OB, int32_t *__restrict__ counters, const int32_t *__restrict__ offsets,
-               float4 *__restrict__ crec, int32_t *__restrict__ cids) {
-    extern __shared__ int32_t s_hist[];
-    const int n = blockIdx.y;
-    const int nt = OB * OB;
-    const ViewRange vr = view_range(first_idx, num_points, n, P0_shared);
-    constexpr int ITEMS = 8;
-    const int64_t chunk0 = (int64_t)blockIdx.x * (256 * ITEMS);
-    if (chunk0 >= vr.count) return;
-    for (int t = threadIdx.x; t < nt; t += 256) s_hist[t] = 0;
-    __syncthreads();
-    int tile[ITEMS];
-#pragma unroll
-    for (int j = 0; j < ITEMS; ++j) {
-        tile[j] = -1;
-        const int64_t i = chunk0 + j * 256 + threadIdx.x;
-        if (i < vr.count && visible[vr.first + i]) {
-            const float4 A = __ldg(&rec[2 * (vr.first + i)]);
-            tile[j] = occ_tile_of(centre_pixel(A.x, S), centre_pixel(A.y, S), OB);
-            atomicAdd(&s_hist[tile[j]], 1);
-        }
-    }
-    __syncthreads();
-    // PASS 0 counts up; PASS 1 claims its range by counting the same counter back down to zero, so the counters are
-    // clean again for the next call (no memset, no cursor copy)
-    int32_t *cnt = counters + (int64_t)n * nt;
-    for (int t = threadIdx.x; t < nt; t += 256) {
-        const int v = s_hist[t];
-        if (v) {
-            if (PASS == 0) atomicAdd(&cnt[t], v);
-            else s_hist[t] = offsets[(int64_t)n * nt + t] + atomicSub(&cnt[t], v) - v;
-        }
-    }
-    if (PASS == 0) return;
-    __syncthreads();
-    // (the record is read again here -- an L2 hit -- rather than carried in 32 registers across the two barriers)
-#pragma unroll
-    for (int j = 0; j < ITEMS; ++j)
-        if (tile[j] >= 0) {
-            const int64_t p = vr.first + chunk0 + j * 256 + threadIdx.x;
-            const float4 A = __ldg(&rec[2 * p]);
-            const float ry = __ldg(&rec[2 * p + 1]).x;
-            const int slot = atomicAdd(&s_hist[tile[j]], 1);
-            crec[slot] = make_float4(A.x, A.y, A.w, ry);
-            cids[slot] = occ_store_id(p, A.z);
-        }
-}
-
-// Cell-level variant: the bins are the PIXELS (occ_cell, kernels.cuh), so a tile's compact list comes out ordered by pixel
-// row, then column.  Consecutive splats of a list then sit in the same or the
+// Bin the visible splats by the PIXEL that contains their (clamped) centre (occ_cell, kernels.cuh): one entry per
+// splat, so the lists are bounded by P and no host round trip is needed.  A tile's compact list comes out ordered by
+// pixel row, then column.  Consecutive splats of a list then sit in the same or the
 // next pixel -- the splats a warp of the tile kernel works on together read (nearly) the same shared-memory rows and
 // columns, which turns its 4-way bank conflicts into broadcasts.  Two million bins per 8 views do not fit a block
-// histogram: plain global atomics (1.5M visible splats over 0.5M occupied cells -- no hot spots).
+// histogram: plain global atomics (1.5M visible splats over 0.5M occupied cells -- no hot spots).  PASS 0 counts;
+// PASS 1 claims its slot by counting the same counter back down to zero, so the counters are clean again for the
+// next call, and scatters the compact records.  Slots are int32: occ_backward requires Ptot < INT32_MAX.
+// ---------------------------------------------------------------------------------------------
 template <int PASS>
 __global__ void __launch_bounds__(256)
 occ_cellbin_kernel(const float4 *__restrict__ rec, const uint8_t *__restrict__ visible,
@@ -259,16 +209,17 @@ struct SelectPacked {
     }
 };
 // The compact records {px, py, rx, ry} of the visible splats, contiguous per view:
-// [tile_offsets[n*nt], tile_offsets[(n+1)*nt]).
+// [tile_offsets[n*nc], tile_offsets[(n+1)*nc]) with nc cells per view.  nc and the record indices are int:
+// occ_backward requires OB*OB*OCC_CELLS <= INT32_MAX and Ptot < INT32_MAX.
 struct SelectCompact {
     using Index = int;
     const float4 *crec;
     const int32_t *tile_offsets;
-    int nt;
+    int nc;
     int pass;
     __device__ __forceinline__ void range(int n, int &beg, int &end) const {
-        beg = __ldg(&tile_offsets[(int64_t)n * nt]);
-        end = __ldg(&tile_offsets[(int64_t)(n + 1) * nt]);
+        beg = __ldg(&tile_offsets[(int64_t)n * nc]);
+        end = __ldg(&tile_offsets[(int64_t)(n + 1) * nc]);
     }
     __device__ __forceinline__ bool load(int i, float &rx, float &ry) const {
         const float4 c = __ldg(&crec[i]);
@@ -411,15 +362,18 @@ __host__ __device__ __forceinline__ bool occ_fits(float r, int S, int R_box) {
 }
 
 __global__ void __launch_bounds__(256)
-occ_parts_kernel(const int32_t *__restrict__ tile_offsets, int cs, const float *__restrict__ rs, int nt_view, int64_t nt,
+occ_parts_kernel(const int32_t *__restrict__ tile_offsets, const float *__restrict__ rs, int nt_view, int64_t nt,
                  int S, int R_box, int32_t *__restrict__ parts) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t > nt) return;
     int p = 0;
-    if (t < nt && occ_fits(rs[t / nt_view], S, R_box)) p = (tile_offsets[(t + 1) * cs] - tile_offsets[t * cs] + OCC_ITEM - 1) / OCC_ITEM;
+    if (t < nt && occ_fits(rs[t / nt_view], S, R_box))
+        p = (tile_offsets[(t + 1) * OCC_CELLS] - tile_offsets[t * OCC_CELLS] + OCC_ITEM - 1) / OCC_ITEM;
     parts[t] = p;   // parts[nt] = 0 so that the scan's last entry is the total
 }
 
+// Tile numbers (item_tile) and item numbers (part_off) are int32: occ_backward requires its bound on the items,
+// max_items = Ptot / OCC_ITEM + nt + 1, below INT32_MAX.
 __global__ void __launch_bounds__(256)
 occ_items_kernel(const int32_t *__restrict__ part_off, int64_t nt, int32_t *__restrict__ item_tile) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -430,8 +384,8 @@ occ_items_kernel(const int32_t *__restrict__ part_off, int64_t nt, int32_t *__re
 struct OccTileArgs {
     const float4 *crec;          // compact tile-ordered records {px, py, rx, ry}
     const int32_t *cids;         // packed splat id of every compact record (occ_store_id: -1 behind the camera)
-    const int32_t *tile_offsets; // (N*OB*OB*cs + 1): list of tile t = [tile_offsets[t*cs], tile_offsets[(t+1)*cs])
-    int cs;                      // bins per tile: 1 (tile-level binning) or OCC_CELLS (cell-level, lists ordered by pixel)
+    const int32_t *tile_offsets; // (N*OB*OB*OCC_CELLS + 1) cell offsets: list of tile t (ordered by pixel) =
+                                 // [tile_offsets[t*OCC_CELLS], tile_offsets[(t+1)*OCC_CELLS])
     const int32_t *part_off;     // (N*OB*OB + 1) exclusive scan of the items per tile; last = number of items
     const int32_t *item_tile;    // tile (n*OB*OB + tile) of every item
     int *group_counter;          // next group of items to hand out (zero at launch)
@@ -658,7 +612,7 @@ occ_tile_kernel(const __grid_constant__ OccTileArgs a) {
             const int n = t / (OB * OB), tile = t - n * OB * OB;
             const int ty = tile / OB, tx = tile - ty * OB;
             const int p = item - a.part_off[t], parts = a.part_off[t + 1] - a.part_off[t];
-            const int tb = a.tile_offsets[(int64_t)t * a.cs], count = a.tile_offsets[(int64_t)(t + 1) * a.cs] - tb;
+            const int tb = a.tile_offsets[(int64_t)t * OCC_CELLS], count = a.tile_offsets[(int64_t)(t + 1) * OCC_CELLS] - tb;
             const int per = (count + parts - 1) / parts;
             const int beg = tb + p * per;
             const int cnt = max(0, min(count - p * per, per));
@@ -912,8 +866,12 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
     const size_t win_elems = (size_t)2 * (side * side + OCC_SLACK) + 2 * side + OCC_SLACK;
     const size_t smem = 2 * win_elems * sizeof(float) + 2 * (size_t)OCC_ITEM * sizeof(float4) + 2 * sizeof(OccItem) +
                         4 * sizeof(unsigned long long);
-    const bool tiles_ok = (size_t)OB * OB * sizeof(int32_t) <= 200 * 1024 && nt + 1 < (int64_t)INT32_MAX &&
-                          Ptot < (int64_t)INT32_MAX;
+    // The limits of the staged path, each stated at the kernel that has it (occ_cellbin_kernel, SelectCompact,
+    // occ_items_kernel, occ_planes_kernel).  Cells are indexed in int64 everywhere (occ_cell, every offset read), so
+    // their total needs no limit of its own.
+    const int64_t max_items = Ptot / OCC_ITEM + nt + 1;   // >= nt + 1
+    const bool tiles_ok = max_items < (int64_t)INT32_MAX && Ptot < (int64_t)INT32_MAX &&
+                          (int64_t)OB * OB * OCC_CELLS <= (int64_t)INT32_MAX && OB * OCC_TILE + 2 * R_box <= 65535;
     if (!tiles_ok) R_box = 0;
     int rc;
     DSS_CUDA_TRY(cudaMemsetAsync(grad_xy, 0, (size_t)Ptot * 2 * sizeof(float), st));
@@ -922,9 +880,7 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
         float4 *crec = nullptr;
         float *planes = nullptr;
         const int PAD = R_box, W = OB * OCC_TILE + 2 * PAD, Hp = W;
-        // bins: pixels (lists ordered by pixel inside a tile) unless that needs more than 32M counters
-        const int cs = (!ctx->occ_tilebin && nt * OCC_CELLS <= ((int64_t)32 << 20)) ? OCC_CELLS : 1;
-        const int64_t nc = nt * cs;
+        const int64_t nc = nt * OCC_CELLS;
         if ((rc = ctx_get(ctx, BUF_OCC_COUNTS, (size_t)(nc + 1), &counts))) return rc;
         if ((rc = ctx_get(ctx, BUF_TILE_OFFSETS, (size_t)(nc + 1), &offsets))) return rc;
         if ((rc = ctx_get(ctx, BUF_OCC_IDS, (size_t)(Ptot > 0 ? Ptot : 1), &cids))) return rc;
@@ -936,36 +892,20 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
             const bool clean = ctx->occ_counts_ptr == counts && ctx->occ_counts_elems >= (size_t)(nc + 1);
             ctx->occ_counts_ptr = nullptr;   // restored below; an error in between forces the memset next time
             if (!clean) DSS_CUDA_TRY(cudaMemsetAsync(counts, 0, ctx->cap[BUF_OCC_COUNTS], st));
-            if (cs == 1) {
-                dim3 bgrid((unsigned)((P0 + 2047) / 2048), N);
-                const size_t hist = (size_t)OB * OB * sizeof(int32_t);
-                if (hist > 48 * 1024) {
-                    DSS_CUDA_TRY(cudaFuncSetAttribute(occ_bin_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist));
-                    DSS_CUDA_TRY(cudaFuncSetAttribute(occ_bin_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist));
-                }
-                occ_bin_kernel<0><<<bgrid, 256, hist, st>>>(rec, visible, first_idx, num_points, P0, S, OB, counts, nullptr,
-                                                            nullptr, nullptr);
-                DSS_LAUNCH_CHECK(ctx);
-                if ((rc = exclusive_scan_i32(ctx, counts, offsets, nc + 1, st))) return rc;
-                occ_bin_kernel<1><<<bgrid, 256, hist, st>>>(rec, visible, first_idx, num_points, P0, S, OB, counts, offsets,
-                                                            crec, cids);
-                DSS_LAUNCH_CHECK(ctx);
+            dim3 bgrid(grid_blocks(P0, 256 * 4, ctx->sm_count, 8), N);
+            if (cell_counts) {
+                // the forward's blend epilogue has counted already (one count per visible splat, same cells): take a
+                // copy -- pass 1 counts the working copy back down to zero, the caller's tensor stays intact
+                DSS_CUDA_TRY(cudaMemcpyAsync(counts, cell_counts, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
             } else {
-                dim3 bgrid(grid_blocks(P0, 256 * 4, ctx->sm_count, 8), N);
-                if (cell_counts) {
-                    // the forward's blend epilogue has counted already (one count per visible splat, same cells): take a
-                    // copy -- pass 1 counts the working copy back down to zero, the caller's tensor stays intact
-                    DSS_CUDA_TRY(cudaMemcpyAsync(counts, cell_counts, (size_t)nc * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-                } else {
-                    occ_cellbin_kernel<0><<<bgrid, 256, 0, st>>>(rec, visible, first_idx, num_points, P0, S, OB, counts, nullptr,
-                                                                 nullptr, nullptr);
-                    DSS_LAUNCH_CHECK(ctx);
-                }
-                if ((rc = exclusive_scan_i32(ctx, counts, offsets, nc + 1, st))) return rc;
-                occ_cellbin_kernel<1><<<bgrid, 256, 0, st>>>(rec, visible, first_idx, num_points, P0, S, OB, counts, offsets,
-                                                             crec, cids);
+                occ_cellbin_kernel<0><<<bgrid, 256, 0, st>>>(rec, visible, first_idx, num_points, P0, S, OB, counts, nullptr,
+                                                             nullptr, nullptr);
                 DSS_LAUNCH_CHECK(ctx);
             }
+            if ((rc = exclusive_scan_i32(ctx, counts, offsets, nc + 1, st))) return rc;
+            occ_cellbin_kernel<1><<<bgrid, 256, 0, st>>>(rec, visible, first_idx, num_points, P0, S, OB, counts, offsets,
+                                                         crec, cids);
+            DSS_LAUNCH_CHECK(ctx);
             ctx->occ_counts_ptr = counts;
             ctx->occ_counts_elems = ctx->cap[BUF_OCC_COUNTS] / sizeof(int32_t);
         }
@@ -976,7 +916,7 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
             DSS_CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)N * 4 * 256 * sizeof(unsigned int), st));
             dim3 grid(grid_blocks(P0 / 4 + 1, 256, ctx->sm_count, 1), N);
             for (int pass = 0; pass < 4; ++pass) {
-                select_hist_kernel<<<grid, 256, 0, st>>>(SelectCompact{crec, offsets, OB * OB * cs, pass}, hist);
+                select_hist_kernel<<<grid, 256, 0, st>>>(SelectCompact{crec, offsets, OB * OB * OCC_CELLS, pass}, hist);
                 DSS_LAUNCH_CHECK(ctx);
             }
             select_final_kernel<<<N, 32, 0, st>>>(hist, radii_s, rs);
@@ -990,11 +930,10 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
         }
         // work items: parts per tile -> scan -> tile of every item
         int32_t *parts = nullptr, *item_tile = nullptr;
-        const int64_t max_items = Ptot / OCC_ITEM + nt + 1;
         if ((rc = ctx_get(ctx, BUF_OCC_PARTS, (size_t)(2 * (nt + 1) + 4), &parts))) return rc;
         if ((rc = ctx_get(ctx, BUF_OCC_ITEMS, (size_t)max_items, &item_tile))) return rc;
         int32_t *part_off = parts + (nt + 1);
-        occ_parts_kernel<<<(unsigned)((nt + 1 + 255) / 256), 256, 0, st>>>(offsets, cs, rs, OB * OB, nt, S, R_box, parts);
+        occ_parts_kernel<<<(unsigned)((nt + 1 + 255) / 256), 256, 0, st>>>(offsets, rs, OB * OB, nt, S, R_box, parts);
         DSS_LAUNCH_CHECK(ctx);
         if ((rc = exclusive_scan_i32(ctx, parts, part_off, nt + 1, st))) return rc;
         occ_items_kernel<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(part_off, nt, item_tile);
@@ -1003,7 +942,6 @@ int occ_backward(dss_ctx *ctx, const float4 *rec, const uint8_t *visible, float 
         a.crec = crec;
         a.cids = cids;
         a.tile_offsets = offsets;
-        a.cs = cs;
         a.part_off = part_off;
         a.item_tile = item_tile;
         a.group_counter = parts + 2 * (nt + 1);

@@ -1,8 +1,8 @@
 """The whole fused backward (dss_render_backward) against its float64 reference (tests/util.py render_backward_f64) on
 the forward's own fragments, in the configurations the operator tests do not reach: packed clouds with ragged and empty
 views and rows no view covers, per-splat h (the Vrk_isotropic layout), a z-buffer loss, K > 8 (the pixel-parallel
-forward, whose blend epilogue counts the backward's binning cells too), the tile-level backward binning with more than 96
-views, filtered slots, and a staged-window hint left by a different call.
+forward, whose blend epilogue counts the backward's binning cells too), a backward binning of more than 2^25 cells over
+more than 96 views, filtered slots, and a staged-window hint left by a different call.
 
 Each case checks the clipped NDC gradient the library writes (grad_ndc), the position gradient per packed row and the
 point / colour gradients autograd returns."""
@@ -208,9 +208,9 @@ def test_k12_backward_takes_the_forward_cell_counts(cuda_device, layout):
     assert k12 == k5, (k12, k5)
 
 
-# ---- 129 shared views at S = 512: tile-level backward binning (N * 16^2 * 1024 > 32M cells), and views past the
-#      96 whose radii the staged-window hint reads, with search radii too large for the window it sizes ------------
-def test_129_views_tile_binning_and_unhinted_views(cuda_device):
+# ---- 129 shared views at S = 512: a backward binning of N * 16^2 * 1024 > 2^25 cells, and views past the 96 whose
+#      radii the staged-window hint reads, with search radii too large for the window it sizes ----------------------
+def test_129_views_many_cells_and_unhinted_views(cuda_device):
     d = cuda_device
     P0, S = 300, 512
     pts, nrm, col = sphere_cloud(P0, seed=9)

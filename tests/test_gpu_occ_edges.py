@@ -168,6 +168,7 @@ CASES = [
     ("small_box", ("random", [0, "none", 7, 8, "big"], 3), 128, 1, "4x1 4x1 4x2 g g"),
     ("default_box", ("random", [19, 20, 0], 4), 96, 0, "4x5 g 4x1"),
     ("tile_binning", ("random", [3] * 33, 5), 1024, 3, "4x1"),
+    ("s8192", ("random", [3], 6), 8192, 3, "4x1"),
     ("disc_edge_r5", ("disc_edge", 128, None), 128, 5, "4x2"),
     ("disc_edge_r10_tile", ("disc_edge", 256, 10), 256, 10, "4x3"),
     ("disc_edge_r10_generic", ("disc_edge", 256, 10), 256, 1, "g"),
@@ -221,8 +222,8 @@ def test_occ_gather_per_point_bound(cuda_device, case):
 def test_occ_dispatch_coverage():
     """the cases above reach every path: all 8 lane mappings with and without a power-of-two S, both sides of every
     `need` bracket edge and the largest need at R_box = 40, hh = 0 (rs = 0, and nothing visible), the last window that
-    fits and the first that does not, rs >= 4, one launch that mixes mappings and the generic kernel, and one with
-    tile-level binning"""
+    fits and the first that does not, rs >= 4, one launch that mixes mappings and the generic kernel, one that bins
+    more than 2^25 cells (the large scan and the scratch it needs), and one view of 256 x 256 tiles (S = 8192)"""
     maps, needs, seen = set(), set(), set()
     for case in CASES:
         cid, spec, S, _, _ = case
@@ -251,7 +252,9 @@ def test_occ_dispatch_coverage():
         if len(kinds) == 2 and len({p for p in paths if p[0] == "tile"}) > 1:
             seen.add("mixed")
         if len(rs) * ((S + 31) // 32) ** 2 * 1024 > (32 << 20):
-            seen.add("tile_binning")
+            seen.add("over_2p25_cells")
+        if "tile" in kinds and S >= 8192:
+            seen.add("s8192_tiles")
         # work items of <= 128 splats per tile, handed out in groups of 4 to at most 2 persistent CTAs per SM
         live = d["vis"] > 0
         view = np.repeat(np.arange(len(rs)), d["num"])[live]
@@ -265,8 +268,8 @@ def test_occ_dispatch_coverage():
     assert maps == {(lps, ppl, p2) for _, lps, ppl in MAPPINGS for p2 in (True, False)}, maps
     for lo, hi in ((8, 10), (16, 18), (24, 26), (32, 34), (40, 42), (48, 50), (64, 66)):
         assert lo in needs and hi in needs, (lo, hi)
-    want = {"last_fit", "first_no_fit", "rs0", "none_visible", "largest_need", "rs_ge_4", "mixed", "tile_binning",
-            "items_per_tile", "groups_over_ctas"}
+    want = {"last_fit", "first_no_fit", "rs0", "none_visible", "largest_need", "rs_ge_4", "mixed", "over_2p25_cells",
+            "s8192_tiles", "items_per_tile", "groups_over_ctas"}
     assert want <= seen, want - seen
     print("mappings (lanes, pairs, pow2): %s; needs: %s; %s" % (sorted(maps), sorted(needs), sorted(seen)))
 
