@@ -23,7 +23,7 @@ from .cloud import clouds_share_points
 from .knn import knn_sq_dists
 
 __all__ = ["PointFragments", "PointsRasterizationSettings", "SurfaceSplatting", "rasterize_elliptical_points",
-           "EllipticalRasterizer", "kMaxPointsPerBin"]
+           "EllipticalRasterizer", "kMaxPointsPerBin", "point_sq_spacing", "splat_variance_scale"]
 
 kMaxPointsPerBin = 22   # pytorch3d constant the reference (mis)uses as a bound on bins per side (rasterizer.py:725-730)
 
@@ -74,6 +74,25 @@ def _splat_params(rs: PointsRasterizationSettings, cameras, kwargs=None) -> Spla
                        radii_backward_scaler=float(rs.radii_backward_scaler),
                        clip_pts_grad=float(rs.clip_pts_grad if rs.clip_pts_grad is not None else -1.0),
                        backface_culling=bool(rs.backface_culling), znear=f(znear), zfar=f(zfar))
+
+
+def point_sq_spacing(points, frnn_radius=0.2):
+    """(P,) 0.5 x the largest squared distance from every point of ONE cloud to its 6 nearest neighbours within
+    ``frnn_radius`` (rasterizer.py:313-326); 0.5e-3 for every point of a cloud of fewer than 7 points."""
+    if points.shape[0] < 7:   # "knn search is unreliable, set sq_dist manually" (rasterizer.py:320-321)
+        return torch.full((points.shape[0],), 0.5e-3, device=points.device)
+    d2 = knn_sq_dists(points.detach(), K=7, radius=frnn_radius)[:, 1:]
+    return 0.5 * d2.max(dim=-1)[0]
+
+
+def splat_variance_scale(per_cloud, Vrk_invariant):
+    """The variance scale h of the reconstruction kernel from :func:`point_sq_spacing` of every cloud (view) of the
+    batch (rasterizer.py:293-402): ``Vrk_invariant`` h_n = clamp(mean, 5e-5, 1e-3) per view -> (N,), else
+    (``Vrk_isotropic``) h_p = clamp(spacing, 5e-5, 0.01) per point -> (P,) packed."""
+    if Vrk_invariant:
+        return torch.stack([h.mean().clamp(5e-5, 1e-3) if h.numel() else h.new_tensor(1e-3)
+                            for h in per_cloud]).float()
+    return torch.cat(per_cloud).clamp(5e-5, 0.01).float()
 
 
 class SurfaceSplatting(nn.Module):
@@ -127,7 +146,6 @@ class SurfaceSplatting(nn.Module):
         Vrk_isotropic: per point h_p = clamp(0.5 max_{6NN} d^2, 5e-5, 0.01), cached        -> (P,)"""
         rs = kwargs.get("raster_settings", self.raster_settings)
         num = point_clouds.num_points_per_cloud()
-        dev = point_clouds.device
         if not (rs.Vrk_invariant or rs.Vrk_isotropic):
             raise NotImplementedError("anisotropic Vrk (curvature frames + batched SVD, rasterizer.py:256-291) "
                                       "is outside the hot path; use Vrk_invariant or Vrk_isotropic")
@@ -138,19 +156,11 @@ class SurfaceSplatting(nn.Module):
         shared = clouds_share_points(point_clouds)
         per_cloud = []
         for n, pts in enumerate(pts_list):
-            if shared and n > 0:
-                per_cloud.append(per_cloud[0])
-                continue
-            if pts.shape[0] < 7:   # "knn search is unreliable, set sq_dist manually" (rasterizer.py:320-321)
-                per_cloud.append(torch.full((pts.shape[0],), 0.5e-3, device=dev))
-                continue
-            d2 = knn_sq_dists(pts.detach(), K=7, radius=self.frnn_radius)[:, 1:]
-            per_cloud.append(0.5 * d2.max(dim=-1)[0])
-        if rs.Vrk_invariant:
-            return torch.stack([h.mean().clamp(5e-5, 1e-3) if h.numel() else h.new_tensor(1e-3)
-                                for h in per_cloud]).float()
-        self._Vrk_h = torch.cat(per_cloud).clamp(5e-5, 0.01).float()
-        return self._Vrk_h
+            per_cloud.append(per_cloud[0] if shared and n > 0 else point_sq_spacing(pts, self.frnn_radius))
+        h = splat_variance_scale(per_cloud, rs.Vrk_invariant)
+        if not rs.Vrk_invariant:
+            self._Vrk_h = h
+        return h
 
     def _get_per_point_info(self, point_clouds, **kwargs):
         """radii (P,2), ellipse_params (P,3), cutoff_threshold (P,), scaler (P,) -- rasterizer.py:525-565,

@@ -20,7 +20,8 @@ import torch
 
 from . import _lib
 
-__all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points"]
+__all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
+           "point_filters", "set_point_filters"]
 
 
 class SplatParams(NamedTuple):
@@ -339,6 +340,48 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     image, idx, weights, visible, records, scaler = outs[:6]
     zbuf, qvalue = (outs[6], outs[7]) if return_fragments else (None, None)
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
+
+
+def point_filters(out: RenderOutput, mask_img):
+    """The visibility and inmask point filters of the reference's ``Model.forward`` (point_modeling.py:172-173,
+    188-212) for the SHARED cloud that ``render_points`` drew in ``out``: ``visibility`` = visible in any view,
+    ``inmask`` = visibility and, in any view, torch's ``grid_sample(mask, clamp(-xy, -1, 1))`` (bilinear, reflection
+    padding, align_corners=False) != 0 at the NDC position the render projected the point to (csrc/point_filter.cu).
+    A non-finite projected position is outside the mask.
+
+    ``mask_img``: the N ground-truth masks, (N,H,W) or (N,1,H,W), float32, uint8 or bool, any strides (read in place),
+    of any size H x W.  Returns ``(visibility, inmask)``, (P0,) bool.  One launch, no host synchronisation."""
+    N = out.image.shape[0]
+    P = out.records.shape[0]
+    if out.image.dim() != 4 or tuple(out.records.shape[1:]) != (8,) or P % N or tuple(out.visible.shape) != (P,):
+        raise RuntimeError("out must be the RenderOutput of a shared cloud: records (N*P0, 8) and visible (N*P0,)")
+    if mask_img.dim() == 4 and mask_img.shape[1] == 1:
+        mask_img = mask_img[:, 0]
+    if mask_img.dim() != 3 or mask_img.shape[0] != N or mask_img.shape[1] < 1 or mask_img.shape[2] < 1:
+        raise RuntimeError("mask_img must have shape (%d, H, W) or (%d, 1, H, W), got %s" % (N, N, tuple(mask_img.shape)))
+    if mask_img.dtype not in (torch.float32, torch.uint8, torch.bool):
+        raise TypeError("mask_img must be float32, uint8 or bool, got %s" % mask_img.dtype)
+    dev = _lib.require_cuda(out.records, out.visible, mask_img)
+    P0 = P // N
+    visibility = torch.empty((P0,), dtype=torch.bool, device=dev)
+    inmask = torch.empty((P0,), dtype=torch.bool, device=dev)
+    strides = (C.c_int64 * 3)(*mask_img.stride())
+    with torch.cuda.device(dev):
+        rc = _lib.load().dss_point_filters(
+            _lib.ctx(dev), _lib.ptr(out.records), _lib.ptr(out.visible), 1, N, P0, _lib.ptr(mask_img),
+            int(mask_img.dtype != torch.float32), strides, int(mask_img.shape[1]), int(mask_img.shape[2]),
+            _lib.ptr(visibility), _lib.ptr(inmask), _lib.stream_ptr(dev))
+    _lib.check(rc, "dss_point_filters")
+    return visibility, inmask
+
+
+def set_point_filters(points_filter, out: RenderOutput, mask_img):
+    """Set ``points_filter`` (a ``PointCloudsFilters``) to the (1, P0) ``visibility`` and ``inmask`` of
+    :func:`point_filters`, the filters ``ProjectionLoss`` / ``RepulsionLoss`` read: one call in place of
+    point_modeling.py:188-212.  Returns ``points_filter``."""
+    visibility, inmask = point_filters(out, mask_img)
+    points_filter.set_filter(visibility=visibility[None], inmask=inmask[None])
+    return points_filter
 
 
 def make_shading(lights, view_matrices, shininess=64.0) -> Shading:

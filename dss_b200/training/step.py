@@ -1,0 +1,243 @@
+"""The reference's training step on the fused path: ``Trainer.compute_loss`` + ``loss.backward()``
+(DSS/training/trainer.py:275-331, DSS/models/point_modeling.py:135-214) for one shared cloud of P0 points and a batch of
+N views, with the settings ``configs/dss.yml`` trains with:
+
+1. ``F.normalize(normals)`` (point_modeling.py:84-86);
+2. the splat size from a K-NN of the current points (rasterizer.py:293-342, ``Vrk_invariant`` / ``Vrk_isotropic``);
+3. ``render_points`` with fused shading: the batch's lights, and camera centres derived from the batch's view matrices;
+4. ``image_loss`` (trainer.py:332-376);
+5. ``point_filters``: the visibility and inmask filters (point_modeling.py:172-173, 188-212);
+6. the fused ``ProjectionLoss`` and ``RepulsionLoss`` over a rebuilt K-NN (trainer.py:305-319), each skipped when its
+   lambda is 0;
+7. ``loss.backward()``.
+
+Gradients land on the step's OWN leaves (``step.points``, ``step.normals``, ``step.colours``: fresh copies of what was
+passed in, the ones named in ``learn`` requiring grad); the optimizer stays with the caller, who updates those leaves in
+place.  ``step.loss`` holds the trainer's loss dict as device scalars, ``step.image`` the render, ``step.visibility`` and
+``step.inmask`` the (P0,) filters.
+
+:class:`TrainStep` runs the step eagerly.  :class:`GraphedTrainStep` captures it once in a CUDA graph: every piece is
+free of host synchronisation, so one replay computes the whole step.  Between replays ``load()`` copies the next batch
+into the step's static inputs.  Host-side settings are frozen into a capture; when one of them changes (``params``, e.g.
+its ``radii_backward_scaler``, which the trainer's scheduler lowers, or a lambda), or when another library call has
+reallocated the scratch buffers the graph uses, the next ``replay()`` captures again.
+"""
+import ctypes as C
+
+import torch
+import torch.nn.functional as F
+
+from .. import _lib
+from ..core.cloud import PointClouds3D, PointCloudsFilters
+from ..core.lighting import pack_lights
+from ..core.rasterizer import point_sq_spacing, splat_variance_scale
+from ..core.texture import camera_centres
+from ..ops import Shading, SplatParams, point_filters, render_points
+from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
+
+__all__ = ["TrainStep", "GraphedTrainStep"]
+
+_LEARNABLE = ("points", "normals", "colours")
+
+
+class TrainStep:
+    """One training step, eager.  ``points``, ``normals``, ``colours`` (P0,3) float32 CUDA: the world cloud and its
+    albedo.  ``params``: the rasterizer settings (``SplatParams``).  The remaining settings default to the trainer's and
+    ``configs/dss.yml``'s.  ``step(img, mask_img, proj, view, lights)`` runs the step on a batch and returns the loss dict:
+    ``img`` (N,H,W,3) float32 ground truth (any strides), ``mask_img`` (N,H,W) or (N,1,H,W) float32, uint8 or bool,
+    ``proj`` / ``view`` (N,4,4) as ``render_points`` takes them, ``lights`` a ``DirectionalLights`` / ``PointLights``
+    of batch 1 or N (dss_b200.core.lighting)."""
+
+    def __init__(self, points, normals, colours, params: SplatParams, *, learn=("points", "normals"),
+                 Vrk_invariant=True, frnn_radius=0.2, shininess=64.0, lambda_dr_rgb=1.0, lambda_dr_silhouette=1.0,
+                 lambda_dr_proj=0.01, lambda_dr_repel=0.0, knn_k=12, filter_scale=2.0, sharpness_sigma=0.75,
+                 grad_sync=None):
+        dev = _lib.require_cuda(points, normals, colours)
+        for name, t in (("points", points), ("normals", normals), ("colours", colours)):
+            if t.dtype != torch.float32 or t.dim() != 2 or tuple(t.shape) != (points.shape[0], 3):
+                raise RuntimeError("%s must be a float32 (P0, 3) tensor, got %s %s" % (name, t.dtype, tuple(t.shape)))
+        if any(name not in _LEARNABLE for name in learn):
+            raise ValueError("learn takes names out of %s, got %s" % (_LEARNABLE, tuple(learn)))
+        if grad_sync is not None and grad_sync.world_size > 1:
+            raise NotImplementedError("the training step does not take the multi-GPU gradient exchange; call "
+                                      "render_points(..., grad_sync=...) eagerly")
+        self.device = dev
+        leaf = lambda t, name: t.detach().clone().requires_grad_(name in learn)
+        self.points, self.normals, self.colours = leaf(points, "points"), leaf(normals, "normals"), \
+            leaf(colours, "colours")
+        self.params = params
+        self.Vrk_invariant, self.frnn_radius, self.shininess = bool(Vrk_invariant), float(frnn_radius), float(shininess)
+        self.lambda_dr_rgb, self.lambda_dr_silhouette = float(lambda_dr_rgb), float(lambda_dr_silhouette)
+        self.lambda_dr_proj, self.lambda_dr_repel = float(lambda_dr_proj), float(lambda_dr_repel)
+        self.knn_k, self.filter_scale, self.sharpness_sigma = int(knn_k), float(filter_scale), float(sharpness_sigma)
+        # the cloud's point count as a device tensor made once: PointClouds3D would build it from a host list, a copy
+        # that a capture cannot take
+        self._num = torch.full((1,), points.shape[0], dtype=torch.int64, device=dev)
+        self.loss = self.image = self.visibility = self.inmask = None
+
+    def settings(self):
+        """every host-side value the step bakes into its launches"""
+        return (tuple(self.params), self.Vrk_invariant, self.frnn_radius, self.shininess, self.lambda_dr_rgb,
+                self.lambda_dr_silhouette, self.lambda_dr_proj, self.lambda_dr_repel, self.knn_k, self.filter_scale,
+                self.sharpness_sigma)
+
+    def _check_batch(self, img, mask_img, proj, view):
+        _lib.require_cuda(self.points, img, mask_img, proj, view)
+        if not fused_image_loss_targets(img, mask_img):
+            raise TypeError("img must be float32 and mask_img float32, uint8 or bool, neither requiring grad; got %s "
+                            "and %s" % (img.dtype, mask_img.dtype))
+        N = proj.shape[0]
+        if tuple(proj.shape) != (N, 4, 4) or tuple(view.shape) != (N, 4, 4):
+            raise RuntimeError("proj and view must have shape (N, 4, 4)")
+        S = int(self.params.image_size)
+        if tuple(img.shape) != (N, S, S, 3):
+            raise RuntimeError("img must have shape (N, S, S, 3) = %s, got %s" % ((N, S, S, 3), tuple(img.shape)))
+
+    def __call__(self, img, mask_img, proj, view, lights):
+        self._check_batch(img, mask_img, proj, view)
+        rows, ambient, kind = pack_lights(lights)
+        return self._run(img, mask_img, proj, view, rows.detach(), ambient.detach(), kind)
+
+    def _run(self, img, mask_img, proj, view, rows, ambient, light_type):
+        for t in (self.points, self.normals, self.colours):
+            t.grad = None
+        N, dev = proj.shape[0], self.device
+        normals = F.normalize(self.normals, dim=-1)
+        with torch.no_grad():
+            # the one cloud's spacing, the rule of SurfaceSplatting._compute_h for its N views
+            h = splat_variance_scale([point_sq_spacing(self.points, self.frnn_radius)], self.Vrk_invariant).repeat(N)
+        shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
+        out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading)
+        loss = image_loss(out.image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette)
+        visibility, inmask = point_filters(out, mask_img)
+        cloud = PointClouds3D([self.points], [normals])
+        cloud._cache["num"] = self._num
+        points_filter = PointCloudsFilters(dev, visibility=visibility[None], inmask=inmask[None])
+        zero = torch.zeros((), dtype=torch.float32, device=dev)
+        reg = {}
+        for key, lam, cls in (("loss_dr_proj", self.lambda_dr_proj, ProjectionLoss),
+                              ("loss_dr_repel", self.lambda_dr_repel, RepulsionLoss)):
+            reg[key] = zero
+            if lam > 0:
+                fn = cls(reduction="mean", knn_k=self.knn_k, filter_scale=self.filter_scale,
+                         sharpness_sigma=self.sharpness_sigma)
+                reg[key] = fn(cloud, rebuild_knn=True, points_filter=points_filter) * lam
+        # trainer.py:313: loss = proj + repel + the image loss
+        total = reg["loss_dr_proj"] + reg["loss_dr_repel"] + loss["loss"]
+        total.backward()
+        self.loss = {"loss": total.detach(), "loss_dr_rgb": loss["loss_dr_rgb"].detach(),
+                     "loss_dr_silhouette": loss["loss_dr_silhouette"].detach(),
+                     "loss_dr_proj": reg["loss_dr_proj"].detach(), "loss_dr_repel": reg["loss_dr_repel"].detach()}
+        self.image, self.visibility, self.inmask = out.image.detach(), visibility, inmask
+        return self.loss
+
+
+class GraphedTrainStep(TrainStep):
+    """:class:`TrainStep` captured in a CUDA graph.  The step owns static copies of the first batch
+    (``step.img``, ``step.mask_img``, ``step.proj``, ``step.view`` and the packed light rows); ``load(img, mask_img,
+    proj, view, lights)`` copies the next batch into them in place (same shapes, same kind of lights) and ``replay()``
+    runs the step on them::
+
+        step = GraphedTrainStep(points, normals, colours, params, img, mask_img, proj, view, lights)
+        for batch in loader:
+            step.load(*batch)
+            step.replay()            # step.loss, step.image, step.visibility, step.inmask; gradients on the leaves
+            optimizer.step()         # over step.points, step.normals: updated in place
+
+    ``replay()`` captures again, first, when :meth:`settings` differ from those of the capture (``step.params =
+    step.params._replace(radii_backward_scaler=...)``, ``step.lambda_dr_proj = ...``).  As for ``GraphedRenderStep``,
+    the forward's tile-list capacity is frozen into the capture: replays stay correct when the lists outgrow it, and
+    :meth:`stale` tells when a new capture (:meth:`capture`) would be faster.  The capture holds the library's scratch
+    buffers; when a library call outside the step has reallocated them (the library's scratch total changed), the next
+    ``replay()`` captures again too."""
+
+    def __init__(self, points, normals, colours, params: SplatParams, img, mask_img, proj, view, lights, warmup=3,
+                 **settings):
+        super().__init__(points, normals, colours, params, **settings)
+        self._check_batch(img, mask_img, proj, view)
+        rows, ambient, self._light_type = pack_lights(lights)
+        # static inputs (clone keeps a permuted view's strides)
+        self.img, self.mask_img = img.detach().clone(), mask_img.detach().clone()
+        self.proj, self.view = proj.detach().float().contiguous().clone(), view.detach().float().contiguous().clone()
+        self.lights, self.ambient = rows.detach().clone(), ambient.detach().clone()
+        self._warmup = max(1, int(warmup))
+        self.graph = None
+        self.capture()
+
+    def _eager(self):
+        return self._run(self.img, self.mask_img, self.proj, self.view, self.lights, self.ambient, self._light_type)
+
+    def capture(self):
+        """warm up on a side stream (sizes the library's scratch and the caching allocator), then capture the step"""
+        dev = self.device
+        self.graph = None
+        s = torch.cuda.Stream(device=dev)
+        s.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(s):
+            for _ in range(self._warmup):
+                self._eager()
+        torch.cuda.current_stream(dev).wait_stream(s)
+        torch.cuda.synchronize(dev)
+        self._capacity_at_capture = self._tile_total()
+        for t in (self.points, self.normals, self.colours):
+            t.grad = None
+        graph = torch.cuda.CUDAGraph(keep_graph=True)    # (kept for kernel_nodes)
+        with torch.cuda.graph(graph):
+            self._eager()
+        graph.instantiate()
+        # the library's scratch only grows, by reallocation: a different total means that a buffer the graph uses moved
+        self.graph, self._captured, self._scratch = graph, self.settings(), _lib.scratch_bytes(dev)
+        # what every replay rewrites: re-attached after each replay, so that an optimizer's zero_grad(set_to_none=True)
+        # or an eager call in between does not detach them
+        self._outputs = (self.loss, self.image, self.visibility, self.inmask)
+        self._grads = tuple(t.grad for t in (self.points, self.normals, self.colours))
+
+    def load(self, img, mask_img, proj, view, lights):
+        """copy the next batch into the static inputs (no synchronisation)"""
+        self._check_batch(img, mask_img, proj, view)
+        rows, ambient, kind = pack_lights(lights)
+        if kind != self._light_type or rows.shape != self.lights.shape or ambient.shape != self.ambient.shape:
+            raise ValueError("the lights must keep the kind and shape of the capture: %s %s, got %s %s"
+                             % (self._light_type, tuple(self.lights.shape), kind, tuple(rows.shape)))
+        for dst, src in ((self.img, img), (self.mask_img, mask_img), (self.proj, proj), (self.view, view),
+                         (self.lights, rows), (self.ambient, ambient)):
+            if dst.shape != src.shape or dst.dtype != src.dtype:
+                raise ValueError("load() takes a batch of the capture's shapes and dtypes: %s %s, got %s %s"
+                                 % (tuple(dst.shape), dst.dtype, tuple(src.shape), src.dtype))
+            dst.copy_(src.detach())
+
+    def replay(self):
+        if self.settings() != self._captured or _lib.scratch_bytes(self.device) != self._scratch:
+            self.capture()
+        self.graph.replay()
+        self.loss, self.image, self.visibility, self.inmask = self._outputs
+        for t, g in zip((self.points, self.normals, self.colours), self._grads):
+            t.grad = g
+        return self.loss
+
+    def _tile_total(self):
+        return int(_lib.load().dss_debug_tile_total(_lib.ctx(self.device)))
+
+    def stale(self, slack=1.2) -> bool:
+        """True when the tile lists have outgrown what they were at capture time by more than `slack` (the replay is
+        still correct, but a new capture will be faster); as GraphedRenderStep.stale"""
+        now = self._tile_total()
+        return self._capacity_at_capture > 0 and now > slack * 1.25 * self._capacity_at_capture
+
+    def kernel_nodes(self) -> int:
+        """the number of kernel launches one replay makes (kernel nodes of the captured graph)"""
+        rt = C.CDLL("libcudart.so.12")
+        g = C.c_void_p(self.graph.raw_cuda_graph())
+        count = C.c_size_t(0)
+        if rt.cudaGraphGetNodes(g, None, C.byref(count)):
+            raise RuntimeError("cudaGraphGetNodes failed")
+        nodes = (C.c_void_p * count.value)()
+        if rt.cudaGraphGetNodes(g, nodes, C.byref(count)):
+            raise RuntimeError("cudaGraphGetNodes failed")
+        kinds = C.c_int(0)
+        n = 0
+        for node in nodes:
+            if rt.cudaGraphNodeGetType(C.c_void_p(node), C.byref(kinds)):
+                raise RuntimeError("cudaGraphNodeGetType failed")
+            n += kinds.value == 0     # cudaGraphNodeTypeKernel
+        return n

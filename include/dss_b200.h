@@ -247,6 +247,21 @@ DSS_API int dss_image_loss_backward(dss_ctx *ctx, const float *pred, const float
                                     const float *grad_loss_rgb, const float *grad_loss_sil, float *grad_pred,
                                     void *stream);
 
+/* ---- point filters of the training step -------------------------------------------------------------------------
+ * Model.forward's visibility and inmask filters (DSS/models/point_modeling.py:172-173, 188-212) of one SHARED cloud of
+ * P0 points seen by N cameras (shared_cloud must be 1: packed clouds return DSS_E_INVALID), from the forward's records
+ * (N*P0, 8) f32, 8-byte aligned, and visible (N*P0,) bytes of dss_render_forward:
+ *   visibility[i] = any_n visible[n*P0 + i],
+ *   inmask[i]     = visibility[i] && any_n sample_n(clamp(-x, -1, 1), clamp(-y, -1, 1)) != 0,
+ * x, y the record's NDC position of (view n, point i) and sample_n torch's grid_sample of mask n (bilinear, reflection
+ * padding, align_corners = False), its arithmetic restated in ATen's order.  A non-finite x or y is outside the mask.
+ * mask n at mask[n*s0 + y*s1 + x*s2], mask_strides = {s0, s1, s2} (host array, in elements), H x W independent of the
+ * render size, f32 (mask_kind 0) or bytes (mask_kind 1: bool / uint8).  Outputs (P0,) bytes, 0 or 1.
+ * One launch, one thread per point; deterministic; no scratch, no host synchronisation. */
+DSS_API int dss_point_filters(dss_ctx *ctx, const float *records, const uint8_t *visible, int shared_cloud, int N,
+                              int64_t P0, const void *mask, int mask_kind, const int64_t *mask_strides, int H, int W,
+                              uint8_t *visibility, uint8_t *inmask, void *stream);
+
 /* ---- fused renderer path (what bench.py times) ----------------------------------------------
  * One call per direction for SurfaceSplattingRenderer.forward / its autograd backward
  * (DSS/core/renderer.py:36-82, DSS/core/rasterizer.py:584-664,749-977).  All pointers device. */
