@@ -86,8 +86,13 @@ _SIGNATURES = {
                                          C.c_double, C.c_double, vp, vp, vp, vp, vp]),
     "dss_image_loss_backward": (C.c_int, [vp, vp, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                           C.c_double, C.c_double, vp, vp, vp, vp, vp, vp]),
+    "dss_image_loss_partial": (C.c_int, [vp, vp, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,
+                                         C.c_double, C.c_double, vp, vp]),
+    "dss_image_loss_finish": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, vp, vp, vp, vp]),
     "dss_point_filters": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp, C.c_int, C.POINTER(C.c_int64),
                                     C.c_int, C.c_int, vp, vp, vp]),
+    "dss_point_filters_gated": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp, C.c_int,
+                                          C.POINTER(C.c_int64), C.c_int, C.c_int, vp, vp, vp, vp]),
     "dss_preprocess": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),

@@ -14,6 +14,10 @@
 // writes the view's totals; the last block to finish (an integer counter; no float atomics) adds the N totals in a
 // fixed order and writes the loss scalars.  Backward: one pass, the coefficients of view n from the totals and the
 // upstream gradients of the three scalars, read from device memory.  Bit-reproducible; no host synchronisation.
+// View-sharded (each rank holds some of the views): dss_image_loss_partial runs both forward passes but, instead of the
+// scalars, puts the rank's view count into the fifth slot of the total row; the caller sums that row over the ranks
+// and image_loss_finish_kernel writes the scalars from it.  The backward reads M and the view count from the (summed)
+// total row and I_n, U_n from the rank's own view rows.
 #include "common.cuh"
 
 namespace dss {
@@ -79,9 +83,21 @@ __global__ void __launch_bounds__(IL_THREADS) image_loss_partials_kernel(const _
     if (threadIdx.x < IL_SUMS) partials[((int64_t)n * gridDim.x + blockIdx.x) * IL_SUMS + threadIdx.x] = v;
 }
 
-// grad_finish_kernel's output rows: view m's totals, then, in the last block, the loss scalars
+// the three loss scalars from the total row's sums over Nv views of HW pixels each
+__device__ __forceinline__ void il_scalars(double M, double abs_rgb, double abs_sil, double iou, double Nv,
+                                           double npix, double lambda_rgb, double lambda_sil, int use_rgb, int use_sil,
+                                           float *loss, float *loss_rgb, float *loss_sil) {
+    const double rgb = (use_rgb && M > 0.0) ? lambda_rgb * (abs_rgb / M) : 0.0;
+    const double sil = use_sil ? lambda_sil * (0.01 * (iou / Nv) + abs_sil / npix) : 0.0;
+    *loss_rgb = (float)rgb;
+    *loss_sil = (float)sil;
+    *loss = (float)(rgb + sil);
+}
+
+// grad_finish_kernel's output rows: view m's totals, then, in the last block, the total row and either the loss scalars
+// or (loss == nullptr: one rank's share of a view-sharded loss) the view count in the row's fifth slot
 struct ImageLossRows {
-    double *totals;              // (N + 1, IL_SUMS): the views', then (M, sum |d rgb|, sum |m - alpha|, sum_n iou_n, 0)
+    double *totals;              // (N + 1, IL_SUMS): the views', then (M, sum |d rgb|, sum |m - alpha|, sum_n iou_n, 0 or N)
     unsigned int *done;
     float *loss, *loss_rgb, *loss_sil;
     double lambda_rgb, lambda_sil, npix;
@@ -110,21 +126,26 @@ struct ImageLossRows {
         if (k < 4) sAll[k] = s;
         __syncthreads();
         if (k != 0) return;
-        const double M = sAll[0];
-        const double rgb = (use_rgb && M > 0.0) ? lambda_rgb * (sAll[1] / M) : 0.0;
-        const double sil = use_sil ? lambda_sil * (0.01 * (sAll[3] / N) + sAll[2] / npix) : 0.0;
         double *row = totals + (int64_t)N * IL_SUMS;
-        row[0] = sAll[0], row[1] = sAll[1], row[2] = sAll[2], row[3] = sAll[3], row[4] = 0.0;
-        *loss_rgb = (float)rgb;
-        *loss_sil = (float)sil;
-        *loss = (float)(rgb + sil);
+        row[0] = sAll[0], row[1] = sAll[1], row[2] = sAll[2], row[3] = sAll[3], row[4] = loss ? 0.0 : (double)N;
+        if (loss)
+            il_scalars(sAll[0], sAll[1], sAll[2], sAll[3], N, npix, lambda_rgb, lambda_sil, use_rgb, use_sil, loss,
+                       loss_rgb, loss_sil);
     }
 };
 
+// the scalars of a view-sharded loss from its total row summed over the ranks (the fifth slot: the view count)
+__global__ void image_loss_finish_kernel(const double *row, double HW, double lambda_rgb, double lambda_sil,
+                                         int use_rgb, int use_sil, float *loss, float *loss_rgb, float *loss_sil) {
+    const double Nv = row[4];
+    il_scalars(row[0], row[1], row[2], row[3], Nv, Nv * HW, lambda_rgb, lambda_sil, use_rgb, use_sil, loss, loss_rgb,
+               loss_sil);
+}
+
 struct ImageLossGradArgs {
-    const double *totals;                          // as ImageLossRows writes them
+    const double *totals;                          // as ImageLossRows writes them, the total row maybe summed over ranks
     const float *g_loss, *g_rgb, *g_sil;           // upstream gradients of the three scalars (device)
-    double lambda_rgb, lambda_sil, npix;
+    double lambda_rgb, lambda_sil;
     float4 *grad;                                  // (N, H*W) d L / d rgba
 };
 
@@ -132,6 +153,8 @@ __global__ void __launch_bounds__(IL_THREADS) image_loss_backward_kernel(const _
                                                                           const __grid_constant__ ImageLossGradArgs b) {
     const int n = blockIdx.y, N = gridDim.y;
     const double gl = *b.g_loss;
+    // the view count of the loss: this call's N, or, for a view-sharded loss, the total row's fifth slot
+    const double Nt = b.totals[(int64_t)N * IL_SUMS + 4], Nv = Nt > 0.0 ? Nt : (double)N, npix = Nv * (double)a.HW;
     // rgb: sign(pred - gt) w_rgb inside mask_pred; alpha: sign(alpha - m) w_l1 - m A + (1 - m) B, where
     // d(1 - I/E)/d alpha = -(m E - I (1 - m) dE/dU) / E^2 gives A = w_iou / E and B = w_iou I dE/dU / E^2
     float w_rgb = 0.0f;
@@ -141,10 +164,10 @@ __global__ void __launch_bounds__(IL_THREADS) image_loss_backward_kernel(const _
         w_rgb = M > 0.0 ? (float)(b.lambda_rgb * (gl + (double)*b.g_rgb) / M) : 0.0f;
     }
     if (a.use_sil) {
-        const double ws = b.lambda_sil * (gl + (double)*b.g_sil), w_iou = 0.01 * ws / N;
+        const double ws = b.lambda_sil * (gl + (double)*b.g_sil), w_iou = 0.01 * ws / Nv;
         const double I = b.totals[(int64_t)n * IL_SUMS + 3], U = b.totals[(int64_t)n * IL_SUMS + 4];
         const double E = il_eps_denom(U);
-        w_l1 = ws / b.npix;
+        w_l1 = ws / npix;
         A = w_iou / E;
         B = fabs(U) >= IL_EPS ? w_iou * I / (E * E) : 0.0;
     }
@@ -193,20 +216,16 @@ static int il_args(ImageLossArgs &a, const float *pred, const float *gt, const i
     return DSS_OK;
 }
 
-}  // namespace dss
-
-extern "C" {
-
-int dss_image_loss_forward(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
-                           const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb, double lambda_sil,
-                           double *totals, float *loss, float *loss_rgb, float *loss_sil, void *stream) {
-    using namespace dss;
+// both forward passes; loss == nullptr: a rank's share of a view-sharded loss (no scalars, the view count in the row)
+static int il_forward(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides, const void *mask,
+                      int mask_kind, int N, int H, int W, double lambda_rgb, double lambda_sil, double *totals,
+                      float *loss, float *loss_rgb, float *loss_sil, void *stream) {
     cudaStream_t st = (cudaStream_t)stream;
     DSS_REQUIRE(ctx != nullptr, "ctx is null");
     ImageLossArgs a;
     int rc = il_args(a, pred, gt, gt_strides, mask, mask_kind, N, H, W, lambda_rgb, lambda_sil);
     if (rc) return rc;
-    DSS_REQUIRE(totals && loss && loss_rgb && loss_sil, "null pointer");
+    DSS_REQUIRE(totals != nullptr, "null pointer");
     const unsigned int blocks = il_blocks(ctx, N, a.HW, 4);
     const size_t np = (size_t)N * blocks * IL_SUMS;
     double *partials = nullptr;
@@ -219,6 +238,39 @@ int dss_image_loss_forward(dss_ctx *ctx, const float *pred, const float *gt, con
     rows.lambda_rgb = lambda_rgb, rows.lambda_sil = lambda_sil, rows.npix = (double)N * (double)a.HW;
     rows.use_rgb = a.use_rgb, rows.use_sil = a.use_sil;
     grad_finish_kernel<IL_SUMS><<<dim3(1, N), 256, 0, st>>>(partials, (int)blocks, N, 1, rows);
+    DSS_LAUNCH_CHECK(ctx);
+    return DSS_OK;
+}
+
+}  // namespace dss
+
+extern "C" {
+
+int dss_image_loss_forward(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
+                           const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb, double lambda_sil,
+                           double *totals, float *loss, float *loss_rgb, float *loss_sil, void *stream) {
+    using namespace dss;
+    DSS_REQUIRE(loss && loss_rgb && loss_sil, "null pointer");
+    return il_forward(ctx, pred, gt, gt_strides, mask, mask_kind, N, H, W, lambda_rgb, lambda_sil, totals, loss,
+                      loss_rgb, loss_sil, stream);
+}
+
+int dss_image_loss_partial(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
+                           const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb, double lambda_sil,
+                           double *totals, void *stream) {
+    return dss::il_forward(ctx, pred, gt, gt_strides, mask, mask_kind, N, H, W, lambda_rgb, lambda_sil, totals,
+                           nullptr, nullptr, nullptr, stream);
+}
+
+int dss_image_loss_finish(dss_ctx *ctx, const double *total_row, int H, int W, double lambda_rgb, double lambda_sil,
+                          float *loss, float *loss_rgb, float *loss_sil, void *stream) {
+    using namespace dss;
+    DSS_REQUIRE(ctx != nullptr, "ctx is null");
+    DSS_REQUIRE(H >= 1 && W >= 1 && (int64_t)H * W <= (int64_t)INT32_MAX, "size out of range");
+    DSS_REQUIRE(total_row && loss && loss_rgb && loss_sil, "null pointer");
+    image_loss_finish_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(total_row, (double)H * (double)W, lambda_rgb,
+                                                                lambda_sil, lambda_rgb > 0.0, lambda_sil > 0.0, loss,
+                                                                loss_rgb, loss_sil);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
@@ -237,7 +289,7 @@ int dss_image_loss_backward(dss_ctx *ctx, const float *pred, const float *gt, co
     DSS_REQUIRE((reinterpret_cast<uintptr_t>(grad_pred) & 15) == 0, "grad_pred must be 16-byte aligned");
     ImageLossGradArgs b;
     b.totals = totals, b.g_loss = grad_loss, b.g_rgb = grad_loss_rgb, b.g_sil = grad_loss_sil;
-    b.lambda_rgb = lambda_rgb, b.lambda_sil = lambda_sil, b.npix = (double)N * (double)a.HW;
+    b.lambda_rgb = lambda_rgb, b.lambda_sil = lambda_sil;
     b.grad = reinterpret_cast<float4 *>(grad_pred);
     image_loss_backward_kernel<<<dim3(il_blocks(ctx, N, a.HW, 8), N), IL_THREADS, 0, st>>>(a, b);
     DSS_LAUNCH_CHECK(ctx);

@@ -21,7 +21,7 @@ import torch
 from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
-           "point_filters", "set_point_filters"]
+           "point_filters", "point_filters_no_views", "set_point_filters"]
 
 
 class SplatParams(NamedTuple):
@@ -342,7 +342,7 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
 
 
-def point_filters(out: RenderOutput, mask_img):
+def point_filters(out: RenderOutput, mask_img, group=None):
     """The visibility and inmask point filters of the reference's ``Model.forward`` (point_modeling.py:172-173,
     188-212) for the SHARED cloud that ``render_points`` drew in ``out``: ``visibility`` = visible in any view,
     ``inmask`` = visibility and, in any view, torch's ``grid_sample(mask, clamp(-xy, -1, 1))`` (bilinear, reflection
@@ -350,7 +350,12 @@ def point_filters(out: RenderOutput, mask_img):
     A non-finite projected position is outside the mask.
 
     ``mask_img``: the N ground-truth masks, (N,H,W) or (N,1,H,W), float32, uint8 or bool, any strides (read in place),
-    of any size H x W.  Returns ``(visibility, inmask)``, (P0,) bool.  One launch, no host synchronisation."""
+    of any size H x W.  Returns ``(visibility, inmask)``, (P0,) bool.  One launch, no host synchronisation.
+
+    ``group``: a torch.distributed process group whose ranks each rendered some of the views of one shared cloud: the
+    filters are then those of all the views, the same on every rank (exact: ORs of bytes).  Two launches and two
+    all-reduces (MAX) of P0 bytes: this rank's visibility, ORed over the ranks, gates ``dss_point_filters_gated``,
+    whose inmask is ORed over the ranks in turn.  A rank without views calls :func:`point_filters_no_views`."""
     N = out.image.shape[0]
     P = out.records.shape[0]
     if out.image.dim() != 4 or tuple(out.records.shape[1:]) != (8,) or P % N or tuple(out.visible.shape) != (P,):
@@ -363,16 +368,38 @@ def point_filters(out: RenderOutput, mask_img):
         raise TypeError("mask_img must be float32, uint8 or bool, got %s" % mask_img.dtype)
     dev = _lib.require_cuda(out.records, out.visible, mask_img)
     P0 = P // N
-    visibility = torch.empty((P0,), dtype=torch.bool, device=dev)
-    inmask = torch.empty((P0,), dtype=torch.bool, device=dev)
     strides = (C.c_int64 * 3)(*mask_img.stride())
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_point_filters(
-            _lib.ctx(dev), _lib.ptr(out.records), _lib.ptr(out.visible), 1, N, P0, _lib.ptr(mask_img),
-            int(mask_img.dtype != torch.float32), strides, int(mask_img.shape[1]), int(mask_img.shape[2]),
-            _lib.ptr(visibility), _lib.ptr(inmask), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_point_filters")
-    return visibility, inmask
+    head = (out.records, out.visible, 1, N, P0, mask_img, int(mask_img.dtype != torch.float32), strides,
+            int(mask_img.shape[1]), int(mask_img.shape[2]))
+
+    def launch(name, *tail):
+        args = [_lib.ptr(a) if isinstance(a, torch.Tensor) or a is None else a for a in head + tail]
+        with torch.cuda.device(dev):
+            rc = getattr(_lib.load(), name)(_lib.ctx(dev), *args, _lib.stream_ptr(dev))
+        _lib.check(rc, name)
+
+    if group is None:
+        visibility = torch.empty((P0,), dtype=torch.bool, device=dev)
+        inmask = torch.empty((P0,), dtype=torch.bool, device=dev)
+        launch("dss_point_filters", visibility, inmask)
+        return visibility, inmask
+    import torch.distributed as dist
+    visibility, inmask = (torch.empty((P0,), dtype=torch.uint8, device=dev) for _ in range(2))
+    launch("dss_point_filters", visibility, inmask)
+    dist.all_reduce(visibility, op=dist.ReduceOp.MAX, group=group)
+    launch("dss_point_filters_gated", visibility, visibility, inmask)
+    dist.all_reduce(inmask, op=dist.ReduceOp.MAX, group=group)
+    return visibility.view(torch.bool), inmask.view(torch.bool)
+
+
+def point_filters_no_views(P0, device, group):
+    """:func:`point_filters` with ``group`` on a rank that holds no views of the batch: the same two all-reduces, with
+    zero contributions, so that the ranks with views do not wait for it.  Returns the (P0,) filters of all views."""
+    import torch.distributed as dist
+    visibility, inmask = (torch.zeros((int(P0),), dtype=torch.uint8, device=device) for _ in range(2))
+    dist.all_reduce(visibility, op=dist.ReduceOp.MAX, group=group)
+    dist.all_reduce(inmask, op=dist.ReduceOp.MAX, group=group)
+    return visibility.view(torch.bool), inmask.view(torch.bool)
 
 
 def set_point_filters(points_filter, out: RenderOutput, mask_img):

@@ -462,12 +462,12 @@ class IouLoss(BaseLoss):
         return 1.0 - intersect / eps_denom(union)
 
 
-def _image_loss_inputs(rgba, img, mask_img):
+def _image_loss_inputs(rgba, img, mask_img, min_views=1):
     """shape and device checks shared by both routes; returns the mask as (N,H,W)"""
     if rgba.dim() != 4 or rgba.shape[-1] != 4:
         raise RuntimeError("rgba must have shape (N, H, W, 4), got %s" % (tuple(rgba.shape),))
     N, H, W = rgba.shape[:3]
-    if N < 1 or H < 1 or W < 1:
+    if N < min_views or H < 1 or W < 1:
         raise RuntimeError("rgba must hold at least one pixel, got %s" % (tuple(rgba.shape),))
     if tuple(img.shape) != (N, H, W, 3):
         raise RuntimeError("img must have shape (N, H, W, 3) = %s, got %s" % ((N, H, W, 3), tuple(img.shape)))
@@ -478,9 +478,15 @@ def _image_loss_inputs(rgba, img, mask_img):
     return mask_img.reshape(N, H, W)
 
 
-def image_loss_torch(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0):
+def image_loss_torch(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0, group=None):
     """Trainer.calc_dr_loss (trainer.py:332-376) in torch ops, line for line, its host synchronisations included (the
-    ``mask_pred.sum() > 0`` branch and the boolean index); any dtype and device.  The float64 reference of the tests."""
+    ``mask_pred.sum() > 0`` branch and the boolean index); any dtype and device.  The float64 reference of the tests.
+
+    ``group``: a torch.distributed process group whose ranks each hold some of the views (any number, 0 included):
+    the loss is then the one over all their views, the same on every rank, and each rank's ``rgba`` receives its
+    views' share of the gradient (see :func:`image_loss`)."""
+    if group is not None:
+        return _image_loss_torch_sharded(rgba, img, mask_img, lambda_rgb, lambda_silhouette, group)
     mask_img = _image_loss_inputs(rgba, img, mask_img)
     img_pred, mask_img_pred = rgba[..., :3], rgba[..., 3]
     zero = rgba.new_zeros(())
@@ -499,6 +505,42 @@ def image_loss_torch(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0)
             "loss_dr_silhouette": loss_dr_silhouette, "loss_image_gradients": zero}
 
 
+def _image_loss_torch_sharded(rgba, img, mask_img, lambda_rgb, lambda_silhouette, group):
+    """image_loss_torch over the views of all the ranks of ``group``: the rank's sums (M, sum |d rgb| over mask_pred,
+    sum |m - alpha|, sum_n iou_n, its view count) are summed over the ranks, the loss values are formed from those sums
+    and the gradient is that of this rank's terms, the normalisers (M, the view count) held constant"""
+    import torch.distributed as dist
+    mask_img = _image_loss_inputs(rgba, img, mask_img, min_views=0)
+    N, H, W = rgba.shape[:3]
+    img_pred, mask_img_pred = rgba[..., :3], rgba[..., 3]
+    mask_pred = mask_img.bool() & mask_img_pred.bool()
+    s_rgb = (img - img_pred).abs()[mask_pred].sum()
+    s_sil = (mask_img.float() - mask_img_pred).abs().sum()
+    dims = (1, 2)
+    intersect = (mask_img.float() * mask_img_pred).sum(dims)
+    union = (mask_img.float() + mask_img_pred - mask_img.float() * mask_img_pred).sum(dims)
+    s_iou = (1.0 - intersect / eps_denom(union)).sum()
+    row = torch.stack([mask_pred.sum().to(torch.float64), s_rgb.detach().to(torch.float64),
+                       s_sil.detach().to(torch.float64), s_iou.detach().to(torch.float64),
+                       torch.tensor(float(N), dtype=torch.float64, device=rgba.device)])
+    dist.all_reduce(row, op=dist.ReduceOp.SUM, group=group)
+    M, n_views = float(row[0]), float(row[4])
+
+    def term(value, local):      # the value over all ranks, the gradient of this rank's share
+        return value.to(rgba.dtype) + (local - local.detach())
+
+    zero = rgba.new_zeros(())
+    loss_dr_silhouette = zero
+    loss_dr_rgb = zero
+    if lambda_rgb > 0 and M > 0:
+        loss_dr_rgb = term(row[1] / M * lambda_rgb, s_rgb / M * lambda_rgb)
+    if lambda_silhouette > 0:
+        value = (0.01 * (row[3] / n_views) + row[2] / (n_views * H * W)) * lambda_silhouette
+        loss_dr_silhouette = term(value, (0.01 * (s_iou / n_views) + s_sil / (n_views * H * W)) * lambda_silhouette)
+    return {"loss": loss_dr_rgb + loss_dr_silhouette + zero, "loss_dr_rgb": loss_dr_rgb,
+            "loss_dr_silhouette": loss_dr_silhouette, "loss_image_gradients": zero}
+
+
 def _image_loss_call(name, rgba, img, mask, lambda_rgb, lambda_sil, *tail):
     N, H, W = rgba.shape[:3]
     dev = rgba.device
@@ -512,15 +554,30 @@ def _image_loss_call(name, rgba, img, mask, lambda_rgb, lambda_sil, *tail):
 
 class _ImageLoss(torch.autograd.Function):
     """dss_image_loss_forward (the three loss scalars and the per-view totals) and dss_image_loss_backward (the RGBA
-    gradient, from the upstream gradients of the three scalars on the device)."""
+    gradient, from the upstream gradients of the three scalars on the device).  With a process group:
+    dss_image_loss_partial, the total row summed over the ranks (one all-reduce of 5 doubles), dss_image_loss_finish;
+    the backward reads the summed row."""
 
     @staticmethod
-    def forward(ctx, rgba, img, mask, lambda_rgb, lambda_sil):
-        N, dev = rgba.shape[0], rgba.device
+    def forward(ctx, rgba, img, mask, lambda_rgb, lambda_sil, group=None):
+        (N, H, W), dev = rgba.shape[:3], rgba.device
         totals = torch.empty((N + 1, 5), dtype=torch.float64, device=dev)
         loss, loss_rgb, loss_sil = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(3))
-        _image_loss_call("dss_image_loss_forward", rgba, img, mask, lambda_rgb, lambda_sil, totals, loss, loss_rgb,
-                         loss_sil)
+        if group is None:
+            _image_loss_call("dss_image_loss_forward", rgba, img, mask, lambda_rgb, lambda_sil, totals, loss, loss_rgb,
+                             loss_sil)
+        else:
+            import torch.distributed as dist
+            if N:
+                _image_loss_call("dss_image_loss_partial", rgba, img, mask, lambda_rgb, lambda_sil, totals)
+            else:
+                totals.zero_()
+            dist.all_reduce(totals[N], op=dist.ReduceOp.SUM, group=group)
+            with torch.cuda.device(dev):
+                rc = _lib.load().dss_image_loss_finish(_lib.ctx(dev), _lib.ptr(totals[N]), H, W, float(lambda_rgb),
+                                                       float(lambda_sil), _lib.ptr(loss), _lib.ptr(loss_rgb),
+                                                       _lib.ptr(loss_sil), _lib.stream_ptr(dev))
+            _lib.check(rc, "dss_image_loss_finish")
         ctx.lambdas = (lambda_rgb, lambda_sil)
         ctx.save_for_backward(rgba, img, mask, totals)
         return loss, loss_rgb, loss_sil
@@ -529,9 +586,10 @@ class _ImageLoss(torch.autograd.Function):
     def backward(ctx, g_loss, g_rgb, g_sil):
         rgba, img, mask, totals = ctx.saved_tensors
         grad = torch.empty_like(rgba, memory_format=torch.contiguous_format)
-        ups = [g.to(torch.float32).contiguous() for g in (g_loss, g_rgb, g_sil)]
-        _image_loss_call("dss_image_loss_backward", rgba, img, mask, *ctx.lambdas, totals, *ups, grad)
-        return grad, None, None, None, None
+        if rgba.shape[0]:
+            ups = [g.to(torch.float32).contiguous() for g in (g_loss, g_rgb, g_sil)]
+            _image_loss_call("dss_image_loss_backward", rgba, img, mask, *ctx.lambdas, totals, *ups, grad)
+        return grad, None, None, None, None, None
 
 
 def fused_image_loss_targets(img, mask_img):
@@ -542,7 +600,7 @@ def fused_image_loss_targets(img, mask_img):
         and not img.requires_grad and not mask_img.requires_grad
 
 
-def image_loss(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0):
+def image_loss(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0, group=None):
     """The image loss of the training step, ``Trainer.calc_dr_loss`` (trainer.py:332-376) on the renderer's RGBA:
     the masked RGB L1 (``L1Loss``, mean over the pixels where both masks are non-zero) times ``lambda_rgb`` and the
     silhouette L1 plus 0.01 x ``IouLoss`` times ``lambda_silhouette``; a term whose lambda is not > 0 is absent.
@@ -554,15 +612,21 @@ def image_loss(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0):
 
     float32 CUDA inputs take the fused route (csrc/image_loss.cu: two launches forward, one backward, no host
     synchronisation, bit-reproducible), which differentiates ``rgba``; every other dtype or device, and targets that
-    require grad, run :func:`image_loss_torch`."""
-    mask = _image_loss_inputs(rgba, img, mask_img)
+    require grad, run :func:`image_loss_torch`.
+
+    ``group``: a torch.distributed process group whose ranks each hold some of the N views of one batch (a rank may
+    hold none: N = 0 there).  Every rank must call with the same lambdas and H x W.  The loss is then the one over all
+    the views -- M, N·H·W and the view count summed over the ranks, one all-reduce of 5 doubles -- the same values on
+    every rank, and each rank's ``rgba`` receives the gradient of its own views.  The fused route makes one launch more
+    than without a group and still no host synchronisation."""
+    mask = _image_loss_inputs(rgba, img, mask_img, min_views=0 if group is not None else 1)
     if not (rgba.is_cuda and rgba.dtype == torch.float32 and fused_image_loss_targets(img, mask)):
-        return image_loss_torch(rgba, img, mask_img, lambda_rgb, lambda_silhouette)
+        return image_loss_torch(rgba, img, mask_img, lambda_rgb, lambda_silhouette, group=group)
     lambda_rgb, lambda_silhouette = float(lambda_rgb), float(lambda_silhouette)
     rgba_c = rgba.contiguous()
     if rgba_c.data_ptr() % 16:
         rgba_c = rgba_c.clone()
     mask = mask.contiguous()
-    loss, loss_rgb, loss_sil = _ImageLoss.apply(rgba_c, img, mask, lambda_rgb, lambda_silhouette)
+    loss, loss_rgb, loss_sil = _ImageLoss.apply(rgba_c, img, mask, lambda_rgb, lambda_silhouette, group)
     zero = torch.zeros((), dtype=torch.float32, device=rgba.device)
     return {"loss": loss, "loss_dr_rgb": loss_rgb, "loss_dr_silhouette": loss_sil, "loss_image_gradients": zero}

@@ -16,7 +16,9 @@ passed in, the ones named in ``learn`` requiring grad); the optimizer stays with
 place.  ``step.loss`` holds the trainer's loss dict as device scalars, ``step.image`` the render, ``step.visibility`` and
 ``step.inmask`` the (P0,) filters.
 
-:class:`TrainStep` runs the step eagerly.  :class:`GraphedTrainStep` captures it once in a CUDA graph: every piece is
+:class:`TrainStep` runs the step eagerly, on one GPU or, with a ``GradSync`` of world size G > 1, view-sharded over G
+ranks: each rank holds the whole cloud and passes its own views, and every rank finishes with the loss, filters and
+gradients of one step over all the views.  :class:`GraphedTrainStep` runs on one GPU.  :class:`GraphedTrainStep` captures it once in a CUDA graph: every piece is
 free of host synchronisation, so one replay computes the whole step.  Between replays ``load()`` copies the next batch
 into the step's static inputs.  Host-side settings are frozen into a capture; when one of them changes (``params``, e.g.
 its ``radii_backward_scaler``, which the trainer's scheduler lowers, or a lambda), or when another library call has
@@ -25,6 +27,7 @@ reallocated the scratch buffers the graph uses, the next ``replay()`` captures a
 import ctypes as C
 
 import torch
+import torch.distributed as dist
 import torch.nn.functional as F
 
 from .. import _lib
@@ -32,7 +35,7 @@ from ..core.cloud import PointClouds3D, PointCloudsFilters
 from ..core.lighting import pack_lights
 from ..core.rasterizer import point_sq_spacing, splat_variance_scale
 from ..core.texture import camera_centres
-from ..ops import Shading, SplatParams, point_filters, render_points
+from ..ops import Shading, SplatParams, point_filters, point_filters_no_views, render_points
 from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
 
 __all__ = ["TrainStep", "GraphedTrainStep"]
@@ -46,7 +49,17 @@ class TrainStep:
     ``configs/dss.yml``'s.  ``step(img, mask_img, proj, view, lights)`` runs the step on a batch and returns the loss dict:
     ``img`` (N,H,W,3) float32 ground truth (any strides), ``mask_img`` (N,H,W) or (N,1,H,W) float32, uint8 or bool,
     ``proj`` / ``view`` (N,4,4) as ``render_points`` takes them, ``lights`` a ``DirectionalLights`` / ``PointLights``
-    of batch 1 or N (dss_b200.core.lighting)."""
+    of batch 1 or N (dss_b200.core.lighting).
+
+    ``grad_sync``: a ``dss_b200.parallel.GradSync`` of world size G > 1 shards the step by views.  Every rank builds its
+    TrainStep from the same cloud and settings and calls ``step`` with its own views (``assign_views`` deals them; a
+    rank may hold none: pass tensors of batch 0, its lights are not read), in the same order as the other ranks.
+    The loss is the one over all the views (image-loss sums, one all-reduce of 5 doubles), the point filters those of
+    all the views (two all-reduces of P0 bytes), the render gradients arrive summed over the ranks through
+    ``GradSync``, and the regularisers run replicated on every rank: each rank ends with the same ``step.loss``,
+    ``step.visibility``, ``step.inmask`` and gradients on its leaves, so identical optimizer steps keep the replicas
+    identical.  The ranks must agree on P0, the kind of lights, the lambdas and ``params``; that is not checked (it would
+    take a host synchronisation).  With G = 1 or no ``grad_sync`` the step runs as on one GPU."""
 
     def __init__(self, points, normals, colours, params: SplatParams, *, learn=("points", "normals"),
                  Vrk_invariant=True, frnn_radius=0.2, shininess=64.0, lambda_dr_rgb=1.0, lambda_dr_silhouette=1.0,
@@ -58,9 +71,10 @@ class TrainStep:
                 raise RuntimeError("%s must be a float32 (P0, 3) tensor, got %s %s" % (name, t.dtype, tuple(t.shape)))
         if any(name not in _LEARNABLE for name in learn):
             raise ValueError("learn takes names out of %s, got %s" % (_LEARNABLE, tuple(learn)))
-        if grad_sync is not None and grad_sync.world_size > 1:
-            raise NotImplementedError("the training step does not take the multi-GPU gradient exchange; call "
-                                      "render_points(..., grad_sync=...) eagerly")
+        self._sync = grad_sync if grad_sync is not None and grad_sync.world_size > 1 else None
+        # image_loss and point_filters take None as "not sharded": GradSync's default group is named explicitly
+        self._group = None if self._sync is None else (grad_sync.group if grad_sync.group is not None
+                                                       else dist.group.WORLD)
         self.device = dev
         leaf = lambda t, name: t.detach().clone().requires_grad_(name in learn)
         self.points, self.normals, self.colours = leaf(points, "points"), leaf(normals, "normals"), \
@@ -95,6 +109,8 @@ class TrainStep:
 
     def __call__(self, img, mask_img, proj, view, lights):
         self._check_batch(img, mask_img, proj, view)
+        if self._sync is not None and proj.shape[0] == 0:
+            return self._run(img, mask_img, proj, view, None, None, None)
         rows, ambient, kind = pack_lights(lights)
         return self._run(img, mask_img, proj, view, rows.detach(), ambient.detach(), kind)
 
@@ -103,13 +119,25 @@ class TrainStep:
             t.grad = None
         N, dev = proj.shape[0], self.device
         normals = F.normalize(self.normals, dim=-1)
-        with torch.no_grad():
-            # the one cloud's spacing, the rule of SurfaceSplatting._compute_h for its N views
-            h = splat_variance_scale([point_sq_spacing(self.points, self.frnn_radius)], self.Vrk_invariant).repeat(N)
-        shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
-        out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading)
-        loss = image_loss(out.image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette)
-        visibility, inmask = point_filters(out, mask_img)
+        if N == 0:
+            # a rank of a view-sharded step without views: the collectives of the others, with zero contributions
+            S = int(self.params.image_size)
+            image = torch.zeros((0, S, S, 4), dtype=torch.float32, device=dev)
+            loss = image_loss(image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette, group=self._group)
+            visibility, inmask = point_filters_no_views(self.points.shape[0], dev, self._group)
+            rendered = _NoViews.apply(self.points, normals, self.colours, self._sync)
+        else:
+            with torch.no_grad():
+                # the one cloud's spacing, the rule of SurfaceSplatting._compute_h for its N views
+                h = splat_variance_scale([point_sq_spacing(self.points, self.frnn_radius)],
+                                         self.Vrk_invariant).repeat(N)
+            shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
+            out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading,
+                                grad_sync=self._sync)
+            loss = image_loss(out.image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette,
+                              group=self._group)
+            visibility, inmask = point_filters(out, mask_img, group=self._group)
+            image, rendered = out.image, None
         cloud = PointClouds3D([self.points], [normals])
         cloud._cache["num"] = self._num
         points_filter = PointCloudsFilters(dev, visibility=visibility[None], inmask=inmask[None])
@@ -124,12 +152,37 @@ class TrainStep:
                 reg[key] = fn(cloud, rebuild_knn=True, points_filter=points_filter) * lam
         # trainer.py:313: loss = proj + repel + the image loss
         total = reg["loss_dr_proj"] + reg["loss_dr_repel"] + loss["loss"]
+        if rendered is not None:
+            total = total + rendered
         total.backward()
         self.loss = {"loss": total.detach(), "loss_dr_rgb": loss["loss_dr_rgb"].detach(),
                      "loss_dr_silhouette": loss["loss_dr_silhouette"].detach(),
                      "loss_dr_proj": reg["loss_dr_proj"].detach(), "loss_dr_repel": reg["loss_dr_repel"].detach()}
-        self.image, self.visibility, self.inmask = out.image.detach(), visibility, inmask
+        self.image, self.visibility, self.inmask = image.detach(), visibility, inmask
         return self.loss
+
+
+class _NoViews(torch.autograd.Function):
+    """The render of a view-sharded step's rank that holds no views: 0 forward; backward, the all-reduces that
+    render_points' backward makes through GradSync (d albedo and d normal on its side stream, then d position), with
+    zero contributions, so that this rank receives the other ranks' render gradients."""
+
+    @staticmethod
+    def forward(ctx, points, normals, albedo, sync):
+        ctx.sync, ctx.P0 = sync, points.shape[0]
+        return points.new_zeros(())
+
+    @staticmethod
+    def backward(ctx, grad):
+        sync, dev = ctx.sync, grad.device
+        g_points, g_normals, g_albedo = (torch.zeros((ctx.P0, 3), dtype=torch.float32, device=dev) for _ in range(3))
+        main, side = torch.cuda.current_stream(dev), sync.side_stream(dev)
+        side.wait_stream(main)
+        with torch.cuda.stream(side):
+            sync.reduce_early(g_albedo, g_normals)
+        sync.reduce_late(g_points)
+        sync.join(dev)
+        return g_points, g_normals, g_albedo, None
 
 
 class GraphedTrainStep(TrainStep):
@@ -153,6 +206,10 @@ class GraphedTrainStep(TrainStep):
 
     def __init__(self, points, normals, colours, params: SplatParams, img, mask_img, proj, view, lights, warmup=3,
                  **settings):
+        sync = settings.get("grad_sync")
+        if sync is not None and sync.world_size > 1:
+            raise NotImplementedError("GraphedTrainStep runs on one GPU; a view-sharded step runs eagerly: "
+                                      "TrainStep(..., grad_sync=...)")
         super().__init__(points, normals, colours, params, **settings)
         self._check_batch(img, mask_img, proj, view)
         rows, ambient, self._light_type = pack_lights(lights)

@@ -236,7 +236,13 @@ DSS_API int dss_surface_regulariser(dss_ctx *ctx, int kind, const float *points,
  * the three scalars (device f32 scalars): rgb sign(pred - gt) lambda_rgb (g_loss + g_rgb) / M inside mask_pred, else 0;
  * alpha lambda_sil (g_loss + g_sil) (sign(alpha - m) / (N H W) - 0.01 (m E_n - I_n (1 - m) dE_n) / (N E_n^2)) with
  * E_n = eps_denom(U_n) and dE_n = [|U_n| >= 1e-17]; sign(0) = sign(NaN) = 0, as torch's abs backward.
- * Deterministic: fixed-order fp64 sums, no float atomics; no host synchronisation; partial sums in context scratch. */
+ * Deterministic: fixed-order fp64 sums, no float atomics; no host synchronisation; partial sums in context scratch.
+ * View-sharded loss (each rank holds some of the views, the loss is the one over all of them): dss_image_loss_partial
+ * (2 launches) writes the rank's totals as dss_image_loss_forward does, no scalars, and N in row N's fifth slot; the
+ * caller sums row N over the ranks (5 doubles) and dss_image_loss_finish (1 launch) writes the three scalars from the
+ * summed row: M and N above are then the sums over all ranks (at least one view in all).  dss_image_loss_backward on
+ * these totals takes its M and N from the summed row (a non-zero fifth slot replaces its own N) and I_n, U_n from the
+ * rank's view rows. */
 DSS_API int dss_image_loss_forward(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
                                    const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb,
                                    double lambda_sil, double *totals, float *loss, float *loss_rgb, float *loss_sil,
@@ -246,6 +252,11 @@ DSS_API int dss_image_loss_backward(dss_ctx *ctx, const float *pred, const float
                                     double lambda_sil, const double *totals, const float *grad_loss,
                                     const float *grad_loss_rgb, const float *grad_loss_sil, float *grad_pred,
                                     void *stream);
+DSS_API int dss_image_loss_partial(dss_ctx *ctx, const float *pred, const float *gt, const int64_t *gt_strides,
+                                   const void *mask, int mask_kind, int N, int H, int W, double lambda_rgb,
+                                   double lambda_sil, double *totals, void *stream);
+DSS_API int dss_image_loss_finish(dss_ctx *ctx, const double *total_row, int H, int W, double lambda_rgb,
+                                  double lambda_sil, float *loss, float *loss_rgb, float *loss_sil, void *stream);
 
 /* ---- point filters of the training step -------------------------------------------------------------------------
  * Model.forward's visibility and inmask filters (DSS/models/point_modeling.py:172-173, 188-212) of one SHARED cloud of
@@ -257,10 +268,17 @@ DSS_API int dss_image_loss_backward(dss_ctx *ctx, const float *pred, const float
  * padding, align_corners = False), its arithmetic restated in ATen's order.  A non-finite x or y is outside the mask.
  * mask n at mask[n*s0 + y*s1 + x*s2], mask_strides = {s0, s1, s2} (host array, in elements), H x W independent of the
  * render size, f32 (mask_kind 0) or bytes (mask_kind 1: bool / uint8).  Outputs (P0,) bytes, 0 or 1.
- * One launch, one thread per point; deterministic; no scratch, no host synchronisation. */
+ * One launch, one thread per point; deterministic; no scratch, no host synchronisation.
+ * dss_point_filters_gated: the same with visibility[i] = visibility_gate[i] != 0 in place of the any over this call's
+ * views (NULL: as dss_point_filters).  A view-sharded step passes the visibility ORed over the ranks, so that inmask
+ * ORed over the ranks is the filter of all the views. */
 DSS_API int dss_point_filters(dss_ctx *ctx, const float *records, const uint8_t *visible, int shared_cloud, int N,
                               int64_t P0, const void *mask, int mask_kind, const int64_t *mask_strides, int H, int W,
                               uint8_t *visibility, uint8_t *inmask, void *stream);
+DSS_API int dss_point_filters_gated(dss_ctx *ctx, const float *records, const uint8_t *visible, int shared_cloud,
+                                    int N, int64_t P0, const void *mask, int mask_kind, const int64_t *mask_strides,
+                                    int H, int W, const uint8_t *visibility_gate, uint8_t *visibility,
+                                    uint8_t *inmask, void *stream);
 
 /* ---- fused renderer path (what bench.py times) ----------------------------------------------
  * One call per direction for SurfaceSplattingRenderer.forward / its autograd backward
