@@ -46,6 +46,7 @@ class RenderArgs(C.Structure):
         ("albedo", vp), ("lights", vp), ("ambient", vp), ("cam_centres", vp), ("shaded", vp),
         ("grad_albedo", vp), ("grad_normals_world", vp), ("grad_points_shading", vp),
         ("cell_counts", vp),
+        ("frames", vp),
     ]
 
 
@@ -80,6 +81,7 @@ _SIGNATURES = {
     "dss_zbuf_backward": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int, vp, vp]),
     "dss_knn_points": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_float,
                                  vp, vp, vp]),
+    "dss_local_frames": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int64, vp, vp, vp]),
     "dss_surface_regulariser": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int64, vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp, C.c_float, C.c_float, vp, vp, vp]),
     "dss_image_loss_forward": (C.c_int, [vp, vp, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,

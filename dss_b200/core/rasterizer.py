@@ -17,13 +17,13 @@ import torch.autograd as autograd
 import torch.nn as nn
 
 from .. import _C
-from ..ops import SplatParams, preprocess_points
+from ..ops import LOCAL_FRAME_K, SplatParams, local_frames, preprocess_points
 from .camera import camera_matrices
 from .cloud import clouds_share_points
 from .knn import knn_sq_dists
 
 __all__ = ["PointFragments", "PointsRasterizationSettings", "SurfaceSplatting", "rasterize_elliptical_points",
-           "EllipticalRasterizer", "kMaxPointsPerBin", "point_sq_spacing", "splat_variance_scale"]
+           "EllipticalRasterizer", "kMaxPointsPerBin", "point_sq_spacing", "splat_variance_scale", "cloud_frames"]
 
 kMaxPointsPerBin = 22   # pytorch3d constant the reference (mis)uses as a bound on bins per side (rasterizer.py:725-730)
 
@@ -95,6 +95,20 @@ def splat_variance_scale(per_cloud, Vrk_invariant):
     return torch.cat(per_cloud).clamp(5e-5, 0.01).float()
 
 
+def cloud_frames(point_clouds, shared):
+    """The anisotropic kernel's :func:`local_frames` of a batch of clouds: of the one cloud when ``shared`` (every view
+    renders the same points: (P0,8)), else of every cloud of the packed batch ((P,8)).  A cloud of at most 8 points raises
+    ValueError, as mathHelper.py:57-61 does (the counts are read on the host, as there)."""
+    num = point_clouds.num_points_per_cloud()
+    counts = [int(c) for c in num.tolist()]
+    if min(counts) <= LOCAL_FRAME_K:
+        raise ValueError("the anisotropic kernel (Vrk_invariant and Vrk_isotropic off) needs clouds of more than %d "
+                         "points (the neighbourhood size), got %d" % (LOCAL_FRAME_K, min(counts)))
+    if shared:
+        return local_frames(point_clouds.points_list()[0])
+    return local_frames(point_clouds.points_packed(), point_clouds.cloud_to_packed_first_idx(), num)
+
+
 class SurfaceSplatting(nn.Module):
     """rasterizer.py:102-664.  Outputs per point the screen-space extent and centre of projection, and per
     pixel the K nearest splats."""
@@ -143,12 +157,13 @@ class SurfaceSplatting(nn.Module):
     def _compute_h(self, point_clouds, refresh=True, **kwargs):
         """Variance scale of the reconstruction kernel (rasterizer.py:293-402):
         Vrk_invariant: per view h = clamp(mean_p(0.5 max_{6NN} d^2), 5e-5, 1e-3)          -> (N,)
-        Vrk_isotropic: per point h_p = clamp(0.5 max_{6NN} d^2, 5e-5, 0.01), cached        -> (P,)"""
+        Vrk_isotropic: per point h_p = clamp(0.5 max_{6NN} d^2, 5e-5, 0.01), cached        -> (P,)
+        neither (anisotropic, rasterizer.py:256-291): no h                                 -> None
+        (the splat shape then comes from :meth:`_compute_frames`)"""
         rs = kwargs.get("raster_settings", self.raster_settings)
         num = point_clouds.num_points_per_cloud()
         if not (rs.Vrk_invariant or rs.Vrk_isotropic):
-            raise NotImplementedError("anisotropic Vrk (curvature frames + batched SVD, rasterizer.py:256-291) "
-                                      "is outside the hot path; use Vrk_invariant or Vrk_isotropic")
+            return None
         if (not rs.Vrk_invariant and not refresh and self._Vrk_h is not None
                 and self._Vrk_h.shape[0] == int(num.sum())):
             return self._Vrk_h
@@ -162,6 +177,12 @@ class SurfaceSplatting(nn.Module):
             self._Vrk_h = h
         return h
 
+    def _compute_frames(self, point_clouds, shared=False):
+        """Anisotropic kernel (``Vrk_invariant`` and ``Vrk_isotropic`` off, rasterizer.py:256-291): the
+        :func:`local_frames` records of the clouds, recomputed every forward as in the reference; (P0,8) of the one
+        cloud when ``shared``, else (P,8) packed.  Clouds of at most 8 points raise ValueError (mathHelper.py:57-61)."""
+        return cloud_frames(point_clouds, shared)
+
     def _get_per_point_info(self, point_clouds, **kwargs):
         """radii (P,2), ellipse_params (P,3), cutoff_threshold (P,), scaler (P,) -- rasterizer.py:525-565,
         fused into one kernel (dss_preprocess).  Also returns ``ndc`` whose z is -1 for filtered points."""
@@ -172,13 +193,21 @@ class SurfaceSplatting(nn.Module):
         h = kwargs.get("Vrk_h", None)
         if h is None:
             h = self._compute_h(point_clouds, **kwargs)
+        frames = None
+        if h is None:
+            # anisotropic: the frames of every (view's) cloud, indexed like the packed points
+            shared = clouds_share_points(point_clouds) and len(point_clouds) > 1
+            frames = self._compute_frames(point_clouds, shared)
+            if shared:
+                frames = frames.repeat(len(point_clouds), 1)
         normals = point_clouds.normals_packed()
         if normals is None:
             raise ValueError("surface splatting needs point normals")
         prm = _splat_params(rs, cameras, kwargs)
-        return preprocess_points(point_clouds.points_packed(), normals, proj.to(dev), view.to(dev), h.to(dev), prm,
+        return preprocess_points(point_clouds.points_packed(), normals, proj.to(dev), view.to(dev),
+                                 h.to(dev) if h is not None else None, prm,
                                  first_idx=point_clouds.cloud_to_packed_first_idx(),
-                                 num_points=point_clouds.num_points_per_cloud(), shared_cloud=False)
+                                 num_points=point_clouds.num_points_per_cloud(), shared_cloud=False, frames=frames)
 
     def _empty_fragments(self, batch_size, **kwargs):
         rs = kwargs.get("raster_settings", self.raster_settings)

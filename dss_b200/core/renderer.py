@@ -61,20 +61,27 @@ class SurfaceSplattingRenderer(nn.Module):
         dev = point_clouds.device
         proj, view = camera_matrices(cameras)
         prm = _splat_params(rs, cameras, kwargs)
+        shared = clouds_share_points(point_clouds) and clouds_equal_sized(point_clouds)
+        frames = None
         with torch.no_grad():
             h = kwargs.get("Vrk_h", None)
             if h is None:
                 h = rast._compute_h(point_clouds, **kwargs)
+            if h is None:
+                # anisotropic splats: the frames of the one cloud (shared) or of every packed cloud
+                frames = rast._compute_frames(point_clouds, shared)
+            else:
+                h = h.to(dev)
         feats = point_clouds.features_packed()[:, :3].contiguous()
         verbose = kwargs.get("verbose", False)
-        if clouds_share_points(point_clouds) and clouds_equal_sized(point_clouds):
+        if shared:
             out = render_points(point_clouds.points_list()[0], point_clouds.normals_list()[0], feats, proj.to(dev),
-                                view.to(dev), h.to(dev), prm, shared_cloud=True, return_fragments=verbose)
+                                view.to(dev), h, prm, shared_cloud=True, return_fragments=verbose, frames=frames)
         else:
             out = render_points(point_clouds.points_packed(), point_clouds.normals_packed(), feats, proj.to(dev),
-                                view.to(dev), h.to(dev), prm, first_idx=point_clouds.cloud_to_packed_first_idx(),
+                                view.to(dev), h, prm, first_idx=point_clouds.cloud_to_packed_first_idx(),
                                 num_points=point_clouds.num_points_per_cloud(), shared_cloud=False,
-                                return_fragments=verbose)
+                                return_fragments=verbose, frames=frames)
         pcf = kwargs.get("point_clouds_filter", None)
         if pcf is not None:
             num = point_clouds.num_points_per_cloud()

@@ -151,10 +151,14 @@ __device__ __forceinline__ V3 shade_point(const float *sL, int n_lights, int lig
 // exactly like the reference treats points behind the camera (rasterize_points.cu:87-88).
 // rec: the (P,2) records (g.records or context scratch); zrange: (N,2) float bits, min / max view depth of the
 // renderable splats, or null.  SHADE: write the shaded colour of every (view, point) to g.shaded.
+// FRAMES (anisotropic splats, rasterizer.py:256-291, 425-439): the world variance is l1 f1 f1^T + l2 f2 f2^T from the
+// g.frames record of the point instead of h (I - n n^T); with u = (f1.J0, f1.J1), v = (f2.J0, f2.J1):
+//   Vk = l1 u u^T + l2 v v^T,   |det Mk| = |u0 v1 - u1 v0|
+// and the rest (G = Vk + aa I, conic, radii, scaler, filters, shading) is shared.  The body is one inlined function
+// so that the two kernels without frames keep the code they had.
 // ---------------------------------------------------------------------------------------------
-template <bool SHADE>
-__global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__ dss_render_args g, float4 *rec,
-                                                         int32_t *zrange) {
+template <bool SHADE, bool FRAMES>
+__device__ __forceinline__ void preprocess_splats(const dss_render_args &g, float4 *rec, int32_t *zrange) {
     __shared__ float sM[16], sV[16];
     __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
     const int n = blockIdx.y;
@@ -191,14 +195,29 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
             J0[k] = sM[k * 4 + 0] * it - sM[k * 4 + 3] * x * it2;
             J1[k] = sM[k * 4 + 1] * it - sM[k * 4 + 3] * y * it2;
         }
-        // T = J^T (I - n n^T) J
-        const float nj0 = n0 * J0[0] + n1 * J0[1] + n2 * J0[2];
-        const float nj1 = n0 * J1[0] + n1 * J1[1] + n2 * J1[2];
-        const float T00 = (J0[0] * J0[0] + J0[1] * J0[1] + J0[2] * J0[2]) - nj0 * nj0;
-        const float T01 = (J0[0] * J1[0] + J0[1] * J1[1] + J0[2] * J1[2]) - nj0 * nj1;
-        const float T11 = (J1[0] * J1[0] + J1[1] * J1[1] + J1[2] * J1[2]) - nj1 * nj1;
-        const float hh = g.h_per_splat ? g.h[s] : g.h[n];
-        const float G00 = fmaf(hh, T00, aa), G01 = hh * T01, G11 = fmaf(hh, T11, aa);
+        float G00, G01, G11;
+        float T00, T01, T11;        // without frames: T = J^T (I - n n^T) J
+        float u0, u1, v0, v1;       // with frames: Sk WJk = [u; v]
+        if (FRAMES) {
+            // u_k = f1.J_k, v_k = f2.J_k (rasterizer.py:289-291, 428-439)
+            const float4 fa = reinterpret_cast<const float4 *>(g.frames)[2 * src];
+            const float4 fb = reinterpret_cast<const float4 *>(g.frames)[2 * src + 1];
+            u0 = fa.x * J0[0] + fa.y * J0[1] + fa.z * J0[2];
+            u1 = fa.x * J1[0] + fa.y * J1[1] + fa.z * J1[2];
+            v0 = fb.x * J0[0] + fb.y * J0[1] + fb.z * J0[2];
+            v1 = fb.x * J1[0] + fb.y * J1[1] + fb.z * J1[2];
+            G00 = fmaf(fa.w * u0, u0, fmaf(fb.w * v0, v0, aa));
+            G01 = fmaf(fa.w * u0, u1, fb.w * v0 * v1);
+            G11 = fmaf(fa.w * u1, u1, fmaf(fb.w * v1, v1, aa));
+        } else {
+            const float nj0 = n0 * J0[0] + n1 * J0[1] + n2 * J0[2];
+            const float nj1 = n0 * J1[0] + n1 * J1[1] + n2 * J1[2];
+            T00 = (J0[0] * J0[0] + J0[1] * J0[1] + J0[2] * J0[2]) - nj0 * nj0;
+            T01 = (J0[0] * J1[0] + J0[1] * J1[1] + J0[2] * J1[2]) - nj0 * nj1;
+            T11 = (J1[0] * J1[0] + J1[1] * J1[1] + J1[2] * J1[2]) - nj1 * nj1;
+            const float hh = g.h_per_splat ? g.h[s] : g.h[n];
+            G00 = fmaf(hh, T00, aa), G01 = hh * T01, G11 = fmaf(hh, T11, aa);
+        }
         const float detG = G00 * G11 - G01 * G01;
         const float idet = rcp_approx(detG);
         const float ea = G11 * idet, eb = -2.0f * G01 * idet, ec = G00 * idet;   // rasterizer.py:543-551
@@ -206,8 +225,9 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
         const float iden = rcp_approx(den);
         const float ry = fast_sqrt(py_eps_sqrt(4.0f * ea * g.cutoff_threshold * iden));
         const float rx = fast_sqrt(py_eps_sqrt(4.0f * ec * g.cutoff_threshold * iden));
-        const float detT = fmaxf(T00 * T11 - T01 * T01, 0.0f);
-        const float sc = fast_sqrt(detT) *
+        // |det Mk|: sqrt(det T) = |det(Sk WJk)| for the orthonormal tangent frame of I - n n^T
+        const float detM = FRAMES ? fabsf(u0 * v1 - u1 * v0) : fast_sqrt(fmaxf(T00 * T11 - T01 * T01, 0.0f));
+        const float sc = detM *
                          rcp_approx(py_eps_denom(fast_sqrt(py_eps_sqrt(detG * (4.0f * CUDART_PI_F * CUDART_PI_F)))));  // :558-559
         // filters (rasterizer.py:187-192, :152): view-space depth range, optional backface
         bool keep = (zv >= g.znear) && (zv <= g.zfar);
@@ -270,6 +290,18 @@ __global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__
             atomicMax(&zrange[2 * n + 1], zhi);
         }
     }
+}
+
+template <bool SHADE>
+__global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__ dss_render_args g, float4 *rec,
+                                                         int32_t *zrange) {
+    preprocess_splats<SHADE, false>(g, rec, zrange);
+}
+
+template <bool SHADE>
+__global__ void __launch_bounds__(256) preprocess_frames_kernel(const __grid_constant__ dss_render_args g, float4 *rec,
+                                                                int32_t *zrange) {
+    preprocess_splats<SHADE, true>(g, rec, zrange);
 }
 
 // d L / d shaded (N*P0,3) -> d albedo, d normal, d position (through the shading) per world point, summed over the views:
@@ -410,12 +442,21 @@ static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, c
         if (rc) return rc;
     }
     if (g->P == 0 || g->P0 == 0) return DSS_OK;
-    DSS_REQUIRE(g->points_world && g->normals_world && g->proj && g->view && g->h, "null input array");
+    DSS_REQUIRE(g->points_world && g->normals_world && g->proj && g->view && (g->h || g->frames), "null input array");
+    DSS_REQUIRE(!(g->h && g->frames), "pass exactly one of h and frames");
+    DSS_REQUIRE(!g->frames || (reinterpret_cast<uintptr_t>(g->frames) & 15) == 0, "frames must be 16-byte aligned");
     int32_t *zr = reinterpret_cast<int32_t *>(zrange);
     dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 8), g->n_views);
     StageScope prof(ctx, ST_PREPROCESS, st);
-    if (g->shade && g->shaded) preprocess_kernel<true><<<grid, 256, 0, st>>>(*g, rec, zr);
-    else preprocess_kernel<false><<<grid, 256, 0, st>>>(*g, rec, zr);
+    const bool shade = g->shade && g->shaded;
+    if (g->frames) {
+        if (shade) preprocess_frames_kernel<true><<<grid, 256, 0, st>>>(*g, rec, zr);
+        else preprocess_frames_kernel<false><<<grid, 256, 0, st>>>(*g, rec, zr);
+    } else if (shade) {
+        preprocess_kernel<true><<<grid, 256, 0, st>>>(*g, rec, zr);
+    } else {
+        preprocess_kernel<false><<<grid, 256, 0, st>>>(*g, rec, zr);
+    }
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }

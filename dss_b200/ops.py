@@ -21,7 +21,7 @@ import torch
 from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
-           "point_filters", "point_filters_no_views", "set_point_filters"]
+           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames"]
 
 
 class SplatParams(NamedTuple):
@@ -127,19 +127,37 @@ def _layout(points, proj, first_idx, num_points, shared):
     return N, P, P   # P0 is only an upper bound on the points of one view in packed mode
 
 
+def _splat_shape(h, frames, rows, N, P):
+    """(h_c, frames_c) for the kernel: exactly one of the isotropic / invariant scale h ((N,) or (P,)) and the
+    anisotropic frames ((rows, 8) records of :func:`local_frames`, rows = P0 for a shared cloud, P packed)"""
+    if (h is None) == (frames is None):
+        raise RuntimeError("pass exactly one of h (isotropic / invariant splats) and frames (anisotropic splats)")
+    if frames is None:
+        h_c = _lib.as_f32(h.detach().reshape(-1), "h")
+        if h_c.numel() not in (N, P):
+            raise RuntimeError("h must have N or P elements")
+        return h_c, None
+    f = _lib.as_f32(frames.detach(), "frames")
+    if tuple(f.shape) != (rows, 8):
+        raise RuntimeError("frames must have shape (%d, 8), got %s" % (rows, tuple(f.shape)))
+    if f.data_ptr() % 16:
+        f = f.clone()
+    return None, f
+
+
 class _RenderFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, normals, colours, proj, view, h, first_idx, num_points, shared, prm, want_frags,
-                grad_sync=None, shading=None, cam_centres=None, lights=None, ambient=None):
+                grad_sync=None, shading=None, cam_centres=None, lights=None, ambient=None, frames=None):
         # cam_centres, lights and ambient are the shading's tensors, passed on their own so that autograd tracks them
-        dev = _lib.require_cuda(points, normals, colours, proj, view, h, first_idx, num_points)
+        dev = _lib.require_cuda(points, normals, colours, proj, view, h, first_idx, num_points, frames)
         points_c = _lib.as_f32(points.detach(), "points")
         normals_c = _lib.as_f32(normals.detach(), "normals")
         colours_c = _lib.as_f32(colours.detach(), "colours")
         proj_c = _lib.as_f32(proj.detach(), "proj")
         view_c = _lib.as_f32(view.detach(), "view")
-        h_c = _lib.as_f32(h.detach().reshape(-1), "h")
         N, P0, P = _layout(points_c, proj_c, first_idx, num_points, shared)
+        h_c, frames_c = _splat_shape(h, frames, P0 if shared else P, N, P)
         if shading is not None:
             if tuple(colours_c.shape) != (P0, 3):
                 raise RuntimeError("fused shading takes the per-point albedo as colours: (%d, 3) for a %s, got %s"
@@ -154,8 +172,6 @@ class _RenderFunction(torch.autograd.Function):
                                % (P, " or (%d, 3)" % P0 if shared else "", tuple(colours_c.shape)))
         if tuple(proj_c.shape) != (N, 4, 4) or tuple(view_c.shape) != (N, 4, 4):
             raise RuntimeError("proj and view must have shape (N,4,4)")
-        if h_c.numel() not in (N, P):
-            raise RuntimeError("h must have N or P elements")
         S, K = int(prm.image_size), int(prm.points_per_pixel)
         if K > _lib.MAX_POINTS_PER_PIXEL:
             raise RuntimeError("Must have points_per_pixel <= %d" % _lib.MAX_POINTS_PER_PIXEL)
@@ -177,6 +193,7 @@ class _RenderFunction(torch.autograd.Function):
         npts = num_points.contiguous() if num_points is not None else None
         a = _lib.RenderArgs()
         _fill_common(a, points_c, normals_c, colours_c, proj_c, view_c, h_c, fi, npts, shared, N, P0, P, prm)
+        a.frames = _lib.ptr(frames_c)
         a.shared_colours = int(shared_col)
         shaded = None
         if shading is not None:
@@ -306,14 +323,14 @@ class _RenderFunction(torch.autograd.Function):
                     light_backward()
                 grad_sync.reduce_late(grad_points)
                 grad_sync.join(dev)
-        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb)
+        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb, None)
         if shade is not None:
             return (grad_points, grad_normals, grad_albedo) + cams
         return (grad_points, None, grad_colours) + cams
 
 
 def render_points(points, normals, colours, proj, view, h, params: SplatParams, first_idx=None, num_points=None,
-                  shared_cloud=True, return_fragments=False, grad_sync=None, shading=None) -> RenderOutput:
+                  shared_cloud=True, return_fragments=False, grad_sync=None, shading=None, frames=None) -> RenderOutput:
     """Render ``N`` views of an oriented point cloud to RGBA.
 
     points, normals : (P0,3) when ``shared_cloud`` (one cloud seen from N cameras) else packed (P,3)
@@ -321,7 +338,11 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
                       features used by every view of a shared cloud (gradient then summed over the views)
     proj, view      : (N,4,4) full-projection and world-to-view matrices, row-vector convention; when they require
                       grad they receive the gradient of the screen positions (proj: x, y; view: the depth)
-    h               : (N,) per-view or (P,) per-splat variance scale (rasterizer.py:293-402)
+    h               : (N,) per-view or (P,) per-splat variance scale (rasterizer.py:293-402), or None with ``frames``
+    frames          : anisotropic splats (``Vrk_invariant`` and ``Vrk_isotropic`` off, rasterizer.py:256-291): the
+                      (P0,8) (shared cloud) or (P,8) (packed) records of :func:`local_frames`, in place of ``h``; the
+                      splat's world variance is l1 f1 f1^T + l2 f2 f2^T.  Constants, as in the reference: the normals
+                      then receive only the shading's gradient
     shading         : optional Shading -- `colours` is then the per-point albedo, (P0,3) for a shared cloud or (P,3),
                       one row per packed point, for packed clouds, and the colour of every (view, point) is computed in
                       the preprocess kernel: albedo * (ambient + diffuse) + specular (DSS/core/texture.py:74-127), with
@@ -336,7 +357,7 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     outs = _RenderFunction.apply(points, normals, colours, proj, view, h, first_idx, num_points,
                                  bool(shared_cloud), params, bool(return_fragments), grad_sync, shading,
                                  *((shading.cam_centres, shading.lights, shading.ambient) if shading is not None
-                                   else (None, None, None)))
+                                   else (None, None, None)), frames)
     image, idx, weights, visible, records, scaler = outs[:6]
     zbuf, qvalue = (outs[6], outs[7]) if return_fragments else (None, None)
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
@@ -428,15 +449,16 @@ def make_shading(lights, view_matrices, shininess=64.0) -> Shading:
 
 
 def preprocess_points(points, normals, proj, view, h, params: SplatParams, first_idx=None, num_points=None,
-                      shared_cloud=True):
-    """Per-(point,view) screen-space info only (rasterizer.py:525-565 + the transform of :614).
+                      shared_cloud=True, frames=None):
+    """Per-(point,view) screen-space info only (rasterizer.py:525-565 + the transform of :614).  Pass exactly one of
+    ``h`` and ``frames``, as for :func:`render_points`.
 
     Returns dict(ndc (P,3), ellipse_params (P,3), radii (P,2), scaler (P,), cutoff_threshold (P,))."""
-    dev = _lib.require_cuda(points, normals, proj, view, h, first_idx, num_points)
+    dev = _lib.require_cuda(points, normals, proj, view, h, first_idx, num_points, frames)
     points_c, normals_c = _lib.as_f32(points.detach(), "points"), _lib.as_f32(normals.detach(), "normals")
     proj_c, view_c = _lib.as_f32(proj.detach(), "proj"), _lib.as_f32(view.detach(), "view")
-    h_c = _lib.as_f32(h.detach().reshape(-1), "h")
     N, P0, P = _layout(points_c, proj_c, first_idx, num_points, shared_cloud)
+    h_c, frames_c = _splat_shape(h, frames, P0 if shared_cloud else P, N, P)
     f32 = dict(dtype=torch.float32, device=dev)
     ndc, ell = torch.empty((P, 3), **f32), torch.empty((P, 3), **f32)
     radii, scaler = torch.empty((P, 2), **f32), torch.empty((P,), **f32)
@@ -444,9 +466,50 @@ def preprocess_points(points, normals, proj, view, h, params: SplatParams, first
     npts = num_points.contiguous() if num_points is not None else None
     a = _lib.RenderArgs()
     _fill_common(a, points_c, normals_c, None, proj_c, view_c, h_c, fi, npts, shared_cloud, N, P0, P, params)
+    a.frames = _lib.ptr(frames_c)
     a.ndc, a.ellipse, a.radii, a.scaler = _lib.ptr(ndc), _lib.ptr(ell), _lib.ptr(radii), _lib.ptr(scaler)
     with torch.cuda.device(dev):
         rc = _lib.load().dss_preprocess(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
     _lib.check(rc, "dss_preprocess")
     return {"ndc": ndc, "ellipse_params": ell, "radii": radii, "scaler": scaler,
             "cutoff_threshold": torch.full((P,), float(params.cutoff_threshold), **f32)}
+
+
+LOCAL_FRAME_K = 8   # neighbourhood of the anisotropic kernel (rasterizer.py:272-273)
+
+
+def local_frames(points, first_idx=None, num_points=None):
+    """Per-point principal frames of the anisotropic reconstruction kernel (``Vrk_invariant`` and ``Vrk_isotropic``
+    off: DSS/core/rasterizer.py:256-291 over DSS/utils/mathHelper.py:34-91).  ``points`` (P0,3), one cloud, or packed
+    (P,3) with ``first_idx`` / ``num_points`` (N,) int64 as for ``knn_points_packed``.
+
+    Returns (P0|P, 8) float32 records {f1.xyz, l1, f2.xyz, l2}: l0 <= l1 <= l2 the eigenvalues of the population
+    covariance of each point's 8 nearest neighbours (itself included) and f1, f2 the eigenvectors of the two largest,
+    solved in float64 (csrc/local_frames.cu).  Rows with fewer than 8 finite neighbours (a non-finite point, a packed
+    cloud of fewer than 8 points) are NaN.  Two launches (the K-NN and the frames kernel), no host synchronisation; a
+    single cloud of at most 8 points raises ValueError as the reference does (mathHelper.py:57-61), packed clouds are
+    not checked on the host.  No gradients (the reference computes the frames under no_grad)."""
+    from .frnn_grid import knn_points_packed
+    dev = _lib.require_cuda(points, first_idx, num_points)
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3)")
+    if (first_idx is None) != (num_points is None):
+        raise RuntimeError("pass both first_idx and num_points, or neither")
+    pts = _lib.as_f32(points.detach(), "points")
+    P = pts.shape[0]
+    single = first_idx is None
+    if single:
+        if P <= LOCAL_FRAME_K:
+            raise ValueError("the anisotropic kernel needs clouds of more than %d points (the neighbourhood size), "
+                             "got %d" % (LOCAL_FRAME_K, P))
+        first_idx = torch.zeros((1,), dtype=torch.int64, device=dev)
+        num_points = torch.full((1,), P, dtype=torch.int64, device=dev)
+    fi, npts = first_idx.contiguous(), num_points.contiguous()
+    _, idx = knn_points_packed(pts, fi, npts, LOCAL_FRAME_K, -1.0)
+    frames = torch.empty((P, 8), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.load().dss_local_frames(_lib.ctx(dev), _lib.ptr(pts), _lib.ptr(None if single else fi),
+                                          _lib.ptr(None if single else npts), int(npts.shape[0]), P, _lib.ptr(idx),
+                                          _lib.ptr(frames), _lib.stream_ptr(dev))
+    _lib.check(rc, "dss_local_frames")
+    return frames

@@ -3,7 +3,8 @@
 N views, with the settings ``configs/dss.yml`` trains with:
 
 1. ``F.normalize(normals)`` (point_modeling.py:84-86);
-2. the splat size from a K-NN of the current points (rasterizer.py:293-342, ``Vrk_invariant`` / ``Vrk_isotropic``);
+2. the splat size from a K-NN of the current points (rasterizer.py:293-342, ``Vrk_invariant`` / ``Vrk_isotropic``), or,
+   with both off (``configs/default.yaml``), the anisotropic splats' local frames (rasterizer.py:256-291);
 3. ``render_points`` with fused shading: the batch's lights, and camera centres derived from the batch's view matrices;
 4. ``image_loss`` (trainer.py:332-376);
 5. ``point_filters``: the visibility and inmask filters (point_modeling.py:172-173, 188-212);
@@ -35,7 +36,8 @@ from ..core.cloud import PointClouds3D, PointCloudsFilters
 from ..core.lighting import pack_lights
 from ..core.rasterizer import point_sq_spacing, splat_variance_scale
 from ..core.texture import camera_centres
-from ..ops import Shading, SplatParams, point_filters, point_filters_no_views, render_points
+from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, local_frames, point_filters, point_filters_no_views,
+                   render_points)
 from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
 
 __all__ = ["TrainStep", "GraphedTrainStep"]
@@ -59,18 +61,26 @@ class TrainStep:
     ``GradSync``, and the regularisers run replicated on every rank: each rank ends with the same ``step.loss``,
     ``step.visibility``, ``step.inmask`` and gradients on its leaves, so identical optimizer steps keep the replicas
     identical.  The ranks must agree on P0, the kind of lights, the lambdas and ``params``; that is not checked (it would
-    take a host synchronisation).  With G = 1 or no ``grad_sync`` the step runs as on one GPU."""
+    take a host synchronisation).  With G = 1 or no ``grad_sync`` the step runs as on one GPU.
+
+    ``Vrk_invariant`` / ``Vrk_isotropic`` select the splat shape as in the rasterizer settings: one h per view, one h
+    per point, or, with both False (``configs/default.yaml``), anisotropic splats from the local frames of every point's
+    8 nearest neighbours (``local_frames``, computed every step from the current points; a view-sharded step computes
+    them on every rank from the same cloud, no collective).  The anisotropic kernel needs P0 > 8."""
 
     def __init__(self, points, normals, colours, params: SplatParams, *, learn=("points", "normals"),
-                 Vrk_invariant=True, frnn_radius=0.2, shininess=64.0, lambda_dr_rgb=1.0, lambda_dr_silhouette=1.0,
-                 lambda_dr_proj=0.01, lambda_dr_repel=0.0, knn_k=12, filter_scale=2.0, sharpness_sigma=0.75,
-                 grad_sync=None):
+                 Vrk_invariant=True, Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0, lambda_dr_rgb=1.0,
+                 lambda_dr_silhouette=1.0, lambda_dr_proj=0.01, lambda_dr_repel=0.0, knn_k=12, filter_scale=2.0,
+                 sharpness_sigma=0.75, grad_sync=None):
         dev = _lib.require_cuda(points, normals, colours)
         for name, t in (("points", points), ("normals", normals), ("colours", colours)):
             if t.dtype != torch.float32 or t.dim() != 2 or tuple(t.shape) != (points.shape[0], 3):
                 raise RuntimeError("%s must be a float32 (P0, 3) tensor, got %s %s" % (name, t.dtype, tuple(t.shape)))
         if any(name not in _LEARNABLE for name in learn):
             raise ValueError("learn takes names out of %s, got %s" % (_LEARNABLE, tuple(learn)))
+        if not (Vrk_invariant or Vrk_isotropic) and points.shape[0] <= LOCAL_FRAME_K:
+            raise ValueError("the anisotropic kernel (Vrk_invariant and Vrk_isotropic off) needs more than %d points, "
+                             "got %d" % (LOCAL_FRAME_K, points.shape[0]))
         self._sync = grad_sync if grad_sync is not None and grad_sync.world_size > 1 else None
         # image_loss and point_filters take None as "not sharded": GradSync's default group is named explicitly
         self._group = None if self._sync is None else (grad_sync.group if grad_sync.group is not None
@@ -81,6 +91,7 @@ class TrainStep:
             leaf(colours, "colours")
         self.params = params
         self.Vrk_invariant, self.frnn_radius, self.shininess = bool(Vrk_invariant), float(frnn_radius), float(shininess)
+        self.Vrk_isotropic = bool(Vrk_isotropic)
         self.lambda_dr_rgb, self.lambda_dr_silhouette = float(lambda_dr_rgb), float(lambda_dr_silhouette)
         self.lambda_dr_proj, self.lambda_dr_repel = float(lambda_dr_proj), float(lambda_dr_repel)
         self.knn_k, self.filter_scale, self.sharpness_sigma = int(knn_k), float(filter_scale), float(sharpness_sigma)
@@ -91,9 +102,9 @@ class TrainStep:
 
     def settings(self):
         """every host-side value the step bakes into its launches"""
-        return (tuple(self.params), self.Vrk_invariant, self.frnn_radius, self.shininess, self.lambda_dr_rgb,
-                self.lambda_dr_silhouette, self.lambda_dr_proj, self.lambda_dr_repel, self.knn_k, self.filter_scale,
-                self.sharpness_sigma)
+        return (tuple(self.params), self.Vrk_invariant, self.Vrk_isotropic, self.frnn_radius, self.shininess,
+                self.lambda_dr_rgb, self.lambda_dr_silhouette, self.lambda_dr_proj, self.lambda_dr_repel, self.knn_k,
+                self.filter_scale, self.sharpness_sigma)
 
     def _check_batch(self, img, mask_img, proj, view):
         _lib.require_cuda(self.points, img, mask_img, proj, view)
@@ -127,13 +138,18 @@ class TrainStep:
             visibility, inmask = point_filters_no_views(self.points.shape[0], dev, self._group)
             rendered = _NoViews.apply(self.points, normals, self.colours, self._sync)
         else:
+            h = frames = None
             with torch.no_grad():
-                # the one cloud's spacing, the rule of SurfaceSplatting._compute_h for its N views
-                h = splat_variance_scale([point_sq_spacing(self.points, self.frnn_radius)],
-                                         self.Vrk_invariant).repeat(N)
+                if self.Vrk_invariant or self.Vrk_isotropic:
+                    # the one cloud's spacing, the rule of SurfaceSplatting._compute_h for its N views
+                    h = splat_variance_scale([point_sq_spacing(self.points, self.frnn_radius)],
+                                             self.Vrk_invariant).repeat(N)
+                else:
+                    # anisotropic: the one cloud's local frames, shared by its N views
+                    frames = local_frames(self.points)
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
             out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading,
-                                grad_sync=self._sync)
+                                grad_sync=self._sync, frames=frames)
             loss = image_loss(out.image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette,
                               group=self._group)
             visibility, inmask = point_filters(out, mask_img, group=self._group)

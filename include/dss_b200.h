@@ -196,6 +196,20 @@ DSS_API int dss_knn_points(dss_ctx *ctx, const float *queries, const int64_t *qu
                            const int64_t *num_points, int N, int64_t Pq, int64_t P, int K, float radius,
                            float *sq_dists, int32_t *idxs, void *stream);
 
+/* ---- local frames of the anisotropic kernel ------------------------------------------------------------------------
+ * Replaces estimate_pointcloud_local_coord_frames(neighborhood_size=8, disambiguate_directions=False) and the frame /
+ * curvature selection of _compute_anisotropic_Vrk (DSS/utils/mathHelper.py:34-91, DSS/core/rasterizer.py:256-291).
+ * knn_idx (P,8) int32: every row's 8 nearest neighbours as dss_knn_points writes them for K = 8, r = -1 (local to the
+ * cloud, the point itself included).  Per row: the population covariance C of the 8 neighbours about their mean,
+ * diagonalised in float64 (fixed cyclic Jacobi sweeps), rounded once: frames (P,8) f32, 16-byte aligned,
+ * {f1.xyz, l1, f2.xyz, l2} with l0 <= l1 <= l2 the eigenvalues and f2 the eigenvector of the largest.  Where
+ * l1 - l0 <= 2^-40 l2, f1 = normalize(f2 x e_k), e_k the axis of the smallest |f2_k|; where l2 - l0 <= 2^-40 l2 too,
+ * f2 = e_x.  A row with a -1 neighbour is all NaN.  first_idx / num_points (N,) int64 as for dss_knn_points, or both
+ * NULL with N = 1: one cloud of P rows.  Rows outside every range are not written.  One launch, one thread per row; no
+ * scratch, no atomics, no host synchronisation. */
+DSS_API int dss_local_frames(dss_ctx *ctx, const float *points, const int64_t *first_idx, const int64_t *num_points,
+                             int N, int64_t P, const int32_t *knn_idx, float *frames, void *stream);
+
 /* ---- surface regularisers of the training step (SURVEY.md section 8(f) row 2) -----------------------------------
  * Replaces the torch bodies of ProjectionLoss (kind 0) and RepulsionLoss (kind 1) (DSS/training/losses.py:282-497) on
  * packed clouds (points, normals (P,3); first_idx, num_points as for dss_knn_points).  knn_dists (P, K-1+self_col) f32
@@ -368,6 +382,12 @@ typedef struct dss_render_args {
      * up to a multiple of 4), read by the backward, whose binning then skips its counting pass over all P splats.  Give
      * the same tensor to both calls or NULL to both. */
     int32_t *cell_counts;
+    /* anisotropic splats (Vrk_invariant = Vrk_isotropic = false, rasterizer.py:256-291, 425-439): the (P0,8) (shared
+     * cloud) or (P,8) (packed) records {f1.xyz, l1, f2.xyz, l2} of dss_local_frames, indexed like the points.  The
+     * splat's world variance is then l1 f1 f1^T + l2 f2 f2^T and |det Mk| = |det([f1 f2]^T J)|, in place of
+     * h (I - n n^T); `h` must be NULL.  NULL: the isotropic / invariant kernel with `h`.  The normals still shade and
+     * cull. */
+    const float *frames;
 } dss_render_args;
 #define DSS_MAX_LIGHTS 8
 
