@@ -12,7 +12,7 @@ import math
 
 import torch
 
-__all__ = ["FoVPerspectiveCameras", "look_at_view_transform", "look_at_rotation", "camera_matrices"]
+__all__ = ["FoVPerspectiveCameras", "look_at_view_transform", "look_at_rotation", "camera_matrices", "CameraSampler"]
 
 
 class _Transform:
@@ -151,3 +151,43 @@ def camera_matrices(cameras, **kwargs):
     proj = cameras.get_full_projection_transform().get_matrix()
     view = cameras.get_world_to_view_transform().get_matrix()
     return proj.float().contiguous(), view.float().contiguous()
+
+
+class CameraSampler:
+    """Random cameras looking at (about) the origin from varying distances, in batches (DSS/core/camera.py:6-71):
+    distances uniform in ``distance_range`` (sorted descending with ``sort_distance``), azimuth uniform in [-180, 180),
+    elevation in [-90, 90) degrees and ``at`` uniform in [-0.05, 0.05)^3, through :func:`look_at_view_transform`.
+    Iterating yields ``camera_type(R=..., T=..., **camera_params)`` of ``num_cams_batch`` cameras (the last batch may be
+    smaller).  All draws come from ``generator`` (a ``torch.Generator``; None: torch's global one)."""
+
+    def __init__(self, num_cams_total, num_cams_batch, distance_range=(5, 10), sort_distance=True,
+                 camera_type=FoVPerspectiveCameras, camera_params=None, generator=None):
+        self.num_cams_total, self.num_cams_batch = int(num_cams_total), int(num_cams_batch)
+        self.sort_distance = sort_distance
+        self.camera_type = camera_type
+        self.camera_params = {} if camera_params is None else dict(camera_params)
+        rng = torch.as_tensor(distance_range, dtype=torch.float32).reshape(-1, 2)
+        n, g = self.num_cams_total, generator
+        distances = torch.rand(n, generator=g) * (rng[:, 1] - rng[:, 0]) + rng[:, 0]
+        if sort_distance:
+            distances, _ = distances.sort(descending=True)
+        azim = torch.rand(n, generator=g) * 360 - 180
+        elev = torch.rand(n, generator=g) * 180 - 90
+        at = torch.rand((n, 3), generator=g) * 0.1 - 0.05
+        self.distances, self.azim, self.elev, self.at = distances, azim, elev, at
+        self.R, self.T = look_at_view_transform(distances, elev, azim, at=at, degrees=True)
+        self._idx = 0
+
+    def __len__(self):
+        return (self.R.shape[0] + self.num_cams_batch - 1) // self.num_cams_batch
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        if self._idx >= len(self):
+            raise StopIteration
+        start = self._idx * self.num_cams_batch
+        end = min(start + self.num_cams_batch, self.R.shape[0])
+        self._idx += 1
+        return self.camera_type(R=self.R[start:end], T=self.T[start:end], **self.camera_params)

@@ -68,6 +68,11 @@ enum BufId {
     BUF_LIGHT,        // per-block fp64 partial sums of the light gradients
     BUF_REGULARISER,  // denoised normals (P,3) and per-cloud bounding boxes of the surface regularisers
     BUF_IMAGE_LOSS,   // per-block fp64 partial sums of the image loss, and the finish's block counter
+    BUF_MESH_SCREEN,  // mesh rasterizer: screen-space vertices {x, y, z, 0} of a chunk of views
+    BUF_MESH_OFFSETS, //   per (view, face) pixel-centre counts, then their exclusive 64-bit scan (+ total)
+    BUF_MESH_RECTS,   //   per (view, face) pixel-index rectangle {column lo, row lo, width, 0}
+    BUF_MESH_BLOCKS,  //   per-tile sums of the 64-bit scan
+    BUF_MESH_KEYS,    //   per-pixel closest (depth, face) key
     NUM_BUFS
 };
 

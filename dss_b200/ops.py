@@ -21,7 +21,7 @@ import torch
 from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
-           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames"]
+           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh"]
 
 
 class SplatParams(NamedTuple):
@@ -513,3 +513,56 @@ def local_frames(points, first_idx=None, num_points=None):
                                           _lib.ptr(frames), _lib.stream_ptr(dev))
     _lib.check(rc, "dss_local_frames")
     return frames
+
+
+class MeshRender(NamedTuple):
+    image: Optional[torch.Tensor]   # (N,S,S,4) flat-shaded rgb + coverage, or None without shading
+    pix_to_face: torch.Tensor       # (N,S,S) int32 face index in the mesh, -1 where no face covers the pixel
+    zbuf: torch.Tensor              # (N,S,S) float32 view-space depth of that face, -1 where none
+
+
+def render_mesh(verts, faces, proj, view, image_size, shading: Optional[Shading] = None) -> MeshRender:
+    """Rasterize one opaque triangle mesh into N views: the closest face per pixel and, with ``shading``, its flat
+    shading -- pytorch3d's ``MeshRasterizer`` (blur_radius 0, faces_per_pixel 1, no perspective correction, no back-face
+    culling) + ``HardFlatShader`` as the reference's scripts/create_mvr_data_from_mesh.py uses them (csrc/mesh_raster.cu;
+    the rules are in include/dss_b200.h).
+
+    verts (V,3) f32, faces (F,3) integer (every index in [0, V), checked here), proj / view (N,4,4) as for
+    :func:`render_points`.  ``shading``: a :class:`Shading` (:func:`make_shading`), lights shared or per view,
+    directional or point; the vertex colours and materials are ones.  Forward only (no gradients).  Background pixels
+    are (1, 1, 1, 0); alpha is the coverage mask."""
+    dev = _lib.require_cuda(verts, faces, proj, view)
+    v = _lib.as_f32(verts.detach(), "verts")
+    if v.dim() != 2 or v.shape[1] != 3:
+        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
+        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
+    V, F = v.shape[0], faces.shape[0]
+    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
+        raise ValueError("face indices must lie in [0, %d)" % V)
+    if V >= 2 ** 31 or F >= 2 ** 31:
+        raise ValueError("at most 2^31 - 1 vertices and faces")
+    f = faces.detach().to(torch.int32).contiguous()
+    proj_c, view_c = _lib.as_f32(proj.detach(), "proj"), _lib.as_f32(view.detach(), "view")
+    N = proj_c.shape[0]
+    if tuple(proj_c.shape) != (N, 4, 4) or tuple(view_c.shape) != (N, 4, 4) or N < 1:
+        raise RuntimeError("proj and view must have shape (N,4,4), N >= 1")
+    S = int(image_size)
+    if S < 1:
+        raise RuntimeError("image_size must be positive")
+    pix_to_face = torch.empty((N, S, S), dtype=torch.int32, device=dev)
+    zbuf = torch.empty((N, S, S), dtype=torch.float32, device=dev)
+    image = None
+    sh_args = (0, 0, 0, 0.0, None, None, None)
+    if shading is not None:
+        sh = _check_shading(shading, N, dev)
+        image = torch.empty((N, S, S, 4), dtype=torch.float32, device=dev)
+        sh_args = (int(sh.lights.shape[-2]), sh.light_type, int(sh.lights.dim() == 3), sh.shininess, sh.lights,
+                   sh.ambient, sh.cam_centres)
+    with torch.cuda.device(dev):
+        rc = _lib.load().dss_rasterize_mesh(
+            _lib.ctx(dev), _lib.ptr(v), V, _lib.ptr(f), F, _lib.ptr(proj_c), _lib.ptr(view_c), N, S,
+            *sh_args[:4], *(_lib.ptr(t) for t in sh_args[4:]), _lib.ptr(pix_to_face), _lib.ptr(zbuf), _lib.ptr(image),
+            _lib.stream_ptr(dev))
+    _lib.check(rc, "dss_rasterize_mesh")
+    return MeshRender(image, pix_to_face, zbuf)

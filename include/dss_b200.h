@@ -424,6 +424,29 @@ DSS_API int dss_light_backward(dss_ctx *ctx, const dss_render_args *args, float 
 /* per-(point,view) preprocess only (rasterizer.py:443-565 fused): writes ndc, ellipse, radii, scaler. */
 DSS_API int dss_preprocess(dss_ctx *ctx, const dss_render_args *args, void *stream);
 
+/* ---- opaque triangle meshes (training data from a mesh) -------------------------------------------------------------
+ * pytorch3d's rasterize_meshes + HardFlatShader as the reference's scripts/create_mvr_data_from_mesh.py:147-208 calls
+ * them (blur_radius 0, perspective_correct off, cull_backfaces off, only the front fragment), for one mesh verts (V,3)
+ * f32 / faces (F,3) i32 seen by N cameras proj / view (N,4,4), row-vector convention as in dss_render_args.
+ * Per view every vertex gets screen x, y = its NDC (the splat preprocess's expression) and z = its view-space depth;
+ * pixel (row, col) has the centre pix_to_ndc of index (S-1-col, S-1-row) as in the point rasterizer.  With
+ * E(p, a, b) = (p.x - a.x)(b.y - a.y) - (p.y - a.y)(b.x - a.x), a face is skipped when max(z0, z1, z2) < 0, when
+ * |E(v0, v1, v2)| <= 1e-8, or at pixels outside its closed xy bounding box; otherwise, with den = E(v2, v0, v1) + 1e-8,
+ *   w0 = E(p, v1, v2) / den,  w1 = E(p, v2, v0) / den,  w2 = E(p, v0, v1) / den,  pz = (w0 z0 + w1 z1) + w2 z2,
+ * it covers the pixel when w0 > 0 && w1 > 0 && w2 > 0 && pz >= 0.  The covering face with the smallest pz wins, ties to
+ * the smaller face index.  Outputs (caller-allocated, N*S*S each): pix_to_face i32 (face index, -1: none) and zbuf f32
+ * (pz, -0 written as +0; -1: none).  rgba (N,S,S,4) f32 or NULL: flat shading, the fused shading's formula (see
+ * dss_render_args.shade) with albedo 1 at the face centroid, normal normalize(cross(v1 - v0, v2 - v0)) and view n's
+ * lights and camera centre; background (1, 1, 1, 0).  n_lights, light_type, lights_per_view, shininess, lights, ambient
+ * and cam_centres as the dss_render_args fields of the same names, read only with rgba.  A face with an index outside
+ * [0, V) covers nothing.  Deterministic (a 64-bit integer atomicMin per covered (face, pixel)); no host
+ * synchronisation; views are processed in chunks that bound the context's scratch. */
+DSS_API int dss_rasterize_mesh(dss_ctx *ctx, const float *verts, int64_t V, const int32_t *faces, int64_t F,
+                               const float *proj, const float *view, int N, int image_size, int n_lights,
+                               int light_type, int lights_per_view, float shininess, const float *lights,
+                               const float *ambient, const float *cam_centres, int32_t *pix_to_face, float *zbuf,
+                               float *rgba, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
