@@ -65,6 +65,8 @@ _SIGNATURES = {
     "dss_debug_raster_stats": (C.c_int, [vp, C.c_int, C.POINTER(C.c_uint64)]),
     "dss_debug_limit_tile_capacity": (C.c_int, [vp, C.c_int64]),
     "dss_debug_tile_total": (C.c_int64, [vp]),
+    "dss_debug_bin_no_rects": (C.c_int, [vp, C.c_int]),
+    "dss_debug_tile_lists": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, C.c_int64, vp, vp]),
     "dss_exclusive_scan_i32": (C.c_int, [vp, vp, vp, C.c_int64, vp]),
     "dss_grid_insert_points_2d": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp]),
     "dss_grid_counting_sort_2d": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp]),
@@ -198,6 +200,23 @@ def raster_stats(enable, device=None):
 def limit_tile_capacity(max_entries, device=None):
     """testing: cap the forward's tile-list buffer (0 = no cap) so that the overflow path runs (see the header)."""
     check(load().dss_debug_limit_tile_capacity(ctx(device), int(max_entries)), "dss_debug_limit_tile_capacity")
+
+
+def bin_no_rects(on, device=None):
+    """testing: bin the forward tile lists with separate count and scatter passes (DSS_BIN_NORECTS) or not."""
+    check(load().dss_debug_bin_no_rects(ctx(device), int(bool(on))), "dss_debug_bin_no_rects")
+
+
+def tile_lists(n_views, n_offsets, n_ids, device=None):
+    """testing: (zrange (n_views, 2) float32, offsets (n_offsets,) int32, ids (n_ids,) int32) of the last forward,
+    copied from the context's scratch on the current stream."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+    zr = torch.empty(n_views, 2, dtype=torch.float32, device=dev)
+    off = torch.empty(n_offsets, dtype=torch.int32, device=dev)
+    ids = torch.empty(n_ids, dtype=torch.int32, device=dev)
+    check(load().dss_debug_tile_lists(ctx(device), int(n_views), ptr(zr), int(n_offsets), ptr(off), int(n_ids),
+                                      ptr(ids), stream_ptr(device)), "dss_debug_tile_lists")
+    return zr, off, ids
 
 
 def scratch_bytes(device=None):

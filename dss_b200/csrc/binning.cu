@@ -4,6 +4,7 @@
 // (N,B,B,M) int32 tensor filled by 64 CTAs that brute-force all B^2 bins per point, every splat
 // computes its bin rectangle in O(1), counts go through an on-device exclusive scan and ids are
 // scattered into exact-size CSR lists.
+#include "binning.cuh"
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -36,89 +37,6 @@ int pack_records(dss_ctx *ctx, const float *points, const float *radii, const fl
     pack_records_kernel<<<(unsigned)((P + 255) / 256), 256, 0, st>>>(points, radii, ellipse, P, rec);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Bin range of an interval [p0, p1] -- the reference's closed fp32 predicate
-//     (p0 <= b1(b)) && (b0(b) <= p1),   b0(b) = PixToNdc(b*bin) - 1/S,  b1(b) = PixToNdc((b+1)*bin-1) + 1/S
-// (DSS/csrc/rasterize_points.cu:355-383) is monotone in b, so the overlapping bins form a contiguous
-// range [lo, hi].  We estimate it arithmetically and fix it up with the exact predicate, which makes
-// the membership bit-identical to the reference's brute-force loop at O(1) cost.
-// ---------------------------------------------------------------------------------------------
-// (pix_to_ndc_fast: for a power-of-two S the division-free form is bit-identical to the reference's expression,
-//  see common.cuh -- the edges are evaluated up to eight times per splat and axis, the IEEE division dominated the
-//  instruction count of both binning kernels)
-struct EdgeCtx {
-    int bin, S, B;
-    float inv_S, half_pix;
-};
-__device__ __forceinline__ EdgeCtx make_edge_ctx(int bin, int S, int B) {
-    EdgeCtx e;
-    e.bin = bin;
-    e.S = S;
-    e.B = B;
-    e.inv_S = 1.0f / (float)S;
-    e.half_pix = 1.0f / S;
-    return e;
-}
-template <bool POW2>
-__device__ __forceinline__ float bin_lo_edge_eval(int b, const EdgeCtx &e) {
-    return pix_to_ndc_fast(b * e.bin, e.S, e.inv_S, POW2) - e.half_pix;
-}
-template <bool POW2>
-__device__ __forceinline__ float bin_hi_edge_eval(int b, const EdgeCtx &e) {
-    return pix_to_ndc_fast((b + 1) * e.bin - 1, e.S, e.inv_S, POW2) + e.half_pix;
-}
-template <bool POW2>
-__device__ __forceinline__ float bin_lo_edge(int b, const EdgeCtx &e) { return bin_lo_edge_eval<POW2>(b, e); }
-template <bool POW2>
-__device__ __forceinline__ float bin_hi_edge(int b, const EdgeCtx &e) { return bin_hi_edge_eval<POW2>(b, e); }
-// (tried and dropped: the B edges tabulated once per block in shared memory -- the same float values, 12 loads instead
-//  of 12 x (IMAD, I2F, FFMA, FADD) per splat: bin_count did not get faster and bin_scatter got slower; the fix-up loops
-//  are latency chains either way and the table reads went through generic loads)
-
-template <bool POW2>
-__device__ __forceinline__ void bin_range(float p0, float p1, const EdgeCtx &e, int &lo, int &hi) {
-    const int B = e.B;
-    const float scale = (float)e.S / (2.0f * (float)e.bin);
-    // estimates: the bin that contains the end point (exact unless the point sits within rounding of an edge; NaN/inf are
-    // handled by the clamps).  The fix-up loops below correct any start in either direction, so the estimate only sets
-    // their trip count: two predicate evaluations per bound from here, three from the "one bin outside" start used before
-    // (the edge arithmetic is most of bin_count_kernel's instructions)
-    float e0 = floorf((p0 + 1.0f) * scale);
-    float e1 = floorf((p1 + 1.0f) * scale);
-    lo = (e0 >= 0.0f) ? ((e0 < (float)B) ? (int)e0 : B) : 0;          // NaN -> 0
-    hi = (e1 >= 0.0f) ? ((e1 < (float)B) ? (int)e1 : B - 1) : -1;    // NaN -> -1
-    if (hi > B - 1) hi = B - 1;
-    // lo = smallest b with p0 <= b1(b)
-    while (lo > 0 && p0 <= bin_hi_edge<POW2>(lo - 1, e)) --lo;
-    while (lo < B && !(p0 <= bin_hi_edge<POW2>(lo, e))) ++lo;
-    // hi = largest b with b0(b) <= p1
-    while (hi < B - 1 && bin_lo_edge<POW2>(hi + 1, e) <= p1) ++hi;
-    while (hi >= 0 && !(bin_lo_edge<POW2>(hi, e) <= p1)) --hi;
-}
-
-struct BinRect {
-    int x0, x1, y0, y1;
-    bool empty;
-};
-
-template <bool POW2>
-__device__ __forceinline__ BinRect splat_bin_rect(const float4 A, const float ry, int bin, int S, int B) {
-    BinRect r;
-    r.empty = true;
-    r.x0 = r.y0 = 0;
-    r.x1 = r.y1 = -1;
-    if (A.z < 0) return r;  // behind the camera (rasterize_points.cu:351-352); also NaN-safe below
-    const float px0 = A.x - A.w, px1 = A.x + A.w;
-    const float py0 = A.y - ry, py1 = A.y + ry;
-    const EdgeCtx e = make_edge_ctx(bin, S, B);
-    bin_range<POW2>(py0, py1, e, r.y0, r.y1);
-    if (r.y0 > r.y1) return r;
-    bin_range<POW2>(px0, px1, e, r.x0, r.x1);
-    if (r.x0 > r.x1) return r;
-    r.empty = false;
-    return r;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -190,15 +108,6 @@ constexpr int BIN_THREADS = 256;
 constexpr int BIN_ITEMS = 16;   // splats per thread (32 measured slower: fewer, longer blocks)
 constexpr int BIN_CHUNK = BIN_THREADS * BIN_ITEMS;
 constexpr int BIN_MAX_SMEM_TILES = 48 * 1024;   // 192 KB of histogram at most
-
-// tile rectangle + depth slice of a splat in one register: 7 bits per coordinate (B <= 128), 4 bits of slice
-constexpr int BIN_PACK_MAX_B = 128;
-constexpr unsigned int BIN_PACK_EMPTY = 0xffffffffu;
-__device__ __forceinline__ unsigned int pack_rect(const BinRect &r, int slice) {
-    return r.empty ? BIN_PACK_EMPTY
-                   : (unsigned int)r.x0 | ((unsigned int)r.x1 << 7) | ((unsigned int)r.y0 << 14) | ((unsigned int)r.y1 << 21) |
-                         ((unsigned int)slice << 28);
-}
 
 template <bool SMEM, bool POW2>
 __global__ void __launch_bounds__(BIN_THREADS)
@@ -394,6 +303,69 @@ int bin_scatter(dss_ctx *ctx, const float4 *rec, const int64_t *first_idx, const
         }
         DSS_LAUNCH_CHECK(ctx);
     }
+    return DSS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Scatter of lists that the fused preprocess counted (render.cu, preprocess_splats<..., BIN>): each preprocess block
+// stored the packed rectangle of its splats and, per non-empty bin, the value its flush atomic returned -- the block's
+// offset inside the bin.  This kernel runs on the same grid with the same grid-stride loop, so block b of view n sees
+// exactly the splats block b counted: its cursors are the scanned bin offsets plus its own offsets, and the slots are
+// claimed with shared-memory atomics only.  block_offsets: (N, gridDim.x, B*B*NS), entries of empty bins unset (never
+// read back, the block has no splat in them).
+// ---------------------------------------------------------------------------------------------
+constexpr int SCATTER_BATCH = 8;   // rectangle words per thread whose loads are issued together
+
+__global__ void __launch_bounds__(PREPROCESS_THREADS)
+bin_scatter_counted_kernel(const int64_t *__restrict__ first_idx, const int64_t *__restrict__ num_points,
+                           int64_t P0_shared, int B, int NS, const int32_t *__restrict__ offsets,
+                           const int32_t *__restrict__ block_offsets, const unsigned int *__restrict__ rects,
+                           int32_t *__restrict__ ids, int ids_capacity) {
+    extern __shared__ int32_t s_cur[];
+    const int n = blockIdx.y;
+    const int nt = B * B * NS;
+    const ViewRange vr = view_range(first_idx, num_points, n, P0_shared);
+    const int32_t *off = offsets + (int64_t)n * nt;
+    const int32_t *own = block_offsets + ((int64_t)n * gridDim.x + blockIdx.x) * nt;
+    // (unsigned: the unset entries of empty bins may hold anything)
+#pragma unroll 8
+    for (int t = threadIdx.x; t < nt; t += PREPROCESS_THREADS) s_cur[t] = (int32_t)((unsigned int)off[t] + (unsigned int)own[t]);
+    __syncthreads();
+    const int64_t stride = (int64_t)gridDim.x * PREPROCESS_THREADS;
+    for (int64_t i0 = (int64_t)blockIdx.x * PREPROCESS_THREADS + threadIdx.x; i0 < vr.count; i0 += SCATTER_BATCH * stride) {
+        unsigned int pr[SCATTER_BATCH];
+#pragma unroll
+        for (int j = 0; j < SCATTER_BATCH; ++j) {
+            const int64_t i = i0 + j * stride;
+            pr[j] = i < vr.count ? __ldg(&rects[vr.first + i]) : BIN_PACK_EMPTY;
+        }
+#pragma unroll
+        for (int j = 0; j < SCATTER_BATCH; ++j) {
+            if (pr[j] == BIN_PACK_EMPTY) continue;
+            const int x0 = pr[j] & 127, x1 = (pr[j] >> 7) & 127, y0 = (pr[j] >> 14) & 127, y1 = (pr[j] >> 21) & 127,
+                      sl = pr[j] >> 28;
+            const int32_t p = (int32_t)(vr.first + i0 + j * stride);
+            for (int by = y0; by <= y1; ++by)
+                for (int bx = x0; bx <= x1; ++bx) {
+                    const int slot = atomicAdd(&s_cur[(by * B + bx) * NS + sl], 1);
+                    if (slot < ids_capacity) ids[slot] = p;
+                }
+        }
+    }
+}
+
+int bin_scatter_counted(dss_ctx *ctx, const int64_t *first_idx, const int64_t *num_points, int N, int64_t P0, int B,
+                        int NS, const int32_t *offsets, const int32_t *block_offsets, unsigned int blocks,
+                        const unsigned int *rects, int32_t *ids, int64_t ids_capacity, cudaStream_t st) {
+    if (P0 == 0) return DSS_OK;
+    const int cap = (int)(ids_capacity > (int64_t)INT32_MAX ? (int64_t)INT32_MAX : ids_capacity);
+    const size_t smem = (size_t)B * B * NS * sizeof(int32_t);
+    int rc = prepare_smem(bin_scatter_counted_kernel, smem);
+    if (rc) return rc;
+    StageScope prof(ctx, ST_BIN_SCATTER, st);
+    bin_scatter_counted_kernel<<<dim3(blocks, N), PREPROCESS_THREADS, smem, st>>>(first_idx, num_points, P0, B, NS, offsets,
+                                                                           block_offsets, rects, ids, cap);
+    DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }
 

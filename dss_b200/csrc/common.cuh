@@ -61,6 +61,7 @@ enum BufId {
     BUF_OCC_IDS,      // packed splat id of every compact record
     BUF_TILE_ORDER,   // launch order of the forward tiles
     BUF_BIN_RECTS,    // packed tile rectangle + depth slice of every splat (count pass -> scatter pass)
+    BUF_BIN_BLOCK_OFFSETS,  // fused route: every preprocess block's offset inside each tile-list bin it touched
     BUF_KNN_COUNTS,   // 3-D grid of the K-NN search: points per cell
     BUF_KNN_OFFSETS,  //   exclusive scan of the counts
     BUF_KNN_SORTED,   //   points in cell order {x, y, z, index}

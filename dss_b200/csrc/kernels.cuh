@@ -54,6 +54,31 @@ int bin_scatter(dss_ctx *ctx, const float4 *rec, const int64_t *first_idx, const
                 int64_t P0, int S, int bin, int NS, const float *zrange, const int32_t *offsets, int32_t *cursors,
                 int32_t *ids, int64_t ids_capacity, const unsigned int *rects, cudaStream_t st);
 
+// Threads per block of the preprocess.  The fused route's scatter (bin_scatter_counted) runs on the preprocess's grid
+// and partition of the splats, so both use this.
+constexpr int PREPROCESS_THREADS = 256;
+
+// Tile lists that the preprocess counted (dss_render_forward): counts already hold the per-(view, tile, slice) sizes,
+// rects the packed rectangle of every splat, block_offsets (N, blocks, B*B*NS) the offset of every preprocess block
+// inside each bin it touched.
+struct CountedBins {
+    const unsigned int *rects;
+    const int32_t *block_offsets;
+    unsigned int blocks;   // preprocess blocks per view
+};
+int bin_scatter_counted(dss_ctx *ctx, const int64_t *first_idx, const int64_t *num_points, int N, int64_t P0, int B,
+                        int NS, const int32_t *offsets, const int32_t *block_offsets, unsigned int blocks,
+                        const unsigned int *rects, int32_t *ids, int64_t ids_capacity, cudaStream_t st);
+
+// Tile grid and depth slices of the forward lists for N views of S x S pixels and K points per pixel; packed: the lists
+// can be binned with per-block histograms and the packed rectangle word (B <= 128, <= 16 slices, histogram <= 192 KB, and
+// neither DSS_BIN_DIRECT nor DSS_BIN_NORECTS).  Fails when the N*B*B*NS bins do not fit the int32 offsets.
+struct TilePlan {
+    int B, NS;
+    bool packed;
+};
+int plan_tiles(dss_ctx *ctx, int N, int S, int K, TilePlan *plan);
+
 // Depth slicing shared by the binning and raster kernels (identical arithmetic on both sides).
 struct SliceMap {
     float zmin, dz, inv_dz;
@@ -122,9 +147,11 @@ struct RasterArgs {
 
 int raster_forward(dss_ctx *ctx, const RasterArgs &a, cudaStream_t st);
 
-// bin + rasterize, shared by dss_splat_points and dss_render_forward.  Synchronises once.
+// bin + rasterize, shared by dss_splat_points and dss_render_forward.  Synchronises once.  counted: the preprocess
+// already counted the lists (the plan_tiles plan of this call, packed) and a.zrange holds the depth ranges; null: count
+// here.
 int bin_and_raster(dss_ctx *ctx, RasterArgs a, const int64_t *first_idx, const int64_t *num_points,
-                   int64_t P0, cudaStream_t st);
+                   int64_t P0, cudaStream_t st, const CountedBins *counted = nullptr);
 
 int visibility_from_idx(dss_ctx *ctx, const int32_t *idx, int64_t num_pixels, int K, int64_t P,
                         uint8_t *visible, cudaStream_t st);

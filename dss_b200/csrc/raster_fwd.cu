@@ -703,42 +703,55 @@ int raster_forward(dss_ctx *ctx, const RasterArgs &a, cudaStream_t st) {
     return launch_raster<DSS_MAX_POINTS_PER_PIXEL>(ctx, a, st);
 }
 
-int bin_and_raster(dss_ctx *ctx, RasterArgs a, const int64_t *first_idx, const int64_t *num_points,
-                   int64_t P0, cudaStream_t st) {
-    const int S = a.S;
-    const bool scatter_path = a.K <= 8;
-    a.B = (S + RASTER_TILE - 1) / RASTER_TILE;
-    a.NS = scatter_path ? choose_depth_slices(a.B) : 1;
-    if (a.NS > 1 && ctx->ns_override > 0 && ctx->ns_override < a.NS) a.NS = ctx->ns_override;
-    a.first_idx = first_idx;
-    a.num_points = num_points;
-    a.P0 = P0;
-    const int64_t nb = (int64_t)a.N * a.B * a.B * a.NS;
+int plan_tiles(dss_ctx *ctx, int N, int S, int K, TilePlan *plan) {
+    const int B = (S + RASTER_TILE - 1) / RASTER_TILE;
+    int NS = K <= 8 ? choose_depth_slices(B) : 1;   // the sliced rasterizer (K <= 8) walks its lists by depth slice
+    if (NS > 1 && ctx->ns_override > 0 && ctx->ns_override < NS) NS = ctx->ns_override;
+    const int64_t nb = (int64_t)N * B * B * NS;
     if (nb + 1 >= (int64_t)INT32_MAX) {
         set_error("too many tiles (%lld)", (long long)nb);
         return DSS_E_INVALID;
     }
+    plan->B = B;
+    plan->NS = NS;
+    // (the packed rectangle needs B <= 128 tiles per side and <= 16 slices, like the block histograms)
+    plan->packed = B <= 128 && NS <= 16 && (int64_t)B * B * NS <= 48 * 1024 && !ctx->bin_direct && !ctx->bin_no_rects;
+    return DSS_OK;
+}
+
+int bin_and_raster(dss_ctx *ctx, RasterArgs a, const int64_t *first_idx, const int64_t *num_points,
+                   int64_t P0, cudaStream_t st, const CountedBins *counted) {
+    const int S = a.S;
+    const bool scatter_path = a.K <= 8;
+    TilePlan plan;
+    int rc;
+    if ((rc = plan_tiles(ctx, a.N, S, a.K, &plan))) return rc;
+    a.B = plan.B;
+    a.NS = plan.NS;
+    a.first_idx = first_idx;
+    a.num_points = num_points;
+    a.P0 = P0;
+    const int64_t nb = (int64_t)a.N * a.B * a.B * a.NS;
     int32_t *counts = nullptr, *offsets = nullptr;
     int32_t *ids = nullptr;
     float *zrange = const_cast<float *>(a.zrange);   // non-null: the caller's preprocess already produced it
-    int rc;
     if ((rc = ctx_get(ctx, BUF_TILE_COUNTS, (size_t)(nb + 1), &counts))) return rc;
     if ((rc = ctx_get(ctx, BUF_TILE_OFFSETS, (size_t)(nb + 1), &offsets))) return rc;
-    if (a.NS > 1 && zrange == nullptr) {
-        if ((rc = ctx_get(ctx, BUF_ZRANGE, (size_t)(2 * a.N), &zrange))) return rc;
-        if ((rc = compute_zrange(ctx, a.rec, first_idx, num_points, a.N, P0, zrange, st))) return rc;
+    unsigned int *rects = nullptr;
+    if (counted) {
+        if ((rc = exclusive_scan_i32(ctx, counts, offsets, nb + 1, st))) return rc;
+    } else {
+        if (a.NS > 1 && zrange == nullptr) {
+            if ((rc = ctx_get(ctx, BUF_ZRANGE, (size_t)(2 * a.N), &zrange))) return rc;
+            if ((rc = compute_zrange(ctx, a.rec, first_idx, num_points, a.N, P0, zrange, st))) return rc;
+        }
+        const int64_t Ptot = (first_idx == nullptr) ? (int64_t)a.N * P0 : P0;
+        if (plan.packed && Ptot > 0 && (rc = ctx_get(ctx, BUF_BIN_RECTS, (size_t)Ptot, &rects))) return rc;
+        if ((rc = bin_count_and_scan(ctx, a.rec, first_idx, num_points, a.N, P0, S, RASTER_TILE, a.NS, zrange, counts,
+                                     offsets, rects, st)))
+            return rc;
     }
     a.zrange = zrange;
-    // (the packed rectangle needs B <= 128 tiles per side and <= 16 slices, like the block histograms)
-    unsigned int *rects = nullptr;
-    {
-        const int64_t Ptot = (first_idx == nullptr) ? (int64_t)a.N * P0 : P0;
-        if (a.B <= 128 && a.NS <= 16 && (int64_t)a.B * a.B * a.NS <= 48 * 1024 && !ctx->bin_direct && !ctx->bin_no_rects && Ptot > 0)
-            if ((rc = ctx_get(ctx, BUF_BIN_RECTS, (size_t)Ptot, &rects))) return rc;
-    }
-    if ((rc = bin_count_and_scan(ctx, a.rec, first_idx, num_points, a.N, P0, S, RASTER_TILE, a.NS, zrange, counts,
-                                 offsets, rects, st)))
-        return rc;
     a.tile_offsets = offsets;
     a.stats = nullptr;
     if (ctx->raster_stats) {
@@ -782,9 +795,13 @@ int bin_and_raster(dss_ctx *ctx, RasterArgs a, const int64_t *first_idx, const i
         set_error("internal: tile list buffer too small for the pixel-parallel path");
         return DSS_E_CAPACITY;
     }
-    if ((rc = bin_scatter(ctx, a.rec, first_idx, num_points, a.N, P0, S, RASTER_TILE, a.NS, zrange, offsets, counts, ids,
-                          a.ids_capacity, rects, st)))
-        return rc;
+    if (counted)
+        rc = bin_scatter_counted(ctx, first_idx, num_points, a.N, P0, a.B, a.NS, offsets, counted->block_offsets,
+                                 counted->blocks, counted->rects, ids, a.ids_capacity, st);
+    else
+        rc = bin_scatter(ctx, a.rec, first_idx, num_points, a.N, P0, S, RASTER_TILE, a.NS, zrange, offsets, counts, ids,
+                         a.ids_capacity, rects, st);
+    if (rc) return rc;
     a.tile_ids = ids;
     if ((rc = raster_forward(ctx, a, st))) return rc;
     // hint for the next call: whatever total the device has published by now (this call's, if the GPU is ahead of
@@ -819,6 +836,32 @@ int dss_debug_limit_tile_capacity(dss_ctx *ctx, int64_t max_entries) {
     DSS_REQUIRE(ctx != nullptr, "ctx is null");
     DSS_REQUIRE(max_entries >= 0 && max_entries <= (int64_t)INT32_MAX, "bad limit");
     ctx->tile_cap_limit = max_entries;
+    return DSS_OK;
+}
+
+int dss_debug_bin_no_rects(dss_ctx *ctx, int on) {
+    DSS_REQUIRE(ctx != nullptr, "ctx is null");
+    ctx->bin_no_rects = on ? 1 : 0;
+    return DSS_OK;
+}
+
+int dss_debug_tile_lists(dss_ctx *ctx, int n_views, float *zrange, int64_t n_offsets, int32_t *offsets, int64_t n_ids,
+                         int32_t *ids, void *stream) {
+    using namespace dss;
+    DSS_REQUIRE(ctx != nullptr, "ctx is null");
+    DSS_REQUIRE(n_views >= 0 && n_offsets >= 0 && n_ids >= 0, "negative size");
+    const struct {
+        BufId id;
+        void *dst;
+        size_t bytes;
+    } copies[3] = {{BUF_ZRANGE, zrange, (size_t)n_views * 2 * sizeof(float)},
+                   {BUF_TILE_OFFSETS, offsets, (size_t)n_offsets * sizeof(int32_t)},
+                   {BUF_TILE_IDS, ids, (size_t)n_ids * sizeof(int32_t)}};
+    for (const auto &c : copies) {
+        if (!c.dst || c.bytes == 0) continue;
+        DSS_REQUIRE(c.bytes <= ctx->cap[c.id], "more entries than the scratch holds");
+        DSS_CUDA_TRY(cudaMemcpyAsync(c.dst, ctx->buf[c.id], c.bytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    }
     return DSS_OK;
 }
 

@@ -2,6 +2,7 @@
 // orchestration (gradient clip + chain to world space).
 #include <math_constants.h>
 
+#include "binning.cuh"
 #include "common.cuh"
 #include "kernels.cuh"
 #include "shading.cuh"
@@ -40,6 +41,30 @@ __device__ __forceinline__ float fast_sqrt(float x) {
 __device__ __forceinline__ float py_eps_denom(float d) { return eps_denom(d, 1e-17f); }
 __device__ __forceinline__ float py_eps_sqrt(float s) { return fmaxf(fabsf(s), 1e-17f); }
 
+// View-space depth of world point p in view n (sV: the view's matrix) after the preprocess's filters
+// (rasterizer.py:187-192, :152): the depth range and, with backface culling, the normal n facing the camera.  A filtered
+// point gets -1.  The preprocess and the depth-range pre-pass of the fused route both call this, so that the pre-pass
+// finds exactly the depths the records will hold.
+__device__ __forceinline__ float kept_view_depth(const dss_render_args &g, const float *sV, float p0, float p1, float p2,
+                                                 float n0, float n1, float n2) {
+    const float zv = fmaf(p0, sV[2], fmaf(p1, sV[6], fmaf(p2, sV[10], sV[14])));
+    bool keep = (zv >= g.znear) && (zv <= g.zfar);
+    if (g.backface_culling) {
+        const float nz = n0 * sV[2] + n1 * sV[6] + n2 * sV[10];
+        keep = keep && (nz < 0.0f);
+    }
+    return keep ? zv : -1.0f;
+}
+
+// Counting inputs and outputs of the fused route's preprocess (BIN != 0 below).
+struct PreprocessBins {
+    const float *zrange;        // (N,2) depth ranges of the views (depth_range_kernel)
+    int32_t *counts;            // (N*B*B*NS) list sizes, zeroed by the caller
+    unsigned int *rects;        // (P,) packed tile rectangle + depth slice of every splat
+    int32_t *block_offsets;     // (N, gridDim.x, B*B*NS) each block's offset inside the bins it touches
+    int B, NS;
+};
+
 // ---------------------------------------------------------------------------------------------
 // One thread per (view, point).  Fuses DSS/core/rasterizer.py:183-217 (depth filter), :148-181
 // (backface filter), :443-496 (_compute_WJk), :293-342 (global/isotropic Vrk with Sk^T Sk = I - n n^T),
@@ -54,11 +79,21 @@ __device__ __forceinline__ float py_eps_sqrt(float s) { return fmaxf(fabsf(s), 1
 //   Vk = l1 u u^T + l2 v v^T,   |det Mk| = |u0 v1 - u1 v0|
 // and the rest (G = Vk + aa I, conic, radii, scaler, filters, shading) is shared.  The body is one inlined function
 // so that the two kernels without frames keep the code they had.
+// BIN (the fused route, 1: S a power of two, 2: any S): the thread also bins the splat it has just written, with the
+// binning's own functions on the same register values (bin_count_kernel reads them back from the record), stores the
+// packed rectangle and counts it in the block's histogram of the B*B*NS bins (dynamic shared memory).  At the end each
+// non-empty bin is added to the view's count with one atomic, whose return value -- the block's offset inside the bin --
+// goes to the block's row of pb.block_offsets for bin_scatter_counted.  The depth slices need the view's depth range
+// before the first record exists: pb.zrange comes from depth_range_kernel, and the kernel makes no zrange atomics.
 // ---------------------------------------------------------------------------------------------
-template <bool SHADE, bool FRAMES>
-__device__ __forceinline__ void preprocess_splats(const dss_render_args &g, float4 *rec, int32_t *zrange) {
+constexpr int FLUSH_BATCH = 8;   // histogram bins per thread whose flush atomics are in flight together
+
+template <bool SHADE, bool FRAMES, int BIN>
+__device__ __forceinline__ void preprocess_splats(const dss_render_args &g, float4 *rec, int32_t *zrange,
+                                                  const PreprocessBins &pb) {
     __shared__ float sM[16], sV[16];
     __shared__ float sL[DSS_MAX_LIGHTS * 9 + 6];   // lights, ambient (3), camera centre (3)
+    extern __shared__ int32_t s_hist[];            // BIN: B*B*NS counters
     const int n = blockIdx.y;
     if (threadIdx.x < 16) {
         sM[threadIdx.x] = g.proj[n * 16 + threadIdx.x];
@@ -66,7 +101,11 @@ __device__ __forceinline__ void preprocess_splats(const dss_render_args &g, floa
     }
     constexpr bool shade = SHADE;
     if (shade) stage_view_shading(sL, g, n);
+    const int nt = pb.B * pb.B * pb.NS;
+    if (BIN)
+        for (int t = threadIdx.x; t < nt; t += PREPROCESS_THREADS) s_hist[t] = 0;
     __syncthreads();
+    const SliceMap slices = make_slice_map(BIN ? pb.zrange : nullptr, n, pb.NS);
     const ViewRange vr = view_range(g.shared_cloud ? nullptr : g.first_idx, g.num_points, n, g.P0);
     const float pix = 2.0f / (float)g.image_size;
     const float aa = g.antialiasing_sigma * pix * pix;
@@ -82,7 +121,6 @@ __device__ __forceinline__ void preprocess_splats(const dss_render_args &g, floa
         const float x = fmaf(p0, sM[0], fmaf(p1, sM[4], fmaf(p2, sM[8], sM[12])));
         const float y = fmaf(p0, sM[1], fmaf(p1, sM[5], fmaf(p2, sM[9], sM[13])));
         const float t = fmaf(p0, sM[3], fmaf(p1, sM[7], fmaf(p2, sM[11], sM[15])));
-        float zv = fmaf(p0, sV[2], fmaf(p1, sV[6], fmaf(p2, sV[10], sV[14])));
         const float te = py_eps_denom(t);
         const float t2 = py_eps_denom(t * t);
         const float it = rcp_approx(te), it2 = rcp_approx(t2);
@@ -127,13 +165,7 @@ __device__ __forceinline__ void preprocess_splats(const dss_render_args &g, floa
         const float detM = FRAMES ? fabsf(u0 * v1 - u1 * v0) : fast_sqrt(fmaxf(T00 * T11 - T01 * T01, 0.0f));
         const float sc = detM *
                          rcp_approx(py_eps_denom(fast_sqrt(py_eps_sqrt(detG * (4.0f * CUDART_PI_F * CUDART_PI_F)))));  // :558-559
-        // filters (rasterizer.py:187-192, :152): view-space depth range, optional backface
-        bool keep = (zv >= g.znear) && (zv <= g.zfar);
-        if (g.backface_culling) {
-            const float nz = n0 * sV[2] + n1 * sV[6] + n2 * sV[10];
-            keep = keep && (nz < 0.0f);
-        }
-        if (!keep) zv = -1.0f;
+        const float zv = kept_view_depth(g, sV, p0, p1, p2, n0, n1, n2);
         if (zv >= 0.0f && zv < 3.0e38f) {
             const int zb = __float_as_int(zv + 0.0f);
             zlo = min(zlo, zb);
@@ -169,6 +201,33 @@ __device__ __forceinline__ void preprocess_splats(const dss_render_args &g, floa
             g.shaded[s * 3 + 1] = c.y;
             g.shaded[s * 3 + 2] = c.z;
         }
+        if (BIN) {
+            const BinRect r = splat_bin_rect<BIN == 1>(make_float4(xn, yn, zv, rx), ry, RASTER_TILE, g.image_size, pb.B);
+            const int sl = r.empty ? 0 : depth_slice(slices, zv);
+            pb.rects[s] = pack_rect(r, sl);
+            if (!r.empty)
+                for (int by = r.y0; by <= r.y1; ++by)
+                    for (int bx = r.x0; bx <= r.x1; ++bx) atomicAdd(&s_hist[(by * pb.B + bx) * pb.NS + sl], 1);
+        }
+    }
+    if (BIN) {
+        __syncthreads();
+        int32_t *cnt = pb.counts + (int64_t)n * nt;
+        int32_t *own = pb.block_offsets + ((int64_t)n * gridDim.x + blockIdx.x) * nt;
+        // the atomics of a batch are issued before their results are stored (a store between two atomics would make
+        // each one wait for the previous one's round trip)
+        for (int t0 = threadIdx.x; t0 < nt; t0 += FLUSH_BATCH * PREPROCESS_THREADS) {
+            int v[FLUSH_BATCH], r[FLUSH_BATCH];
+#pragma unroll
+            for (int j = 0; j < FLUSH_BATCH; ++j) {
+                const int t = t0 + j * PREPROCESS_THREADS;
+                v[j] = t < nt ? s_hist[t] : 0;
+                r[j] = v[j] ? atomicAdd(&cnt[t], v[j]) : 0;
+            }
+#pragma unroll
+            for (int j = 0; j < FLUSH_BATCH; ++j)
+                if (v[j]) own[t0 + j * PREPROCESS_THREADS] = r[j];
+        }
     }
     if (zrange) {   // one pair of atomics per block
         __shared__ int s_lo[8], s_hi[8];
@@ -190,16 +249,75 @@ __device__ __forceinline__ void preprocess_splats(const dss_render_args &g, floa
     }
 }
 
-template <bool SHADE>
-__global__ void __launch_bounds__(256) preprocess_kernel(const __grid_constant__ dss_render_args g, float4 *rec,
-                                                         int32_t *zrange) {
-    preprocess_splats<SHADE, false>(g, rec, zrange);
+template <bool SHADE, int BIN>
+__global__ void __launch_bounds__(PREPROCESS_THREADS)
+preprocess_kernel(const __grid_constant__ dss_render_args g, float4 *rec, int32_t *zrange, const PreprocessBins pb) {
+    preprocess_splats<SHADE, false, BIN>(g, rec, zrange, pb);
 }
 
-template <bool SHADE>
-__global__ void __launch_bounds__(256) preprocess_frames_kernel(const __grid_constant__ dss_render_args g, float4 *rec,
-                                                                int32_t *zrange) {
-    preprocess_splats<SHADE, true>(g, rec, zrange);
+template <bool SHADE, int BIN>
+__global__ void __launch_bounds__(PREPROCESS_THREADS)
+preprocess_frames_kernel(const __grid_constant__ dss_render_args g, float4 *rec, int32_t *zrange, const PreprocessBins pb) {
+    preprocess_splats<SHADE, true, BIN>(g, rec, zrange, pb);
+}
+
+typedef void (*PreprocessKernel)(const dss_render_args, float4 *, int32_t *, const PreprocessBins);
+template <int BIN>
+static PreprocessKernel preprocess_kernel_for(bool frames, bool shade) {
+    if (frames) return shade ? preprocess_frames_kernel<true, BIN> : preprocess_frames_kernel<false, BIN>;
+    return shade ? preprocess_kernel<true, BIN> : preprocess_kernel<false, BIN>;
+}
+
+// Depth range pre-pass of the fused route: zrange[n] = {min, max} (float bits) of kept_view_depth over the renderable
+// points of view n -- what the preprocess's own zrange atomics find, before the preprocess runs.  zrange must hold
+// {0x7f7fffff, 0} per view (init_zrange).  A shared cloud is read once: one thread per world point takes it through all
+// the views (grid (blocks, 1)); a packed cloud has a range per view (grid (blocks, N)).  Each warp folds its depths of a
+// view into the block's shared pair, each block folds its pairs into zrange.
+__global__ void __launch_bounds__(256) depth_range_kernel(const __grid_constant__ dss_render_args g, int32_t *zrange) {
+    extern __shared__ float s_view[];   // nv view matrices (16 floats each), then {min, max} per view
+    const int v0 = g.shared_cloud ? 0 : blockIdx.y, nv = g.shared_cloud ? g.n_views : 1;
+    int32_t *s_z = reinterpret_cast<int32_t *>(s_view + nv * 16);
+    for (int i = threadIdx.x; i < nv * 16; i += blockDim.x) s_view[i] = g.view[v0 * 16 + i];
+    for (int i = threadIdx.x; i < nv; i += blockDim.x) {
+        s_z[2 * i] = 0x7f7fffff;
+        s_z[2 * i + 1] = 0;
+    }
+    __syncthreads();
+    const ViewRange vr = view_range(g.shared_cloud ? nullptr : g.first_idx, g.num_points, v0, g.P0);
+    const int lane = threadIdx.x & 31;
+    for (int64_t w = (int64_t)blockIdx.x * blockDim.x + (threadIdx.x - lane); w < vr.count;
+         w += (int64_t)gridDim.x * blockDim.x) {   // warp-uniform trip count: the reductions below take all lanes
+        const int64_t i = w + lane, src = vr.first + i;
+        const bool in = i < vr.count;
+        float p0 = 0.f, p1 = 0.f, p2 = 0.f, n0 = 0.f, n1 = 0.f, n2 = 0.f;
+        if (in) {
+            p0 = g.points_world[src * 3 + 0];
+            p1 = g.points_world[src * 3 + 1];
+            p2 = g.points_world[src * 3 + 2];
+            if (g.backface_culling) {
+                n0 = g.normals_world[src * 3 + 0];
+                n1 = g.normals_world[src * 3 + 1];
+                n2 = g.normals_world[src * 3 + 2];
+            }
+        }
+        for (int v = 0; v < nv; ++v) {
+            const float zv = in ? kept_view_depth(g, s_view + v * 16, p0, p1, p2, n0, n1, n2) : -1.0f;
+            int zlo = 0x7f7fffff, zhi = 0;
+            if (zv >= 0.0f && zv < 3.0e38f) zlo = zhi = __float_as_int(zv + 0.0f);
+            zlo = __reduce_min_sync(0xffffffffu, zlo);
+            zhi = __reduce_max_sync(0xffffffffu, zhi);
+            if (lane == 0 && zlo <= zhi) {
+                atomicMin(&s_z[2 * v], zlo);
+                atomicMax(&s_z[2 * v + 1], zhi);
+            }
+        }
+    }
+    __syncthreads();
+    for (int v = threadIdx.x; v < nv; v += blockDim.x) {
+        if (s_z[2 * v] > s_z[2 * v + 1]) continue;   // no renderable point of view v in this block
+        atomicMin(&zrange[2 * (v0 + v)], s_z[2 * v]);
+        atomicMax(&zrange[2 * (v0 + v) + 1], s_z[2 * v + 1]);
+    }
 }
 
 // d L / d shaded (N*P0,3) -> d albedo, d normal, d position (through the shading) per world point, summed over the views:
@@ -334,28 +452,82 @@ static int check_common(const dss_render_args *g) {
     return DSS_OK;
 }
 
+static int check_preprocess_inputs(const dss_render_args *g) {
+    DSS_REQUIRE(g->points_world && g->normals_world && g->proj && g->view && (g->h || g->frames), "null input array");
+    DSS_REQUIRE(!(g->h && g->frames), "pass exactly one of h and frames");
+    DSS_REQUIRE(!g->frames || (reinterpret_cast<uintptr_t>(g->frames) & 15) == 0, "frames must be 16-byte aligned");
+    return DSS_OK;
+}
+
 static int run_preprocess(dss_ctx *ctx, const dss_render_args *g, float4 *rec, cudaStream_t st, float *zrange = nullptr) {
     if (zrange) {
         int rc = init_zrange(ctx, zrange, g->n_views, st);
         if (rc) return rc;
     }
     if (g->P == 0 || g->P0 == 0) return DSS_OK;
-    DSS_REQUIRE(g->points_world && g->normals_world && g->proj && g->view && (g->h || g->frames), "null input array");
-    DSS_REQUIRE(!(g->h && g->frames), "pass exactly one of h and frames");
-    DSS_REQUIRE(!g->frames || (reinterpret_cast<uintptr_t>(g->frames) & 15) == 0, "frames must be 16-byte aligned");
-    int32_t *zr = reinterpret_cast<int32_t *>(zrange);
-    dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 8), g->n_views);
+    int rc = check_preprocess_inputs(g);
+    if (rc) return rc;
+    dim3 grid(grid_blocks(g->P0, PREPROCESS_THREADS, ctx->sm_count, 8), g->n_views);
     StageScope prof(ctx, ST_PREPROCESS, st);
-    const bool shade = g->shade && g->shaded;
-    if (g->frames) {
-        if (shade) preprocess_frames_kernel<true><<<grid, 256, 0, st>>>(*g, rec, zr);
-        else preprocess_frames_kernel<false><<<grid, 256, 0, st>>>(*g, rec, zr);
-    } else if (shade) {
-        preprocess_kernel<true><<<grid, 256, 0, st>>>(*g, rec, zr);
-    } else {
-        preprocess_kernel<false><<<grid, 256, 0, st>>>(*g, rec, zr);
-    }
+    preprocess_kernel_for<0>(g->frames != nullptr, g->shade && g->shaded)<<<grid, PREPROCESS_THREADS, 0, st>>>(
+        *g, rec, reinterpret_cast<int32_t *>(zrange), PreprocessBins{});
     DSS_LAUNCH_CHECK(ctx);
+    return DSS_OK;
+}
+
+// The fused route's preprocess, which also counts the forward tile lists of `plan` (packed): the depth-range pre-pass,
+// then the counting preprocess.  Fills zrange, the list sizes in BUF_TILE_COUNTS, the packed rectangles and the block
+// offsets, and describes them in *out for bin_and_raster.  The grid is COUNTING_WAVES waves of the counting kernel over
+// all views (at the occupancy its B*B*NS-counter histogram allows), at most one block per 256 points of a view.
+// Every block flushes its whole histogram, so fewer blocks make a cheaper preprocess; but bin_scatter_counted runs on
+// the same grid, and its id stores -- most of its time -- fill each block's slots of a list over the block's whole
+// lifetime: long-lived blocks leave partly written sectors of the (larger than L2) id buffer to be evicted and merged
+// in DRAM.  On the 1M-point / 8 x 512^2 workload (bench.py, H100 SXM, 700 W) 1, 2, 3, 4, 6 and 8 waves gave
+// preprocess + scatter 0.561, 0.524, 0.484, 0.490, 0.513, 0.533 ms and 3 waves the best step (DESIGN.md section 6).
+constexpr int COUNTING_WAVES = 3;
+
+static int run_counting_preprocess(dss_ctx *ctx, const dss_render_args *g, const TilePlan &plan, float4 *rec,
+                                   float *zrange, CountedBins *out, cudaStream_t st) {
+    int rc = check_preprocess_inputs(g);
+    if (rc) return rc;
+    const int N = g->n_views;
+    const int64_t nt = (int64_t)plan.B * plan.B * plan.NS;
+    const int S = g->image_size;
+    PreprocessKernel kern = (S & (S - 1)) == 0 ? preprocess_kernel_for<1>(g->frames != nullptr, g->shade && g->shaded)
+                                               : preprocess_kernel_for<2>(g->frames != nullptr, g->shade && g->shaded);
+    const size_t smem = (size_t)nt * sizeof(int32_t);
+    if (smem > 48 * 1024)
+        DSS_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    DSS_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, PREPROCESS_THREADS, smem));
+    int64_t blocks = (int64_t)COUNTING_WAVES * (per_sm > 0 ? per_sm : 1) * ctx->sm_count / N;
+    const int64_t need = (g->P0 + PREPROCESS_THREADS - 1) / PREPROCESS_THREADS;
+    if (blocks > need) blocks = need;
+    if (blocks < 1) blocks = 1;
+    PreprocessBins pb;
+    pb.zrange = zrange;
+    pb.B = plan.B;
+    pb.NS = plan.NS;
+    if ((rc = ctx_get(ctx, BUF_TILE_COUNTS, (size_t)(N * nt + 1), &pb.counts))) return rc;
+    if ((rc = ctx_get(ctx, BUF_BIN_RECTS, (size_t)g->P, &pb.rects))) return rc;
+    if ((rc = ctx_get(ctx, BUF_BIN_BLOCK_OFFSETS, (size_t)(N * blocks * nt), &pb.block_offsets))) return rc;
+    DSS_CUDA_TRY(cudaMemsetAsync(pb.counts, 0, (size_t)(N * nt + 1) * sizeof(int32_t), st));
+    {
+        StageScope prof(ctx, ST_BIN_COUNT, st);
+        if ((rc = init_zrange(ctx, zrange, N, st))) return rc;
+        const int nv = g->shared_cloud ? N : 1;
+        dim3 grid(grid_blocks(g->P0, 256, ctx->sm_count, 4), g->shared_cloud ? 1 : N);
+        depth_range_kernel<<<grid, 256, (size_t)nv * 18 * sizeof(float), st>>>(*g, reinterpret_cast<int32_t *>(zrange));
+        DSS_LAUNCH_CHECK(ctx);
+    }
+    {
+        StageScope prof(ctx, ST_PREPROCESS, st);
+        kern<<<dim3((unsigned int)blocks, N), PREPROCESS_THREADS, smem, st>>>(*g, rec, nullptr, pb);
+        DSS_LAUNCH_CHECK(ctx);
+    }
+    out->rects = pb.rects;
+    out->block_offsets = pb.block_offsets;
+    out->blocks = (unsigned int)blocks;
     return DSS_OK;
 }
 
@@ -699,7 +871,14 @@ int dss_render_forward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     DSS_REQUIRE((reinterpret_cast<uintptr_t>(rec) & 15) == 0, "records must be 16-byte aligned");
     float *zrange = nullptr;
     if ((rc = ctx_get(ctx, BUF_ZRANGE, (size_t)(2 * g->n_views), &zrange))) return rc;
-    if ((rc = run_preprocess(ctx, g, rec, st, zrange))) return rc;
+    // the preprocess counts the tile lists itself wherever the binning would use block histograms and packed rectangles
+    TilePlan plan;
+    if ((rc = plan_tiles(ctx, g->n_views, g->image_size, g->points_per_pixel, &plan))) return rc;
+    CountedBins counted;
+    const bool count_here = plan.packed && g->P > 0 && g->P0 > 0;
+    if (count_here) rc = run_counting_preprocess(ctx, g, plan, rec, zrange, &counted, st);
+    else rc = run_preprocess(ctx, g, rec, st, zrange);
+    if (rc) return rc;
     if (g->visible) DSS_CUDA_TRY(cudaMemsetAsync(g->visible, 0, (size_t)g->P, st));
     // fused count pass of the backward's binning (see RasterArgs::cell_counts)
     int32_t *cell_counts = nullptr;
@@ -727,8 +906,9 @@ int dss_render_forward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     a.weights = g->weights;
     a.visible = g->visible;
     a.cell_counts = cell_counts;
-    a.zrange = zrange;   // already filled by the preprocess kernel
-    return bin_and_raster(ctx, a, g->shared_cloud ? nullptr : g->first_idx, g->num_points, g->P0, st);
+    a.zrange = zrange;   // already filled by the preprocess or its pre-pass
+    return bin_and_raster(ctx, a, g->shared_cloud ? nullptr : g->first_idx, g->num_points, g->P0, st,
+                          count_here ? &counted : nullptr);
 }
 
 int dss_colour_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {

@@ -83,6 +83,17 @@ DSS_API int64_t dss_debug_tile_total(const dss_ctx *ctx);
  * buffer is sized from the previous call without the host ever waiting for the device.  Results must not change. */
 DSS_API int dss_debug_limit_tile_capacity(dss_ctx *ctx, int64_t max_entries);
 
+/* Testing: on != 0 bins the forward tile lists as DSS_BIN_NORECTS=1 does -- separate count and scatter passes over the
+ * records, the depth ranges from the preprocess -- instead of counting them in the preprocess of dss_render_forward.
+ * Both must produce the same depth ranges, offsets and lists (as sets). */
+DSS_API int dss_debug_bin_no_rects(dss_ctx *ctx, int on);
+
+/* Testing: copies the last forward's binning from the context's scratch, queued on `stream`: the depth ranges of
+ * n_views views (2 floats each) into zrange, the first n_offsets tile-list offsets into offsets and the first n_ids list
+ * entries into ids (each skipped when its pointer is NULL).  Fails when a count exceeds what the scratch holds. */
+DSS_API int dss_debug_tile_lists(dss_ctx *ctx, int n_views, float *zrange, int64_t n_offsets, int32_t *offsets,
+                                 int64_t n_ids, int32_t *ids, void *stream);
+
 /* ---- exclusive prefix sum -----------------------------------------------------------------
  * Replaces prefix_sum.prefix_sum_cuda(grid_cnt, num_grids, grid_off)
  * (external/prefix_sum/prefix_sum.h:6-21, prefix_sum.cu:74-87,135-205): exclusive int32 scan of the
