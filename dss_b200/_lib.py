@@ -47,6 +47,7 @@ class RenderArgs(C.Structure):
         ("grad_albedo", vp), ("grad_normals_world", vp), ("grad_points_shading", vp),
         ("cell_counts", vp),
         ("frames", vp),
+        ("deterministic_colours", C.c_int32),
     ]
 
 
@@ -99,6 +100,7 @@ _SIGNATURES = {
                                           C.POINTER(C.c_int64), C.c_int, C.c_int, vp, vp, vp, vp]),
     "dss_rasterize_mesh": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
+    "dss_chamfer": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int64, C.c_int, vp, vp]),
     "dss_preprocess": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),

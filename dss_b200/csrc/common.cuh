@@ -74,6 +74,8 @@ enum BufId {
     BUF_MESH_RECTS,   //   per (view, face) pixel-index rectangle {column lo, row lo, width, 0}
     BUF_MESH_BLOCKS,  //   per-tile sums of the 64-bit scan
     BUF_MESH_KEYS,    //   per-pixel closest (depth, face) key
+    BUF_COLOUR_FIXED, // deterministic colour backward: per-record 64-bit fixed-point sums and the call's scale
+    BUF_CHAMFER,      // chamfer distance: fp64 per-block partials, then both directions' K = 1 rows (dist, index)
     NUM_BUFS
 };
 

@@ -171,5 +171,10 @@ int zbuf_backward(dss_ctx *ctx, const int32_t *idx, const float *grad_zbuf, int6
 int colour_backward(dss_ctx *ctx, const int32_t *idx, const float *weights, const float *grad_image,
                     int64_t num_pixels, int K, float *grad_colours, int64_t colour_P0, int64_t pixels_per_view,
                     cudaStream_t st);
+// per-record colours (P,3) of views of pixels_per_view pixels, deterministic: 64-bit fixed-point sums (backward.cu);
+// zeroes grad_colours first
+int colour_backward_fixed(dss_ctx *ctx, const int32_t *idx, const float *weights, const float *grad_image,
+                          int64_t num_pixels, int K, float *grad_colours, int64_t P, int64_t pixels_per_view,
+                          cudaStream_t st);
 
 }  // namespace dss

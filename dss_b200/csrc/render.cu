@@ -409,8 +409,15 @@ static int run_colour_backward(dss_ctx *ctx, const dss_render_args *g, cudaStrea
     const int N = g->n_views, S = g->image_size, K = g->points_per_pixel;
     const int64_t npix = (int64_t)N * S * S;
     const int64_t cP0 = (g->shared_cloud && g->shared_colours && !g->shade) ? g->P0 : 0;
-    DSS_CUDA_TRY(cudaMemsetAsync(g->grad_colours, 0, (size_t)(cP0 > 0 ? cP0 : g->P) * 3 * sizeof(float), on));
-    int rc = colour_backward(ctx, g->idx, g->weights, g->grad_image, npix, K, g->grad_colours, cP0, (int64_t)S * S, on);
+    int rc;
+    if (g->shade && g->deterministic_colours) {
+        // the training step's d shaded: summed in fixed point, the same bits every run
+        rc = colour_backward_fixed(ctx, g->idx, g->weights, g->grad_image, npix, K, g->grad_colours, g->P,
+                                   (int64_t)S * S, on);
+    } else {
+        DSS_CUDA_TRY(cudaMemsetAsync(g->grad_colours, 0, (size_t)(cP0 > 0 ? cP0 : g->P) * 3 * sizeof(float), on));
+        rc = colour_backward(ctx, g->idx, g->weights, g->grad_image, npix, K, g->grad_colours, cP0, (int64_t)S * S, on);
+    }
     if (rc || !g->shade) return rc;
     // shading backward: d shaded (P,3) -> d albedo, d normal, d position, per world point (shared cloud) or packed row
     DSS_REQUIRE(g->grad_albedo && g->grad_normals_world && g->grad_points_shading && g->points_world,

@@ -21,7 +21,7 @@ import torch
 from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
-           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh"]
+           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh", "chamfer_distance"]
 
 
 class SplatParams(NamedTuple):
@@ -148,7 +148,8 @@ def _splat_shape(h, frames, rows, N, P):
 class _RenderFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, normals, colours, proj, view, h, first_idx, num_points, shared, prm, want_frags,
-                grad_sync=None, shading=None, cam_centres=None, lights=None, ambient=None, frames=None):
+                grad_sync=None, shading=None, cam_centres=None, lights=None, ambient=None, frames=None,
+                deterministic=False):
         # cam_centres, lights and ambient are the shading's tensors, passed on their own so that autograd tracks them
         dev = _lib.require_cuda(points, normals, colours, proj, view, h, first_idx, num_points, frames)
         points_c = _lib.as_f32(points.detach(), "points")
@@ -211,6 +212,7 @@ class _RenderFunction(torch.autograd.Function):
         ctx.set_materialize_grads(False)
         ctx.save_for_backward(points_c, proj_c, view_c, records, idx, weights, visible, fi, npts)
         ctx.shading = (shading, normals_c, colours_c) if shading is not None else None
+        ctx.deterministic = bool(deterministic)
         ctx.cell_counts = cell_counts
         ctx.meta = (shared, prm, N, P0, P, want_frags, shared_col, grad_sync)
         outs = (image, idx, weights, visible, records, scaler)
@@ -252,6 +254,7 @@ class _RenderFunction(torch.autograd.Function):
             alloc = torch.empty if shared else torch.zeros
             grad_albedo, grad_normals, grad_pshade = (alloc((P0, 3), dtype=torch.float32, device=dev) for _ in range(3))
             _fill_shading(a, sh, albedo_c)
+            a.deterministic_colours = int(ctx.deterministic)
             a.normals_world = _lib.ptr(normals_c)
             a.grad_albedo, a.grad_normals_world = _lib.ptr(grad_albedo), _lib.ptr(grad_normals)
             a.grad_points_shading = _lib.ptr(grad_pshade)
@@ -323,14 +326,15 @@ class _RenderFunction(torch.autograd.Function):
                     light_backward()
                 grad_sync.reduce_late(grad_points)
                 grad_sync.join(dev)
-        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb, None)
+        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb, None, None)
         if shade is not None:
             return (grad_points, grad_normals, grad_albedo) + cams
         return (grad_points, None, grad_colours) + cams
 
 
 def render_points(points, normals, colours, proj, view, h, params: SplatParams, first_idx=None, num_points=None,
-                  shared_cloud=True, return_fragments=False, grad_sync=None, shading=None, frames=None) -> RenderOutput:
+                  shared_cloud=True, return_fragments=False, grad_sync=None, shading=None, frames=None,
+                  deterministic=False) -> RenderOutput:
     """Render ``N`` views of an oriented point cloud to RGBA.
 
     points, normals : (P0,3) when ``shared_cloud`` (one cloud seen from N cameras) else packed (P,3)
@@ -353,11 +357,14 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     grad_sync       : optional dss_b200.parallel.GradSync -- the backward then returns gradients already summed over the
                       ranks of a view-sharded step, the collectives overlapped with the backward kernels (not with
                       fused shading of packed clouds)
+    deterministic   : with ``shading``, the backward sums d L / d shaded in 64-bit fixed point, so that its gradients are
+                      the same bits on every run (the training step asks for it: the loop's resume relies on it); off,
+                      float atomics add those terms in arrival order, which is faster at large P
     """
     outs = _RenderFunction.apply(points, normals, colours, proj, view, h, first_idx, num_points,
                                  bool(shared_cloud), params, bool(return_fragments), grad_sync, shading,
                                  *((shading.cam_centres, shading.lights, shading.ambient) if shading is not None
-                                   else (None, None, None)), frames)
+                                   else (None, None, None)), frames, bool(deterministic))
     image, idx, weights, visible, records, scaler = outs[:6]
     zbuf, qvalue = (outs[6], outs[7]) if return_fragments else (None, None)
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
@@ -566,3 +573,80 @@ def render_mesh(verts, faces, proj, view, image_size, shading: Optional[Shading]
             _lib.stream_ptr(dev))
     _lib.check(rc, "dss_rasterize_mesh")
     return MeshRender(image, pix_to_face, zbuf)
+
+
+def _chamfer_input(points, lengths, normals, name):
+    """pytorch3d's _handle_pointcloud_input in the dss_knn_points layout: a cloud object gives its packed rows and its
+    own normals; a padded (N,P,3) tensor is passed as packed with gaps (cloud n owns rows [n P, n P + lengths[n]))."""
+    if hasattr(points, "points_packed"):
+        pts, nrm = points.points_packed(), points.normals_packed()
+        first, num = points.cloud_to_packed_first_idx(), points.num_points_per_cloud()
+        N = len(points)
+    else:
+        if not torch.is_tensor(points) or points.dim() != 3 or points.shape[2] != 3:
+            raise ValueError("%s must be a PointClouds3D or a padded (N, P, 3) tensor" % name)
+        if normals is not None and tuple(normals.shape) != tuple(points.shape):
+            raise ValueError("%s_normals must have the shape of %s, got %s" % (name, name, tuple(normals.shape)))
+        N, P = points.shape[0], points.shape[1]
+        pts, nrm = points.reshape(N * P, 3), None if normals is None else normals.reshape(N * P, 3)
+        if lengths is not None and (not torch.is_tensor(lengths) or lengths.dim() != 1 or lengths.shape[0] != N):
+            raise ValueError("Expected %s_lengths to be of shape (N,) = (%d,), got %s"
+                             % (name, N, tuple(lengths.shape) if torch.is_tensor(lengths) else type(lengths).__name__))
+        first = torch.arange(N, dtype=torch.int64, device=points.device) * P
+        # a length outside [0, P] would read another cloud's or no storage: clamped on the device, no host sync
+        num = (torch.full((N,), P, dtype=torch.int64, device=points.device) if lengths is None
+               else lengths.to(device=points.device, dtype=torch.int64).clamp(0, P))
+    for t in (pts, nrm):
+        if t is not None and t.requires_grad:
+            raise RuntimeError("chamfer_distance is an evaluation metric without a backward: pass tensors that do not "
+                               "require grad (detach them, or call it under torch.no_grad())")
+    return pts, nrm, first.contiguous(), num.contiguous(), N
+
+
+def chamfer_distance(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None, batch_reduction="mean",
+                     point_reduction="mean"):
+    """pytorch3d's ``chamfer_distance`` [ext, pytorch3d 0.4.0] as the reference's ``Trainer.evaluate_3d`` calls it
+    (DSS/training/trainer.py:158-160), forward only (csrc/chamfer.cu, the rules in include/dss_b200.h).
+
+    ``x`` / ``y``: ``PointClouds3D`` (their own lengths and normals are used) or padded (N,P,3) float32 CUDA tensors with
+    optional ``*_lengths`` (N,) and ``*_normals`` (N,P,3).  Per cloud n: the sum over x's rows of the squared distance
+    to the nearest row of y (smallest (distance, index)), the same from y to x, and with both normals the sums of
+    1 - |cosine_similarity(eps=1e-6)| against the nearest row's normal.  ``point_reduction`` "mean" divides each sum by
+    its cloud's length, "sum" keeps it; ``batch_reduction`` "mean" or "sum" reduces over n, ``None`` keeps (N,).
+    Returns ``(cham_x + cham_y, cham_norm_x + cham_norm_y or None)`` as float32 device tensors.  A row without a
+    neighbour (a NaN or infinite coordinate, an empty other cloud) makes its cloud's terms NaN; padding rows are never
+    read.  No gradients: inputs that require grad raise RuntimeError.  No host synchronisation."""
+    if batch_reduction not in ("mean", "sum", None):
+        raise ValueError('batch_reduction must be one of ["mean", "sum"] or None')
+    if point_reduction not in ("mean", "sum"):
+        raise ValueError('point_reduction must be one of ["mean", "sum"]')
+    sums, xc, yc, with_normals = _chamfer_sums(x, y, x_lengths, y_lengths, x_normals, y_normals)
+    terms = sums
+    if point_reduction == "mean":
+        terms = sums / torch.stack([xc, yc, xc, yc], 1).to(torch.float64)
+    if batch_reduction is not None:
+        terms = terms.sum(0)
+        if batch_reduction == "mean":
+            terms = terms / sums.shape[0]
+    dist = (terms[..., 0] + terms[..., 1]).float()
+    return dist, (terms[..., 2] + terms[..., 3]).float() if with_normals else None
+
+
+def _chamfer_sums(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normals=None):
+    """dss_chamfer on chamfer_distance's inputs -> (sums (N,4) float64 {sum_x d, sum_y d, sum_x c, sum_y c}, x lengths,
+    y lengths, whether both normals were given)"""
+    xp, xn, xf, xc, N = _chamfer_input(x, x_lengths, x_normals, "x")
+    yp, yn, yf, yc, Ny = _chamfer_input(y, y_lengths, y_normals, "y")
+    dev = _lib.require_cuda(xp, xn, xf, xc, yp, yn, yf, yc)
+    if Ny != N:
+        raise ValueError("y does not have the correct shape: %d clouds against %d" % (Ny, N))
+    with_normals = xn is not None and yn is not None
+    xp, yp = _lib.as_f32(xp, "x"), _lib.as_f32(yp, "y")
+    xn, yn = (_lib.as_f32(xn, "x_normals"), _lib.as_f32(yn, "y_normals")) if with_normals else (None, None)
+    sums = torch.zeros((N, 4), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib.load().dss_chamfer(_lib.ctx(dev), _lib.ptr(xp), _lib.ptr(xn), _lib.ptr(xf), _lib.ptr(xc),
+                                     xp.shape[0], _lib.ptr(yp), _lib.ptr(yn), _lib.ptr(yf), _lib.ptr(yc), yp.shape[0],
+                                     N, _lib.ptr(sums), _lib.stream_ptr(dev))
+    _lib.check(rc, "dss_chamfer")
+    return sums, xc, yc, with_normals

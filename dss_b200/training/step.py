@@ -149,6 +149,7 @@ class TrainStep:
                     frames = local_frames(self.points)
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
             out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading,
+                                deterministic=True,
                                 grad_sync=self._sync, frames=frames)
             loss = image_loss(out.image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette,
                               group=self._group)

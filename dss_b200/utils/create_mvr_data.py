@@ -33,7 +33,7 @@ from ..core.lighting import DirectionalLights, PointLights
 from .io import read_mesh, save_obj
 
 __all__ = ["get_tri_color_lights_for_view", "get_light_for_view", "light_value_dict", "sample_points_from_mesh",
-           "normalize_mesh", "write_mvr_data", "create_mvr_data", "main"]
+           "ico_sphere", "normalize_mesh", "write_mvr_data", "create_mvr_data", "main"]
 
 CAMERAS_TYPE = "pytorch3d.renderer.cameras.FoVPerspectiveCameras"
 LIGHTS_TYPE = {False: "DSS.core.lighting.DirectionalLights", True: "DSS.core.lighting.PointLights"}
@@ -122,6 +122,34 @@ def sample_points_from_mesh(verts, faces, num_samples, generator=None):
     points = w0 * v0[fidx] + w1 * v1[fidx] + w2 * v2[fidx]
     normals = F.normalize(cross, dim=1, eps=1e-6)[fidx]
     return points, normals
+
+
+_ICO_T = (1.0 + 5.0 ** 0.5) / 2.0
+_ICO_VERTS = ((-1, _ICO_T, 0), (1, _ICO_T, 0), (-1, -_ICO_T, 0), (1, -_ICO_T, 0), (0, -1, _ICO_T), (0, 1, _ICO_T),
+              (0, -1, -_ICO_T), (0, 1, -_ICO_T), (_ICO_T, 0, -1), (_ICO_T, 0, 1), (-_ICO_T, 0, -1), (-_ICO_T, 0, 1))
+_ICO_FACES = ((0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2),
+              (10, 7, 6), (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11),
+              (6, 2, 10), (8, 6, 7), (9, 8, 1))
+
+
+def ico_sphere(level=0):
+    """Unit icosphere as pytorch3d's ``ico_sphere(level)`` builds it: the icosahedron, then ``level`` times every face
+    split into four at its edge midpoints, the new vertices pushed onto the unit sphere.  10 4^level + 2 vertices,
+    20 4^level faces, counter-clockwise seen from outside.  Returns (verts (V,3) float32, faces (F,3) int64) on the
+    CPU."""
+    verts = torch.tensor(_ICO_VERTS, dtype=torch.float64)
+    verts = verts / verts.norm(dim=1, keepdim=True)
+    faces = torch.tensor(_ICO_FACES, dtype=torch.int64)
+    for _ in range(int(level)):
+        F_, V = faces.shape[0], verts.shape[0]
+        edges = torch.cat([faces[:, [0, 1]], faces[:, [1, 2]], faces[:, [2, 0]]]).sort(dim=1).values
+        unique, inverse = torch.unique(edges, dim=0, return_inverse=True)
+        mid = verts[unique[:, 0]] + verts[unique[:, 1]]
+        verts = torch.cat([verts, mid / mid.norm(dim=1, keepdim=True)])
+        ab, bc, ca = (inverse[k * F_:(k + 1) * F_] + V for k in range(3))
+        a, b, c = faces.unbind(1)
+        faces = torch.cat([torch.stack(f, 1) for f in ((a, ab, ca), (b, bc, ab), (c, ca, bc), (ab, bc, ca))])
+    return verts.float(), faces
 
 
 def normalize_mesh(verts):

@@ -399,6 +399,9 @@ typedef struct dss_render_args {
      * h (I - n n^T); `h` must be NULL.  NULL: the isotropic / invariant kernel with `h`.  The normals still shade and
      * cull. */
     const float *frames;
+    /* with `shade`: != 0 sums the colour scatter into d L / d shaded in 64-bit fixed point (the same bits on every run,
+     * see dss_colour_backward); 0 adds it with float atomics (faster at large P).  The training step sets it. */
+    int32_t deterministic_colours;
 } dss_render_args;
 #define DSS_MAX_LIGHTS 8
 
@@ -410,6 +413,9 @@ DSS_API int dss_render_forward(dss_ctx *ctx, const dss_render_args *args, void *
  * grad_colours == NULL skips the colour scatter (see dss_colour_backward). */
 DSS_API int dss_render_backward(dss_ctx *ctx, const dss_render_args *args, void *stream);
 /* The colour half of the backward alone (norm_weighted_sum backward: grad_colours[idx_k] += g_rgb * w_k), on `stream`.
+ * With `shade` and `deterministic_colours` the per-record d L / d shaded is summed in 64-bit fixed point (one scale per
+ * call, each term rounded once) and is the same bits on every run; otherwise float atomics add the terms in arrival
+ * order.
  * Lets a data-parallel caller start the all-reduce of the colour gradients while dss_render_backward (called with
  * grad_colours == NULL on another stream) is still busy with the occupancy path (dss_b200/parallel.py). */
 DSS_API int dss_colour_backward(dss_ctx *ctx, const dss_render_args *args, void *stream);
@@ -457,6 +463,22 @@ DSS_API int dss_rasterize_mesh(dss_ctx *ctx, const float *verts, int64_t V, cons
                                int light_type, int lights_per_view, float shininess, const float *lights,
                                const float *ambient, const float *cam_centres, int32_t *pix_to_face, float *zbuf,
                                float *rgba, void *stream);
+
+/* ---- chamfer distance (evaluation only, no backward) ----------------------------------------------------------------
+ * The sums behind pytorch3d's chamfer_distance as Trainer.evaluate_3d calls it (DSS/training/trainer.py:144-171).  x
+ * (Px,3) and y (Py,3) f32 hold N clouds each in the dss_knn_points layout (cloud n owns rows [first[n], first[n] +
+ * num[n]); gaps allowed, overlaps not); x_normals / y_normals are indexed like the points, both or neither may be NULL.
+ * For every query row its nearest row of the other cloud n -- the smallest (squared distance, index), the
+ * dss_knn_points rule and its float32 distance -- gives d; with normals, c = 1 - |cos| of the two normals, where
+ * cos = sum_k (a_k / max(|a|, 1e-6)) (b_k / max(|b|, 1e-6)) in fp64 (torch's cosine_similarity, eps = 1e-6).  A row
+ * without a neighbour (a NaN or infinite coordinate, or an empty other cloud) gives d = c = NaN.
+ * Output sums (N,4) f64: {sum_x d, sum_y d, sum_x c, sum_y c} (the normal sums are 0 without normals).  Two K = 1
+ * searches (their rows in context scratch), one thread per query row of both directions writing fp64 per-block
+ * partials, one fixed-order finish: deterministic, no atomics on floats, no host synchronisation, capturable.  x and y
+ * may be the same rows (the tie rule holds there too). */
+DSS_API int dss_chamfer(dss_ctx *ctx, const float *x, const float *x_normals, const int64_t *x_first,
+                        const int64_t *x_num, int64_t Px, const float *y, const float *y_normals,
+                        const int64_t *y_first, const int64_t *y_num, int64_t Py, int N, double *sums, void *stream);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,137 @@
+"""Time the training loop's pieces: ops.chamfer_distance (csrc/chamfer.cu) at 8000 ground-truth points against 5 000,
+100 000 and 1 000 000 model points with normals, next to a torch brute force (torch.cdist in chunks on the GPU), and the
+loop of dss_b200.training.train at configs/dss.yml's settings (5000 points, 8 views per batch, 512^2) next to bare
+GraphedTrainStep.replay() on the same batches.
+
+    python scripts/train_loop_time.py [--iters 20] [--loop-its 200] [--out results.json]
+
+CUDA events around each chamfer call, median after warm-up.  The loop's rate is taken between two of its own logged
+records (each ends in a host synchronisation), after the capture and a warm-up.  Prints one JSON line with the card name
+and its power limit."""
+import argparse
+import json
+import os
+import shutil
+import sys
+import tempfile
+import time
+
+import torch
+import torch.nn.functional as F
+import yaml
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "scripts"))
+
+from dss_b200.ops import chamfer_distance  # noqa: E402
+from mesh_raster_time import card, timed  # noqa: E402
+
+
+def torch_chamfer(x, y, xn, yn, budget=1 << 28):
+    """pytorch3d's chamfer_distance (mean, mean) for one cloud each, as chunked torch.cdist on the device"""
+    def one_way(q, p, qn, pn):
+        chunk = max(1, budget // p.shape[0])
+        d, c = [], []
+        for s in range(0, q.shape[0], chunk):
+            m, a = (torch.cdist(q[s:s + chunk], p) ** 2).min(1)
+            d.append(m)
+            c.append(1 - F.cosine_similarity(qn[s:s + chunk], pn[a], dim=1, eps=1e-6).abs())
+        return torch.cat(d).mean(), torch.cat(c).mean()
+    dx, cx = one_way(x, y, xn, yn)
+    dy, cy = one_way(y, x, yn, xn)
+    return dx + dy, cx + cy
+
+
+def chamfer_times(dev, warmup, iters):
+    g = torch.Generator().manual_seed(0)
+    gt = F.normalize(torch.randn(8000, 3, generator=g), dim=1).to(dev)
+    gtn = gt.clone()
+    out = {}
+    for P in (5000, 100000, 1000000):
+        y = (F.normalize(torch.randn(P, 3, generator=g), dim=1) * 0.9 + 0.01 * torch.randn(P, 3, generator=g)).to(dev)
+        yn = F.normalize(torch.randn(P, 3, generator=g), dim=1).to(dev)
+        ours = chamfer_distance(gt[None], y[None], x_normals=gtn[None], y_normals=yn[None])
+        ref = torch_chamfer(gt, y, gtn, yn)
+        out["chamfer_ms_8000x%d" % P] = timed(
+            lambda: chamfer_distance(gt[None], y[None], x_normals=gtn[None], y_normals=yn[None]), warmup, iters)
+        out["torch_cdist_ms_8000x%d" % P] = timed(lambda: torch_chamfer(gt, y, gtn, yn), 1, max(3, iters // 4))
+        out["rel_diff_8000x%d" % P] = [float((ours[k] - ref[k]).abs() / ref[k].abs()) for k in (0, 1)]
+    return out
+
+
+def loop_times(dev, loop_its, tmp):
+    from dss_b200.training.config import load_config
+    from dss_b200.training.train import Trainer
+    from dss_b200.utils.create_mvr_data import main as create
+    from dss_b200.utils.io import save_obj
+    from tests.test_mesh_data import torus
+    verts, faces = torus(nu=192, nv=96)
+    save_obj(os.path.join(tmp, "torus.obj"), verts.numpy(), faces.numpy())
+    data_dir = create(["--points", os.path.join(tmp, "torus.obj"), "--output", os.path.join(tmp, "data"),
+                       "--num_cameras", "64", "--image-size", "512", "--tri_color_light", "--point_lights"])[0]
+    cfg_path = os.path.join(tmp, "dss.yml")
+    warm = 40
+    with open(cfg_path, "w") as f:
+        yaml.safe_dump({
+            "name": "time", "data": {"data_dir": data_dir},
+            "model": {"model_kwargs": {"n_points_per_cloud": 5000, "learn_colors": False}},
+            "renderer": {"raster_params": {"Vrk_invariant": True, "Vrk_isotropic": False, "clip_pts_grad": 0.05,
+                                           "cutoff_threshold": 1.0, "depth_merging_threshold": 0.05,
+                                           "image_size": 512, "points_per_pixel": 5, "radii_backward_scaler": 5}},
+            "training": {"out_dir": os.path.join(tmp, "out"), "batch_size": 8, "lambda_dr_proj": 0.01,
+                         "lambda_dr_repel": 0.0, "steps_dss_backward_radii": 200, "print_every": warm,
+                         "validate_every": 0, "checkpoint_every": 0}}, f)
+    t = Trainer(load_config(cfg_path))
+    t.run(exit_after=-1, max_it=warm + loop_its + 1)
+    with open(os.path.join(t.out_dir, "metrics.jsonl")) as f:
+        recs = [json.loads(line) for line in f]
+    first = next(r for r in recs if r["it"] >= warm)
+    last = recs[-1]
+    res = {"loop_it_per_s": (last["it"] - first["it"]) / (last["time"] - first["time"]),
+           "loop_its_timed": last["it"] - first["it"]}
+    # bare replays of the same step on batches already on the device
+    step = t.step
+    batches = [t._batch(t.order[i:i + 8]) for i in range(0, 64, 8)]
+    torch.cuda.synchronize()
+    for b in batches:
+        step.load(*b)
+        step.replay()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for i in range(loop_its):
+        step.load(*batches[i % len(batches)])
+        step.replay()
+    torch.cuda.synchronize()
+    res["replay_it_per_s"] = loop_its / (time.perf_counter() - t0)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    ev = t.evaluate()
+    res["validation_ms_5000_vs_8000"] = (time.perf_counter() - t0) * 1e3
+    res["chamfer_point_at_end"] = ev["chamfer_point"]
+    return res
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--iters", type=int, default=20)
+    ap.add_argument("--loop-its", type=int, default=200)
+    ap.add_argument("--out", default=None)
+    opt = ap.parse_args()
+    dev = torch.device("cuda:0")
+    res = chamfer_times(dev, opt.warmup, opt.iters)
+    tmp = tempfile.mkdtemp(prefix="dss_loop_time_")
+    try:
+        res.update(loop_times(dev, opt.loop_its, tmp))
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
+    res["card"], res["power_limit"] = card()
+    print(json.dumps(res))
+    if opt.out:
+        with open(opt.out, "w") as f:
+            json.dump(res, f)
+
+
+if __name__ == "__main__":
+    main()
