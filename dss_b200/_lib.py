@@ -101,6 +101,7 @@ _SIGNATURES = {
     "dss_rasterize_mesh": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
     "dss_chamfer": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int64, C.c_int, vp, vp]),
+    "dss_point_mesh_distance": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, vp, vp]),
     "dss_preprocess": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),

@@ -14,7 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdss_b200.so")
 SOURCES = ["ctx.cu", "binning.cu", "raster_fwd.cu", "backward.cu", "occ_backward.cu", "knn.cu", "render.cu",
-           "regularisers.cu", "image_loss.cu", "point_filter.cu", "local_frames.cu", "mesh_raster.cu", "chamfer.cu"]
+           "regularisers.cu", "image_loss.cu", "point_filter.cu", "local_frames.cu", "mesh_raster.cu", "chamfer.cu",
+           "mesh_distance.cu"]
 HEADERS = ["binning.cuh", "common.cuh", "kernels.cuh", "shading.cuh", os.path.join("..", "..", "include", "dss_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper)

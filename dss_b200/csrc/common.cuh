@@ -76,6 +76,11 @@ enum BufId {
     BUF_MESH_KEYS,    //   per-pixel closest (depth, face) key
     BUF_COLOUR_FIXED, // deterministic colour backward: per-record 64-bit fixed-point sums and the call's scale
     BUF_CHAMFER,      // chamfer distance: fp64 per-block partials, then both directions' K = 1 rows (dist, index)
+    BUF_PMD_STATE,    // point-mesh distance: face bounding box, grid parameters and the reference total
+    BUF_PMD_TRIS,     //   the usable faces' vertices, 3 float4 per face
+    BUF_PMD_COUNTS,   //   face references per grid cell
+    BUF_PMD_OFFSETS,  //   exclusive scan of the counts
+    BUF_PMD_REFS,     //   face indices in cell order
     NUM_BUFS
 };
 

@@ -21,7 +21,8 @@ import torch
 from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
-           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh", "chamfer_distance"]
+           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh", "chamfer_distance",
+           "PointMeshDistance", "point_mesh_distance"]
 
 
 class SplatParams(NamedTuple):
@@ -650,3 +651,47 @@ def _chamfer_sums(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normal
                                      N, _lib.ptr(sums), _lib.stream_ptr(dev))
     _lib.check(rc, "dss_chamfer")
     return sums, xc, yc, with_normals
+
+
+class PointMeshDistance(NamedTuple):
+    sq_dists: torch.Tensor            # (P,) float32 squared distance to the nearest face, NaN for a non-finite query
+    face_idx: torch.Tensor            # (P,) int64 that face, -1 where there is none
+    closest: Optional[torch.Tensor]   # (P,3) float32 the closest point on it, or None when not asked for
+
+
+def point_mesh_distance(points, verts, faces, return_closest=False, _face_tests=None) -> PointMeshDistance:
+    """Exact distance from every point to one triangle mesh (csrc/mesh_distance.cu; the rules are in
+    include/dss_b200.h): each face is the closed triangle of its vertices, distances are formed in float64 and rounded
+    once, a tie goes to the smaller face index, and the result equals a brute force over all faces.
+
+    points (P,3) and verts (V,3) float32 CUDA tensors, faces (F,3) integer with every index in [0, V) (checked here).
+    A point with a NaN or infinite coordinate gets NaN / -1; faces on a non-finite vertex are never nearest; without a
+    usable face every point gets NaN / -1.  Forward only: inputs that require grad raise RuntimeError.  The call
+    synchronises the host once, to size the search structure."""
+    dev = _lib.require_cuda(points, verts, faces)
+    for name, t in (("points", points), ("verts", verts)):
+        if t.requires_grad:
+            raise RuntimeError("point_mesh_distance has no backward: pass %s that does not require grad (detach it, "
+                               "or call it under torch.no_grad())" % name)
+    p, v = _lib.as_f32(points, "points"), _lib.as_f32(verts, "verts")
+    if p.dim() != 2 or p.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3), got %s" % (tuple(p.shape),))
+    if v.dim() != 2 or v.shape[1] != 3:
+        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
+        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
+    P, V, F = p.shape[0], v.shape[0], faces.shape[0]
+    if P >= 2 ** 31 or V >= 2 ** 31 or F >= 2 ** 31:
+        raise ValueError("at most 2^31 - 1 points, vertices and faces")
+    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
+        raise ValueError("face indices must lie in [0, %d)" % V)
+    f = faces.to(torch.int32).contiguous()
+    sq = torch.empty(P, dtype=torch.float32, device=dev)
+    idx = torch.empty(P, dtype=torch.int32, device=dev)
+    closest = torch.empty((P, 3), dtype=torch.float32, device=dev) if return_closest else None
+    with torch.cuda.device(dev):
+        rc = _lib.load().dss_point_mesh_distance(_lib.ctx(dev), _lib.ptr(p), P, _lib.ptr(v), V, _lib.ptr(f), F,
+                                                 _lib.ptr(sq), _lib.ptr(idx), _lib.ptr(closest), _lib.ptr(_face_tests),
+                                                 _lib.stream_ptr(dev))
+    _lib.check(rc, "dss_point_mesh_distance")
+    return PointMeshDistance(sq, idx.long(), closest)

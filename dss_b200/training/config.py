@@ -126,6 +126,19 @@ def check_config(cfg, resolution, has_lights):
         raise ValueError("the data directory has no lights_%d entries: the loop shades with the data's lights")
 
 
+SELECTION_METRICS = ("chamfer_point", "chamfer_normal", "p2f_avg")
+
+
+def selection_metric(cfg):
+    """``training.model_selection_metric`` if the loop can select by it: the chamfer distances of the reference's
+    trainer, or ``p2f_avg``, the mean distance of the cloud's points to ``<data_dir>/mesh.obj``."""
+    metric = cfg["training"]["model_selection_metric"]
+    if metric not in SELECTION_METRICS:
+        raise NotImplementedError("model_selection_metric %r: the loop selects by one of %s"
+                                  % (metric, ", ".join(SELECTION_METRICS)))
+    return metric
+
+
 def splat_params(cfg, znear, zfar):
     """``SplatParams`` of ``renderer.raster_params`` (``bin_size`` / ``max_points_per_bin`` are accepted and ignored, as
     ``PointsRasterizationSettings`` ignores them) with the data cameras' depth range."""

@@ -16,8 +16,10 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   trainer.py:114-123): see :func:`radii_backward_scaler` and :func:`compound_lambda_proj`.
 - every ``print_every`` iterations the losses go to ``<out>/<logfile>`` and one JSON line to ``<out>/metrics.jsonl``
   (the loop's only host synchronisations besides validation); every ``validate_every`` (it > 0) the chamfer distances
-  of the ground-truth cloud against the current one (trainer.py:144-171), and on improvement ``model_best.pt`` and
-  ``val/best.ply``; ``model.pt`` every ``checkpoint_every``, ``model_%d.pt`` every ``backup_every``.
+  of the ground-truth cloud against the current one (trainer.py:144-171), and on improvement of
+  ``training.model_selection_metric`` ``model_best.pt`` and ``val/best.ply``.  With the metric ``p2f_avg`` the loop
+  reads ``<data_dir>/mesh.obj`` once (it must exist) and every validation adds ``p2f_avg`` / ``p2f_std``, the mean and
+  population standard deviation of the exact distances of the cloud's points to that mesh; ``model.pt`` every ``checkpoint_every``, ``model_%d.pt`` every ``backup_every``.
 - ``training.resume_from`` (in ``<out>``) is loaded when it exists, and the run continues where it stopped, mid-epoch
   included: a resumed run computes what an uninterrupted one does.  (The reference starts a new epoch.)
 - ``--exit-after S`` saves ``model.pt`` and exits with status 3 once S seconds have passed (checked after every
@@ -40,8 +42,9 @@ from ..core.lighting import DirectionalLights, PointLights
 from ..ops import chamfer_distance
 from ..utils.create_mvr_data import ico_sphere, sample_points_from_mesh
 from ..utils.dataset import MVRData
+from ..utils.evaluate import p2f_stats
 from ..utils.io import read_mesh, save_ply
-from .config import check_config, load_config, splat_params, step_settings
+from .config import check_config, load_config, selection_metric, splat_params, step_settings
 from .step import GraphedTrainStep
 
 __all__ = ["radii_backward_scaler", "compound_lambda_proj", "initial_cloud", "make_optimizer", "make_lr_scheduler",
@@ -152,6 +155,13 @@ class Trainer:
         V = len(self.data)
         lights = [self.data[i].get("lights") for i in range(V)]
         check_config(cfg, self.data.resolution, all(l is not None for l in lights))
+        self.mesh = None
+        if selection_metric(cfg) == "p2f_avg":
+            mesh_path = os.path.join(dc["data_dir"], "mesh.obj")
+            if not os.path.isfile(mesh_path):
+                raise ValueError("model_selection_metric p2f_avg measures against %s, which does not exist" % mesh_path)
+            verts, faces = read_mesh(mesh_path)
+            self.mesh = (torch.from_numpy(verts).float().to(self.dev), torch.from_numpy(faces).to(self.dev))
         kind = str(self.data.data_dict["lights_type"]) if "lights_type" in self.data.data_dict else ""
         self.light_cls = PointLights if "PointLights" in kind else DirectionalLights
         vec = "location" if self.light_cls is PointLights else "direction"
@@ -174,9 +184,6 @@ class Trainer:
         self.sign = {"minimize": -1, "maximize": 1}.get(tr["model_selection_mode"])
         if self.sign is None:
             raise ValueError("model_selection_mode must be either maximize or minimize.")
-        if tr["model_selection_metric"] not in ("chamfer_point", "chamfer_normal"):
-            raise NotImplementedError("model_selection_metric %r: the loop selects by chamfer_point or chamfer_normal"
-                                      % tr["model_selection_metric"])
         self.best = -self.sign * math.inf
         self.radii_init = self.params.radii_backward_scaler
         self.lambda_dr_proj = self.settings["lambda_dr_proj"]
@@ -240,11 +247,15 @@ class Trainer:
         return self.step.points.detach(), F.normalize(self.step.normals.detach(), dim=-1)
 
     def evaluate(self):
-        """trainer.py:144-171: chamfer distances of the ground truth (x) against the current cloud (y)"""
+        """trainer.py:144-171: chamfer distances of the ground truth (x) against the current cloud (y); selecting by
+        p2f_avg, also the mean and population standard deviation of the points' distances to the data's mesh"""
         points, normals = self.cloud()
         with torch.no_grad():
             cd_p, cd_n = chamfer_distance(PointClouds3D([self.gt[0]], [self.gt[1]]), PointClouds3D([points], [normals]))
-        return {"chamfer_point": float(cd_p), "chamfer_normal": float(cd_n)}
+        ev = {"chamfer_point": float(cd_p), "chamfer_normal": float(cd_n)}
+        if self.mesh is not None:
+            _, ev["p2f_avg"], ev["p2f_std"] = p2f_stats(points, self.mesh)
+        return ev
 
     def save(self, name):
         s = self.step

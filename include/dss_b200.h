@@ -480,6 +480,29 @@ DSS_API int dss_chamfer(dss_ctx *ctx, const float *x, const float *x_normals, co
                         const int64_t *x_num, int64_t Px, const float *y, const float *y_normals,
                         const int64_t *y_first, const int64_t *y_num, int64_t Py, int N, double *sums, void *stream);
 
+/* ---- point-to-mesh distance (evaluation only, no backward) ---------------------------------------------------------
+ * The point-to-surface term of the reference's scripts/evaluatePointClouds.py, exact.  queries (P,3) f32, one mesh
+ * verts (V,3) f32 / faces (F,3) i32.  Every face is the closed convex hull of its three vertices, so a zero-area face
+ * is a segment or a point.  For every query q:
+ *   sq_dist[q]  (P,) f32: the smallest squared Euclidean distance from q to any face, computed in fp64 from the f32
+ *               inputs (the closest point of a face by its Voronoi regions, every operation rounded on its own; a face
+ *               whose edge vectors have an exactly zero cross product takes the closest of its three edges) and
+ *               rounded once to f32;
+ *   face_idx[q] (P,) i32: the face attaining it, an exact fp64 tie to the smaller face index;
+ *   closest     (P,3) f32 or NULL (not written): the closest point on that face, each coordinate rounded once.
+ * A query with a NaN or infinite coordinate gets NaN / -1 (closest NaN).  A face with an index outside [0, V) or a
+ * non-finite vertex is ignored: never nearest, and it does not shape the acceleration structure (as in
+ * dss_rasterize_mesh).  Without any usable face every query gets NaN / -1.  The result equals a brute force over all
+ * faces: a uniform grid over the usable faces' bounding box (built on the device, its cell size from the face density,
+ * at most 2^21 cells) only decides which faces a query tests, and each query's search stops once no untested face can
+ * be nearer (DESIGN.md).  Deterministic (integer atomics only).  The call synchronises the host ONCE, after counting
+ * the grid's face references, to size that list in the context's scratch (so it cannot be captured in a CUDA graph);
+ * more than 2^31 - 1 references is DSS_E_CAPACITY.  face_tests (P,) i32 or NULL: for measuring the search, the number
+ * of face distances each query evaluated. */
+DSS_API int dss_point_mesh_distance(dss_ctx *ctx, const float *queries, int64_t P, const float *verts, int64_t V,
+                                    const int32_t *faces, int64_t F, float *sq_dist, int32_t *face_idx, float *closest,
+                                    int32_t *face_tests, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
