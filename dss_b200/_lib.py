@@ -102,6 +102,11 @@ _SIGNATURES = {
                                      C.c_int, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
     "dss_chamfer": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int64, C.c_int, vp, vp]),
     "dss_point_mesh_distance": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, vp, C.c_int64, vp, vp, vp, vp, vp]),
+    "dss_poisson_solve": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int, vp, C.POINTER(C.c_float), C.POINTER(C.c_float),
+                                    C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_int),
+                                    C.POINTER(C.c_float), vp]),
+    "dss_marching_tetrahedra": (C.c_int, [vp, vp, C.c_int, C.POINTER(C.c_float), C.c_float, vp, C.c_int64, vp,
+                                          C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp]),
     "dss_preprocess": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),

@@ -81,6 +81,11 @@ enum BufId {
     BUF_PMD_COUNTS,   //   face references per grid cell
     BUF_PMD_OFFSETS,  //   exclusive scan of the counts
     BUF_PMD_REFS,     //   face indices in cell order
+    BUF_PSN_STATE,    // Poisson solve: the samples' box, the CG state and the fp64 per-block partials
+    BUF_PSN_GRID,     //   8 node arrays of the finest level: cell map, residual, then S (3 x 64 bit) / p, q, 1 / diag
+    BUF_PSN_COARSE,   //   the previous level's solution, for the prolongation
+    BUF_PSN_CELLS,    //   per occupied cell: 36 fixed-point entries of its block of Q, then the 64 float entries
+    BUF_MT,           // marching tetrahedra: totals, per-node vertex counts / bases, per-cube face counts / bases, masks
     NUM_BUFS
 };
 

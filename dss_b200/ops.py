@@ -22,7 +22,7 @@ from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
            "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh", "chamfer_distance",
-           "PointMeshDistance", "point_mesh_distance"]
+           "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra"]
 
 
 class SplatParams(NamedTuple):
@@ -695,3 +695,84 @@ def point_mesh_distance(points, verts, faces, return_closest=False, _face_tests=
                                                  _lib.stream_ptr(dev))
     _lib.check(rc, "dss_point_mesh_distance")
     return PointMeshDistance(sq, idx.long(), closest)
+
+
+class PoissonMesh(NamedTuple):
+    verts: torch.Tensor               # (V,3) float32 on the device of the input
+    faces: torch.Tensor               # (F,3) int64, each face's normal pointing outwards
+    grid: Optional[torch.Tensor]      # (R+1, R+1, R+1) float32 chi (negative inside), or None when not asked for
+    origin: torch.Tensor              # (3,) float32 (CPU): the centre c the grid is placed around
+    side: float                       # L, the grid's edge length: node (i, j, k) lies at c + (h (i, j, k) - 0.5) L
+    iterations: int                   # CG iterations of the finest level
+    residual: float                   # its final relative residual |r| / |b|
+
+
+def marching_tetrahedra(grid, origin, side):
+    """The chi = 0 surface of a node grid (csrc/poisson.cu; the rules are in include/dss_b200.h): every cube split into
+    6 Kuhn tetrahedra, one vertex per crossing edge, faces oriented from chi < 0 (inside) to chi >= 0 (outside).
+
+    grid (R+1, R+1, R+1) float32 CUDA tensor, x-major; origin the centre c (3 numbers or a tensor), side the edge L:
+    node (i, j, k) lies at c + (h (i, j, k) - 0.5) L with h = 1 / R.  Returns (verts (V,3) float32, faces (F,3) int64),
+    vertices ordered by (node, edge direction), faces by (cube, tetrahedron, triangle).  Synchronises the host twice:
+    once to size the outputs, once in the call that fills them."""
+    dev = _lib.require_cuda(grid)
+    g = _lib.as_f32(grid, "grid")
+    if g.dim() != 3 or g.shape[0] != g.shape[1] or g.shape[0] != g.shape[2] or g.shape[0] < 2:
+        raise RuntimeError("grid must have shape (R+1, R+1, R+1) with R >= 1, got %s" % (tuple(g.shape),))
+    if g.requires_grad:
+        raise RuntimeError("marching_tetrahedra has no backward: pass a grid that does not require grad")
+    R = g.shape[0] - 1
+    c = (C.c_float * 3)(*[float(v) for v in (origin.tolist() if torch.is_tensor(origin) else origin)])
+    nv, nf = C.c_int64(0), C.c_int64(0)
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.dss_marching_tetrahedra(_lib.ctx(dev), _lib.ptr(g), R, c, float(side), None, 0, None, 0,
+                                         C.byref(nv), C.byref(nf), _lib.stream_ptr(dev))
+        if rc == _lib.DSS_E_CAPACITY and nv.value < 2 ** 31 and nf.value < 2 ** 31:
+            verts = torch.empty((nv.value, 3), dtype=torch.float32, device=dev)
+            faces = torch.empty((nf.value, 3), dtype=torch.int32, device=dev)
+            rc = lib.dss_marching_tetrahedra(_lib.ctx(dev), _lib.ptr(g), R, c, float(side), _lib.ptr(verts),
+                                             nv.value, _lib.ptr(faces), nf.value, C.byref(nv), C.byref(nf),
+                                             _lib.stream_ptr(dev))
+        else:
+            verts = torch.empty((0, 3), dtype=torch.float32, device=dev)
+            faces = torch.empty((0, 3), dtype=torch.int32, device=dev)
+    _lib.check(rc, "dss_marching_tetrahedra")
+    return verts, faces.long()
+
+
+def poisson_reconstruction(points, normals, depth=8, return_grid=False) -> PoissonMesh:
+    """Screened Poisson surface reconstruction of an oriented cloud (csrc/poisson.cu; the discretisation is in
+    include/dss_b200.h): the indicator chi on the 2^depth grid around the usable samples, then its chi = 0 surface by
+    :func:`marching_tetrahedra`.  What the reference's ``Generator.generate_mesh`` gets from pymeshlab's
+    ``surface_reconstruction_screened_poisson(depth=8)``, with trilinear elements instead of Kazhdan's B-splines.
+
+    points, normals (P,3) float32 CUDA tensors; a row with a non-finite value or a zero normal is ignored, normals need
+    not be unit.  depth in [2, 9].  Without a usable sample, or when they all coincide, the mesh is empty.  The result
+    is the same bits for any order of the rows.  Forward only: inputs that require grad raise RuntimeError.  The host
+    synchronises once every few dozen CG iterations (DESIGN.md)."""
+    dev = _lib.require_cuda(points, normals)
+    for name, t in (("points", points), ("normals", normals)):
+        if t.requires_grad:
+            raise RuntimeError("poisson_reconstruction has no backward: pass %s that does not require grad (detach it, "
+                               "or call it under torch.no_grad())" % name)
+    p, n = _lib.as_f32(points, "points"), _lib.as_f32(normals, "normals")
+    if p.dim() != 2 or p.shape[1] != 3 or n.shape != p.shape:
+        raise RuntimeError("points and normals must both have shape (P, 3), got %s and %s"
+                           % (tuple(p.shape), tuple(n.shape)))
+    if not 2 <= int(depth) <= 9:
+        raise ValueError("depth must lie in [2, 9], got %r" % (depth,))
+    depth = int(depth)
+    P, R = p.shape[0], 1 << depth
+    if P >= 2 ** 31:
+        raise ValueError("at most 2^31 - 1 samples")
+    chi = torch.empty((R + 1, R + 1, R + 1), dtype=torch.float32, device=dev)
+    c, L = (C.c_float * 3)(), C.c_float(0.0)
+    its, res = C.c_int(0), C.c_double(0.0)
+    with torch.cuda.device(dev):
+        rc = _lib.load().dss_poisson_solve(_lib.ctx(dev), _lib.ptr(p), _lib.ptr(n), P, depth, _lib.ptr(chi), c,
+                                           C.byref(L), C.byref(its), C.byref(res), None, None, _lib.stream_ptr(dev))
+    _lib.check(rc, "dss_poisson_solve")
+    origin = torch.tensor(list(c), dtype=torch.float32)
+    verts, faces = marching_tetrahedra(chi, origin, L.value)
+    return PoissonMesh(verts, faces, chi if return_grid else None, origin, L.value, its.value, res.value)

@@ -89,8 +89,10 @@ def read_ply(path):
     return {"points": pts, "normals": nrm, "colors": col, "properties": data}
 
 
-def save_ply(filename, points, colors=None, normals=None, binary=True):
-    """DSS/utils/io.py:89-146.  points (N, 2 or 3); colors (N, 3 or 4), scaled by 255 when max <= 1; normals (N, 2 or 3)."""
+def save_ply(filename, points, colors=None, normals=None, binary=True, faces=None):
+    """DSS/utils/io.py:89-146.  points (N, 2 or 3); colors (N, 3 or 4), scaled by 255 when max <= 1; normals (N, 2 or 3).
+    faces (F, 3) integer indices into the points, or None: a ``face`` element (``property list uchar int
+    vertex_indices``) after the vertices, as trimesh writes a mesh; without it the file is unchanged."""
     points = np.asarray(points)
     if points.ndim != 2:
         raise ValueError("points must be (N, 2 or 3)")
@@ -122,17 +124,30 @@ def save_ply(filename, points, colors=None, normals=None, binary=True):
     d = os.path.dirname(filename)
     if d and not os.path.exists(d):
         os.makedirs(d)
+    if faces is not None:
+        faces = np.asarray(faces).reshape(-1, 3)
+        if faces.size and (faces.min() < 0 or faces.max() >= n):
+            raise ValueError("face index out of range [0, %d)" % n)
     type_names = {"<f4": "float", "u1": "uchar"}
     header = ["ply", "format %s 1.0" % ("binary_little_endian" if binary else "ascii"), "element vertex %d" % n]
     header += ["property %s %s" % (type_names[t], name) for name, t in fields]
+    if faces is not None:
+        header += ["element face %d" % len(faces), "property list uchar int vertex_indices"]
     header += ["end_header"]
     with open(filename, "wb") as f:
         f.write(("\n".join(header) + "\n").encode("ascii"))
         if binary:
             f.write(rec.tobytes())
+            if faces is not None:
+                frec = np.empty(len(faces), dtype=np.dtype([("n", "u1"), ("i", "<i4", (3,))]))
+                frec["n"] = 3
+                frec["i"] = faces
+                f.write(frec.tobytes())
         else:
             for row in rec:
                 f.write((" ".join(repr(float(v)) if isinstance(v, np.floating) else str(int(v)) for v in row) + "\n").encode("ascii"))
+            if faces is not None:
+                f.writelines(("3 %d %d %d\n" % tuple(int(i) for i in t)).encode("ascii") for t in faces)
 
 
 def _fan(poly):

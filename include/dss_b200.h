@@ -503,6 +503,73 @@ DSS_API int dss_point_mesh_distance(dss_ctx *ctx, const float *queries, int64_t 
                                     const int32_t *faces, int64_t F, float *sq_dist, int32_t *face_idx, float *closest,
                                     int32_t *face_tests, void *stream);
 
+/* ---- screened Poisson surface reconstruction (forward only) ---------------------------------------------------------
+ * The surface of the reference's Generator.generate_mesh (DSS/models/point_modeling.py:256-282, pymeshlab's
+ * surface_reconstruction_screened_poisson(depth=8)), restated as Kazhdan & Hoppe's screened Poisson reconstruction on a
+ * dense grid with first-order (trilinear) elements.  The discretisation:
+ *   - usable sample: finite coordinates and normal, |n| > 0; its unit normal n / |n| (fp64).  Other rows are ignored.
+ *   - domain: c = centre of the usable samples' bounding box, L = 1.1 x its longest side, both rounded to float32 as
+ *     c_k = (float)(0.5 (lo_k + hi_k)) and L = (float)(1.1 max_k (hi_k - lo_k)) in fp64.  A sample maps to
+ *     u = (p - c) / L + 0.5 (fp64, from the float32 c and L), inside [0.045, 0.955]^3.
+ *   - grid: R = 2^depth cells per axis, h = 1 / R, nodes u = h (i, j, k) for i, j, k in [0, R], stored x-major:
+ *     node (i, j, k) at (i (R+1) + j) (R+1) + k.  phi_n is the trilinear hat of node n.
+ *   - A = h^2 x (cells holding at least one usable sample), a = A / N_usable;  V = sum_n V_n phi_n,
+ *     V_n = (a / h^3) sum_p phi_n(u_p) n_p.
+ *   - chi minimises  integral over [0,1]^3 of |grad chi - V|^2  +  alpha a sum_p chi(u_p)^2,  alpha =
+ *     DSS_POISSON_POINT_WEIGHT: (K + alpha a Q) chi = b with K_nm = int grad phi_n . grad phi_m, Q_nm = sum_p phi_n(u_p)
+ *     phi_m(u_p), b_n = int grad phi_n . V; natural (Neumann) boundary, every node an unknown.  On the tensor basis
+ *     K = K1(x)M1(x)M1 + M1(x)K1(x)M1 + M1(x)M1(x)K1 and b = (D1(x)M1(x)M1) V_x + (M1(x)D1(x)M1) V_y + (M1(x)M1(x)D1) V_z
+ *     with the 1-D mass M1, stiffness K1 and D1[n][m] = int phi_n' phi_m.
+ *   - iso-value 0: 1^T K = 0 and sum_n b_n = 0, so sum_p chi(u_p) = 0 at the solution.  chi < 0 inside, > 0 outside.
+ * Degenerate input (no usable sample, or all of them one point): chi = 1 everywhere (an empty surface), 0 iterations.
+ *
+ * dss_poisson_solve: points, normals (P,3) f32; depth in [2, DSS_POISSON_MAX_DEPTH].  Writes chi ((R+1)^3 f32, device)
+ * and, on the host, center[3] = c, *side = L, *iterations and *residual (|r| / |b| of the depth-d system's CG, both 0
+ * when degenerate; either pointer may be NULL).  level_iterations (host, depth + 1 ints) and level_ms (host, 2 (depth +
+ * 1) floats: set-up and CG milliseconds of each level) are optional; entries of levels not solved are 0.
+ * Solver: cascadic, Jacobi-preconditioned CG in float32 with fp64 dot products, matrix-free (the 27-point stencil of K
+ * and the 8 x 8 block of Q of every occupied cell).  Levels min(depth, DSS_POISSON_FIRST_DEPTH) .. depth are solved in
+ * turn, each from the trilinear prolongation of the previous level's chi (the first from 0); only the depth-d system
+ * defines the result.  Each level stops when |r| / |b| <= DSS_POISSON_TOLERANCE or after DSS_POISSON_MAX_ITERATIONS.
+ * Deterministic: every sample-to-grid sum (S_n, the blocks of Q, the occupied-cell count) is an integer (64-bit fixed
+ * point, 2^-30) atomic, so the result is the same bits for any order of the samples; dot products are per-block fp64
+ * partials added in a fixed order.  Host synchronisations: one after the bounding box, then one every
+ * DSS_POISSON_CHECK_EVERY CG iterations of each level (the CG state stays on the device in between).  Workspace (context
+ * scratch, kept for later calls): 8 node arrays of the finest level ((R+1)^3 x 4 bytes each: 0.54 GB at depth 9, 67 MB
+ * at depth 8), the previous level's solution (1/8 of one), and 544 bytes per cell for min(N_usable, R^3) cells.
+ *
+ * dss_marching_tetrahedra: the chi = 0 surface of a node grid chi ((R+1)^3 f32, the layout above) placed by center[3]
+ * (host) and side: node (i, j, k) lies at c + (h (i, j, k) - 0.5) L.  A node with chi < 0 is inside; chi >= 0 (0 too)
+ * and NaN are outside.  Every cube is split into the 6 Kuhn tetrahedra around its corner (0,0,0) - (1,1,1) diagonal, in
+ * the order of the axis permutations xyz, xzy, yxz, yzx, zxy, zyx (tetrahedron sigma: corners 0, e_s1, e_s1 + e_s2,
+ * (1,1,1)), so neighbouring cubes agree on every face and the mesh is closed without a case table.
+ * Vertices: one per crossing edge (a, a + d), d one of the 7 directions d = (dx, dy, dz) != 0 in {0,1}^3 (direction
+ * number 4 dx + 2 dy + dz), ordered by (node index of a, direction number).  In float32, each operation rounded once:
+ *   t = (0 - chi_a) / (chi_b - chi_a);  g_k = (float)i_k + t where d_k = 1, (float)i_k where d_k = 0;
+ *   vertex_k = c_k + (g_k h - 0.5) L   with h = 1 / R (the products and differences in that order, no fused ops).
+ * Faces: per tetrahedron with k of its 4 corners inside, none for k = 0 or 4; for k = 1 or 3 one triangle on the 3
+ * edges of the lone corner; for k = 2 the quad (i0 o0, i0 o1, i1 o1, i1 o0) of the inside corners i0 < i1 and outside
+ * corners o0 < o1 (local order, o0 and o1 swapped when (i0, i1, o0, o1) is an odd permutation of the positively
+ * oriented tetrahedron), split along i0 o0 - i1 o1 into (q0, q1, q2), (q0, q2, q3).  Every face's right-hand normal
+ * points from inside to outside (along the input normals of a reconstruction).  Faces are ordered by (cube index,
+ * tetrahedron, triangle); cube (i, j, k) has index (i R + j) R + k.
+ * Count, exclusive scan (dss_exclusive_scan_i32) and write: the call synchronises the host once, after counting, and
+ * writes *n_verts / *n_faces (host).  When they exceed max_verts / max_faces nothing is written and DSS_E_CAPACITY is
+ * returned (call again with outputs that size); more than 2^31 - 1 of either is DSS_E_CAPACITY as well.  verts (V,3)
+ * f32, faces (F,3) i32. */
+#define DSS_POISSON_MAX_DEPTH 9
+#define DSS_POISSON_FIRST_DEPTH 4      /* the cascade's coarsest level */
+#define DSS_POISSON_POINT_WEIGHT 4.0   /* alpha: pymeshlab's default point weight */
+#define DSS_POISSON_TOLERANCE 1e-6     /* relative residual |r| / |b| that ends a level's CG */
+#define DSS_POISSON_MAX_ITERATIONS 2000
+#define DSS_POISSON_CHECK_EVERY 32     /* CG iterations queued between two host reads of the convergence state */
+DSS_API int dss_poisson_solve(dss_ctx *ctx, const float *points, const float *normals, int64_t P, int depth,
+                              float *chi, float *center, float *side, int *iterations, double *residual,
+                              int *level_iterations, float *level_ms, void *stream);
+DSS_API int dss_marching_tetrahedra(dss_ctx *ctx, const float *chi, int R, const float *center, float side,
+                                    float *verts, int64_t max_verts, int32_t *faces, int64_t max_faces,
+                                    int64_t *n_verts, int64_t *n_faces, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
