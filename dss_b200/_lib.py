@@ -17,6 +17,8 @@ DSS_E_CAPACITY = -4
 MAX_POINTS_PER_PIXEL = 64
 MAX_SHARED_VIEWS = 256
 MAX_LIGHTS = 8
+PD_MONTECARLO_RATE = 20     # DSS_PD_MONTECARLO_RATE
+PD_MAX_PROBES = 64          # DSS_PD_MAX_PROBES
 
 _lib = None
 _ctx = {}
@@ -107,6 +109,10 @@ _SIGNATURES = {
                                     C.POINTER(C.c_float), vp]),
     "dss_marching_tetrahedra": (C.c_int, [vp, vp, C.c_int, C.POINTER(C.c_float), C.c_float, vp, C.c_int64, vp,
                                           C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp]),
+    "dss_sample_mesh_poisson_disk": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, C.c_int64, C.c_int, C.c_uint64, vp,
+                                               vp, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_double), vp]),
+    "dss_poisson_disk_stats": (C.c_int, [vp, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_int64),
+                                         C.POINTER(C.c_int), C.POINTER(C.c_float)]),
     "dss_preprocess": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_forward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),
     "dss_render_backward": (C.c_int, [vp, C.POINTER(RenderArgs), vp]),

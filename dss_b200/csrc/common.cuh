@@ -86,6 +86,11 @@ enum BufId {
     BUF_PSN_COARSE,   //   the previous level's solution, for the prolongation
     BUF_PSN_CELLS,    //   per occupied cell: 36 fixed-point entries of its block of Q, then the 64 float entries
     BUF_MT,           // marching tetrahedra: totals, per-node vertex counts / bases, per-cube face counts / bases, masks
+    BUF_PDS_STATE,    // Poisson-disk sampling: the face box, A_max, the weight total and the round state
+    BUF_PDS_FACES,    //   per face: fp64 area, then the weights and their 64-bit exclusive scan (+ total), tile sums
+    BUF_PDS_POOL,     //   the Monte Carlo pool: points and normals (float4 each)
+    BUF_PDS_SORTED,   //   the pool in cell order (points with their pool index, normals), cells, round state, flags
+    BUF_PDS_GRID,     //   samples per cell, then their exclusive scan
     NUM_BUFS
 };
 
@@ -131,6 +136,12 @@ struct dss_ctx {
     int bin_direct;     // tuning (env DSS_BIN_DIRECT): tile binning with plain global atomics instead of per-block histograms
     double stage_ms[dss::NUM_STAGES];
     int64_t stage_calls[dss::NUM_STAGES];
+    // the last dss_sample_mesh_poisson_disk call (dss_poisson_disk_stats)
+    int pd_probes;
+    double pd_radii[DSS_PD_MAX_PROBES];
+    int64_t pd_counts[DSS_PD_MAX_PROBES];
+    int pd_rounds[DSS_PD_MAX_PROBES];
+    float pd_ms[4];
 };
 
 namespace dss {
@@ -200,6 +211,30 @@ __device__ __forceinline__ int f2ord(float f) {
     return i >= 0 ? i : i ^ 0x7fffffff;
 }
 __device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
+
+struct D3 {
+    double x, y, z;
+};
+
+__device__ __forceinline__ D3 d3(double x, double y, double z) {
+    D3 r;
+    r.x = x, r.y = y, r.z = z;
+    return r;
+}
+
+// fp64 vector arithmetic with every operation rounded on its own (no contraction), so that an oracle performing the
+// same operations in the same order in float64 (tests/point_mesh_oracle.py, tests/poisson_disk_oracle.py) gives the
+// same bits.
+__device__ __forceinline__ D3 dsub(D3 a, D3 b) { return d3(__dsub_rn(a.x, b.x), __dsub_rn(a.y, b.y), __dsub_rn(a.z, b.z)); }
+__device__ __forceinline__ double ddot(D3 a, D3 b) {
+    return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
+}
+__device__ __forceinline__ D3 daxpy(D3 a, double t, D3 u) {        // a + t u
+    return d3(__dadd_rn(a.x, __dmul_rn(t, u.x)), __dadd_rn(a.y, __dmul_rn(t, u.y)), __dadd_rn(a.z, __dmul_rn(t, u.z)));
+}
+__device__ __forceinline__ double ddiff(double a, double b, double c, double d) {   // a b - c d
+    return __dsub_rn(__dmul_rn(a, b), __dmul_rn(c, d));
+}
 
 // sum of acc[k] over the block (blockDim.x a multiple of 32, at most 256) in a fixed order; thread k < K
 // returns sum k, the others 0

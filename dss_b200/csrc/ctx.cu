@@ -256,6 +256,94 @@ int exclusive_scan_i32(dss_ctx *ctx, const int32_t *in, int32_t *out, int64_t n,
     return DSS_OK;
 }
 
+// ---------------------------------------------------------------------------------------------
+// 64-bit exclusive scan in place, three launches: per-tile sums, one block scanning the tile sums (and writing the
+// grand total to v[n]), then each tile applied from its carry.  Integer sums, so the result does not depend on the
+// order of anything.  Used by the mesh rasterizer (pixel items per (view, face)) and the Poisson-disk sampler (face
+// weights).
+// ---------------------------------------------------------------------------------------------
+
+// exclusive scan of v over the block (SCAN_THREADS threads); returns the block total through `total`
+__device__ __forceinline__ int64_t block_exclusive_scan_i64(int64_t v, int64_t &total) {
+    __shared__ int64_t sWarp[SCAN_THREADS / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int64_t inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int64_t u = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += u;
+    }
+    if (lane == 31) sWarp[warp] = inc;
+    __syncthreads();
+    int64_t before = 0;
+    total = 0;
+#pragma unroll
+    for (int w = 0; w < SCAN_THREADS / 32; ++w) {
+        if (w < warp) before += sWarp[w];
+        total += sWarp[w];
+    }
+    __syncthreads();
+    return before + inc - v;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) scan_i64_tiles_kernel(const int64_t *v, int64_t n,
+                                                                      int64_t *tile_sums) {
+    const int64_t base = (int64_t)blockIdx.x * SCAN_TILE + (int64_t)threadIdx.x * SCAN_ITEMS;
+    int64_t s = 0;
+#pragma unroll
+    for (int k = 0; k < SCAN_ITEMS; ++k) s += base + k < n ? v[base + k] : 0;
+    int64_t total;
+    block_exclusive_scan_i64(s, total);
+    if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
+}
+
+// one block: exclusive scan of the tile sums in place; the grand total goes to v[n]
+__global__ void __launch_bounds__(SCAN_THREADS) scan_i64_sums_kernel(int64_t *tile_sums, int64_t tiles, int64_t *v,
+                                                                     int64_t n) {
+    int64_t carry = 0;
+    for (int64_t b0 = 0; b0 < tiles; b0 += SCAN_THREADS) {
+        const int64_t b = b0 + threadIdx.x;
+        const int64_t x = b < tiles ? tile_sums[b] : 0;
+        int64_t total;
+        const int64_t ex = block_exclusive_scan_i64(x, total);
+        if (b < tiles) tile_sums[b] = carry + ex;
+        carry += total;
+    }
+    if (threadIdx.x == 0) v[n] = carry;
+}
+
+__global__ void __launch_bounds__(SCAN_THREADS) scan_i64_apply_kernel(int64_t *v, int64_t n,
+                                                                      const int64_t *tile_sums) {
+    const int64_t base = (int64_t)blockIdx.x * SCAN_TILE + (int64_t)threadIdx.x * SCAN_ITEMS;
+    int64_t x[SCAN_ITEMS], s = 0;
+#pragma unroll
+    for (int k = 0; k < SCAN_ITEMS; ++k) {
+        x[k] = base + k < n ? v[base + k] : 0;
+        s += x[k];
+    }
+    int64_t total;
+    int64_t run = tile_sums[blockIdx.x] + block_exclusive_scan_i64(s, total);
+#pragma unroll
+    for (int k = 0; k < SCAN_ITEMS; ++k) {
+        if (base + k < n) v[base + k] = run;
+        run += x[k];
+    }
+}
+
+int64_t scan_i64_tiles(int64_t n) { return (n + SCAN_TILE - 1) / SCAN_TILE; }
+
+int exclusive_scan_i64(dss_ctx *ctx, int64_t *v, int64_t n, int64_t *tile_sums, cudaStream_t st) {
+    if (n <= 0) return DSS_OK;
+    const int64_t tiles = scan_i64_tiles(n);
+    scan_i64_tiles_kernel<<<(unsigned int)tiles, SCAN_THREADS, 0, st>>>(v, n, tile_sums);
+    DSS_LAUNCH_CHECK(ctx);
+    scan_i64_sums_kernel<<<1, SCAN_THREADS, 0, st>>>(tile_sums, tiles, v, n);
+    DSS_LAUNCH_CHECK(ctx);
+    scan_i64_apply_kernel<<<(unsigned int)tiles, SCAN_THREADS, 0, st>>>(v, n, tile_sums);
+    DSS_LAUNCH_CHECK(ctx);
+    return DSS_OK;
+}
+
 }  // namespace dss
 
 extern "C" {

@@ -36,6 +36,11 @@ int publish_words(dss_ctx *ctx, const void *src_device, void *dst_pinned_host, i
 
 int exclusive_scan_i32(dss_ctx *ctx, const int32_t *in, int32_t *out, int64_t n, cudaStream_t st);
 
+// 64-bit exclusive scan of v[0, n) in place; the total goes to v[n] (v holds n + 1 entries).  tile_sums: scratch of
+// scan_i64_tiles(n) entries.  Three launches, no host synchronisation.
+int64_t scan_i64_tiles(int64_t n);
+int exclusive_scan_i64(dss_ctx *ctx, int64_t *v, int64_t n, int64_t *tile_sums, cudaStream_t st);
+
 int pack_records(dss_ctx *ctx, const float *points, const float *radii, const float *ellipse, int64_t P,
                  float4 *rec, cudaStream_t st);
 

@@ -46,29 +46,6 @@ struct PmdState {       // device scratch of one call
     PmdGrid grid;
 };
 
-struct D3 {
-    double x, y, z;
-};
-
-__device__ __forceinline__ D3 d3(double x, double y, double z) {
-    D3 r;
-    r.x = x, r.y = y, r.z = z;
-    return r;
-}
-
-// Every operation below is rounded on its own (no contraction), so that tests/point_mesh_oracle.py, which performs the
-// same operations in the same order in torch float64, gives the same bits.
-__device__ __forceinline__ D3 dsub(D3 a, D3 b) { return d3(__dsub_rn(a.x, b.x), __dsub_rn(a.y, b.y), __dsub_rn(a.z, b.z)); }
-__device__ __forceinline__ double ddot(D3 a, D3 b) {
-    return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
-}
-__device__ __forceinline__ D3 daxpy(D3 a, double t, D3 u) {        // a + t u
-    return d3(__dadd_rn(a.x, __dmul_rn(t, u.x)), __dadd_rn(a.y, __dmul_rn(t, u.y)), __dadd_rn(a.z, __dmul_rn(t, u.z)));
-}
-__device__ __forceinline__ double ddiff(double a, double b, double c, double d) {   // a b - c d
-    return __dsub_rn(__dmul_rn(a, b), __dmul_rn(c, d));
-}
-
 // closest point of the closed segment [a, b]; a point when a == b
 __device__ __forceinline__ D3 seg_closest(D3 p, D3 a, D3 b) {
     const D3 ab = dsub(b, a), ap = dsub(p, a);

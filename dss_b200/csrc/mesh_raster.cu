@@ -9,20 +9,19 @@
 //   1. screen_kernel : one thread per (view, vertex): NDC x, y as the splat preprocess forms them, view-space z.
 //   2. count_kernel  : one thread per (view, face): the rectangle of pixel centres inside the face's closed bounding
 //                      box (exact, by the pixel-centre expression itself) and its size; 0 for skipped faces.
-//   3. a 64-bit exclusive scan of the sizes (3 launches).
+//   3. a 64-bit exclusive scan of the sizes (exclusive_scan_i64, 3 launches).
 //   4. item_kernel   : one thread per (face, pixel) item, found by binary search over the scan: the coverage test and
 //                      a 64-bit atomicMin of (depth bits << 32 | face) into the pixel's key.  Faces of any size spread
 //                      evenly over the grid; the minimum does not depend on the order of the atomics.
 //   5. resolve_kernel: one thread per pixel writes pix_to_face, zbuf and (optionally) the shaded RGBA.
 // No float atomics, no host synchronisation (the item kernel reads the total from the device).
 #include "common.cuh"
+#include "kernels.cuh"
 #include "shading.cuh"
 
 namespace dss {
 
 constexpr int MESH_THREADS = 256;
-constexpr int MESH_SCAN_ITEMS = 8;                                   // scan entries per thread
-constexpr int MESH_SCAN_TILE = MESH_THREADS * MESH_SCAN_ITEMS;       // 2048
 constexpr int64_t MESH_CHUNK_ENTRIES = (int64_t)1 << 23;             // (view, face) entries per chunk
 constexpr int64_t MESH_CHUNK_PIXELS = (int64_t)1 << 25;              // pixel keys per chunk
 constexpr unsigned long long MESH_EMPTY = ~0ull;
@@ -110,75 +109,6 @@ __global__ void __launch_bounds__(MESH_THREADS) mesh_count_kernel(const int32_t 
         }
         counts[e] = cnt;
         rects[e] = r;
-    }
-}
-
-// ---- 64-bit exclusive scan of the counts (tiles of 2048 entries) ----------------------------------------------------
-
-// exclusive scan of v over the block (MESH_THREADS threads); returns the block total through `total`
-__device__ __forceinline__ int64_t block_exclusive_scan(int64_t v, int64_t &total) {
-    __shared__ int64_t sWarp[MESH_THREADS / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int64_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int64_t u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += u;
-    }
-    if (lane == 31) sWarp[warp] = inc;
-    __syncthreads();
-    int64_t before = 0;
-    total = 0;
-#pragma unroll
-    for (int w = 0; w < MESH_THREADS / 32; ++w) {
-        if (w < warp) before += sWarp[w];
-        total += sWarp[w];
-    }
-    __syncthreads();
-    return before + inc - v;
-}
-
-__global__ void __launch_bounds__(MESH_THREADS) mesh_scan_tiles_kernel(const int64_t *counts, int64_t M,
-                                                                       int64_t *tile_sums) {
-    const int64_t base = (int64_t)blockIdx.x * MESH_SCAN_TILE + (int64_t)threadIdx.x * MESH_SCAN_ITEMS;
-    int64_t s = 0;
-#pragma unroll
-    for (int k = 0; k < MESH_SCAN_ITEMS; ++k) s += base + k < M ? counts[base + k] : 0;
-    int64_t total;
-    block_exclusive_scan(s, total);
-    if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
-}
-
-// one block: exclusive scan of the tile sums in place; the grand total goes to offsets[M]
-__global__ void __launch_bounds__(MESH_THREADS) mesh_scan_sums_kernel(int64_t *tile_sums, int64_t tiles,
-                                                                      int64_t *offsets, int64_t M) {
-    int64_t carry = 0;
-    for (int64_t b0 = 0; b0 < tiles; b0 += MESH_THREADS) {
-        const int64_t b = b0 + threadIdx.x;
-        const int64_t v = b < tiles ? tile_sums[b] : 0;
-        int64_t total;
-        const int64_t ex = block_exclusive_scan(v, total);
-        if (b < tiles) tile_sums[b] = carry + ex;
-        carry += total;
-    }
-    if (threadIdx.x == 0) offsets[M] = carry;
-}
-
-__global__ void __launch_bounds__(MESH_THREADS) mesh_scan_apply_kernel(int64_t *offsets, int64_t M,
-                                                                       const int64_t *tile_sums) {
-    const int64_t base = (int64_t)blockIdx.x * MESH_SCAN_TILE + (int64_t)threadIdx.x * MESH_SCAN_ITEMS;
-    int64_t v[MESH_SCAN_ITEMS], s = 0;
-#pragma unroll
-    for (int k = 0; k < MESH_SCAN_ITEMS; ++k) {
-        v[k] = base + k < M ? offsets[base + k] : 0;
-        s += v[k];
-    }
-    int64_t total;
-    int64_t run = tile_sums[blockIdx.x] + block_exclusive_scan(s, total);
-#pragma unroll
-    for (int k = 0; k < MESH_SCAN_ITEMS; ++k) {
-        if (base + k < M) offsets[base + k] = run;
-        run += v[k];
     }
 }
 
@@ -318,7 +248,7 @@ int dss_rasterize_mesh(dss_ctx *ctx, const float *verts, int64_t V, const int32_
     int rc;
     if ((rc = ctx_get(ctx, BUF_MESH_KEYS, (size_t)(C * npix), &keys))) return rc;
     if (have_faces) {
-        const int64_t Mmax = C * F, tiles = (Mmax + MESH_SCAN_TILE - 1) / MESH_SCAN_TILE;
+        const int64_t Mmax = C * F, tiles = scan_i64_tiles(Mmax);
         if ((rc = ctx_get(ctx, BUF_MESH_SCREEN, (size_t)(C * V), &screen))) return rc;
         if ((rc = ctx_get(ctx, BUF_MESH_OFFSETS, (size_t)(Mmax + 1), &offsets))) return rc;
         if ((rc = ctx_get(ctx, BUF_MESH_RECTS, (size_t)Mmax, &rects))) return rc;
@@ -329,19 +259,14 @@ int dss_rasterize_mesh(dss_ctx *ctx, const float *verts, int64_t V, const int32_
         const int Cn = (int)(N - n0 < C ? N - n0 : C);
         DSS_CUDA_TRY(cudaMemsetAsync(keys, 0xff, (size_t)(Cn * npix) * sizeof(unsigned long long), st));
         if (have_faces) {
-            const int64_t M = (int64_t)Cn * F, tiles = (M + MESH_SCAN_TILE - 1) / MESH_SCAN_TILE;
+            const int64_t M = (int64_t)Cn * F;
             mesh_screen_kernel<<<dim3(grid_blocks(V, MESH_THREADS, ctx->sm_count, 8), Cn), MESH_THREADS, 0, st>>>(
                 verts, V, proj, view, n0, screen);
             DSS_LAUNCH_CHECK(ctx);
             mesh_count_kernel<<<grid_blocks(M, MESH_THREADS, ctx->sm_count, 8), MESH_THREADS, 0, st>>>(
                 faces, F, V, screen, M, S, offsets, rects);
             DSS_LAUNCH_CHECK(ctx);
-            mesh_scan_tiles_kernel<<<(unsigned int)tiles, MESH_THREADS, 0, st>>>(offsets, M, tile_sums);
-            DSS_LAUNCH_CHECK(ctx);
-            mesh_scan_sums_kernel<<<1, MESH_THREADS, 0, st>>>(tile_sums, tiles, offsets, M);
-            DSS_LAUNCH_CHECK(ctx);
-            mesh_scan_apply_kernel<<<(unsigned int)tiles, MESH_THREADS, 0, st>>>(offsets, M, tile_sums);
-            DSS_LAUNCH_CHECK(ctx);
+            if ((rc = exclusive_scan_i64(ctx, offsets, M, tile_sums, st))) return rc;
             // the item total is on the device: a full grid strides over it
             mesh_item_kernel<<<grid_blocks(INT64_MAX / 2, MESH_THREADS, ctx->sm_count, 8), MESH_THREADS, 0, st>>>(
                 faces, F, screen, V, offsets, rects, M, S, keys);

@@ -776,3 +776,72 @@ def poisson_reconstruction(points, normals, depth=8, return_grid=False) -> Poiss
     origin = torch.tensor(list(c), dtype=torch.float32)
     verts, faces = marching_tetrahedra(chi, origin, L.value)
     return PoissonMesh(verts, faces, chi if return_grid else None, origin, L.value, its.value, res.value)
+
+
+class PoissonDiskSamples(NamedTuple):
+    points: torch.Tensor              # (n,3) float32 on the device of the input, in pool order
+    normals: torch.Tensor             # (n,3) float32 unit normal of each sample's face
+    radius: float                     # the disk radius the count was reached at
+
+
+def sample_points_poisson_disk(verts, faces, num_samples, geodesic=False, seed=0) -> PoissonDiskSamples:
+    """Poisson-disk samples of a triangle mesh (csrc/mesh_sample.cu; the rule is in include/dss_b200.h): a dart throw
+    over a pool of 20 x ``num_samples`` area-weighted samples drawn from ``seed``, at the radius whose count lies within
+    0.5 % of ``num_samples`` (meshlab's ``generate_sampling_poisson_disk`` with ``exactnumflag``, the reference's
+    evaluation ground truth).  ``geodesic`` measures meshlab's approximate geodesic distance instead of the Euclidean
+    one.  The same inputs give the same bits.
+
+    verts (V,3) float32 CUDA tensor, faces (F,3) integer with every index in [0, V) (checked here).  Faces with a
+    non-finite vertex or zero area are never sampled; without a usable face the result is empty with radius 0.
+    Forward only.  The host synchronises once per few selection rounds (DESIGN.md)."""
+    dev = _lib.require_cuda(verts, faces)
+    if verts.requires_grad:
+        raise RuntimeError("sample_points_poisson_disk has no backward: pass verts that do not require grad")
+    v = _lib.as_f32(verts, "verts")
+    if v.dim() != 2 or v.shape[1] != 3:
+        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
+        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
+    N = int(num_samples)
+    if N < 1 or _lib.PD_MONTECARLO_RATE * N >= 2 ** 31:
+        raise ValueError("num_samples must lie in [1, %d], got %r" % ((2 ** 31 - 1) // _lib.PD_MONTECARLO_RATE,
+                                                                     num_samples))
+    V, F = v.shape[0], faces.shape[0]
+    if V >= 2 ** 31 or F >= 2 ** 31:
+        raise ValueError("at most 2^31 - 1 vertices and faces")
+    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
+        raise ValueError("face indices must lie in [0, %d)" % V)
+    f = faces.to(torch.int32).contiguous()
+    n, r = C.c_int64(0), C.c_double(0.0)
+    lib = _lib.load()
+    # room for a count within the tolerance, which is what the search nearly always returns; a call that finds more
+    # (its probes all missed the tolerance) is repeated with room for exactly that many
+    cap = N + N // 200
+    with torch.cuda.device(dev):
+        for _ in range(2):
+            points = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+            normals = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+            rc = lib.dss_sample_mesh_poisson_disk(_lib.ctx(dev), _lib.ptr(v), V, _lib.ptr(f), F, N,
+                                                  int(bool(geodesic)), int(seed) & (2 ** 64 - 1), _lib.ptr(points),
+                                                  _lib.ptr(normals), cap, C.byref(n), C.byref(r), _lib.stream_ptr(dev))
+            if rc != _lib.DSS_E_CAPACITY:
+                break
+            cap = n.value
+    _lib.check(rc, "dss_sample_mesh_poisson_disk")
+    return PoissonDiskSamples(points[:n.value], normals[:n.value], r.value)
+
+
+def poisson_disk_stats(device=None):
+    """{"probes", "radii", "counts", "rounds", "stage_ms"} of the last :func:`sample_points_poisson_disk` call on the
+    device: per probe its radius, sample count and selection rounds; stage_ms the pool build, the radius search, the
+    final selection (0 when the returned probe was the last) and the output, in milliseconds."""
+    probes = C.c_int(0)
+    radii = (C.c_double * _lib.PD_MAX_PROBES)()
+    counts = (C.c_int64 * _lib.PD_MAX_PROBES)()
+    rounds = (C.c_int * _lib.PD_MAX_PROBES)()
+    ms = (C.c_float * 4)()
+    _lib.check(_lib.load().dss_poisson_disk_stats(_lib.ctx(device), C.byref(probes), radii, counts, rounds, ms),
+               "dss_poisson_disk_stats")
+    k = probes.value
+    return {"probes": k, "radii": list(radii[:k]), "counts": list(counts[:k]), "rounds": list(rounds[:k]),
+            "stage_ms": list(ms)}

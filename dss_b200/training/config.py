@@ -9,10 +9,14 @@ import warnings
 
 import yaml
 
-__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "step_settings", "splat_params"]
+__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "step_settings", "splat_params",
+           "EVAL_SAMPLINGS"]
+
+EVAL_SAMPLINGS = ("uniform", "poisson_disk")
 
 # The configs/default.yaml values the loop reads, plus the reference Trainer's keyword defaults it passes on
-# (trainer.py:73-80: n_eval_points, steps_dss_backward_radii) and what is this loop's own (seed, backup_every 0: off).
+# (trainer.py:73-80: n_eval_points, steps_dss_backward_radii) and what is this loop's own (seed, backup_every 0: off,
+# eval_sampling: how the validation's ground truth is drawn from the data's mesh, see train.ground_truth_cloud).
 DEFAULTS = {
     "name": "demo",
     "data": {"type": "MVR", "data_dir": "example_data", "data_dict": "data_dict.npz", "img_folder": "image",
@@ -36,6 +40,7 @@ DEFAULTS = {
         "scheduler_milestones": [500, 800], "scheduler_gamma": 0.5, "logfile": "train.log",
         "resume_from": "model.pt", "model_selection_metric": "chamfer_point", "model_selection_mode": "minimize",
         "n_eval_points": 8000, "steps_dss_backward_radii": 100, "steps_proj": -1, "gamma_proj": 5,
+        "eval_sampling": "uniform",
     },
 }
 

@@ -16,7 +16,8 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   trainer.py:114-123): see :func:`radii_backward_scaler` and :func:`compound_lambda_proj`.
 - every ``print_every`` iterations the losses go to ``<out>/<logfile>`` and one JSON line to ``<out>/metrics.jsonl``
   (the loop's only host synchronisations besides validation); every ``validate_every`` (it > 0) the chamfer distances
-  of the ground-truth cloud against the current one (trainer.py:144-171), and on improvement of
+  of the ground-truth cloud against the current one (trainer.py:144-171; ``training.eval_sampling: poisson_disk`` draws
+  it as the reference does, see :func:`ground_truth_cloud`), and on improvement of
   ``training.model_selection_metric`` ``model_best.pt`` and ``val/best.ply``.  With the metric ``p2f_avg`` the loop
   reads ``<data_dir>/mesh.obj`` once (it must exist) and every validation adds ``p2f_avg`` / ``p2f_std``, the mean and
   population standard deviation of the exact distances of the cloud's points to that mesh; ``model.pt`` every ``checkpoint_every``, ``model_%d.pt`` every ``backup_every``.
@@ -44,7 +45,7 @@ from ..utils.create_mvr_data import ico_sphere, sample_points_from_mesh
 from ..utils.dataset import MVRData
 from ..utils.evaluate import p2f_stats
 from ..utils.io import read_mesh, save_ply
-from .config import check_config, load_config, selection_metric, splat_params, step_settings
+from .config import EVAL_SAMPLINGS, check_config, load_config, selection_metric, splat_params, step_settings
 from .step import GraphedTrainStep
 
 __all__ = ["radii_backward_scaler", "compound_lambda_proj", "initial_cloud", "make_optimizer", "make_lr_scheduler",
@@ -98,14 +99,21 @@ def make_lr_scheduler(optimizer, cfg):
                                                 gamma=float(tr["scheduler_gamma"]))
 
 
-def ground_truth_cloud(data, data_dir, n_eval_points, device):
+def ground_truth_cloud(data, data_dir, n_eval_points, device, sampling="uniform"):
     """(points, normals) the validation measures against: the stored cloud when ``n_eval_points`` <= 0 or equals its
-    size, otherwise ``n_eval_points`` area-weighted samples of ``<data_dir>/mesh.obj`` drawn once from a fixed seed.
-    (The reference samples the mesh with pymeshlab's Poisson-disk sampling, so absolute values differ from its own.)"""
+    size; otherwise, with ``sampling`` "uniform", ``n_eval_points`` area-weighted samples of ``<data_dir>/mesh.obj``
+    drawn once from a fixed seed, and with "poisson_disk" the reference's ``get_pointclouds(num_points=n_eval_points)``:
+    geodesic Poisson-disk samples of that mesh (:meth:`MVRData.get_pointclouds`).  Only those compare with the
+    reference's own chamfer values."""
+    if sampling not in EVAL_SAMPLINGS:
+        raise ValueError("training.eval_sampling must be one of %s, got %r" % (", ".join(EVAL_SAMPLINGS), sampling))
     stored = data.get_pointclouds()
     n = int(n_eval_points)
     if n <= 0 or n == stored.points_packed().shape[0]:
         return stored.points_packed().to(device), stored.normals_packed().to(device)
+    if sampling == "poisson_disk":
+        pc = data.get_pointclouds(num_points=n)
+        return pc.points_packed().to(device), pc.normals_packed().to(device)
     verts, faces = read_mesh(os.path.join(data_dir, "mesh.obj"))
     g = torch.Generator(device=device).manual_seed(EVAL_SEED)
     return sample_points_from_mesh(torch.from_numpy(verts).float().to(device), torch.from_numpy(faces).long().to(device),
@@ -177,7 +185,8 @@ class Trainer:
         if V // self.batch_size < 1:
             raise ValueError("batch_size %d is larger than the %d views: an epoch would have no batch"
                              % (self.batch_size, V))
-        self.gt = ground_truth_cloud(self.data, dc["data_dir"], tr["n_eval_points"], self.dev)
+        self.gt = ground_truth_cloud(self.data, dc["data_dir"], tr["n_eval_points"], self.dev,
+                                     tr.get("eval_sampling", "uniform"))
         # ---- state: fresh, then whatever the checkpoint holds
         self.gen = torch.Generator().manual_seed(int(tr["seed"]))
         self.epoch_it, self.it, self.order, self.pos = -1, -1, None, 0

@@ -61,6 +61,8 @@ class MVRData:
                 raise ValueError("Found unequal number of %s and camera matrices! (%d, %d)"
                                  % (name, len(arr), len(self.camera_mat)))
         self.images, self.masks = images, masks
+        self.data_dir = data_dir          # None when a data_dict file was given: no mesh.obj to sample
+        self._poisson_disk = {}           # get_pointclouds(num_points) samples, per count
         self.n_imgs = len(self.camera_mat) if n_imgs is None else min(int(n_imgs), len(self.camera_mat))
 
     def __len__(self):
@@ -115,11 +117,32 @@ class MVRData:
                                  if isinstance(v, (list, np.ndarray))}
         return out
 
-    def get_pointclouds(self) -> PointClouds3D:
-        """points, normals and colours in object coordinates (dataset.py:107-135, the stored-cloud branch)."""
+    def get_pointclouds(self, num_points=None) -> PointClouds3D:
+        """points, normals and colours in object coordinates (dataset.py:103-135).  With ``num_points`` None or the
+        stored cloud's size, the stored cloud; otherwise ``num_points`` geodesic Poisson-disk samples of
+        ``<data_dir>/mesh.obj`` (:func:`~dss_b200.ops.sample_points_poisson_disk`, seed 0, the reference's
+        ``generate_sampling_poisson_disk(approximategeodesicdistance=True, exactnumflag=True)``) with colours of ones,
+        on the CPU, computed on the current CUDA device once per count.  Raises ValueError when that file is missing."""
         t = lambda k: torch.tensor(np.asarray(self.data_dict[k]), dtype=torch.float32)
-        colors = t("colors") if "colors" in self.data_dict else torch.ones_like(t("points"))
-        return PointClouds3D([t("points")], [t("normals")], [colors])
+        points = t("points")
+        if num_points is None or int(num_points) == points.shape[0]:
+            colors = t("colors") if "colors" in self.data_dict else torch.ones_like(points)
+            return PointClouds3D([points], [t("normals")], [colors])
+        n = int(num_points)
+        if n not in self._poisson_disk:
+            mesh = None if self.data_dir is None else os.path.join(self.data_dir, "mesh.obj")
+            if mesh is None or not os.path.isfile(mesh):
+                raise ValueError("get_pointclouds(%d) samples the data's mesh.obj, which %s" % (
+                    n, "a data_dict file has not" if mesh is None else "does not exist: %s" % mesh))
+            from ..ops import sample_points_poisson_disk
+            from .io import read_mesh
+            verts, faces = read_mesh(mesh)
+            dev = torch.device("cuda", torch.cuda.current_device())
+            s = sample_points_poisson_disk(torch.from_numpy(verts).to(dev), torch.from_numpy(faces).to(dev), n,
+                                           geodesic=True, seed=0)
+            self._poisson_disk[n] = (s.points.cpu(), s.normals.cpu())
+        p, nrm = self._poisson_disk[n]
+        return PointClouds3D([p.clone()], [nrm.clone()], [torch.ones_like(p)])
 
     def get_cameras(self, camera_mat=None, **camera_params):
         """``FoVPerspectiveCameras`` with R, T taken from ``camera_mat`` ((n,4,4) or (4,4); default: all images)

@@ -1,9 +1,11 @@
 """Score predicted point clouds against the ground truth: the reference's scripts/evaluatePointClouds.py.
 
-    python -m dss_b200.utils.evaluate --gt GT --pred DIR [DIR ...] --name PATTERN [--mesh MESH]
+    python -m dss_b200.utils.evaluate --gt GT --pred DIR [DIR ...] --name PATTERN [--mesh MESH] [--gt-samples N]
 
 Per prediction (the files matching ``DIR/**/PATTERN``, ``.ply`` or ``.xyz``) and its ground truth (``--gt`` a file:
-that file for every prediction; a directory: the file with the prediction's basename):
+that file for every prediction; a directory: the file with the prediction's basename; with ``--gt-samples N``, ``--gt``
+is a mesh and its ``N`` Euclidean Poisson-disk samples are every prediction's ground truth -- the reference's
+scripts/poisson_sampling.mlx, :func:`~dss_b200.ops.sample_points_poisson_disk` with seed 0):
 
 - ``cd_forward`` / ``cd_backward``: the squared distance of every predicted point to its nearest ground-truth point,
   and of every ground-truth point to its nearest prediction (K = 1 of the device K-NN, raw coordinates);
@@ -33,11 +35,11 @@ import numpy as np
 import torch
 
 from ..frnn_grid import knn_points_packed
-from ..ops import point_mesh_distance
+from ..ops import point_mesh_distance, sample_points_poisson_disk
 from .io import read_mesh, read_ply, save_ply
 
 __all__ = ["CloudScores", "evaluate_cloud", "p2f_stats", "jet", "read_points", "read_xyz", "write_p2f_xyz", "pair_files",
-           "evaluation_rows", "write_evaluation_csv", "summary_line", "main"]
+           "evaluation_rows", "write_evaluation_csv", "summary_line", "mesh_ground_truth", "main"]
 
 FIELDS = ["name", "CD", "hausdorff", "p2f avg", "p2f std"] + ["nuc_%d" % d for d in range(7)]
 CD_COLOUR_MAX = 0.003
@@ -203,14 +205,22 @@ def p2f_stats(points, mesh):
     return p2f, avg, std
 
 
-def _evaluate_dir(gt, pred_dir, pattern, mesh, device):
+def mesh_ground_truth(path, num_samples, device):
+    """(G,3) float32 device tensor: ``num_samples`` Euclidean Poisson-disk samples of the mesh file ``path`` (seed 0),
+    the ground truth scripts/poisson_sampling.mlx makes of a mesh"""
+    v, f = read_mesh(path)
+    return sample_points_poisson_disk(torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(device),
+                                      torch.from_numpy(np.ascontiguousarray(f)).to(device), int(num_samples)).points
+
+
+def _evaluate_dir(gt, pred_dir, pattern, mesh, device, gt_cloud=None):
     pairs = pair_files(gt, pred_dir, pattern)
     if not pairs:
         print("{:60s} no predictions matching {} (with a ground truth)".format(os.path.basename(pred_dir), pattern))
         return None
     results = []
     for gt_path, pred_path in pairs:
-        gt_pts = torch.from_numpy(read_points(gt_path)).to(device)
+        gt_pts = gt_cloud if gt_cloud is not None else torch.from_numpy(read_points(gt_path)).to(device)
         pred_pts = torch.from_numpy(read_points(pred_path)).to(device)
         s = evaluate_cloud(pred_pts, gt_pts, mesh)
         stem = pred_path[:-4]
@@ -239,7 +249,14 @@ def main(argv=None):
     ap.add_argument("--pred", nargs="+", required=True, help="directories of predictions")
     ap.add_argument("--name", required=True, help="file name pattern of the predictions, e.g. '*.ply'")
     ap.add_argument("--mesh", default=None, help="ground-truth mesh: compute the point-to-surface distances")
+    ap.add_argument("--gt-samples", type=int, default=None, metavar="N",
+                    help="--gt is a mesh: score against N Euclidean Poisson-disk samples of it")
     opt = ap.parse_args(argv)
+    if opt.gt_samples is not None:
+        if os.path.isdir(opt.gt):
+            ap.error("--gt-samples samples one mesh: --gt must be a mesh file, not a directory")
+        if opt.gt_samples < 1:
+            ap.error("--gt-samples must be positive")
     if not torch.cuda.is_available():
         raise RuntimeError("the evaluation needs a CUDA device (sm_90a)")
     device = torch.device("cuda", torch.cuda.current_device())
@@ -248,9 +265,10 @@ def main(argv=None):
         v, f = read_mesh(opt.mesh)
         mesh = (torch.from_numpy(np.ascontiguousarray(v, dtype=np.float32)).to(device),
                 torch.from_numpy(np.ascontiguousarray(f)).to(device))
+    gt_cloud = mesh_ground_truth(opt.gt, opt.gt_samples, device) if opt.gt_samples is not None else None
     print(summary_header())
     for d in opt.pred:
-        _evaluate_dir(opt.gt, d, opt.name, mesh, device)
+        _evaluate_dir(opt.gt, d, opt.name, mesh, device, gt_cloud)
     return 0
 
 

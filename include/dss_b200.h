@@ -570,6 +570,63 @@ DSS_API int dss_marching_tetrahedra(dss_ctx *ctx, const float *chi, int R, const
                                     float *verts, int64_t max_verts, int32_t *faces, int64_t max_faces,
                                     int64_t *n_verts, int64_t *n_faces, void *stream);
 
+/* ---- Poisson-disk sampling of a mesh (evaluation ground truth, no backward) ----------------------------------------
+ * The samples of the reference's MVRDataset.get_pointclouds(num_points) and scripts/poisson_sampling.mlx (meshlab's
+ * Poisson-disk sampling with a Monte Carlo pool of DSS_PD_MONTECARLO_RATE x N samples and an exact-count radius search
+ * to 0.5 %), restated as a rule.  Inputs: one mesh verts (V,3) f32 / faces (F,3) i32, a target count N, a seed and
+ * the geodesic flag.  Every fp64 operation below is rounded on its own (no contraction).
+ *   1. Usable faces: indices in [0, V), finite vertices, area_f = 0.5 sqrt(c . c) > 0 with c = cross(b - a, c - a)
+ *      (component k: the two products, then their difference).  A_max = the largest area, W_f = max(1, ceil(area_f
+ *      2^32 / A_max)) in [1, 2^32] for a usable face, 0 otherwise; P_f = the exclusive 64-bit prefix of the W_f, W the
+ *      total.  A = (double)W A_max 2^-32 is the area the radius search starts from (>= the usable area, within
+ *      F A_max 2^-32 of it).  Without a usable face the result is empty.
+ *   2. Pool of M = DSS_PD_MONTECARLO_RATE N samples.  The draws of sample i are x_k = splitmix64(seed, 3 i + k + 1) for
+ *      k = 0, 1, 2, where splitmix64(s, j) is the j-th output of SplitMix64 seeded with s:
+ *        z = s + j 0x9E3779B97F4A7C15;  z = (z ^ z >> 30) 0xBF58476D1CE4E5B9;  z = (z ^ z >> 27) 0x94D049BB133111EB;
+ *        x = z ^ z >> 31                                                           (all modulo 2^64).
+ *      The face is the f with P_f <= t < P_f + W_f, t = the high 64 bits of the 128-bit product x_0 W (the first
+ *      usable face whose inclusive prefix exceeds t).  u = (x_1 >> 11) 2^-53, v = (x_2 >> 11) 2^-53, s = sqrt(u),
+ *      w0 = 1 - s, w1 = s (1 - v), w2 = s v, the point ((w0 a + w1 b) + w2 c) per coordinate and its normal c / |c|
+ *      (c the face's cross product above), each rounded once to f32.  Pool order is the selection's priority.
+ *   3. Selection at radius r (the sequential dart throw): walk the pool in index order and accept a sample unless an
+ *      accepted sample conflicts with it.  Samples p0 (the later) and p1 (the earlier) conflict when their distance is
+ *      below r.  Euclidean: d2 < r * r with d = p0 - p1 in fp64 from the f32 points and d2 = (dx dx + dy dy) + dz dz.
+ *      Geodesic (meshlab's approximate geodesic distance, libm asin, so not bit-reproducible across libraries): 0 when
+ *      d2 = 0; otherwise d_e = sqrt(d2), and no conflict unless d_e < r; then v = d / d_e, C0 = v . n0, C1 = v . n1
+ *      (the f32 normals), each clamped to [-1, 1], g = (asin C0 - asin C1) / (C0 - C1), or 1 / sqrt(1 - C0 C1) when
+ *      |C0 - C1| < 1e-4, g = max(g, 1), and the distance is d_e g.  g equals arc / chord for two points of a circle, is
+ *      symmetric and >= 1, so every conflict is also a Euclidean one.
+ *   4. The radius: N_tol = floor(N / 200).  Probe r = sqrt(A / (0.7 pi N)) first.  After a probe with n(r) samples:
+ *      stop when |n(r) - N| <= N_tol; otherwise r is a lower bound when n(r) > N, an upper one when n(r) < N, and the
+ *      next probe is 2 r while no upper bound is known, r / 2 while no lower one is, else (lo + hi) / 2.  After
+ *      DSS_PD_MAX_PROBES probes the probe with the smallest |n - N| (the earliest on a tie) is returned.  The radius is
+ *      host fp64 arithmetic.
+ * Output: the accepted samples of the returned probe in pool order, points and normals (n,3) f32; *n_out = n (host),
+ * *radius = its r (host; 0 without a usable face).  When n > max_out nothing is written and DSS_E_CAPACITY is returned
+ * (*n_out tells the size; call again).  N <= 0 and M >= 2^31 are DSS_E_INVALID.
+ * On the device: a face pass (areas, box, A_max), the weights, the 64-bit scan, one thread per pool sample; then per
+ * probe a uniform grid of cell side max(r (1 + 2^-20), extent / DSS_PD_GRID) (27 cells hold every conflict) built by
+ * count, dss_exclusive_scan_i32 and fill, and the lexicographically first maximal independent set of the conflict
+ * graph in pool order, computed in rounds (DESIGN.md): an undecided sample is rejected when an earlier conflicting
+ * sample is accepted and accepted when no earlier conflicting sample is undecided, which is the sequential result.
+ * Deterministic.  Host synchronisations: one after the face pass (box, A_max, W), then one every DSS_PD_CHECK_EVERY
+ * rounds of every probe, and one to size the output: not capturable.  Scratch from the context: ~80 bytes per pool
+ * sample, 16 per face and 8 per grid cell (at most (DSS_PD_GRID + 1)^3 cells). */
+#define DSS_PD_MONTECARLO_RATE 20     /* pool samples per requested sample (poisson_sampling.mlx's MontecarloRate) */
+#define DSS_PD_MAX_PROBES 64          /* radius probes at most */
+#define DSS_PD_CHECK_EVERY 8          /* selection rounds queued between two host reads of the round state */
+#define DSS_PD_GRID 256               /* the selection grid's cell side is at least extent / DSS_PD_GRID */
+DSS_API int dss_sample_mesh_poisson_disk(dss_ctx *ctx, const float *verts, int64_t V, const int32_t *faces, int64_t F,
+                                         int64_t num_samples, int geodesic, uint64_t seed, float *points,
+                                         float *normals, int64_t max_out, int64_t *n_out, double *radius,
+                                         void *stream);
+/* Statistics of the context's last dss_sample_mesh_poisson_disk call, for measuring it (each pointer may be NULL):
+ * *probes; per probe (DSS_PD_MAX_PROBES entries, host) its radius, its count and its selection rounds; stage_ms (4
+ * floats): the pool build, the radius search, the final selection when the returned probe was not the last one, and
+ * the output. */
+DSS_API int dss_poisson_disk_stats(dss_ctx *ctx, int *probes, double *radii, int64_t *counts, int *rounds,
+                                   float *stage_ms);
+
 #ifdef __cplusplus
 }
 #endif
