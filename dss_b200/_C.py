@@ -58,12 +58,8 @@ def splat_points(points, ellipse_params, cutoff_thres, radii, cloud_to_packed_fi
     zbuf = torch.empty((N, S, S, K), dtype=torch.float32, device=dev)
     qvalue = torch.empty((N, S, S, K), dtype=torch.float32, device=dev)
     occ = torch.empty((N, S, S), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_splat_points(
-            _lib.ctx(dev), _lib.ptr(points), _lib.ptr(ellipse_params), _lib.ptr(cutoff_thres), _lib.ptr(radii),
-            _lib.ptr(fi), _lib.ptr(npts), N, P, float(depth_merging_thres), S, K, int(bin_size or 0),
-            _lib.ptr(idx), _lib.ptr(zbuf), _lib.ptr(qvalue), _lib.ptr(occ), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_splat_points")
+    _lib.call("dss_splat_points", dev, points, ellipse_params, cutoff_thres, radii, fi, npts, N, P,
+              float(depth_merging_thres), S, K, int(bin_size or 0), idx, zbuf, qvalue, occ)
     return idx, zbuf, qvalue, occ
 
 
@@ -89,18 +85,13 @@ def _rasterize_coarse_csr(points, radii, cloud_to_packed_first_idx, num_points_p
     fi, npts = cloud_to_packed_first_idx.contiguous(), num_points_per_cloud.contiguous()
     off = torch.empty(N * B * B + 1, dtype=torch.int32, device=dev)
     cap = max(2 * P, 1024)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        for _ in range(2):
-            ids = torch.empty(cap, dtype=torch.int32, device=dev)
-            need = C.c_int64(0)
-            rc = lib.dss_rasterize_coarse(_lib.ctx(dev), _lib.ptr(points), _lib.ptr(radii), _lib.ptr(fi),
-                                          _lib.ptr(npts), N, P, S, bs, _lib.ptr(off), _lib.ptr(ids), cap,
-                                          C.byref(need), _lib.stream_ptr(dev))
-            if rc != _lib.DSS_E_CAPACITY:
-                break
-            cap = int(need.value)
-    _lib.check(rc, "dss_rasterize_coarse")
+    for first in (True, False):
+        ids = torch.empty(cap, dtype=torch.int32, device=dev)
+        need = C.c_int64(0)
+        if _lib.call("dss_rasterize_coarse", dev, points, radii, fi, npts, N, P, S, bs, off, ids, cap, C.byref(need),
+                     capacity=first) != _lib.DSS_E_CAPACITY:
+            break
+        cap = int(need.value)
     return off, ids[: int(need.value)]
 
 
@@ -157,12 +148,8 @@ def _splat_points_occ_backward(points, radii, grad_occ, cloud_to_packed_first_id
     radii = _lib.as_f32(radii.detach(), "radii")
     grad_occ = _lib.as_f32(grad_occ.detach(), "grad_occ")
     out = torch.empty((P, 2), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_occ_backward_slow(
-            _lib.ctx(dev), _lib.ptr(points), _lib.ptr(radii), _lib.ptr(grad_occ), 1, 0,
-            _lib.ptr(cloud_to_packed_first_idx.contiguous()), _lib.ptr(num_points_per_cloud.contiguous()), N, P, S,
-            float(radii_s), _lib.ptr(out), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_occ_backward_slow")
+    _lib.call("dss_occ_backward_slow", dev, points, radii, grad_occ, 1, 0, cloud_to_packed_first_idx.contiguous(),
+              num_points_per_cloud.contiguous(), N, P, S, float(radii_s), out)
     return out
 
 
@@ -197,12 +184,8 @@ def occ_backward(points, radii, visible, rs, grad_occ, cloud_to_packed_first_idx
     rs = _lib.as_f32(rs.detach(), "rs")
     visible = visible.to(torch.uint8).contiguous()
     out = torch.empty((P, 2), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_occ_backward(
-            _lib.ctx(dev), _lib.ptr(points), _lib.ptr(radii), _lib.ptr(visible), _lib.ptr(rs), _lib.ptr(grad_occ),
-            1, 0, _lib.ptr(cloud_to_packed_first_idx.contiguous()), _lib.ptr(num_points_per_cloud.contiguous()),
-            N, P, S, _lib.ptr(out), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_occ_backward")
+    _lib.call("dss_occ_backward", dev, points, radii, visible, rs, grad_occ, 1, 0,
+              cloud_to_packed_first_idx.contiguous(), num_points_per_cloud.contiguous(), N, P, S, out)
     return out
 
 
@@ -214,10 +197,7 @@ def visibility_from_idx(idx, P):
         raise RuntimeError("idx must be int32")
     K = idx.shape[-1]
     vis = torch.empty(P, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_visibility_from_idx(_lib.ctx(dev), _lib.ptr(idx), idx.numel() // K, K, P,
-                                                 _lib.ptr(vis), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_visibility_from_idx")
+    _lib.call("dss_visibility_from_idx", dev, idx, idx.numel() // K, K, P, vis)
     return vis
 
 
@@ -227,12 +207,8 @@ def search_radius(radii, visible, cloud_to_packed_first_idx, num_points_per_clou
     N = num_points_per_cloud.shape[0]
     rs = torch.empty(N, dtype=torch.float32, device=dev)
     radii = _lib.as_f32(radii.detach(), "radii")
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_search_radius(_lib.ctx(dev), _lib.ptr(radii), _lib.ptr(visible.contiguous()),
-                                           _lib.ptr(cloud_to_packed_first_idx.contiguous()),
-                                           _lib.ptr(num_points_per_cloud.contiguous()), N, radii.shape[0],
-                                           float(radii_s), _lib.ptr(rs), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_search_radius")
+    _lib.call("dss_search_radius", dev, radii, visible.contiguous(), cloud_to_packed_first_idx.contiguous(),
+              num_points_per_cloud.contiguous(), N, radii.shape[0], float(radii_s), rs)
     return rs
 
 
@@ -244,9 +220,6 @@ def _backward_zbuf(idx, grad_zbuf, point_z_grad):
     if not point_z_grad.is_contiguous() or point_z_grad.dtype != torch.float32:
         raise RuntimeError("point_z_grad must be a contiguous float32 tensor")
     K = idx.shape[-1]
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_zbuf_backward(_lib.ctx(dev), _lib.ptr(idx.contiguous()),
-                                           _lib.ptr(_lib.as_f32(grad_zbuf, "grad_zbuf")), idx.numel() // K, K,
-                                           _lib.ptr(point_z_grad), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_zbuf_backward")
+    _lib.call("dss_zbuf_backward", dev, idx.contiguous(), _lib.as_f32(grad_zbuf, "grad_zbuf"), idx.numel() // K, K,
+              point_z_grad)
     return None

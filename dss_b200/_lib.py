@@ -179,6 +179,19 @@ def ptr(t):
     return vp(t.data_ptr())
 
 
+def call(name, device, *args, capacity=False):
+    """Call the stream-taking entry point ``name`` on ``device``: the device's context first, then ``args`` (each tensor
+    as its data pointer, everything else as given), then the device's current stream, read now (so that a call inside
+    ``torch.cuda.stream(s)`` runs on ``s``).  Raises RuntimeError on a failed status; with ``capacity`` a
+    DSS_E_CAPACITY status is returned instead, for the callers that size their outputs from a first call."""
+    with torch.cuda.device(device):
+        rc = getattr(load(), name)(ctx(device), *[ptr(a) if isinstance(a, torch.Tensor) else a for a in args],
+                                   stream_ptr(device))
+    if not (capacity and rc == DSS_E_CAPACITY):
+        check(rc, name)
+    return rc
+
+
 def launch_count(device=None):
     return int(load().dss_launch_count(ctx(device)))
 
@@ -228,13 +241,17 @@ def tile_lists(n_views, n_offsets, n_ids, device=None):
     zr = torch.empty(n_views, 2, dtype=torch.float32, device=dev)
     off = torch.empty(n_offsets, dtype=torch.int32, device=dev)
     ids = torch.empty(n_ids, dtype=torch.int32, device=dev)
-    check(load().dss_debug_tile_lists(ctx(device), int(n_views), ptr(zr), int(n_offsets), ptr(off), int(n_ids),
-                                      ptr(ids), stream_ptr(device)), "dss_debug_tile_lists")
+    call("dss_debug_tile_lists", device, int(n_views), zr, int(n_offsets), off, int(n_ids), ids)
     return zr, off, ids
 
 
 def scratch_bytes(device=None):
     return int(load().dss_scratch_bytes(ctx(device)))
+
+
+def tile_total(device=None):
+    """the forward tile-list size the device published last (a mapped pinned word: no synchronisation)"""
+    return int(load().dss_debug_tile_total(ctx(device)))
 
 
 def as_f32(t, name):

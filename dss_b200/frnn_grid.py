@@ -23,12 +23,8 @@ def insert_points_cuda(points, lengths, params, grid_cnt, grid_cell, grid_idx, G
         if not t.is_contiguous():
             raise RuntimeError("output tensors must be contiguous")
     N, P = points.shape[0], points.shape[1]
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_grid_insert_points_2d(
-            _lib.ctx(dev), _lib.ptr(_lib.as_f32(points, "points")), _lib.ptr(lengths.contiguous()),
-            _lib.ptr(_lib.as_f32(params, "params")), _lib.ptr(grid_cnt), _lib.ptr(grid_cell), _lib.ptr(grid_idx),
-            N, P, int(G), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_grid_insert_points_2d")
+    _lib.call("dss_grid_insert_points_2d", dev, _lib.as_f32(points, "points"), lengths.contiguous(),
+              _lib.as_f32(params, "params"), grid_cnt, grid_cell, grid_idx, N, P, int(G))
 
 
 def counting_sort_cuda(points, lengths, grid_cell, grid_idx, grid_off, sorted_points, sorted_points_idxs):
@@ -39,12 +35,9 @@ def counting_sort_cuda(points, lengths, grid_cell, grid_idx, grid_off, sorted_po
         if not t.is_contiguous():
             raise RuntimeError("output tensors must be contiguous")
     N, P, G = points.shape[0], points.shape[1], grid_off.shape[1]
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_grid_counting_sort_2d(
-            _lib.ctx(dev), _lib.ptr(_lib.as_f32(points, "points")), _lib.ptr(lengths.contiguous()),
-            _lib.ptr(grid_cell.contiguous()), _lib.ptr(grid_idx.contiguous()), _lib.ptr(grid_off.contiguous()),
-            _lib.ptr(sorted_points), _lib.ptr(sorted_points_idxs), N, P, G, _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_grid_counting_sort_2d")
+    _lib.call("dss_grid_counting_sort_2d", dev, _lib.as_f32(points, "points"), lengths.contiguous(),
+              grid_cell.contiguous(), grid_idx.contiguous(), grid_off.contiguous(), sorted_points, sorted_points_idxs,
+              N, P, G)
 
 
 def knn_points_packed(points, first_idx, num_points, K, r=-1.0, queries=None, query_first_idx=None, query_num=None,
@@ -66,12 +59,9 @@ def knn_points_packed(points, first_idx, num_points, K, r=-1.0, queries=None, qu
     Pq, P, N = q.shape[0], pts.shape[0], num_points.shape[0]
     d = torch.empty((Pq, K), dtype=torch.float32, device=dev)
     i = torch.empty((Pq, K), dtype=torch.int32, device=dev) if return_idx else None
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_knn_points(
-            _lib.ctx(dev), _lib.ptr(None if queries is None else q), _lib.ptr(None if queries is None else qf.contiguous()),
-            _lib.ptr(None if queries is None else qn.contiguous()), _lib.ptr(pts), _lib.ptr(first_idx.contiguous()),
-            _lib.ptr(num_points.contiguous()), N, Pq, P, int(K), float(r), _lib.ptr(d), _lib.ptr(i), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_knn_points")
+    query_args = (None, None, None) if queries is None else (q, qf.contiguous(), qn.contiguous())
+    _lib.call("dss_knn_points", dev, *query_args, pts, first_idx.contiguous(), num_points.contiguous(), N, Pq, P,
+              int(K), float(r), d, i)
     return d, i
 
 

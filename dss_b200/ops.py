@@ -205,9 +205,7 @@ class _RenderFunction(torch.autograd.Function):
         a.records, a.scaler, a.image, a.idx = _lib.ptr(records), _lib.ptr(scaler), _lib.ptr(image), _lib.ptr(idx)
         a.weights, a.visible, a.zbuf, a.qvalue = _lib.ptr(weights), _lib.ptr(visible), _lib.ptr(zbuf), _lib.ptr(qvalue)
         a.cell_counts = _lib.ptr(cell_counts)
-        with torch.cuda.device(dev):
-            rc = _lib.load().dss_render_forward(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
-        _lib.check(rc, "dss_render_forward")
+        _lib.call("dss_render_forward", dev, C.byref(a))
         # no zero-filled gradients for the outputs nobody differentiates (idx, weights, records ... would cost five
         # fill kernels over ~400 MB per backward); backward() handles None
         ctx.set_materialize_grads(False)
@@ -275,58 +273,49 @@ class _RenderFunction(torch.autograd.Function):
             grad_lights = torch.empty_like(sh.lights) if ctx.needs_input_grad[14] else None
             grad_amb = torch.empty_like(sh.ambient) if ctx.needs_input_grad[15] else None
         want_light = grad_lights is not None or grad_amb is not None
-        lib = _lib.load()
 
         def light_backward():
             # reads the d L / d shaded scratch in grad_colours
             a.grad_colours = _lib.ptr(grad_colours)
-            rc = lib.dss_light_backward(_lib.ctx(dev), C.byref(a), _lib.ptr(grad_lights), _lib.ptr(grad_amb),
-                                        _lib.stream_ptr(dev))
-            _lib.check(rc, "dss_light_backward")
+            _lib.call("dss_light_backward", dev, C.byref(a), grad_lights, grad_amb)
 
         def camera_backward():
             # reads grad_ndc and (shading) the d L / d shaded scratch in grad_colours
             a.grad_colours = _lib.ptr(grad_colours)
-            rc = lib.dss_camera_backward(_lib.ctx(dev), C.byref(a), _lib.ptr(grad_proj), _lib.ptr(grad_view),
-                                         _lib.ptr(grad_cam), _lib.stream_ptr(dev))
-            _lib.check(rc, "dss_camera_backward")
+            _lib.call("dss_camera_backward", dev, C.byref(a), grad_proj, grad_view, grad_cam)
 
-        with torch.cuda.device(dev):
-            if grad_sync is None:
-                rc = lib.dss_render_backward(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
-                _lib.check(rc, "dss_render_backward")
-                if want_cam:
-                    camera_backward()
-                if want_light:
-                    light_backward()
-            else:
-                # data-parallel step (dss_b200/parallel.py): the colour gradients are final after the colour scatter --
-                # reduce them over the ranks on a side stream while the occupancy path runs here
-                main, side = torch.cuda.current_stream(dev), grad_sync.side_stream(dev)
-                side.wait_stream(main)
-                with torch.cuda.stream(side):
-                    rc = lib.dss_colour_backward(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
-                    _lib.check(rc, "dss_colour_backward")
-                    if shade is not None:
-                        shade_done = torch.cuda.Event()
-                        shade_done.record(side)
-                        grad_sync.reduce_early(grad_albedo, grad_normals)
-                    else:
-                        grad_sync.reduce_early(grad_colours)
-                a.grad_colours = _lib.ptr(None)
-                rc = lib.dss_render_backward(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
-                _lib.check(rc, "dss_render_backward")
+        if grad_sync is None:
+            _lib.call("dss_render_backward", dev, C.byref(a))
+            if want_cam:
+                camera_backward()
+            if want_light:
+                light_backward()
+        else:
+            # data-parallel step (dss_b200/parallel.py): the colour gradients are final after the colour scatter --
+            # reduce them over the ranks on a side stream while the occupancy path runs here
+            main, side = torch.cuda.current_stream(dev), grad_sync.side_stream(dev)
+            side.wait_stream(main)
+            with torch.cuda.stream(side):
+                _lib.call("dss_colour_backward", dev, C.byref(a))
                 if shade is not None:
-                    main.wait_event(shade_done)
-                    grad_points += grad_pshade           # position gradient through the shading
-                if want_cam:
-                    # the rank's own views: no collective (shared camera parameters are the caller's to reduce)
-                    camera_backward()
-                if want_light:
-                    # after the shading work of the side stream (waited for above); no collective either
-                    light_backward()
-                grad_sync.reduce_late(grad_points)
-                grad_sync.join(dev)
+                    shade_done = torch.cuda.Event()
+                    shade_done.record(side)
+                    grad_sync.reduce_early(grad_albedo, grad_normals)
+                else:
+                    grad_sync.reduce_early(grad_colours)
+            a.grad_colours = _lib.ptr(None)
+            _lib.call("dss_render_backward", dev, C.byref(a))
+            if shade is not None:
+                main.wait_event(shade_done)
+                grad_points += grad_pshade           # position gradient through the shading
+            if want_cam:
+                # the rank's own views: no collective (shared camera parameters are the caller's to reduce)
+                camera_backward()
+            if want_light:
+                # after the shading work of the side stream (waited for above); no collective either
+                light_backward()
+            grad_sync.reduce_late(grad_points)
+            grad_sync.join(dev)
         cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb, None, None)
         if shade is not None:
             return (grad_points, grad_normals, grad_albedo) + cams
@@ -400,23 +389,16 @@ def point_filters(out: RenderOutput, mask_img, group=None):
     strides = (C.c_int64 * 3)(*mask_img.stride())
     head = (out.records, out.visible, 1, N, P0, mask_img, int(mask_img.dtype != torch.float32), strides,
             int(mask_img.shape[1]), int(mask_img.shape[2]))
-
-    def launch(name, *tail):
-        args = [_lib.ptr(a) if isinstance(a, torch.Tensor) or a is None else a for a in head + tail]
-        with torch.cuda.device(dev):
-            rc = getattr(_lib.load(), name)(_lib.ctx(dev), *args, _lib.stream_ptr(dev))
-        _lib.check(rc, name)
-
     if group is None:
         visibility = torch.empty((P0,), dtype=torch.bool, device=dev)
         inmask = torch.empty((P0,), dtype=torch.bool, device=dev)
-        launch("dss_point_filters", visibility, inmask)
+        _lib.call("dss_point_filters", dev, *head, visibility, inmask)
         return visibility, inmask
     import torch.distributed as dist
     visibility, inmask = (torch.empty((P0,), dtype=torch.uint8, device=dev) for _ in range(2))
-    launch("dss_point_filters", visibility, inmask)
+    _lib.call("dss_point_filters", dev, *head, visibility, inmask)
     dist.all_reduce(visibility, op=dist.ReduceOp.MAX, group=group)
-    launch("dss_point_filters_gated", visibility, visibility, inmask)
+    _lib.call("dss_point_filters_gated", dev, *head, visibility, visibility, inmask)
     dist.all_reduce(inmask, op=dist.ReduceOp.MAX, group=group)
     return visibility.view(torch.bool), inmask.view(torch.bool)
 
@@ -476,9 +458,7 @@ def preprocess_points(points, normals, proj, view, h, params: SplatParams, first
     _fill_common(a, points_c, normals_c, None, proj_c, view_c, h_c, fi, npts, shared_cloud, N, P0, P, params)
     a.frames = _lib.ptr(frames_c)
     a.ndc, a.ellipse, a.radii, a.scaler = _lib.ptr(ndc), _lib.ptr(ell), _lib.ptr(radii), _lib.ptr(scaler)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_preprocess(_lib.ctx(dev), C.byref(a), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_preprocess")
+    _lib.call("dss_preprocess", dev, C.byref(a))
     return {"ndc": ndc, "ellipse_params": ell, "radii": radii, "scaler": scaler,
             "cutoff_threshold": torch.full((P,), float(params.cutoff_threshold), **f32)}
 
@@ -515,11 +495,8 @@ def local_frames(points, first_idx=None, num_points=None):
     fi, npts = first_idx.contiguous(), num_points.contiguous()
     _, idx = knn_points_packed(pts, fi, npts, LOCAL_FRAME_K, -1.0)
     frames = torch.empty((P, 8), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_local_frames(_lib.ctx(dev), _lib.ptr(pts), _lib.ptr(None if single else fi),
-                                          _lib.ptr(None if single else npts), int(npts.shape[0]), P, _lib.ptr(idx),
-                                          _lib.ptr(frames), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_local_frames")
+    _lib.call("dss_local_frames", dev, pts, None if single else fi, None if single else npts, int(npts.shape[0]), P,
+              idx, frames)
     return frames
 
 
@@ -527,6 +504,22 @@ class MeshRender(NamedTuple):
     image: Optional[torch.Tensor]   # (N,S,S,4) flat-shaded rgb + coverage, or None without shading
     pix_to_face: torch.Tensor       # (N,S,S) int32 face index in the mesh, -1 where no face covers the pixel
     zbuf: torch.Tensor              # (N,S,S) float32 view-space depth of that face, -1 where none
+
+
+def _mesh_input(verts, faces):
+    """(verts (V,3) float32, faces (F,3) int32, V, F) of a triangle mesh: faces integer, every index in [0, V), at most
+    2^31 - 1 vertices and faces"""
+    v = _lib.as_f32(verts.detach(), "verts")
+    if v.dim() != 2 or v.shape[1] != 3:
+        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
+    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
+        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
+    V, F = v.shape[0], faces.shape[0]
+    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
+        raise ValueError("face indices must lie in [0, %d)" % V)
+    if V >= 2 ** 31 or F >= 2 ** 31:
+        raise ValueError("at most 2^31 - 1 vertices and faces")
+    return v, faces.detach().to(torch.int32).contiguous(), V, F
 
 
 def render_mesh(verts, faces, proj, view, image_size, shading: Optional[Shading] = None) -> MeshRender:
@@ -540,17 +533,7 @@ def render_mesh(verts, faces, proj, view, image_size, shading: Optional[Shading]
     directional or point; the vertex colours and materials are ones.  Forward only (no gradients).  Background pixels
     are (1, 1, 1, 0); alpha is the coverage mask."""
     dev = _lib.require_cuda(verts, faces, proj, view)
-    v = _lib.as_f32(verts.detach(), "verts")
-    if v.dim() != 2 or v.shape[1] != 3:
-        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
-    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
-        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
-    V, F = v.shape[0], faces.shape[0]
-    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
-        raise ValueError("face indices must lie in [0, %d)" % V)
-    if V >= 2 ** 31 or F >= 2 ** 31:
-        raise ValueError("at most 2^31 - 1 vertices and faces")
-    f = faces.detach().to(torch.int32).contiguous()
+    v, f, V, F = _mesh_input(verts, faces)
     proj_c, view_c = _lib.as_f32(proj.detach(), "proj"), _lib.as_f32(view.detach(), "view")
     N = proj_c.shape[0]
     if tuple(proj_c.shape) != (N, 4, 4) or tuple(view_c.shape) != (N, 4, 4) or N < 1:
@@ -567,12 +550,7 @@ def render_mesh(verts, faces, proj, view, image_size, shading: Optional[Shading]
         image = torch.empty((N, S, S, 4), dtype=torch.float32, device=dev)
         sh_args = (int(sh.lights.shape[-2]), sh.light_type, int(sh.lights.dim() == 3), sh.shininess, sh.lights,
                    sh.ambient, sh.cam_centres)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_rasterize_mesh(
-            _lib.ctx(dev), _lib.ptr(v), V, _lib.ptr(f), F, _lib.ptr(proj_c), _lib.ptr(view_c), N, S,
-            *sh_args[:4], *(_lib.ptr(t) for t in sh_args[4:]), _lib.ptr(pix_to_face), _lib.ptr(zbuf), _lib.ptr(image),
-            _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_rasterize_mesh")
+    _lib.call("dss_rasterize_mesh", dev, v, V, f, F, proj_c, view_c, N, S, *sh_args, pix_to_face, zbuf, image)
     return MeshRender(image, pix_to_face, zbuf)
 
 
@@ -645,11 +623,7 @@ def _chamfer_sums(x, y, x_lengths=None, y_lengths=None, x_normals=None, y_normal
     xp, yp = _lib.as_f32(xp, "x"), _lib.as_f32(yp, "y")
     xn, yn = (_lib.as_f32(xn, "x_normals"), _lib.as_f32(yn, "y_normals")) if with_normals else (None, None)
     sums = torch.zeros((N, 4), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_chamfer(_lib.ctx(dev), _lib.ptr(xp), _lib.ptr(xn), _lib.ptr(xf), _lib.ptr(xc),
-                                     xp.shape[0], _lib.ptr(yp), _lib.ptr(yn), _lib.ptr(yf), _lib.ptr(yc), yp.shape[0],
-                                     N, _lib.ptr(sums), _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_chamfer")
+    _lib.call("dss_chamfer", dev, xp, xn, xf, xc, xp.shape[0], yp, yn, yf, yc, yp.shape[0], N, sums)
     return sums, xc, yc, with_normals
 
 
@@ -673,27 +647,17 @@ def point_mesh_distance(points, verts, faces, return_closest=False, _face_tests=
         if t.requires_grad:
             raise RuntimeError("point_mesh_distance has no backward: pass %s that does not require grad (detach it, "
                                "or call it under torch.no_grad())" % name)
-    p, v = _lib.as_f32(points, "points"), _lib.as_f32(verts, "verts")
+    p = _lib.as_f32(points, "points")
     if p.dim() != 2 or p.shape[1] != 3:
         raise RuntimeError("points must have shape (P, 3), got %s" % (tuple(p.shape),))
-    if v.dim() != 2 or v.shape[1] != 3:
-        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
-    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
-        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
-    P, V, F = p.shape[0], v.shape[0], faces.shape[0]
-    if P >= 2 ** 31 or V >= 2 ** 31 or F >= 2 ** 31:
+    v, f, V, F = _mesh_input(verts, faces)
+    P = p.shape[0]
+    if P >= 2 ** 31:
         raise ValueError("at most 2^31 - 1 points, vertices and faces")
-    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
-        raise ValueError("face indices must lie in [0, %d)" % V)
-    f = faces.to(torch.int32).contiguous()
     sq = torch.empty(P, dtype=torch.float32, device=dev)
     idx = torch.empty(P, dtype=torch.int32, device=dev)
     closest = torch.empty((P, 3), dtype=torch.float32, device=dev) if return_closest else None
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_point_mesh_distance(_lib.ctx(dev), _lib.ptr(p), P, _lib.ptr(v), V, _lib.ptr(f), F,
-                                                 _lib.ptr(sq), _lib.ptr(idx), _lib.ptr(closest), _lib.ptr(_face_tests),
-                                                 _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_point_mesh_distance")
+    _lib.call("dss_point_mesh_distance", dev, p, P, v, V, f, F, sq, idx, closest, _face_tests)
     return PointMeshDistance(sq, idx.long(), closest)
 
 
@@ -724,20 +688,16 @@ def marching_tetrahedra(grid, origin, side):
     R = g.shape[0] - 1
     c = (C.c_float * 3)(*[float(v) for v in (origin.tolist() if torch.is_tensor(origin) else origin)])
     nv, nf = C.c_int64(0), C.c_int64(0)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = lib.dss_marching_tetrahedra(_lib.ctx(dev), _lib.ptr(g), R, c, float(side), None, 0, None, 0,
-                                         C.byref(nv), C.byref(nf), _lib.stream_ptr(dev))
-        if rc == _lib.DSS_E_CAPACITY and nv.value < 2 ** 31 and nf.value < 2 ** 31:
+    verts = torch.empty((0, 3), dtype=torch.float32, device=dev)
+    faces = torch.empty((0, 3), dtype=torch.int32, device=dev)
+    if _lib.call("dss_marching_tetrahedra", dev, g, R, c, float(side), None, 0, None, 0, C.byref(nv), C.byref(nf),
+                 capacity=True) == _lib.DSS_E_CAPACITY:
+        # counts beyond int32 are not allocated: the library refuses them in the second call
+        if nv.value < 2 ** 31 and nf.value < 2 ** 31:
             verts = torch.empty((nv.value, 3), dtype=torch.float32, device=dev)
             faces = torch.empty((nf.value, 3), dtype=torch.int32, device=dev)
-            rc = lib.dss_marching_tetrahedra(_lib.ctx(dev), _lib.ptr(g), R, c, float(side), _lib.ptr(verts),
-                                             nv.value, _lib.ptr(faces), nf.value, C.byref(nv), C.byref(nf),
-                                             _lib.stream_ptr(dev))
-        else:
-            verts = torch.empty((0, 3), dtype=torch.float32, device=dev)
-            faces = torch.empty((0, 3), dtype=torch.int32, device=dev)
-    _lib.check(rc, "dss_marching_tetrahedra")
+        _lib.call("dss_marching_tetrahedra", dev, g, R, c, float(side), verts, verts.shape[0], faces, faces.shape[0],
+                  C.byref(nv), C.byref(nf))
     return verts, faces.long()
 
 
@@ -769,10 +729,7 @@ def poisson_reconstruction(points, normals, depth=8, return_grid=False) -> Poiss
     chi = torch.empty((R + 1, R + 1, R + 1), dtype=torch.float32, device=dev)
     c, L = (C.c_float * 3)(), C.c_float(0.0)
     its, res = C.c_int(0), C.c_double(0.0)
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_poisson_solve(_lib.ctx(dev), _lib.ptr(p), _lib.ptr(n), P, depth, _lib.ptr(chi), c,
-                                           C.byref(L), C.byref(its), C.byref(res), None, None, _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_poisson_solve")
+    _lib.call("dss_poisson_solve", dev, p, n, P, depth, chi, c, C.byref(L), C.byref(its), C.byref(res), None, None)
     origin = torch.tensor(list(c), dtype=torch.float32)
     verts, faces = marching_tetrahedra(chi, origin, L.value)
     return PoissonMesh(verts, faces, chi if return_grid else None, origin, L.value, its.value, res.value)
@@ -797,37 +754,22 @@ def sample_points_poisson_disk(verts, faces, num_samples, geodesic=False, seed=0
     dev = _lib.require_cuda(verts, faces)
     if verts.requires_grad:
         raise RuntimeError("sample_points_poisson_disk has no backward: pass verts that do not require grad")
-    v = _lib.as_f32(verts, "verts")
-    if v.dim() != 2 or v.shape[1] != 3:
-        raise RuntimeError("verts must have shape (V, 3), got %s" % (tuple(v.shape),))
-    if faces.dim() != 2 or faces.shape[1] != 3 or faces.dtype.is_floating_point or faces.dtype == torch.bool:
-        raise RuntimeError("faces must be an integer tensor of shape (F, 3), got %s %s" % (faces.dtype, tuple(faces.shape)))
+    v, f, V, F = _mesh_input(verts, faces)
     N = int(num_samples)
     if N < 1 or _lib.PD_MONTECARLO_RATE * N >= 2 ** 31:
         raise ValueError("num_samples must lie in [1, %d], got %r" % ((2 ** 31 - 1) // _lib.PD_MONTECARLO_RATE,
                                                                      num_samples))
-    V, F = v.shape[0], faces.shape[0]
-    if V >= 2 ** 31 or F >= 2 ** 31:
-        raise ValueError("at most 2^31 - 1 vertices and faces")
-    if F and (int(faces.min()) < 0 or int(faces.max()) >= V):
-        raise ValueError("face indices must lie in [0, %d)" % V)
-    f = faces.to(torch.int32).contiguous()
     n, r = C.c_int64(0), C.c_double(0.0)
-    lib = _lib.load()
     # room for a count within the tolerance, which is what the search nearly always returns; a call that finds more
     # (its probes all missed the tolerance) is repeated with room for exactly that many
     cap = N + N // 200
-    with torch.cuda.device(dev):
-        for _ in range(2):
-            points = torch.empty((cap, 3), dtype=torch.float32, device=dev)
-            normals = torch.empty((cap, 3), dtype=torch.float32, device=dev)
-            rc = lib.dss_sample_mesh_poisson_disk(_lib.ctx(dev), _lib.ptr(v), V, _lib.ptr(f), F, N,
-                                                  int(bool(geodesic)), int(seed) & (2 ** 64 - 1), _lib.ptr(points),
-                                                  _lib.ptr(normals), cap, C.byref(n), C.byref(r), _lib.stream_ptr(dev))
-            if rc != _lib.DSS_E_CAPACITY:
-                break
-            cap = n.value
-    _lib.check(rc, "dss_sample_mesh_poisson_disk")
+    for first in (True, False):
+        points = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+        normals = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+        if _lib.call("dss_sample_mesh_poisson_disk", dev, v, V, f, F, N, int(bool(geodesic)), int(seed) & (2 ** 64 - 1),
+                     points, normals, cap, C.byref(n), C.byref(r), capacity=first) != _lib.DSS_E_CAPACITY:
+            break
+        cap = n.value
     return PoissonDiskSamples(points[:n.value], normals[:n.value], r.value)
 
 

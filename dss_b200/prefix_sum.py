@@ -20,8 +20,5 @@ def prefix_sum_cuda(grid_cnt, num_grids, grid_off):
     if n < 0 or n > grid_cnt.numel() or n > grid_off.numel():
         raise RuntimeError("num_grids=%d out of range" % n)
     src = grid_cnt.contiguous()
-    with torch.cuda.device(dev):
-        rc = _lib.load().dss_exclusive_scan_i32(_lib.ctx(dev), _lib.ptr(src), _lib.ptr(grid_off), n,
-                                                _lib.stream_ptr(dev))
-    _lib.check(rc, "dss_exclusive_scan_i32")
+    _lib.call("dss_exclusive_scan_i32", dev, src, grid_off, n)
     return None

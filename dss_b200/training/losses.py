@@ -123,13 +123,9 @@ class _SurfaceRegulariser(torch.autograd.Function):
         P, N = points.shape[0], num_points.shape[0]
         loss = torch.empty((P,) if kind == 0 else (P, 3), dtype=torch.float32, device=dev)
         coef = torch.empty((P, 3 if kind == 0 else 9), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            rc = _lib.load().dss_surface_regulariser(
-                _lib.ctx(dev), kind, _lib.ptr(points), _lib.ptr(normals), _lib.ptr(first_idx), _lib.ptr(num_points), N,
-                P, _lib.ptr(knn_dists), _lib.ptr(knn_idx), K, self_col, _lib.ptr(knn_points), _lib.ptr(neighbour_points),
-                _lib.ptr(reliable), _lib.ptr(visible),
-                float(sharpness_sigma), float(filter_scale), _lib.ptr(loss), _lib.ptr(coef), _lib.stream_ptr(dev))
-        _lib.check(rc, "dss_surface_regulariser")
+        _lib.call("dss_surface_regulariser", dev, kind, points, normals, first_idx, num_points, N, P, knn_dists,
+                  knn_idx, K, self_col, knn_points, neighbour_points, reliable, visible, float(sharpness_sigma),
+                  float(filter_scale), loss, coef)
         ctx.kind = kind
         ctx.save_for_backward(coef)
         return loss
@@ -541,15 +537,11 @@ def _image_loss_torch_sharded(rgba, img, mask_img, lambda_rgb, lambda_silhouette
             "loss_dr_silhouette": loss_dr_silhouette, "loss_image_gradients": zero}
 
 
-def _image_loss_call(name, rgba, img, mask, lambda_rgb, lambda_sil, *tail):
+def _image_loss_args(rgba, img, mask, lambda_rgb, lambda_sil):
+    """the leading arguments of dss_image_loss_forward, _partial and _backward"""
     N, H, W = rgba.shape[:3]
-    dev = rgba.device
-    strides = (C.c_int64 * 4)(*img.stride())
-    with torch.cuda.device(dev):
-        rc = getattr(_lib.load(), name)(
-            _lib.ctx(dev), _lib.ptr(rgba), _lib.ptr(img), strides, _lib.ptr(mask), int(mask.dtype != torch.float32),
-            N, H, W, float(lambda_rgb), float(lambda_sil), *[_lib.ptr(t) for t in tail], _lib.stream_ptr(dev))
-    _lib.check(rc, name)
+    return (rgba, img, (C.c_int64 * 4)(*img.stride()), mask, int(mask.dtype != torch.float32), N, H, W,
+            float(lambda_rgb), float(lambda_sil))
 
 
 class _ImageLoss(torch.autograd.Function):
@@ -563,21 +555,18 @@ class _ImageLoss(torch.autograd.Function):
         (N, H, W), dev = rgba.shape[:3], rgba.device
         totals = torch.empty((N + 1, 5), dtype=torch.float64, device=dev)
         loss, loss_rgb, loss_sil = (torch.empty((), dtype=torch.float32, device=dev) for _ in range(3))
+        args = _image_loss_args(rgba, img, mask, lambda_rgb, lambda_sil)
         if group is None:
-            _image_loss_call("dss_image_loss_forward", rgba, img, mask, lambda_rgb, lambda_sil, totals, loss, loss_rgb,
-                             loss_sil)
+            _lib.call("dss_image_loss_forward", dev, *args, totals, loss, loss_rgb, loss_sil)
         else:
             import torch.distributed as dist
             if N:
-                _image_loss_call("dss_image_loss_partial", rgba, img, mask, lambda_rgb, lambda_sil, totals)
+                _lib.call("dss_image_loss_partial", dev, *args, totals)
             else:
                 totals.zero_()
             dist.all_reduce(totals[N], op=dist.ReduceOp.SUM, group=group)
-            with torch.cuda.device(dev):
-                rc = _lib.load().dss_image_loss_finish(_lib.ctx(dev), _lib.ptr(totals[N]), H, W, float(lambda_rgb),
-                                                       float(lambda_sil), _lib.ptr(loss), _lib.ptr(loss_rgb),
-                                                       _lib.ptr(loss_sil), _lib.stream_ptr(dev))
-            _lib.check(rc, "dss_image_loss_finish")
+            _lib.call("dss_image_loss_finish", dev, totals[N], H, W, float(lambda_rgb), float(lambda_sil), loss,
+                      loss_rgb, loss_sil)
         ctx.lambdas = (lambda_rgb, lambda_sil)
         ctx.save_for_backward(rgba, img, mask, totals)
         return loss, loss_rgb, loss_sil
@@ -588,7 +577,8 @@ class _ImageLoss(torch.autograd.Function):
         grad = torch.empty_like(rgba, memory_format=torch.contiguous_format)
         if rgba.shape[0]:
             ups = [g.to(torch.float32).contiguous() for g in (g_loss, g_rgb, g_sil)]
-            _image_loss_call("dss_image_loss_backward", rgba, img, mask, *ctx.lambdas, totals, *ups, grad)
+            _lib.call("dss_image_loss_backward", rgba.device, *_image_loss_args(rgba, img, mask, *ctx.lambdas), totals,
+                      *ups, grad)
         return grad, None, None, None, None, None
 
 

@@ -25,8 +25,6 @@ into the step's static inputs.  Host-side settings are frozen into a capture; wh
 its ``radii_backward_scaler``, which the trainer's scheduler lowers, or a lambda), or when another library call has
 reallocated the scratch buffers the graph uses, the next ``replay()`` captures again.
 """
-import ctypes as C
-
 import torch
 import torch.distributed as dist
 import torch.nn.functional as F
@@ -36,6 +34,7 @@ from ..core.cloud import PointClouds3D, PointCloudsFilters
 from ..core.lighting import pack_lights
 from ..core.rasterizer import point_sq_spacing, splat_variance_scale
 from ..core.texture import camera_centres
+from ..graph import GraphedStep
 from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, local_frames, point_filters, point_filters_no_views,
                    render_points)
 from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
@@ -202,7 +201,7 @@ class _NoViews(torch.autograd.Function):
         return g_points, g_normals, g_albedo, None
 
 
-class GraphedTrainStep(TrainStep):
+class GraphedTrainStep(TrainStep, GraphedStep):
     """:class:`TrainStep` captured in a CUDA graph.  The step owns static copies of the first batch
     (``step.img``, ``step.mask_img``, ``step.proj``, ``step.view`` and the packed light rows); ``load(img, mask_img,
     proj, view, lights)`` copies the next batch into them in place (same shapes, same kind of lights) and ``replay()``
@@ -220,6 +219,7 @@ class GraphedTrainStep(TrainStep):
     :meth:`stale` tells when a new capture (:meth:`capture`) would be faster.  The capture holds the library's scratch
     buffers; when a library call outside the step has reallocated them (the library's scratch total changed), the next
     ``replay()`` captures again too."""
+    _OUTPUTS = ("loss", "image", "visibility", "inmask")
 
     def __init__(self, points, normals, colours, params: SplatParams, img, mask_img, proj, view, lights, warmup=3,
                  **settings):
@@ -235,36 +235,11 @@ class GraphedTrainStep(TrainStep):
         self.proj, self.view = proj.detach().float().contiguous().clone(), view.detach().float().contiguous().clone()
         self.lights, self.ambient = rows.detach().clone(), ambient.detach().clone()
         self._warmup = max(1, int(warmup))
-        self.graph = None
+        self._leaves = (self.points, self.normals, self.colours)
         self.capture()
 
     def _eager(self):
         return self._run(self.img, self.mask_img, self.proj, self.view, self.lights, self.ambient, self._light_type)
-
-    def capture(self):
-        """warm up on a side stream (sizes the library's scratch and the caching allocator), then capture the step"""
-        dev = self.device
-        self.graph = None
-        s = torch.cuda.Stream(device=dev)
-        s.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(s):
-            for _ in range(self._warmup):
-                self._eager()
-        torch.cuda.current_stream(dev).wait_stream(s)
-        torch.cuda.synchronize(dev)
-        self._capacity_at_capture = self._tile_total()
-        for t in (self.points, self.normals, self.colours):
-            t.grad = None
-        graph = torch.cuda.CUDAGraph(keep_graph=True)    # (kept for kernel_nodes)
-        with torch.cuda.graph(graph):
-            self._eager()
-        graph.instantiate()
-        # the library's scratch only grows, by reallocation: a different total means that a buffer the graph uses moved
-        self.graph, self._captured, self._scratch = graph, self.settings(), _lib.scratch_bytes(dev)
-        # what every replay rewrites: re-attached after each replay, so that an optimizer's zero_grad(set_to_none=True)
-        # or an eager call in between does not detach them
-        self._outputs = (self.loss, self.image, self.visibility, self.inmask)
-        self._grads = tuple(t.grad for t in (self.points, self.normals, self.colours))
 
     def load(self, img, mask_img, proj, view, lights):
         """copy the next batch into the static inputs (no synchronisation)"""
@@ -279,39 +254,3 @@ class GraphedTrainStep(TrainStep):
                 raise ValueError("load() takes a batch of the capture's shapes and dtypes: %s %s, got %s %s"
                                  % (tuple(dst.shape), dst.dtype, tuple(src.shape), src.dtype))
             dst.copy_(src.detach())
-
-    def replay(self):
-        if self.settings() != self._captured or _lib.scratch_bytes(self.device) != self._scratch:
-            self.capture()
-        self.graph.replay()
-        self.loss, self.image, self.visibility, self.inmask = self._outputs
-        for t, g in zip((self.points, self.normals, self.colours), self._grads):
-            t.grad = g
-        return self.loss
-
-    def _tile_total(self):
-        return int(_lib.load().dss_debug_tile_total(_lib.ctx(self.device)))
-
-    def stale(self, slack=1.2) -> bool:
-        """True when the tile lists have outgrown what they were at capture time by more than `slack` (the replay is
-        still correct, but a new capture will be faster); as GraphedRenderStep.stale"""
-        now = self._tile_total()
-        return self._capacity_at_capture > 0 and now > slack * 1.25 * self._capacity_at_capture
-
-    def kernel_nodes(self) -> int:
-        """the number of kernel launches one replay makes (kernel nodes of the captured graph)"""
-        rt = C.CDLL("libcudart.so.12")
-        g = C.c_void_p(self.graph.raw_cuda_graph())
-        count = C.c_size_t(0)
-        if rt.cudaGraphGetNodes(g, None, C.byref(count)):
-            raise RuntimeError("cudaGraphGetNodes failed")
-        nodes = (C.c_void_p * count.value)()
-        if rt.cudaGraphGetNodes(g, nodes, C.byref(count)):
-            raise RuntimeError("cudaGraphGetNodes failed")
-        kinds = C.c_int(0)
-        n = 0
-        for node in nodes:
-            if rt.cudaGraphNodeGetType(C.c_void_p(node), C.byref(kinds)):
-                raise RuntimeError("cudaGraphNodeGetType failed")
-            n += kinds.value == 0     # cudaGraphNodeTypeKernel
-        return n

@@ -231,3 +231,64 @@ def test_graphed_step_replays_the_eager_step(cuda_device):
             p.add_(0.002 * torch.randn(P0, 3, generator=torch.Generator().manual_seed(it)).to(d))
             c.mul_(0.9)
     assert not step.stale()
+
+
+@pytest.fixture
+def fresh_context(cuda_device):
+    """A library context of the test's own in place of the process's one, so that its scratch starts empty whatever
+    earlier tests rendered; destroyed afterwards, and the process's context restored."""
+    from dss_b200 import _lib
+    index = torch.device(cuda_device).index or 0
+    torch.cuda.synchronize()
+    saved = _lib._ctx.pop(index, None)
+    try:
+        yield
+    finally:
+        torch.cuda.synchronize()
+        own = _lib._ctx.pop(index, None)
+        if own is not None:
+            _lib.load().dss_destroy(own)
+        if saved is not None:
+            _lib._ctx[index] = saved
+
+
+def test_graphed_step_captures_again_when_the_scratch_moved(cuda_device, fresh_context):
+    """A library call that needs more scratch than a captured GraphedRenderStep reallocates the buffers the graph
+    reads; the next replay() must capture again (once) and still give the eager results."""
+    from dss_b200 import _lib
+    from dss_b200.graph import GraphedRenderStep
+    P0, N, S = 20000, 2, 64
+    pts, nrm, col, proj, view, cams = scene(P0, N, seed=29)
+    d = cuda_device
+    prm = SplatParams(image_size=S, znear=0.1, clip_pts_grad=0.05)
+    h = torch.full((N,), 3e-4, device=d)
+    g = (torch.randn(N, S, S, 4, generator=torch.Generator().manual_seed(9)) * 1e-3).to(d)
+    step = GraphedRenderStep(pts.to(d), nrm.to(d), col.to(d), proj.to(d), view.to(d), h, prm, g)
+    p, c = step.points, step.colours
+    graph, scratch = step.graph, _lib.scratch_bytes()
+    # an eager render at a larger image size and cloud grows the tile lists and the per-splat buffers
+    bp, bn, bc, bproj, bview, _ = scene(4 * P0, N, seed=30)
+    render_points(bp.to(d), bn.to(d), bc.to(d), bproj.to(d), bview.to(d), h, prm._replace(image_size=4 * S))
+    torch.cuda.synchronize()
+    assert _lib.scratch_bytes() > scratch
+
+    def eager():
+        pe = p.detach().clone().requires_grad_(True)
+        ce = c.detach().clone().requires_grad_(True)
+        o = render_points(pe, nrm.to(d), ce, proj.to(d), view.to(d), h, prm)
+        o.image.backward(g)
+        return o.image.detach(), pe.grad, ce.grad
+
+    graphs = []
+    for it in range(2):
+        img = step.replay()
+        graphs.append(step.graph)
+        torch.cuda.synchronize()
+        wi, wp, wc = eager()
+        assert img is step.image and torch.equal(img, wi)
+        assert torch.equal(step.grad_points, wp) and step.points.grad is step.grad_points
+        torch.testing.assert_close(step.grad_colours, wc, rtol=1e-4, atol=1e-9)
+        with torch.no_grad():
+            p.add_(0.002 * torch.randn(P0, 3, generator=torch.Generator().manual_seed(it)).to(d))
+    assert graphs[0] is not graph and graphs[1] is graphs[0]    # captured again over the moved scratch, and only once
+    assert not step.stale()
