@@ -9,35 +9,15 @@ library's kernel launches of one eager step and the kernel nodes of the graph.
     python scripts/anisotropic_time.py [--samples 21]
 """
 import argparse
-import os
-import statistics
-import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200 import _lib  # noqa: E402
-from dss_b200.core.lighting import DirectionalLights  # noqa: E402
-from dss_b200.ops import SplatParams, local_frames, render_points  # noqa: E402
-from dss_b200.training.step import GraphedTrainStep, TrainStep  # noqa: E402
-from tests.util import scene  # noqa: E402
-
-
-def timed(fn):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1)
-
-
-def median_ms(fn, samples):
-    for _ in range(3):
-        timed(fn)
-    t = [timed(fn) for _ in range(samples)]
-    return statistics.median(t), min(t), max(t)
+from timing import card, events_ms, launches, spread
+from dss_b200.core.lighting import DirectionalLights
+from dss_b200.ops import SplatParams, local_frames, render_points
+from dss_b200.training.step import GraphedTrainStep, TrainStep
+from tests.util import scene
 
 
 def main():
@@ -47,13 +27,16 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("anisotropic_time.py needs a CUDA device")
     dev = torch.device("cuda:0")
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print("gpu: %s" % (smi or "not measured"))
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
+
+    def samples(fn):
+        t = [events_ms(fn, 1) for _ in range(3 + a.samples)]
+        return spread(t[3:])                            # after 3 warm-up calls
+
     for P0 in (8000, 100000, 1000000):
         pts = scene(P0, 1, seed=0)[0].to(dev)
         print("local_frames P0 = %7d: median %.3f ms (min %.3f max %.3f)"
-              % ((P0,) + median_ms(lambda p=pts: local_frames(p), a.samples)))
+              % (P0, *samples(lambda: local_frames(pts))))
     N, S = 8, 512
     prm = SplatParams(image_size=S, points_per_pixel=5, cutoff_threshold=0.5, depth_merging_threshold=0.05,
                       radii_backward_scaler=5.0, clip_pts_grad=0.05, znear=0.1)
@@ -72,17 +55,13 @@ def main():
         for mode, kw in (("invariant", dict(Vrk_invariant=True)),
                          ("anisotropic", dict(Vrk_invariant=False, Vrk_isotropic=False))):
             eager = TrainStep(pts, nrm, col, prm, **kw)
-            eager(*batch)
-            torch.cuda.synchronize()
-            before = _lib.launch_count()
-            eager(*batch)
-            launches = _lib.launch_count() - before
-            te = median_ms(lambda e=eager: e(*batch), a.samples)
+            n = launches(lambda: eager(*batch), dev)
+            te = samples(lambda: eager(*batch))
             graph = GraphedTrainStep(pts, nrm, col, prm, *batch, **kw)
-            tg = median_ms(graph.replay, a.samples)
+            tg = samples(graph.replay)
             print("P0 = %6d %-11s: %d library launches per eager step, %d graph kernel nodes; eager median %.3f ms "
                   "(min %.3f max %.3f), graph median %.3f ms (min %.3f max %.3f)"
-                  % ((P0, mode, launches, graph.kernel_nodes()) + te + tg))
+                  % (P0, mode, n, graph.kernel_nodes(), *te, *tg))
             del graph, eager
 
 

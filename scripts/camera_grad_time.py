@@ -6,18 +6,13 @@ camera gradients are asked for).
     python scripts/camera_grad_time.py [--rounds 10] [--steps 20]
 """
 import argparse
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200 import _lib  # noqa: E402
-from dss_b200.core.camera import camera_matrices  # noqa: E402
-from dss_b200.ops import SplatParams, render_points  # noqa: E402
-from tests.util import random_cameras, sphere_cloud  # noqa: E402
+from timing import alternate, card, paired, spread, stage_ms
+from dss_b200.core.camera import camera_matrices
+from dss_b200.ops import SplatParams, render_points
+from tests.util import random_cameras, sphere_cloud
 
 
 def main():
@@ -43,39 +38,15 @@ def main():
         pts_d.grad = col_d.grad = pr.grad = vw.grad = None
         render_points(pts_d, nrm_d, col_d, pr, vw, h, prm).image.backward(grad)
 
-    def timed(cam, n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(n):
-            step(cam)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / n
-
-    for cam in (False, True):
-        timed(cam, 3)                                   # warm-up of both shapes
-    ms = {False: [], True: []}
-    for _ in range(a.rounds):
-        for cam in (False, True):
-            ms[cam].append(timed(cam, a.steps))
+    ms = alternate({cam: lambda cam=cam: step(cam) for cam in (False, True)}, a.rounds, a.steps, 3)
     stages = {}
     for cam in (False, True):
-        _lib.profile_enable(True, dev)
-        _lib.profile_reset(dev)
-        for _ in range(a.steps):
-            step(cam)
-        torch.cuda.synchronize()
-        st = _lib.profile_read(dev)
-        _lib.profile_enable(False, dev)
-        stages[cam] = {k: st[k][0] / a.steps for k in ("chain_world", "camera_backward")}
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    med = {k: statistics.median(v) for k, v in ms.items()}
-    diffs = [b - a_ for a_, b in zip(ms[False], ms[True])]
-    print("gpu: %s" % smi)
-    print("step ms without camera grads: median %.4f  (min %.4f max %.4f)" % (med[False], min(ms[False]), max(ms[False])))
-    print("step ms with camera grads:    median %.4f  (min %.4f max %.4f)" % (med[True], min(ms[True]), max(ms[True])))
-    print("paired difference ms: median %.4f  (min %.4f max %.4f)" % (statistics.median(diffs), min(diffs), max(diffs)))
+        st = stage_ms(lambda: step(cam), a.steps, dev)
+        stages[cam] = {k: st[k] for k in ("chain_world", "camera_backward")}
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
+    print("step ms without camera grads: median %.4f  (min %.4f max %.4f)" % spread(ms[False]))
+    print("step ms with camera grads:    median %.4f  (min %.4f max %.4f)" % spread(ms[True]))
+    print("paired difference ms: median %.4f  (min %.4f max %.4f)" % spread(paired(ms[False], ms[True])))
     for cam in (False, True):
         print("stage ms/step (camera grads %s): %s" % (cam, {k: round(v, 4) for k, v in stages[cam].items()}))
 

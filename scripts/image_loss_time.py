@@ -12,18 +12,16 @@ bytes (forward: rgba 16 + gt 12 + mask 4 per pixel; backward: the same again + 1
     python scripts/image_loss_time.py [--rounds 7] [--steps 20]
 """
 import argparse
-import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200.graph import GraphedRenderStep  # noqa: E402
-from dss_b200.ops import SplatParams, render_points  # noqa: E402
-from dss_b200.training.losses import image_loss, image_loss_torch  # noqa: E402
-from tests.util import scene  # noqa: E402
+from timing import alternate, card, spread
+from dss_b200.graph import GraphedRenderStep
+from dss_b200.ops import SplatParams, render_points
+from dss_b200.training.losses import image_loss, image_loss_torch
+from tests.util import scene
 
 
 def main():
@@ -74,36 +72,19 @@ def main():
         else:
             whole_step(v[1])
 
-    def timed(v, n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(n):
-            run(v)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / n
-
     variants = [("loss", r, N, S) for (N, S) in cases for r in ("torch", "fused")]
     variants += [("step", r) for r in ("torch", "fused", "graph")]
-    for v in variants:
-        timed(v, 3)                                     # warm-up of every variant
-    ms = {v: [] for v in variants}
-    for _ in range(a.rounds):
-        for v in variants:
-            ms[v].append(timed(v, a.steps))
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print("gpu: %s" % (smi or "not measured"))
+    ms = alternate({v: lambda v=v: run(v) for v in variants}, a.rounds, a.steps, 3)
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
     for v in variants:
         what = "%d x %d^2 loss" % (v[2], v[3]) if v[0] == "loss" else "8 x 512^2 whole step"
-        print("%-22s %-5s ms: median %.3f  (min %.3f max %.3f)"
-              % (what, v[1], statistics.median(ms[v]), min(ms[v]), max(ms[v])))
+        print("%-22s %-5s ms: median %.3f  (min %.3f max %.3f)" % (what, v[1], *spread(ms[v])))
     for (N, S) in cases:
         t, f = ms[("loss", "torch", N, S)], ms[("loss", "fused", N, S)]
         r = [x / y for x, y in zip(t, f)]
         gb = N * S * S * (2 * (16 + 12 + 4) + 16) / 1e9
         print("%d x %d^2: torch / fused median %.1fx (min %.1f max %.1f); fused %.0f GB/s algorithmic"
-              % (N, S, statistics.median(r), min(r), max(r), gb / (statistics.median(f) / 1e3)))
+              % (N, S, *spread(r), gb / (statistics.median(f) / 1e3)))
 
 
 if __name__ == "__main__":

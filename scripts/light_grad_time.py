@@ -7,19 +7,14 @@ the light kernels (light_backward).
     python scripts/light_grad_time.py [--rounds 10] [--steps 20]
 """
 import argparse
-import os
-import statistics
-import subprocess
-import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200 import _lib  # noqa: E402
-from dss_b200.core.camera import camera_matrices  # noqa: E402
-from dss_b200.core.lighting import DirectionalLights  # noqa: E402
-from dss_b200.ops import SplatParams, make_shading, render_points  # noqa: E402
-from tests.util import random_cameras, sphere_cloud  # noqa: E402
+from timing import alternate, card, paired, spread, stage_ms
+from dss_b200.core.camera import camera_matrices
+from dss_b200.core.lighting import DirectionalLights
+from dss_b200.ops import SplatParams, make_shading, render_points
+from tests.util import random_cameras, sphere_cloud
 
 
 def lights(L, V, per_view, grad, dev):
@@ -60,45 +55,22 @@ def main():
         sh = make_shading(lt, view)
         render_points(pts_d, nrm_d, alb_d, proj, view, h, prm, shading=sh).image.backward(grad)
 
-    def timed(v, n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(n):
-            step(v)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / n
-
-    for v in variants:
-        timed(v, 3)                                     # warm-up of every variant
-    ms = {v: [] for v in variants}
-    for _ in range(a.rounds):
-        for v in variants:
-            ms[v].append(timed(v, a.steps))
+    ms = alternate({v: lambda v=v: step(v) for v in variants}, a.rounds, a.steps, 3)
     stages = {}
     for v in variants:
-        _lib.profile_enable(True, dev)
-        _lib.profile_reset(dev)
-        for _ in range(a.steps):
-            step(v)
-        torch.cuda.synchronize()
-        st = _lib.profile_read(dev)
-        _lib.profile_enable(False, dev)
-        stages[v] = {k: st[k][0] / a.steps for k in ("preprocess", "colour_backward", "light_backward")}
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print("gpu: %s" % smi)
+        st = stage_ms(lambda: step(v), a.steps, dev)
+        stages[v] = {k: st[k] for k in ("preprocess", "colour_backward", "light_backward")}
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
     name = lambda v: "L=%d %-8s %s" % (v[0], "per-view" if v[1] else "shared", "light grads" if v[2] else "no light grads")
     for v in variants:
         print("step ms %s: median %.4f  (min %.4f max %.4f)  stage ms/step %s"
-              % (name(v), statistics.median(ms[v]), min(ms[v]), max(ms[v]), {k: round(x, 4) for k, x in stages[v].items()}))
+              % (name(v), *spread(ms[v]), {k: round(x, 4) for k, x in stages[v].items()}))
     for L in (1, 3):
         for what, (x, y) in (("per-view - shared, no light grads", ((L, False, False), (L, True, False))),
                              ("light grads - none, shared", ((L, False, False), (L, False, True))),
                              ("light grads - none, per-view", ((L, True, False), (L, True, True)))):
-            diffs = [b - a_ for a_, b in zip(ms[x], ms[y])]
             print("L=%d paired difference ms (%s): median %.4f  (min %.4f max %.4f)"
-                  % (L, what, statistics.median(diffs), min(diffs), max(diffs)))
+                  % (L, what, *spread(paired(ms[x], ms[y]))))
 
 
 if __name__ == "__main__":

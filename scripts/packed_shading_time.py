@@ -9,19 +9,16 @@ eager forward+backward steps alternated in one process and timed with CUDA event
     python scripts/packed_shading_time.py [--rounds 8] [--steps 15]
 """
 import argparse
-import os
-import statistics
-import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200.core.camera import camera_matrices  # noqa: E402
-from dss_b200.core.lighting import DirectionalLights  # noqa: E402
-from dss_b200.core.texture import apply_lighting, camera_centres  # noqa: E402
-from dss_b200.ops import SplatParams, make_shading, render_points  # noqa: E402
-from tests.util import random_cameras, sphere_cloud  # noqa: E402
+from timing import alternate, card, paired, spread
+from dss_b200.core.camera import camera_matrices
+from dss_b200.core.lighting import DirectionalLights
+from dss_b200.core.texture import apply_lighting, camera_centres
+from dss_b200.ops import SplatParams, make_shading, render_points
+from tests.util import random_cameras, sphere_cloud
 
 
 def lights(L, dev):
@@ -75,33 +72,15 @@ def main():
             out = render_points(sh_pts, sh_nrm, sh_alb, proj, view, h, prm, shading=make_shading(lt, view, shin))
         out.image.backward(grad)
 
-    def timed(v, n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(n):
-            step(*v)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / n
-
     variants = [(r, L) for L in (1, 3) for r in ("torch", "packed", "shared")]
+    ms = alternate({v: lambda v=v: step(*v) for v in variants}, a.rounds, a.steps, 3)
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
     for v in variants:
-        timed(v, 3)                                     # warm-up of every variant
-    ms = {v: [] for v in variants}
-    for _ in range(a.rounds):
-        for v in variants:
-            ms[v].append(timed(v, a.steps))
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print("gpu: %s" % (smi or "not measured"))
-    for v in variants:
-        print("step ms L=%d %-6s: median %.3f  (min %.3f max %.3f)"
-              % (v[1], v[0], statistics.median(ms[v]), min(ms[v]), max(ms[v])))
+        print("step ms L=%d %-6s: median %.3f  (min %.3f max %.3f)" % (v[1], v[0], *spread(ms[v])))
     for L in (1, 3):
         for x, y in (("torch", "packed"), ("packed", "shared")):
-            diffs = [p - q for p, q in zip(ms[(x, L)], ms[(y, L)])]
             print("L=%d paired difference ms (%s - %s): median %.3f  (min %.3f max %.3f)"
-                  % (L, x, y, statistics.median(diffs), min(diffs), max(diffs)))
+                  % (L, x, y, *spread(paired(ms[(y, L)], ms[(x, L)]))))
 
 
 if __name__ == "__main__":

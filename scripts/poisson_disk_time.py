@@ -10,18 +10,13 @@ one JSON line per case, the card name and its power limit first; --out also writ
 import argparse
 import json
 import os
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-
-from dss_b200.ops import poisson_disk_stats, sample_points_poisson_disk  # noqa: E402
-from dss_b200.utils.create_mvr_data import ico_sphere  # noqa: E402
-from mesh_raster_time import card, timed  # noqa: E402
-from point_mesh_time import torus  # noqa: E402
+from timing import card, median_ms
+from meshes import torus
+from dss_b200.ops import poisson_disk_stats, sample_points_poisson_disk
+from dss_b200.utils.create_mvr_data import ico_sphere
 
 
 def main():
@@ -33,8 +28,8 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device")
     dev = torch.device("cuda:0")
-    name, power = card()
-    lines = [{"card": name, "power_limit": power}]
+    gpu = card()
+    lines = [{"card": gpu["name"], "power_limit": gpu["power_limit"]}]
     print(json.dumps(lines[0]), flush=True)
     meshes = {"ico_sphere(6)": ico_sphere(6), "ico_sphere(8)": ico_sphere(8), "torus": torus()}
     for mesh, (v, f) in meshes.items():
@@ -45,7 +40,7 @@ def main():
 
                 def call():
                     out["s"] = sample_points_poisson_disk(v, f, N, geodesic=geodesic)
-                ms = timed(call, opt.warmup, opt.iters)
+                ms = median_ms(call, opt.warmup, opt.iters)
                 st = poisson_disk_stats()
                 rec = {"mesh": mesh, "faces": int(f.shape[0]), "geodesic": geodesic, "N": N,
                        "samples": int(out["s"].points.shape[0]), "radius": out["s"].radius, "call_ms": round(ms, 3),

@@ -9,20 +9,14 @@ case, the card name and its power limit first."""
 import argparse
 import ctypes as C
 import json
-import os
-import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-
-from dss_b200 import _lib  # noqa: E402
-from dss_b200.ops import marching_tetrahedra, poisson_reconstruction  # noqa: E402
-from dss_b200.utils.create_mvr_data import sample_points_from_mesh  # noqa: E402
-from mesh_raster_time import card, timed  # noqa: E402
-from point_mesh_time import torus  # noqa: E402
+from timing import card, median_ms
+from meshes import torus
+from dss_b200 import _lib
+from dss_b200.ops import marching_tetrahedra, poisson_reconstruction
+from dss_b200.utils.create_mvr_data import sample_points_from_mesh
 
 
 def levels(p, n, depth):
@@ -45,8 +39,8 @@ def main():
     ap.add_argument("--iters", type=int, default=3)
     opt = ap.parse_args()
     dev = torch.device("cuda:0")
-    name, power = card()
-    print(json.dumps({"card": name, "power_limit": power}), flush=True)
+    gpu = card()
+    print(json.dumps({"card": gpu["name"], "power_limit": gpu["power_limit"]}), flush=True)
     v, f = torus()
     v, f = v.to(dev), f[:, [0, 2, 1]].to(dev)     # outward winding
     g = torch.Generator(device=dev).manual_seed(0)
@@ -55,11 +49,11 @@ def main():
         p, n = pts[:P].contiguous(), nrm[:P].contiguous()
         for depth in (8, 9):
             res = {"P": P, "depth": depth}
-            res["total_ms"] = timed(lambda: poisson_reconstruction(p, n, depth=depth), opt.warmup, opt.iters)
+            res["total_ms"] = median_ms(lambda: poisson_reconstruction(p, n, depth=depth), opt.warmup, opt.iters)
             lv, chi, c, L, residual = levels(p, n, depth)
             res["levels"] = lv
             res["residual"] = residual
-            res["extract_ms"] = timed(lambda: marching_tetrahedra(chi, c, L), 1, opt.iters)
+            res["extract_ms"] = median_ms(lambda: marching_tetrahedra(chi, c, L), 1, opt.iters)
             verts, faces = marching_tetrahedra(chi, c, L)
             res["verts"], res["faces"] = int(verts.shape[0]), int(faces.shape[0])
             res["scratch_gb"] = round(_lib.scratch_bytes(dev) / 1e9, 2)

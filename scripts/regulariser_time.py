@@ -8,17 +8,14 @@ events:
     python scripts/regulariser_time.py [--rounds 7] [--steps 10]
 """
 import argparse
-import os
-import statistics
-import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200.core.cloud import PointClouds3D, PointCloudsFilters  # noqa: E402
-from dss_b200.training.losses import ProjectionLoss, RepulsionLoss  # noqa: E402
-from tests.util import sphere_cloud  # noqa: E402
+from timing import alternate, card, spread
+from dss_b200.core.cloud import PointClouds3D, PointCloudsFilters
+from dss_b200.training.losses import ProjectionLoss, RepulsionLoss
+from tests.util import sphere_cloud
 
 
 def main():
@@ -51,33 +48,15 @@ def main():
             out = loss(cloud, points_filter=filt, rebuild_knn=True)
         out.backward()
 
-    def timed(v, n):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(n):
-            step(*v)
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1) / n
-
     variants = [(r, k, P) for P in cases for k in ("projection", "repulsion") for r in ("torch", "fused")]
+    ms = alternate({v: lambda v=v: step(*v) for v in variants}, a.rounds, a.steps, 2)
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
     for v in variants:
-        timed(v, 2)                                     # warm-up of every variant
-    ms = {v: [] for v in variants}
-    for _ in range(a.rounds):
-        for v in variants:
-            ms[v].append(timed(v, a.steps))
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print("gpu: %s" % (smi or "not measured"))
-    for v in variants:
-        print("P=%-8d %-10s %-5s step ms: median %.3f  (min %.3f max %.3f)"
-              % (v[2], v[1], v[0], statistics.median(ms[v]), min(ms[v]), max(ms[v])))
+        print("P=%-8d %-10s %-5s step ms: median %.3f  (min %.3f max %.3f)" % (v[2], v[1], v[0], *spread(ms[v])))
     for P in cases:
         for k in ("projection", "repulsion"):
             r = [t / f for t, f in zip(ms[("torch", k, P)], ms[("fused", k, P)])]
-            print("P=%-8d %-10s torch / fused: median %.1fx  (min %.1f max %.1f)"
-                  % (P, k, statistics.median(r), min(r), max(r)))
+            print("P=%-8d %-10s torch / fused: median %.1fx  (min %.1f max %.1f)" % (P, k, *spread(r)))
 
 
 if __name__ == "__main__":

@@ -12,7 +12,6 @@ import argparse
 import json
 import os
 import shutil
-import sys
 import tempfile
 import time
 
@@ -20,12 +19,8 @@ import torch
 import torch.nn.functional as F
 import yaml
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-
-from dss_b200.ops import chamfer_distance  # noqa: E402
-from mesh_raster_time import card, timed  # noqa: E402
+from timing import card, median_ms
+from dss_b200.ops import chamfer_distance
 
 
 def torch_chamfer(x, y, xn, yn, budget=1 << 28):
@@ -53,9 +48,9 @@ def chamfer_times(dev, warmup, iters):
         yn = F.normalize(torch.randn(P, 3, generator=g), dim=1).to(dev)
         ours = chamfer_distance(gt[None], y[None], x_normals=gtn[None], y_normals=yn[None])
         ref = torch_chamfer(gt, y, gtn, yn)
-        out["chamfer_ms_8000x%d" % P] = timed(
+        out["chamfer_ms_8000x%d" % P] = median_ms(
             lambda: chamfer_distance(gt[None], y[None], x_normals=gtn[None], y_normals=yn[None]), warmup, iters)
-        out["torch_cdist_ms_8000x%d" % P] = timed(lambda: torch_chamfer(gt, y, gtn, yn), 1, max(3, iters // 4))
+        out["torch_cdist_ms_8000x%d" % P] = median_ms(lambda: torch_chamfer(gt, y, gtn, yn), 1, max(3, iters // 4))
         out["rel_diff_8000x%d" % P] = [float((ours[k] - ref[k]).abs() / ref[k].abs()) for k in (0, 1)]
     return out
 
@@ -126,7 +121,8 @@ def main():
         res.update(loop_times(dev, opt.loop_its, tmp))
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
-    res["card"], res["power_limit"] = card()
+    gpu = card()
+    res["card"], res["power_limit"] = gpu["name"], gpu["power_limit"]
     print(json.dumps(res))
     if opt.out:
         with open(opt.out, "w") as f:

@@ -12,14 +12,12 @@ median and range of its samples.  The collectives make every rank wait for the s
 import argparse
 import os
 import socket
-import statistics
 import subprocess
 import sys
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+from timing import card, events_ms, spread
 
 
 def worker(a):
@@ -57,16 +55,9 @@ def worker(a):
     for _ in range(a.warmup):
         step(*batch)
     torch.cuda.synchronize()
-    ms = []
-    for _ in range(a.steps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        step(*batch)
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
+    ms = [events_ms(lambda: step(*batch), 1) for _ in range(a.steps)]
     if rank == 0:
-        print("RESULT %d %.3f %.3f %.3f %d" % (G, statistics.median(ms), min(ms), max(ms), len(mine)))
+        print("RESULT %d %.3f %.3f %.3f %d" % (G, *spread(ms), len(mine)))
     if G > 1:
         dist.destroy_process_group()
 
@@ -87,9 +78,8 @@ def main():
     if not torch.cuda.is_available():
         sys.exit("train_step_sharded_time.py needs a CUDA device")
     have = torch.cuda.device_count()
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip().splitlines()
-    print("gpus: %d visible (%s)" % (have, smi[0] if smi else "model not read"))
+    gpu = card()
+    print("gpus: %d visible (%s, %s)" % (have, gpu["name"], gpu["power_limit"]))
     print("P0 = %d, %d views of 512^2, K = 5" % (a.points, a.views))
     for G in (int(x) for x in a.gpus.split(",")):
         if G > have:

@@ -13,19 +13,16 @@ with the library's kernel launches of one eager step and the kernel nodes of the
     python scripts/train_step_time.py [--samples 21] [--sizes 5000,100000,1000000]
 """
 import argparse
-import os
-import statistics
-import subprocess
 import sys
 
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from dss_b200 import _lib  # noqa: E402
-from dss_b200.core.lighting import DirectionalLights  # noqa: E402
-from dss_b200.ops import SplatParams, point_filters, render_points  # noqa: E402
-from dss_b200.training.step import GraphedTrainStep, TrainStep  # noqa: E402
-from tests.util import scene  # noqa: E402
+from timing import alternate, card, launches, spread
+from dss_b200 import _lib
+from dss_b200.core.lighting import DirectionalLights
+from dss_b200.ops import SplatParams, point_filters, render_points
+from dss_b200.training.step import GraphedTrainStep, TrainStep
+from tests.util import scene
 
 FILTER_REPS = 50
 
@@ -57,37 +54,19 @@ def main():
         img = tgt[..., :3].permute(0, 3, 1, 2).contiguous().permute(0, 2, 3, 1)
         mask = (tgt[..., 3] > 0).float()
         eager = TrainStep(pts, nrm, col, prm)
-        eager(img, mask, proj, view, lights)
-        torch.cuda.synchronize()
-        before = _lib.launch_count()
-        eager(img, mask, proj, view, lights)
-        lib_launches = _lib.launch_count() - before
+        lib_launches = launches(lambda: eager(img, mask, proj, view, lights), dev)
         with torch.no_grad():
             out = render_points(pts, nrm, col, proj, view, h, prm)
         runs[P0] = {"eager": lambda e=eager, b=(img, mask, proj, view, lights): e(*b),
                     "filter": lambda o=out, m=mask: point_filters(o, m),
                     "_args": (pts, nrm, col, prm, img, mask, proj, view, lights), "_launches": lib_launches}
 
-    def timed(fn):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        return e0.elapsed_time(e1)
-
     def measure(variants):
-        for P0, v in variants:
-            for _ in range(3):
-                timed(runs[P0][v])
-        for _ in range(a.samples):
-            for P0, v in variants:
-                ms[(P0, v)].append(timed(runs[P0][v]))
+        return alternate({(P0, v): runs[P0][v] for P0, v in variants}, a.samples, 1, 3)
 
     # the eager steps are timed before any graph exists: an eager call may reallocate the library's scratch, which a
     # graph then captures again at its next replay
-    ms = {(P0, v): [] for P0 in runs for v in ("eager", "graph", "filter")}
-    measure([(P0, "eager") for P0 in runs])
+    ms = measure([(P0, "eager") for P0 in runs])
     graphs = {}
     for P0, r in runs.items():
         graphs[P0] = GraphedTrainStep(*r.pop("_args"))
@@ -114,21 +93,18 @@ def main():
             break
     else:
         sys.exit("the library's scratch kept growing across the graph captures")
-    measure([(P0, v) for P0 in runs for v in ("graph", "filter")])
+    ms.update(measure([(P0, v) for P0 in runs for v in ("graph", "filter")]))
     assert _lib.scratch_bytes() == scratch, "the scratch moved while the graphs were timed"
     for P0, r in runs.items():
         r["_counts"] = (r.pop("_launches"), graphs[P0].kernel_nodes(), float(graphs[P0].loss["loss"]))
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
-    print("gpu: %s" % (smi or "not measured"))
+    print("gpu: %(name)s, %(power_limit)s, %(max_sm_clock)s" % card())
     for P0 in runs:
         lib_launches, nodes, loss = runs[P0]["_counts"]
         print("P0 = %d: %d library kernel launches per eager step, %d kernel nodes per graph replay, loss %.6f"
               % (P0, lib_launches, nodes, loss))
         for v in ("eager", "graph", "filter"):
             t = [x / FILTER_REPS for x in ms[(P0, v)]] if v == "filter" else ms[(P0, v)]
-            print("  %-6s ms: median %.3f  (min %.3f max %.3f, %d samples)"
-                  % (v, statistics.median(t), min(t), max(t), len(t)))
+            print("  %-6s ms: median %.3f  (min %.3f max %.3f, %d samples)" % (v, *spread(t), len(t)))
 
 
 if __name__ == "__main__":

@@ -143,7 +143,7 @@ def test_edges(cuda_device):
 
 def test_at_scale(cuda_device):
     sys.path.insert(0, os.path.join(ROOT, "scripts"))
-    from mesh_raster_time import displaced_sphere
+    from meshes import displaced_sphere
     dev = cuda_device
     v, f = (t.to(dev) for t in displaced_sphere())
     assert f.shape[0] > 600_000
