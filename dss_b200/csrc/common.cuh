@@ -91,6 +91,7 @@ enum BufId {
     BUF_PDS_POOL,     //   the Monte Carlo pool: points and normals (float4 each)
     BUF_PDS_SORTED,   //   the pool in cell order (points with their pool index, normals), cells, round state, flags
     BUF_PDS_GRID,     //   samples per cell, then their exclusive scan
+    BUF_IMAGE_METRICS,  // per-block fp64 partial sums of the image metrics, and the finish's block counter
     NUM_BUFS
 };
 
@@ -253,6 +254,25 @@ __device__ __forceinline__ double block_sum(const double (&acc)[K], double (*sPa
     if (threadIdx.x < K)
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += sPart[w][threadIdx.x];
     return v;
+}
+
+// eps_denom (DSS/utils/mathHelper.py:10-14) of a view's union, NaN kept: sign(u) max(|u|, 1e-17), +1e-17 for u = 0
+constexpr double EPS_DENOM = 1e-17;
+__device__ __forceinline__ double eps_denom_f64(double u) {
+    const double m = fabs(u) < EPS_DENOM ? EPS_DENOM : fabs(u);
+    return u < 0.0 ? -m : m;
+}
+
+// Called by every thread of each of the n_blocks blocks of a finish grid once the block has written its outputs: true
+// in the block that finished last (an integer counter that the pass before reset; no float atomics), which may then
+// read every block's outputs through L2 (__ldcg).
+__device__ __forceinline__ bool finish_last_block(unsigned int *done, int n_blocks) {
+    __shared__ int sLast;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) sLast = atomicAdd(done, 1u) == (unsigned int)n_blocks - 1;
+    __syncthreads();
+    return sLast;
 }
 
 // Pass 2 of the fixed-order fp64 sums (camera and light gradients, image loss) over partials (N, nl, blocks, SUMS).

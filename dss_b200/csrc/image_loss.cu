@@ -24,7 +24,6 @@ namespace dss {
 
 constexpr int IL_THREADS = 256;
 constexpr int IL_SUMS = 5;   // M, sum |d rgb| over mask_pred, sum |m - alpha|, I, U
-constexpr double IL_EPS = 1e-17;   // eps_denom's (DSS/utils/mathHelper.py:10-14)
 
 struct ImageLossArgs {
     const float4 *pred;          // (N, H*W) rgba
@@ -50,12 +49,6 @@ __device__ __forceinline__ float3 il_gt(const ImageLossArgs &a, int n, int64_t p
 
 // torch's sign (as abs' backward takes it): -1, 0 or 1, and 0 for NaN
 __device__ __forceinline__ float il_sign(float d) { return d > 0.0f ? 1.0f : (d < 0.0f ? -1.0f : 0.0f); }
-
-// eps_denom of a view's union, NaN kept; dE / dU is 1 where the clamp passes the gradient (|U| >= eps), else 0
-__device__ __forceinline__ double il_eps_denom(double u) {
-    const double m = fabs(u) < IL_EPS ? IL_EPS : fabs(u);
-    return u < 0.0 ? -m : m;
-}
 
 __global__ void __launch_bounds__(IL_THREADS) image_loss_partials_kernel(const __grid_constant__ ImageLossArgs a,
                                                                           double *partials, unsigned int *done) {
@@ -105,14 +98,9 @@ struct ImageLossRows {
     __device__ __forceinline__ void operator()(const double *tot, int, int m, int k) const {
         __shared__ double sPart[IL_THREADS / 32][4];
         __shared__ double sAll[4];
-        __shared__ int sLast;
         const int N = gridDim.y;
         if (k < IL_SUMS) totals[(int64_t)m * IL_SUMS + k] = tot[k];
-        __threadfence();
-        __syncthreads();
-        if (k == 0) sLast = atomicAdd(done, 1u) == (unsigned int)N - 1;
-        __syncthreads();
-        if (!sLast) return;
+        if (!finish_last_block(done, N)) return;
         // every view's totals are written: add them in view order
         double acc[4] = {0.0, 0.0, 0.0, 0.0};
         for (int v = k; v < N; v += blockDim.x) {
@@ -120,7 +108,7 @@ struct ImageLossRows {
             acc[0] += __ldcg(t);
             acc[1] += __ldcg(t + 1);
             acc[2] += __ldcg(t + 2);
-            acc[3] += 1.0 - __ldcg(t + 3) / il_eps_denom(__ldcg(t + 4));
+            acc[3] += 1.0 - __ldcg(t + 3) / eps_denom_f64(__ldcg(t + 4));
         }
         const double s = block_sum(acc, sPart);
         if (k < 4) sAll[k] = s;
@@ -166,10 +154,10 @@ __global__ void __launch_bounds__(IL_THREADS) image_loss_backward_kernel(const _
     if (a.use_sil) {
         const double ws = b.lambda_sil * (gl + (double)*b.g_sil), w_iou = 0.01 * ws / Nv;
         const double I = b.totals[(int64_t)n * IL_SUMS + 3], U = b.totals[(int64_t)n * IL_SUMS + 4];
-        const double E = il_eps_denom(U);
+        const double E = eps_denom_f64(U);   // dE / dU is 1 where the clamp passes the gradient (|U| >= eps), else 0
         w_l1 = ws / npix;
         A = w_iou / E;
-        B = fabs(U) >= IL_EPS ? w_iou * I / (E * E) : 0.0;
+        B = fabs(U) >= EPS_DENOM ? w_iou * I / (E * E) : 0.0;
     }
     for (int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; p < a.HW; p += (int64_t)gridDim.x * blockDim.x) {
         const int64_t i = n * a.HW + p;

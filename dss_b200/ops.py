@@ -22,7 +22,8 @@ from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
            "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh", "chamfer_distance",
-           "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra"]
+           "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
+           "ImageMetrics", "image_metrics", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
 
 
 class SplatParams(NamedTuple):
@@ -787,3 +788,130 @@ def poisson_disk_stats(device=None):
     k = probes.value
     return {"probes": k, "radii": list(radii[:k]), "counts": list(counts[:k]), "rounds": list(rounds[:k]),
             "stage_ms": list(ms)}
+
+
+class ImageMetrics(NamedTuple):
+    iou: torch.Tensor                 # () float64: mean over the views of 1 - I / eps_denom(U)
+    psnr: torch.Tensor                # () float64: mean over the views of the summed-channel squared error per pixel
+    per_view: torch.Tensor            # (V,5) float64 rows (I, U, E, iou, psnr)
+
+
+def image_metrics(pred_rgba, gt_rgb, gt_mask) -> ImageMetrics:
+    """The reference's image-space validation metrics (``Trainer.eval_step``, DSS/training/trainer.py:173-212) of
+    renders against their ground truth (csrc/image_metrics.cu; the rules are in include/dss_b200.h).
+
+    ``pred_rgba`` (V,s,s,4) float32: the renders, used as they are (no clamping).  ``gt_rgb`` (V,H,W,3) float32, any
+    strides (``img.permute(0, 2, 3, 1)`` of an (V,3,H,W) batch reads in place), and ``gt_mask`` (V,H,W) or (V,1,H,W)
+    float32, uint8 or bool, its value used: the ground truth at the data's resolution, resized to s x s inside the
+    kernel as ``F.interpolate(mode='bilinear', align_corners=False)`` does it (s == H reads it unchanged).  Per view
+    ``iou`` = ``IouLoss`` = 1 - I / eps_denom(U) with I = sum m alpha, U = sum (m + alpha - m alpha) (an empty view
+    scores 1), and ``psnr`` = ``L2Loss(channel_dim=1)`` = the mean over the pixels of the squared RGB error summed over
+    the channels (an error, not a ratio in dB, despite the reference's name); both means are over the views, as
+    ``BaseTrainer.evaluate`` takes them.  Device tensors; two launches, no host synchronisation, the same bits on every
+    call.  No gradients."""
+    dev = _lib.require_cuda(pred_rgba, gt_rgb, gt_mask)
+    pred = _lib.as_f32(pred_rgba.detach(), "pred_rgba")
+    if pred.dim() != 4 or pred.shape[3] != 4 or pred.shape[1] != pred.shape[2] or pred.shape[0] < 1:
+        raise RuntimeError("pred_rgba must have shape (V, s, s, 4), V >= 1, got %s" % (tuple(pred.shape),))
+    V, s = pred.shape[0], pred.shape[1]
+    if gt_rgb.dtype != torch.float32:
+        raise TypeError("gt_rgb must be float32, got %s" % gt_rgb.dtype)
+    if gt_rgb.dim() != 4 or gt_rgb.shape[0] != V or gt_rgb.shape[3] != 3:
+        raise RuntimeError("gt_rgb must have shape (%d, H, W, 3), got %s" % (V, tuple(gt_rgb.shape)))
+    H, W = gt_rgb.shape[1], gt_rgb.shape[2]
+    mask = gt_mask.detach()
+    if mask.dim() == 4 and mask.shape[1] == 1:
+        mask = mask[:, 0]
+    if tuple(mask.shape) != (V, H, W):
+        raise RuntimeError("gt_mask must have shape (%d, %d, %d) or (%d, 1, %d, %d), got %s"
+                           % (V, H, W, V, H, W, tuple(gt_mask.shape)))
+    if mask.dtype not in (torch.float32, torch.uint8, torch.bool):
+        raise TypeError("gt_mask must be float32, uint8 or bool, got %s" % mask.dtype)
+    mask = mask.contiguous()
+    if pred.data_ptr() % 16:
+        pred = pred.clone()
+    per_view = torch.empty((V, 5), dtype=torch.float64, device=dev)
+    means = torch.empty((2,), dtype=torch.float64, device=dev)
+    gt = gt_rgb.detach()
+    _lib.call("dss_image_metrics", dev, pred, s, gt, (C.c_int64 * 4)(*gt.stride()), mask,
+              int(mask.dtype != torch.float32), V, H, W, per_view, means)
+    return ImageMetrics(means[0], means[1], per_view)
+
+
+def shared_cloud_splats(points, n_views, Vrk_invariant=True, Vrk_isotropic=True, frnn_radius=0.2):
+    """``(h, frames)`` for :func:`render_points` of ``n_views`` views of ONE shared cloud, as the training step sizes its
+    splats: the spacing rule of ``SurfaceSplatting._compute_h`` (one h per view with ``Vrk_invariant``, one per point
+    with ``Vrk_isotropic``) or, with both off, the cloud's anisotropic :func:`local_frames`.  Computed without grad."""
+    from .core.rasterizer import point_sq_spacing, splat_variance_scale
+    with torch.no_grad():
+        if Vrk_invariant or Vrk_isotropic:
+            h = splat_variance_scale([point_sq_spacing(points, frnn_radius)], Vrk_invariant).repeat(n_views)
+            return h, None
+        return None, local_frames(points)
+
+
+def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius, shininess):
+    """render(params, views) -> the renders of :func:`render_data_views`, with what does not depend on the views (the
+    cloud's splat sizes, all the views' cameras and lights on the device) computed once"""
+    from .core.camera import camera_matrices
+    from .core.lighting import pack_lights
+    from .core.texture import camera_centres
+    dev = _lib.require_cuda(points, normals, colours)
+    lp = data.light_props(dev)
+    if lp is None:
+        raise ValueError("the data has no lights_%d entries: the views are shaded with the data's lights")
+    light_cls, props = lp
+    # the training loop's matrices and light rows, bit for bit: all the views' projections, then the batch's
+    proj_all = camera_matrices(data.get_cameras())[0].to(dev)
+    view_all = torch.from_numpy(data.camera_mat[:len(data)]).to(dev)
+    p, c = points.detach(), colours.detach()
+    n = torch.nn.functional.normalize(normals.detach(), dim=-1)
+    h1, frames = shared_cloud_splats(p, 1, Vrk_invariant, Vrk_isotropic, frnn_radius)
+
+    def render(params, views):
+        idx = torch.as_tensor(list(views), dtype=torch.int64, device=dev)
+        lights = light_cls(**{k: v.index_select(0, idx) for k, v in props.items()}, device=dev)
+        rows, ambient, kind = pack_lights(lights)
+        view = view_all.index_select(0, idx)
+        with torch.no_grad():
+            shading = Shading(rows, ambient, camera_centres(view).contiguous(), kind, float(shininess))
+            return render_points(p, n, c, proj_all.index_select(0, idx), view,
+                                 None if h1 is None else h1.repeat(idx.shape[0]), params, shading=shading,
+                                 deterministic=True, frames=frames).image
+    return render
+
+
+def render_data_views(points, normals, colours, data, params: SplatParams, views, Vrk_invariant=True,
+                      Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0):
+    """(len(views), S, S, 4) renders, S = ``params.image_size``, of one shared cloud from the cameras of ``data``'s
+    views ``views`` (an ``MVRData``: its ``get_cameras()`` projections and ``camera_mat`` view matrices) with fused
+    shading by each view's own lights (``data.light_props``), as the training step renders a batch: unit normals, the
+    splats of :func:`shared_cloud_splats`, ``colours`` the albedo.  Forward only."""
+    return _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius,
+                               shininess)(params, views)
+
+
+def evaluate_2d(points, normals, colours, data, params: SplatParams, image_size, batch=1, Vrk_invariant=True,
+                Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0):
+    """The reference's ``Trainer.evaluate_2d`` for a point cloud: every view of ``data`` (an ``MVRData`` with images
+    and masks) rendered at ``image_size`` x ``image_size`` with the splat renderer, ``batch`` views at a time
+    (:func:`render_data_views` with ``params`` at that size), scored by :func:`image_metrics` against the view's
+    ground truth.  Returns ``{"iou", "psnr"}`` (float64 device scalars, the means over all the views) and
+    ``"per_view"`` (V,5) float64 rows (I, U, E, iou, psnr).  Renders and ground truth of one batch at a time are on the
+    device; uses no random numbers and none of a training step's buffers."""
+    if data.images is None or data.masks is None:
+        raise ValueError("evaluate_2d needs the data's images and masks")
+    dev = _lib.require_cuda(points, normals, colours)
+    prm = params._replace(image_size=int(image_size))
+    V, B = len(data), max(1, int(batch))
+    render = _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius, shininess)
+    rows = []
+    for i in range(0, V, B):
+        views = list(range(i, min(i + B, V)))
+        image = render(prm, views)
+        rgb = torch.stack([torch.as_tensor(data.images[v]) for v in views]).to(dev).permute(0, 2, 3, 1)
+        mask = torch.stack([torch.as_tensor(data.masks[v]) for v in views]).to(dev)
+        rows.append(image_metrics(image, rgb, mask).per_view)
+    per_view = torch.cat(rows)
+    means = per_view[:, 3:].mean(0)
+    return {"iou": means[0], "psnr": means[1], "per_view": per_view}

@@ -10,7 +10,7 @@ import warnings
 import yaml
 
 __all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "step_settings", "splat_params",
-           "EVAL_SAMPLINGS"]
+           "EVAL_SAMPLINGS", "SELECTION_METRICS", "IMAGE_METRICS", "selection_metric"]
 
 EVAL_SAMPLINGS = ("uniform", "poisson_disk")
 
@@ -131,12 +131,14 @@ def check_config(cfg, resolution, has_lights):
         raise ValueError("the data directory has no lights_%d entries: the loop shades with the data's lights")
 
 
-SELECTION_METRICS = ("chamfer_point", "chamfer_normal", "p2f_avg")
+IMAGE_METRICS = ("iou", "psnr")
+SELECTION_METRICS = ("chamfer_point", "chamfer_normal", "p2f_avg") + IMAGE_METRICS
 
 
 def selection_metric(cfg):
     """``training.model_selection_metric`` if the loop can select by it: the chamfer distances of the reference's
-    trainer, or ``p2f_avg``, the mean distance of the cloud's points to ``<data_dir>/mesh.obj``."""
+    trainer, ``p2f_avg``, the mean distance of the cloud's points to ``<data_dir>/mesh.obj``, or the image-space
+    ``iou`` / ``psnr`` of its ``evaluate_2d`` (:data:`IMAGE_METRICS`, both errors: minimize them)."""
     metric = cfg["training"]["model_selection_metric"]
     if metric not in SELECTION_METRICS:
         raise NotImplementedError("model_selection_metric %r: the loop selects by one of %s"

@@ -32,11 +32,10 @@ import torch.nn.functional as F
 from .. import _lib
 from ..core.cloud import PointClouds3D, PointCloudsFilters
 from ..core.lighting import pack_lights
-from ..core.rasterizer import point_sq_spacing, splat_variance_scale
 from ..core.texture import camera_centres
 from ..graph import GraphedStep
-from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, local_frames, point_filters, point_filters_no_views,
-                   render_points)
+from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, point_filters, point_filters_no_views, render_points,
+                   shared_cloud_splats)
 from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
 
 __all__ = ["TrainStep", "GraphedTrainStep"]
@@ -137,15 +136,7 @@ class TrainStep:
             visibility, inmask = point_filters_no_views(self.points.shape[0], dev, self._group)
             rendered = _NoViews.apply(self.points, normals, self.colours, self._sync)
         else:
-            h = frames = None
-            with torch.no_grad():
-                if self.Vrk_invariant or self.Vrk_isotropic:
-                    # the one cloud's spacing, the rule of SurfaceSplatting._compute_h for its N views
-                    h = splat_variance_scale([point_sq_spacing(self.points, self.frnn_radius)],
-                                             self.Vrk_invariant).repeat(N)
-                else:
-                    # anisotropic: the one cloud's local frames, shared by its N views
-                    frames = local_frames(self.points)
+            h, frames = shared_cloud_splats(self.points, N, self.Vrk_invariant, self.Vrk_isotropic, self.frnn_radius)
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
             out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading,
                                 deterministic=True,

@@ -20,7 +20,10 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   it as the reference does, see :func:`ground_truth_cloud`), and on improvement of
   ``training.model_selection_metric`` ``model_best.pt`` and ``val/best.ply``.  With the metric ``p2f_avg`` the loop
   reads ``<data_dir>/mesh.obj`` once (it must exist) and every validation adds ``p2f_avg`` / ``p2f_std``, the mean and
-  population standard deviation of the exact distances of the cloud's points to that mesh; ``model.pt`` every ``checkpoint_every``, ``model_%d.pt`` every ``backup_every``.
+  population standard deviation of the exact distances of the cloud's points to that mesh.  With ``iou`` or ``psnr``
+  the validation is the reference's ``evaluate_2d`` instead (see :meth:`Trainer.evaluate`): it needs only the images,
+  masks, cameras and lights, so data without a ground-truth cloud (``points`` / ``normals``) or mesh trains;
+  ``model.pt`` every ``checkpoint_every``, ``model_%d.pt`` every ``backup_every``.
 - ``training.resume_from`` (in ``<out>``) is loaded when it exists, and the run continues where it stopped, mid-epoch
   included: a resumed run computes what an uninterrupted one does.  (The reference starts a new epoch.)
 - ``--exit-after S`` saves ``model.pt`` and exits with status 3 once S seconds have passed (checked after every
@@ -39,17 +42,17 @@ import yaml
 
 from ..core.camera import camera_matrices
 from ..core.cloud import PointClouds3D
-from ..core.lighting import DirectionalLights, PointLights
-from ..ops import chamfer_distance
+from ..ops import chamfer_distance, evaluate_2d
 from ..utils.create_mvr_data import ico_sphere, sample_points_from_mesh
 from ..utils.dataset import MVRData
 from ..utils.evaluate import p2f_stats
 from ..utils.io import read_mesh, save_ply
-from .config import EVAL_SAMPLINGS, check_config, load_config, selection_metric, splat_params, step_settings
+from .config import (EVAL_SAMPLINGS, IMAGE_METRICS, check_config, load_config, selection_metric, splat_params,
+                     step_settings)
 from .step import GraphedTrainStep
 
 __all__ = ["radii_backward_scaler", "compound_lambda_proj", "initial_cloud", "make_optimizer", "make_lr_scheduler",
-           "ground_truth_cloud", "Trainer", "main"]
+           "ground_truth_cloud", "load_data", "Trainer", "main"]
 
 EXIT_TIME_LIMIT = 3        # train_mvr.py:221-227
 EVAL_SEED = 0              # the fixed draw of the ground-truth samples
@@ -120,6 +123,16 @@ def ground_truth_cloud(data, data_dir, n_eval_points, device, sampling="uniform"
                                    n, generator=g)
 
 
+def load_data(cfg):
+    """the configuration's ``MVRData`` (its ``data`` block), which must have images and masks"""
+    dc = cfg["data"]
+    data = MVRData(dc["data_dir"], data_dict=dc["data_dict"], n_imgs=dc["n_imgs"], img_folder=dc["img_folder"],
+                   mask_folder=dc["mask_folder"], img_extension=dc["img_extension"], mask_extension=dc["mask_extension"])
+    if data.images is None or data.masks is None:
+        raise ValueError("%s has no images and masks" % dc["data_dir"])
+    return data
+
+
 class _Log:
     """lines to ``<out>/<logfile>`` (and stdout), JSON records to ``<out>/metrics.jsonl``"""
 
@@ -155,27 +168,19 @@ class Trainer:
         os.makedirs(self.val_dir, exist_ok=True)
         self.log = _Log(self.out_dir, tr["logfile"])
         # ---- data: images in host memory, cameras and lights of every view on the device
-        self.data = MVRData(dc["data_dir"], data_dict=dc["data_dict"], n_imgs=dc["n_imgs"], img_folder=dc["img_folder"],
-                            mask_folder=dc["mask_folder"], img_extension=dc["img_extension"],
-                            mask_extension=dc["mask_extension"])
-        if self.data.images is None or self.data.masks is None:
-            raise ValueError("%s has no images and masks" % dc["data_dir"])
+        self.data = load_data(cfg)
         V = len(self.data)
-        lights = [self.data[i].get("lights") for i in range(V)]
-        check_config(cfg, self.data.resolution, all(l is not None for l in lights))
+        lights = self.data.light_props(self.dev)
+        check_config(cfg, self.data.resolution, lights is not None)
+        self.metric = selection_metric(cfg)
         self.mesh = None
-        if selection_metric(cfg) == "p2f_avg":
+        if self.metric == "p2f_avg":
             mesh_path = os.path.join(dc["data_dir"], "mesh.obj")
             if not os.path.isfile(mesh_path):
                 raise ValueError("model_selection_metric p2f_avg measures against %s, which does not exist" % mesh_path)
             verts, faces = read_mesh(mesh_path)
             self.mesh = (torch.from_numpy(verts).float().to(self.dev), torch.from_numpy(faces).to(self.dev))
-        kind = str(self.data.data_dict["lights_type"]) if "lights_type" in self.data.data_dict else ""
-        self.light_cls = PointLights if "PointLights" in kind else DirectionalLights
-        vec = "location" if self.light_cls is PointLights else "direction"
-        self.light_props = {k: torch.stack([torch.as_tensor(l[src]) for l in lights]).to(self.dev)
-                            for k, src in (("ambient_color", "ambient_color"), ("diffuse_color", "diffuse_color"),
-                                           ("specular_color", "specular_color"), (vec, vec))}
+        self.light_cls, self.light_props = lights
         cams = self.data.get_cameras()
         proj, _ = camera_matrices(cams)
         self.proj_all = proj.to(self.dev)
@@ -185,8 +190,15 @@ class Trainer:
         if V // self.batch_size < 1:
             raise ValueError("batch_size %d is larger than the %d views: an epoch would have no batch"
                              % (self.batch_size, V))
-        self.gt = ground_truth_cloud(self.data, dc["data_dir"], tr["n_eval_points"], self.dev,
-                                     tr.get("eval_sampling", "uniform"))
+        self.gt = None
+        if self.metric not in IMAGE_METRICS:
+            missing = [k for k in ("points", "normals") if k not in self.data.data_dict]
+            if missing:
+                raise ValueError("model_selection_metric %s measures against the data's cloud, but %s has no %s; "
+                                 "select by iou or psnr to train without one"
+                                 % (self.metric, os.path.join(dc["data_dir"], dc["data_dict"]), " / ".join(missing)))
+            self.gt = ground_truth_cloud(self.data, dc["data_dir"], tr["n_eval_points"], self.dev,
+                                         tr.get("eval_sampling", "uniform"))
         # ---- state: fresh, then whatever the checkpoint holds
         self.gen = torch.Generator().manual_seed(int(tr["seed"]))
         self.epoch_it, self.it, self.order, self.pos = -1, -1, None, 0
@@ -257,7 +269,16 @@ class Trainer:
 
     def evaluate(self):
         """trainer.py:144-171: chamfer distances of the ground truth (x) against the current cloud (y); selecting by
-        p2f_avg, also the mean and population standard deviation of the points' distances to the data's mesh"""
+        p2f_avg, also the mean and population standard deviation of the points' distances to the data's mesh.
+        Selecting by iou or psnr, instead the image-space metrics of ``Trainer.evaluate_2d`` (trainer.py:173-212,
+        581-586): every view rendered at resolution // 4 (train_mvr.py:135) with the step's shading and splat flags,
+        ``batch_size`` views at a time, scored by :func:`~dss_b200.ops.evaluate_2d`."""
+        if self.metric in IMAGE_METRICS:
+            st = self.step
+            ev = evaluate_2d(st.points, st.normals, st.colours, self.data, self.params,
+                             max(1, self.data.resolution[0] // 4), self.batch_size, st.Vrk_invariant, st.Vrk_isotropic,
+                             st.frnn_radius, st.shininess)
+            return {"iou": float(ev["iou"]), "psnr": float(ev["psnr"])}
         points, normals = self.cloud()
         with torch.no_grad():
             cd_p, cd_n = chamfer_distance(PointClouds3D([self.gt[0]], [self.gt[1]]), PointClouds3D([points], [normals]))
@@ -285,7 +306,7 @@ class Trainer:
         tr = self.cfg["training"]
         print_every, checkpoint_every = int(tr["print_every"]), int(tr["checkpoint_every"])
         backup_every, validate_every = int(tr["backup_every"]), int(tr["validate_every"])
-        metric = tr["model_selection_metric"]
+        metric = self.metric
         V, bs = len(self.data), self.batch_size
         t0 = t0b = time.time()
         try:

@@ -117,6 +117,21 @@ class MVRData:
                                  if isinstance(v, (list, np.ndarray))}
         return out
 
+    def light_props(self, device="cpu"):
+        """``(light class, {property: (V, ...) tensor on device})`` of the views' own ``lights_%d`` entries: the class
+        is ``PointLights`` when ``lights_type`` names it, else ``DirectionalLights``, and
+        ``cls(**{k: v[idx] for k, v in props.items()})`` gives the lights of views ``idx``.  None when a view has no
+        lights."""
+        from ..core.lighting import DirectionalLights, PointLights
+        lights = [self[i].get("lights") for i in range(len(self))]
+        if any(l is None for l in lights):
+            return None
+        kind = str(self.data_dict["lights_type"]) if "lights_type" in self.data_dict else ""
+        cls = PointLights if "PointLights" in kind else DirectionalLights
+        vec = "location" if cls is PointLights else "direction"
+        return cls, {k: torch.stack([torch.as_tensor(l[k]) for l in lights]).to(device)
+                     for k in ("ambient_color", "diffuse_color", "specular_color", vec)}
+
     def get_pointclouds(self, num_points=None) -> PointClouds3D:
         """points, normals and colours in object coordinates (dataset.py:103-135).  With ``num_points`` None or the
         stored cloud's size, the stored cloud; otherwise ``num_points`` geodesic Poisson-disk samples of

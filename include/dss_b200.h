@@ -283,6 +283,23 @@ DSS_API int dss_image_loss_partial(dss_ctx *ctx, const float *pred, const float 
 DSS_API int dss_image_loss_finish(dss_ctx *ctx, const double *total_row, int H, int W, double lambda_rgb,
                                   double lambda_sil, float *loss, float *loss_rgb, float *loss_sil, void *stream);
 
+/* ---- image-space validation metrics -----------------------------------------------------------------------------
+ * Trainer.eval_step (DSS/training/trainer.py:173-212) on V renders of s x s pixels: the ground truth of H x W pixels is
+ * resized to s x s as torch's F.interpolate(mode='bilinear', align_corners=False) without antialias does it, in float32
+ * (src = max((dst + 0.5) H / s - 0.5, 0), i0 = (int)src, i1 = min(i0 + 1, H - 1), weights src - i0 and 1 - (src - i0),
+ * the same for x; s == H returns the input values unchanged), giving g^ and m^; then per view n, in fp64,
+ *   I_n = sum m^ alpha, U_n = sum (m^ + alpha - m^ alpha), E_n = sum_pixels sum_c (g^_c - p_c)^2,
+ *   iou_n = 1 - I_n / eps_denom(U_n) (IouLoss; an empty union gives 1), psnr_n = E_n / s^2 (L2Loss(channel_dim=1)),
+ * on the raw render (no clamping).  pred (V,s,s,4) f32 contiguous, 16-byte aligned; gt rgb f32 at
+ * gt[n*s0 + y*s1 + x*s2 + c*s3] with gt_strides = {s0, s1, s2, s3} (host array, in elements); mask (V,H,W) contiguous,
+ * f32 (mask_kind 0) or bytes (mask_kind 1: bool / uint8), its value used.  s*s, H*W <= 2^31-1, V <= 65535.
+ * Outputs (device, f64): per_view (V, 5) rows (I_n, U_n, E_n, iou_n, psnr_n) and means (2,) (mean_n iou_n,
+ * mean_n psnr_n).  2 launches; deterministic: fixed-order fp64 sums, no float atomics; no host synchronisation;
+ * partial sums in context scratch. */
+DSS_API int dss_image_metrics(dss_ctx *ctx, const float *pred, int s, const float *gt, const int64_t *gt_strides,
+                              const void *mask, int mask_kind, int V, int H, int W, double *per_view, double *means,
+                              void *stream);
+
 /* ---- point filters of the training step -------------------------------------------------------------------------
  * Model.forward's visibility and inmask filters (DSS/models/point_modeling.py:172-173, 188-212) of one SHARED cloud of
  * P0 points seen by N cameras (shared_cloud must be 1: packed clouds return DSS_E_INVALID), from the forward's records
