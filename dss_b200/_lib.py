@@ -87,6 +87,7 @@ _SIGNATURES = {
     "dss_knn_points": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_float,
                                  vp, vp, vp]),
     "dss_local_frames": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int64, vp, vp, vp]),
+    "dss_estimate_normals": (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int64, vp, C.c_int, C.c_int, vp, vp, vp, vp]),
     "dss_surface_regulariser": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int64, vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp, C.c_float, C.c_float, vp, vp, vp]),
     "dss_image_loss_forward": (C.c_int, [vp, vp, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,

@@ -149,6 +149,27 @@ class PointClouds3D:
         """Same geometry, new per-point features (what LightingTexture produces: texture.py:118-127)."""
         return PointClouds3D(self._points, self._normals, features)
 
+    def estimate_normals(self, neighborhood_size: int = 20, disambiguate_directions: bool = True,
+                         assign_to_self: bool = False):
+        """The clouds' normals by :func:`dss_b200.ops.estimate_normals` (DSS/core/cloud.py:210-258), as a padded
+        (N, P, 3) tensor; with ``assign_to_self`` they also replace the clouds' normals.
+
+        Two departures from the reference: ``neighborhood_size`` defaults to 20 (meshlab's K; the reference's 50 is above
+        the device K-NN's limit of 32), and ``disambiguate_directions=True`` orients the normals along a minimum spanning
+        forest from each component's topmost point, so that their signs agree across the surface (outwards on a closed
+        one), where the reference's per-point vote (Tombari et al.) only agrees locally.  ``False`` gives the canonical
+        sign (the largest component positive).  The clouds must be on a CUDA device."""
+        from ..ops import estimate_normals
+        pts = self.points_packed()
+        est = estimate_normals(pts, neighborhood_size, disambiguate_directions, self.cloud_to_packed_first_idx(),
+                               self.num_points_per_cloud())
+        normals = list(est.normals.split([p.shape[0] for p in self._points]))
+        if assign_to_self:
+            self._normals = normals
+            for key in ("np", "npad"):
+                self._cache.pop(key, None)
+        return PointClouds3D(self._points, normals).normals_padded()
+
 
 class PointCloudsFilters:
     """Named per-point boolean masks, padded (N, P_max) (DSS/core/cloud.py:285-360): ``activation`` selects

@@ -92,6 +92,7 @@ enum BufId {
     BUF_PDS_SORTED,   //   the pool in cell order (points with their pool index, normals), cells, round state, flags
     BUF_PDS_GRID,     //   samples per cell, then their exclusive scan
     BUF_IMAGE_METRICS,  // per-block fp64 partial sums of the image metrics, and the finish's block counter
+    BUF_NORMALS,      // normal estimation: unoriented normals, the spanning forest's state, the Euler tours and flags
     NUM_BUFS
 };
 

@@ -6,7 +6,7 @@
 // eigenvalues of the population covariance C = D^T D / 8 and V's columns its eigenvectors.  It keeps the two largest
 // pairs: Vr = F diag(lambda) F^T, Sk = F^T with F = [f1 f2].  Here that is one thread per row: gather the neighbours
 // (the rows dss_knn_points wrote for K = 8, r = -1), form C in float64, diagonalise it by a fixed number of cyclic
-// Jacobi sweeps in float64 and round once to float32 at the output.  Every row takes the same instruction path up to
+// Jacobi sweeps in float64 (sym3_eigen.cuh, shared with normals.cu) and round once to float32 at the output.  Every row takes the same instruction path up to
 // the rotation guards, so the result does not depend on how fast a solver converges, and the launch needs no scratch,
 // no atomics and no host synchronisation (capturable in a CUDA graph).
 //
@@ -18,12 +18,11 @@
 #include <math_constants.h>
 
 #include "common.cuh"
+#include "sym3_eigen.cuh"
 
 namespace dss {
 
 constexpr int LF_K = 8;            // neighbourhood size (rasterizer.py:272-273)
-constexpr int LF_SWEEPS = 6;       // cyclic Jacobi sweeps: 3x3 converges quadratically, 4 reach float64 on any input
-constexpr double LF_DEGENERATE = 0x1p-40;
 
 struct LocalFrameArgs {
     const float *points;       // (P,3)
@@ -33,36 +32,6 @@ struct LocalFrameArgs {
     float *frames;             // (P,8) {f1.xyz, l1, f2.xyz, l2}
     int64_t P;
 };
-
-// one Jacobi rotation of the symmetric A (upper triangle used) in the (p, q) plane; V accumulates the eigenvectors
-// (columns)
-template <int p, int q>
-__device__ __forceinline__ void jacobi_rotate(double (&A)[3][3], double (&V)[3][3]) {
-    const double apq = A[p][q];
-    if (apq == 0.0) return;
-    constexpr int r = 3 - p - q;
-    const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
-    // t = sgn(theta) / (|theta| + sqrt(theta^2 + 1)), the smaller root; theta^2 overflowing gives t = 0 (no rotation)
-    const double t = copysign(1.0, theta) / (fabs(theta) + sqrt(fma(theta, theta, 1.0)));
-    const double c = rsqrt(fma(t, t, 1.0)), s = t * c;
-    const double arp = A[r < p ? r : p][r < p ? p : r], arq = A[r < q ? r : q][r < q ? q : r];
-    A[p][p] -= t * apq;
-    A[q][q] += t * apq;
-    A[p][q] = 0.0;
-    A[r < p ? r : p][r < p ? p : r] = c * arp - s * arq;
-    A[r < q ? r : q][r < q ? q : r] = s * arp + c * arq;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const double vp = V[k][p], vq = V[k][q];
-        V[k][p] = c * vp - s * vq;
-        V[k][q] = s * vp + c * vq;
-    }
-}
-
-__device__ __forceinline__ void normalize3d(double &x, double &y, double &z) {
-    const double il = rsqrt(x * x + y * y + z * z);
-    x *= il, y *= il, z *= il;
-}
 
 __global__ void __launch_bounds__(256) local_frames_kernel(const __grid_constant__ LocalFrameArgs a) {
     const ViewRange cr = view_range(a.first_idx, a.num_points, blockIdx.y, a.P);
@@ -108,44 +77,9 @@ __global__ void __launch_bounds__(256) local_frames_kernel(const __grid_constant
         for (int r = 0; r < 3; ++r)
 #pragma unroll
             for (int c = r; c < 3; ++c) A[r][c] *= 1.0 / LF_K;
-        double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
-#pragma unroll 1
-        for (int sweep = 0; sweep < LF_SWEEPS; ++sweep) {
-            jacobi_rotate<0, 1>(A, V);
-            jacobi_rotate<0, 2>(A, V);
-            jacobi_rotate<1, 2>(A, V);
-        }
-        // ascending order of the eigenvalues (a fixed three-comparator network; ties keep the column order)
-        double l0 = A[0][0], l1 = A[1][1], l2 = A[2][2];
-        double f0[3] = {V[0][0], V[1][0], V[2][0]}, f1[3] = {V[0][1], V[1][1], V[2][1]}, f2[3] = {V[0][2], V[1][2], V[2][2]};
-        auto cswap = [](double &la, double (&fa)[3], double &lb, double (&fb)[3]) {
-            if (lb < la) {
-                const double t = la;
-                la = lb, lb = t;
-#pragma unroll
-                for (int e = 0; e < 3; ++e) {
-                    const double x = fa[e];
-                    fa[e] = fb[e], fb[e] = x;
-                }
-            }
-        };
-        cswap(l0, f0, l1, f1);
-        cswap(l1, f1, l2, f2);
-        cswap(l0, f0, l1, f1);
-        if (l2 - l0 <= LF_DEGENERATE * fabs(l2)) {
-            // isotropic (all lambda equal, e.g. 0 for duplicates): any frame; take the axes
-            f2[0] = 1.0, f2[1] = 0.0, f2[2] = 0.0;
-        }
-        if (l1 - l0 <= LF_DEGENERATE * fabs(l2)) {
-            // the two smallest agree: f1 = normalize(f2 x e_k), e_k the axis of the smallest |f2_k|
-            const double ax = fabs(f2[0]), ay = fabs(f2[1]), az = fabs(f2[2]);
-            const int k = (ax <= ay && ax <= az) ? 0 : (ay <= az ? 1 : 2);
-            // f2 x e_k
-            f1[0] = k == 0 ? 0.0 : (k == 1 ? -f2[2] : f2[1]);
-            f1[1] = k == 0 ? f2[2] : (k == 1 ? 0.0 : -f2[0]);
-            f1[2] = k == 0 ? -f2[1] : (k == 1 ? f2[0] : 0.0);
-            normalize3d(f1[0], f1[1], f1[2]);
-        }
+        double l0, l1, l2, f0[3], f1[3], f2[3];
+        sym3_eigen(A, l0, l1, l2, f0, f1, f2);
+        sym3_fix_degenerate(l0, l1, l2, f1, f2);
         out[0] = make_float4((float)f1[0], (float)f1[1], (float)f1[2], (float)l1);
         out[1] = make_float4((float)f2[0], (float)f2[1], (float)f2[2], (float)l2);
     }

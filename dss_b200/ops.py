@@ -21,7 +21,8 @@ import torch
 from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
-           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "MeshRender", "render_mesh", "chamfer_distance",
+           "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "PointNormals",
+           "estimate_normals", "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
            "ImageMetrics", "image_metrics", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
 
@@ -499,6 +500,54 @@ def local_frames(points, first_idx=None, num_points=None):
     _lib.call("dss_local_frames", dev, pts, None if single else fi, None if single else npts, int(npts.shape[0]), P,
               idx, frames)
     return frames
+
+
+class PointNormals(NamedTuple):
+    normals: torch.Tensor             # (P,3) float32, unit; NaN on an invalid row
+    root: torch.Tensor                # (P,) int32 local index of the row's component root, -1 when not oriented
+    parent: torch.Tensor              # (P,) int32 local index of the row's tree parent, -1 at a root / when not oriented
+
+
+def estimate_normals(points, k=20, orient=True, first_idx=None, num_points=None) -> PointNormals:
+    """Normals of clouds that carry none (csrc/normals.cu; the rules are in include/dss_b200.h and DESIGN.md): PCA over
+    each point's ``k`` nearest neighbours of its cloud (itself included), solved in float64, and with ``orient`` the
+    signs propagated along the minimum spanning forest of the k-NN graph under the weight 1 - |n_i . n_j| from the
+    point of largest z of each component, whose normal is made to point up (Hoppe et al. 1992, meshlab's "Compute
+    normals for point sets").  On a closed surface the normals then point outwards.  Without ``orient`` each normal's
+    component of largest magnitude is positive.  Orientation is consistent within a connected component only:
+    ``root`` tells the components apart.
+
+    ``points`` (P,3) float32 CUDA tensor, one cloud, or packed with ``first_idx`` / ``num_points`` (N,) int64 as for
+    ``knn_points_packed``; each cloud is handled on its own, and packed rows outside every cloud are not written.
+    ``k`` in [3, 32] (meshlab's default 20).  A row with a non-finite point or fewer than ``k`` finite neighbours gets a
+    NaN normal and root = parent = -1.  Two library calls (the K-NN and the estimate), no host synchronisation, the same
+    bits on every call.  No gradients."""
+    from .frnn_grid import knn_points_packed
+    dev = _lib.require_cuda(points, first_idx, num_points)
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3)")
+    if (first_idx is None) != (num_points is None):
+        raise RuntimeError("pass both first_idx and num_points, or neither")
+    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 32:
+        raise ValueError("k must be an integer in [3, 32], got %r" % (k,))
+    k = int(k)
+    pts = _lib.as_f32(points.detach(), "points")
+    P = pts.shape[0]
+    if P >= 2 ** 30:
+        raise ValueError("at most 2^30 - 1 points")
+    if first_idx is None:
+        first_idx = torch.zeros((1,), dtype=torch.int64, device=dev)
+        num_points = torch.full((1,), P, dtype=torch.int64, device=dev)
+    fi, npts = first_idx.contiguous(), num_points.contiguous()
+    normals = torch.empty((P, 3), dtype=torch.float32, device=dev)
+    root = torch.full((P,), -1, dtype=torch.int32, device=dev)
+    parent = torch.full((P,), -1, dtype=torch.int32, device=dev)
+    if P == 0:
+        return PointNormals(normals, root, parent)
+    _, idx = knn_points_packed(pts, fi, npts, k, -1.0)
+    _lib.call("dss_estimate_normals", dev, pts, fi, npts, int(npts.shape[0]), P, idx, k, int(bool(orient)), normals,
+              root, parent)
+    return PointNormals(normals, root, parent)
 
 
 class MeshRender(NamedTuple):

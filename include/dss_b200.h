@@ -221,6 +221,33 @@ DSS_API int dss_knn_points(dss_ctx *ctx, const float *queries, const int64_t *qu
 DSS_API int dss_local_frames(dss_ctx *ctx, const float *points, const int64_t *first_idx, const int64_t *num_points,
                              int N, int64_t P, const int32_t *knn_idx, float *frames, void *stream);
 
+/* ---- normal estimation and orientation ----------------------------------------------------------------------------
+ * PointClouds3D.estimate_normals (DSS/core/cloud.py:210-258) and meshlab's "Compute normals for point sets" with no
+ * smoothing and no viewpoint (scripts/poisson_sampling_pca.mlx), for clouds that carry no normals.  knn_idx (P,k)
+ * int32, 3 <= k <= 32: every row's k nearest neighbours as dss_knn_points writes them for K = k, r = -1 (local to the
+ * cloud, the point itself included); first_idx / num_points (N,) int64 as for dss_knn_points (required; clouds are never
+ * connected).  Outputs (P,3) f32 normals, (P,) int32 root and parent, local to the cloud.
+ *  - A row with a -1 neighbour (a non-finite point, a cloud of fewer than k finite points) is invalid: NaN normal,
+ *    root = parent = -1, and no edge.
+ *  - PCA: the population covariance of the k neighbours about their mean in float64, diagonalised as dss_local_frames
+ *    does; the normal is the eigenvector f0 of the smallest eigenvalue, rounded once.  Where l1 - l0 <= 2^-40 l2
+ *    (collinear neighbours) it is dss_local_frames' f1 = normalize(f2 x e_k), and where all three agree (duplicates)
+ *    e_z.  Its canonical sign makes the component of largest |n_k| (the first such axis) positive.
+ *  - orient == 0: the canonical normals; root = parent = -1.
+ *  - orient != 0: the undirected graph of the edges {i, j}, j != i in i's list; weight w = 1 - |n_i . n_j| in float32,
+ *    each product and sum rounded in the order x, y, z; edges ordered by (w, min(i,j), max(i,j)), so the minimum
+ *    spanning forest is unique.  Per component the root is the point of largest z (ties: the smallest index), flipped
+ *    so that n_z >= 0 (n_z == 0 keeps the canonical sign).  Every other point is flipped exactly when the dot product
+ *    of its normal with its parent's oriented normal (same rounding) is negative; zero does not flip.  root: the
+ *    component's root; parent: the tree parent, -1 at a root.
+ * On the device (DESIGN.md): one PCA thread per row; Boruvka rounds with 64-bit atomicMin keys and pointer jumping,
+ * Euler tours ranked by pointer jumping, and ancestor doubling for the signs, each loop of ceil(log2 P) + 1 launches
+ * that leave early on a flag written on the device.  Deterministic, no host synchronisation: capturable.  Scratch from
+ * the context: 16 bytes per row, and 108 more per row to orient.  P < 2^30. */
+DSS_API int dss_estimate_normals(dss_ctx *ctx, const float *points, const int64_t *first_idx,
+                                 const int64_t *num_points, int N, int64_t P, const int32_t *knn_idx, int k, int orient,
+                                 float *normals, int32_t *root, int32_t *parent, void *stream);
+
 /* ---- surface regularisers of the training step (SURVEY.md section 8(f) row 2) -----------------------------------
  * Replaces the torch bodies of ProjectionLoss (kind 0) and RepulsionLoss (kind 1) (DSS/training/losses.py:282-497) on
  * packed clouds (points, normals (P,3); first_idx, num_points as for dss_knn_points).  knn_dists (P, K-1+self_col) f32
