@@ -11,7 +11,7 @@ from typing import List, Optional, Sequence, Tuple
 
 import torch
 
-__all__ = ["PointClouds3D", "PointCloudsFilters"]
+__all__ = ["PointClouds3D", "PointCloudsFilters", "upsample", "remove_outliers"]
 
 
 def _as_list(x, name):
@@ -170,6 +170,17 @@ class PointClouds3D:
                 self._cache.pop(key, None)
         return PointClouds3D(self._points, normals).normals_padded()
 
+    def upsample(self, n, neighborhood_size: int = 16):
+        """A denser copy by :func:`dss_b200.ops.upsample_points`: every cloud grown to ``n`` points (an int or one per
+        cloud), its normals and features carried to the new points.  The input points keep their indices in every
+        cloud.  The clouds must be on a CUDA device."""
+        from ..ops import upsample_points
+        up = upsample_points(self.points_packed(), n, neighborhood_size, self.normals_packed(), self.features_packed(),
+                             self.cloud_to_packed_first_idx(), self.num_points_per_cloud())
+        sizes = up.num_points.tolist()
+        split = lambda t: None if t is None else list(t.split(sizes))
+        return PointClouds3D(split(up.points), split(up.normals), split(up.features))
+
 
 class PointCloudsFilters:
     """Named per-point boolean masks, padded (N, P_max) (DSS/core/cloud.py:285-360): ``activation`` selects
@@ -207,6 +218,48 @@ class PointCloudsFilters:
         sel = lambda lst: None if lst is None else [t[mask[i, : t.shape[0]]] for i, t in enumerate(lst)]
         return PointClouds3D(sel(point_clouds.points_list()), sel(point_clouds.normals_list()),
                              sel(point_clouds.features_list()))
+
+
+def upsample(points, n_points, num_points=None, neighborhood_size=16, knn_result=None):
+    """The reference's ``upsample`` (DSS/core/cloud.py:555-632) on :func:`dss_b200.ops.upsample_points`: padded
+    ``points`` (N, P, 3) with ``num_points`` (N,) (default: all P) grown to ``n_points`` (an int or (N,)) ->
+    ``(points_padded (N, max n, 3), num_points (N,))``, zero-padded.  Each cloud's input points come first, where the
+    reference puts each round's points in front.  ``knn_result`` must be None: the neighbourhoods are recomputed on the
+    device every round.  Raises ValueError where the reference would loop forever or pad neighbourhoods with zeros (see
+    ``upsample_points``)."""
+    from ..ops import upsample_points
+    if knn_result is not None:
+        raise ValueError("knn_result is not supported: the neighbourhoods are recomputed on the device every round")
+    if points.dim() != 3 or points.shape[2] != 3:
+        raise ValueError("points must be padded (N, P, 3)")
+    N, P = points.shape[0], points.shape[1]
+    dev = points.device
+    if num_points is None:
+        num_points = torch.full((N,), P, dtype=torch.int64, device=dev)
+    first = torch.arange(N, dtype=torch.int64, device=dev) * P
+    up = upsample_points(points.reshape(N * P, 3), n_points, neighborhood_size, first_idx=first,
+                         num_points=num_points.to(device=dev, dtype=torch.int64))
+    return PointClouds3D(list(up.points.split(up.num_points.tolist()))).points_padded(), up.num_points
+
+
+def remove_outliers(pointclouds, neighborhood_size=16, tolerance=0.05):
+    """The reference's ``remove_outliers`` (DSS/core/cloud.py:363-378) on :func:`dss_b200.ops.outlier_ratio`: the points
+    whose ``neighborhood_size`` nearest neighbours (themselves included) are planar, i.e. whose covariance has its
+    smallest eigenvalue below ``tolerance`` of the three's sum, with their normals and features, as a new
+    :class:`PointClouds3D`.  Like the reference, raises ValueError for a cloud of at most ``neighborhood_size`` points;
+    ``neighborhood_size`` is at most 32, the device K-NN's limit.  The clouds must be on a CUDA device."""
+    from ..ops import outlier_ratio
+    sizes = [int(p.shape[0]) for p in pointclouds.points_list()]
+    if any(n <= neighborhood_size for n in sizes):
+        raise ValueError("every cloud needs more than neighborhood_size = %d points, got %s" % (neighborhood_size, sizes))
+    nl, fl = getattr(pointclouds, "normals_list", None), getattr(pointclouds, "features_list", None)
+    normals, features = (nl() if callable(nl) else None), (fl() if callable(fl) else None)
+    num = torch.tensor(sizes, dtype=torch.int64, device=pointclouds.points_list()[0].device)
+    first = torch.cumsum(num, 0) - num
+    keep = outlier_ratio(torch.cat(pointclouds.points_list(), 0), neighborhood_size, tolerance, first, num).keep
+    masks = keep.split(sizes)
+    sel = lambda lst: None if lst is None else [t[m] for t, m in zip(lst, masks)]
+    return PointClouds3D(sel(pointclouds.points_list()), sel(normals), sel(features))
 
 
 # ---- duck typing for foreign cloud containers --------------------------------------------------------------------

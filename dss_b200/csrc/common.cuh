@@ -93,6 +93,7 @@ enum BufId {
     BUF_PDS_GRID,     //   samples per cell, then their exclusive scan
     BUF_IMAGE_METRICS,  // per-block fp64 partial sums of the image metrics, and the finish's block counter
     BUF_NORMALS,      // normal estimation: unoriented normals, the spanning forest's state, the Euler tours and flags
+    BUF_UPSAMPLE,     // upsampling: the round's K-NN rows, select keys, chosen neighbours, flags and their scan, histograms
     NUM_BUFS
 };
 

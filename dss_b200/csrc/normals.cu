@@ -20,6 +20,9 @@
 // Every loop of rounds has a fixed length (ceil(log2 P) + 1, enough for any input) and reads an early-out flag that
 // the previous round wrote on the device, so the launches are fixed and the call can be captured in a CUDA graph.
 // Indices inside are rows of the packed input; clouds are never connected, since every neighbour lies in its cloud.
+//
+// dss_outlier_ratio (remove_outliers, DSS/core/cloud.py:363-378) runs the same PCA (knn_pca) and keeps the row when
+// its smallest eigenvalue is less than `tolerance` of the three's sum.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -79,43 +82,51 @@ __device__ __forceinline__ float dot_rn(float4 a, float4 b) {
     for (int64_t i_ = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i_ < cr.count;                        \
          i_ += (int64_t)gridDim.x * blockDim.x)
 
+// The PCA of one row, shared by the normals and the outlier ratio: the population covariance of the row's k
+// neighbours nb (local to the cloud starting at row `first`) about their mean in float64, and sym3_eigen's solve of it.
+// False, with nothing solved, when a neighbour is -1.
+__device__ __forceinline__ bool knn_pca(const float *points, int64_t first, const int32_t *nb, int k, double &l0,
+                                        double &l1, double &l2, double (&f0)[3], double (&f1)[3], double (&f2)[3]) {
+    bool ok = true;
+    double m[3] = {0.0, 0.0, 0.0};
+    for (int s = 0; s < k; ++s) {
+        const int32_t j = nb[s];
+        ok = ok && j >= 0;
+        const int64_t src = first + (j >= 0 ? j : 0);
+#pragma unroll
+        for (int e = 0; e < 3; ++e) m[e] += (double)points[src * 3 + e];
+    }
+    if (!ok) return false;
+    const double inv_k = 1.0 / k;
+#pragma unroll
+    for (int e = 0; e < 3; ++e) m[e] *= inv_k;
+    double A[3][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
+    for (int s = 0; s < k; ++s) {
+        const int64_t src = first + nb[s];
+        const double d0 = (double)points[src * 3] - m[0], d1 = (double)points[src * 3 + 1] - m[1],
+                     d2 = (double)points[src * 3 + 2] - m[2];
+        A[0][0] = fma(d0, d0, A[0][0]);
+        A[0][1] = fma(d0, d1, A[0][1]);
+        A[0][2] = fma(d0, d2, A[0][2]);
+        A[1][1] = fma(d1, d1, A[1][1]);
+        A[1][2] = fma(d1, d2, A[1][2]);
+        A[2][2] = fma(d2, d2, A[2][2]);
+    }
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = r; c < 3; ++c) A[r][c] *= inv_k;
+    sym3_eigen(A, l0, l1, l2, f0, f1, f2);
+    return true;
+}
+
 // 1. PCA, canonical sign, and the initial state of every later stage
 __global__ void __launch_bounds__(NRM_THREADS) normals_pca_kernel(const __grid_constant__ NormalArgs a) {
     NRM_ROWS(a) {
         const int32_t row = (int32_t)(cr.first + i_);
-        const int32_t *nb = a.knn_idx + (int64_t)row * a.k;
-        bool ok = true;
-        double m[3] = {0.0, 0.0, 0.0};
-        for (int s = 0; s < a.k; ++s) {
-            const int32_t j = nb[s];
-            ok = ok && j >= 0;
-            const int64_t src = cr.first + (j >= 0 ? j : 0);
-#pragma unroll
-            for (int e = 0; e < 3; ++e) m[e] += (double)a.points[src * 3 + e];
-        }
         float4 n = make_float4(CUDART_NAN_F, CUDART_NAN_F, CUDART_NAN_F, 0.0f);
-        if (ok) {
-            const double inv_k = 1.0 / a.k;
-#pragma unroll
-            for (int e = 0; e < 3; ++e) m[e] *= inv_k;
-            double A[3][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
-            for (int s = 0; s < a.k; ++s) {
-                const int64_t src = cr.first + nb[s];
-                const double d0 = (double)a.points[src * 3] - m[0], d1 = (double)a.points[src * 3 + 1] - m[1],
-                             d2 = (double)a.points[src * 3 + 2] - m[2];
-                A[0][0] = fma(d0, d0, A[0][0]);
-                A[0][1] = fma(d0, d1, A[0][1]);
-                A[0][2] = fma(d0, d2, A[0][2]);
-                A[1][1] = fma(d1, d1, A[1][1]);
-                A[1][2] = fma(d1, d2, A[1][2]);
-                A[2][2] = fma(d2, d2, A[2][2]);
-            }
-#pragma unroll
-            for (int r = 0; r < 3; ++r)
-#pragma unroll
-                for (int c = r; c < 3; ++c) A[r][c] *= inv_k;
-            double l0, l1, l2, f0[3], f1[3], f2[3];
-            sym3_eigen(A, l0, l1, l2, f0, f1, f2);
+        double l0, l1, l2, f0[3], f1[3], f2[3];
+        if (knn_pca(a.points, cr.first, a.knn_idx + (int64_t)row * a.k, a.k, l0, l1, l2, f0, f1, f2)) {
             // degenerate rows: the normal is sym3_fix_degenerate's f1 (collinear: perpendicular to the line;
             // duplicates: e_z)
             const bool flat = l1 - l0 <= SYM3_DEGENERATE * fabs(l2);
@@ -136,6 +147,23 @@ __global__ void __launch_bounds__(NRM_THREADS) normals_pca_kernel(const __grid_c
             a.edge_a[row] = -1, a.edge_b[row] = -1;
             a.root_key[row] = 0ull, a.head[row] = -1, a.gparent[row] = -1;
         }
+    }
+}
+
+// The outlier ratio of every row: l0 / ((l0 + l1) + l2) of the same PCA, NaN on an invalid row (and 0 / 0 on a row of
+// duplicates), and keep = ratio < tolerance, both in float64 (NaN is not kept)
+__global__ void __launch_bounds__(NRM_THREADS)
+outlier_ratio_kernel(const float *__restrict__ points, const int64_t *__restrict__ first_idx,
+                     const int64_t *__restrict__ num_points, const int32_t *__restrict__ knn_idx, int k, int64_t P,
+                     double tolerance, double *__restrict__ ratio, uint8_t *__restrict__ keep) {
+    const ViewRange cr = view_range(first_idx, num_points, blockIdx.y, P);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cr.count; i += (int64_t)gridDim.x * blockDim.x) {
+        const int64_t row = cr.first + i;
+        double l0, l1, l2, f0[3], f1[3], f2[3];
+        double r = CUDART_NAN;
+        if (knn_pca(points, cr.first, knn_idx + row * k, k, l0, l1, l2, f0, f1, f2)) r = __ddiv_rn(l0, __dadd_rn(__dadd_rn(l0, l1), l2));
+        ratio[row] = r;
+        keep[row] = r < tolerance ? 1 : 0;
     }
 }
 
@@ -437,6 +465,26 @@ int dss_estimate_normals(dss_ctx *ctx, const float *points, const int64_t *first
         DSS_LAUNCH_CHECK(ctx);
     }
     normals_out_kernel<<<grid, NRM_THREADS, 0, st>>>(a);
+    DSS_LAUNCH_CHECK(ctx);
+    return DSS_OK;
+}
+
+int dss_outlier_ratio(dss_ctx *ctx, const float *points, const int64_t *first_idx, const int64_t *num_points, int N,
+                      int64_t P, const int32_t *knn_idx, int k, double tolerance, double *ratio, uint8_t *keep,
+                      void *stream) {
+    using namespace dss;
+    DSS_REQUIRE(ctx != nullptr, "ctx is null");
+    DSS_REQUIRE(P >= 0 && P < ((int64_t)1 << 30), "P out of range");
+    DSS_REQUIRE(first_idx && num_points, "first_idx and num_points are required");
+    DSS_REQUIRE(N >= 1 && N <= 65535, "N out of range");
+    DSS_REQUIRE(k >= 3 && k <= 32, "k must lie in [3, 32]");
+    if (P == 0) return DSS_OK;
+    DSS_REQUIRE(points && knn_idx && ratio && keep, "null pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    const dim3 grid(grid_blocks(P, NRM_THREADS, ctx->sm_count, 8), N);
+    StageScope prof(ctx, ST_KNN, st);
+    outlier_ratio_kernel<<<grid, NRM_THREADS, 0, st>>>(points, first_idx, num_points, knn_idx, k, P, tolerance, ratio,
+                                                       keep);
     DSS_LAUNCH_CHECK(ctx);
     return DSS_OK;
 }

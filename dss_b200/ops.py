@@ -22,7 +22,8 @@ from . import _lib
 
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
            "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "PointNormals",
-           "estimate_normals", "MeshRender", "render_mesh", "chamfer_distance",
+           "estimate_normals", "Outliers", "outlier_ratio", "Upsampled", "upsample_schedule", "upsample_points",
+           "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
            "ImageMetrics", "image_metrics", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
 
@@ -548,6 +549,161 @@ def estimate_normals(points, k=20, orient=True, first_idx=None, num_points=None)
     _lib.call("dss_estimate_normals", dev, pts, fi, npts, int(npts.shape[0]), P, idx, k, int(bool(orient)), normals,
               root, parent)
     return PointNormals(normals, root, parent)
+
+
+def _packed_layout(pts, first_idx, num_points, dev):
+    if (first_idx is None) != (num_points is None):
+        raise RuntimeError("pass both first_idx and num_points, or neither")
+    if first_idx is None:
+        first_idx = torch.zeros((1,), dtype=torch.int64, device=dev)
+        num_points = torch.full((1,), pts.shape[0], dtype=torch.int64, device=dev)
+    return first_idx.contiguous(), num_points.contiguous()
+
+
+class Outliers(NamedTuple):
+    keep: torch.Tensor                # (P,) bool: ratio < tolerance (False on an invalid row and outside every cloud)
+    ratio: torch.Tensor               # (P,) float64 l0 / (l0 + l1 + l2); NaN on an invalid row and outside every cloud
+
+
+def outlier_ratio(points, k=16, tolerance=0.05, first_idx=None, num_points=None) -> Outliers:
+    """The planarity test of the reference's ``remove_outliers`` (DSS/core/cloud.py:363-378; csrc/normals.cu, the
+    rules are in include/dss_b200.h): ``ratio = l0 / (l0 + l1 + l2)``, the smallest eigenvalue of the population
+    covariance of each point's ``k`` nearest neighbours of its cloud (itself included) over the three, from the same
+    float64 PCA as :func:`estimate_normals`, and ``keep = ratio < tolerance`` in float64.
+
+    ``points`` (P,3) float32 CUDA tensor, one cloud, or packed with ``first_idx`` / ``num_points`` (N,) int64 as for
+    ``knn_points_packed``.  ``k`` in [3, 32].  A row with a non-finite point or fewer than ``k`` finite neighbours, and
+    a row whose neighbours all coincide (0 / 0), get ratio NaN and are not kept.  Two library calls (the K-NN and the
+    ratio), no host synchronisation, so the call can be captured in a CUDA graph; the same bits on every call."""
+    from .frnn_grid import knn_points_packed
+    dev = _lib.require_cuda(points, first_idx, num_points)
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3)")
+    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 32:
+        raise ValueError("k must be an integer in [3, 32], got %r" % (k,))
+    k = int(k)
+    pts = _lib.as_f32(points.detach(), "points")
+    P = pts.shape[0]
+    if P >= 2 ** 30:
+        raise ValueError("at most 2^30 - 1 points")
+    fi, npts = _packed_layout(pts, first_idx, num_points, dev)
+    keep = torch.zeros((P,), dtype=torch.bool, device=dev)
+    ratio = torch.full((P,), float("nan"), dtype=torch.float64, device=dev)
+    if P == 0:
+        return Outliers(keep, ratio)
+    _, idx = knn_points_packed(pts, fi, npts, k, -1.0)
+    _lib.call("dss_outlier_ratio", dev, pts, fi, npts, int(npts.shape[0]), P, idx, k, float(tolerance), ratio, keep)
+    return Outliers(keep, ratio)
+
+
+class Upsampled(NamedTuple):
+    points: torch.Tensor              # (M,3) float32, packed: cloud n owns rows [first_idx[n], first_idx[n] + num_points[n])
+    normals: Optional[torch.Tensor]   # (M,3) float32 or None
+    features: Optional[torch.Tensor]  # (M,D) float32 or None
+    first_idx: torch.Tensor           # (N,) int64
+    num_points: torch.Tensor          # (N,) int64, the targets
+    parents: torch.Tensor             # (M,2) int32 (i, j*) local to the cloud; (-1, -1) on an input row
+
+
+def upsample_schedule(num_points, targets, k=16):
+    """The sizes of every cloud before each round and after the last: a list of R + 1 lists of N ints.  Each round adds
+    ``min(n - c, c // 10)`` points to a cloud of ``c`` points and target ``n``, until every cloud has reached its
+    target.  Raises ValueError for a target below the cloud's size, and for a cloud that has to grow but has at most
+    ``k`` or fewer than 10 points (the rounds would then need missing neighbours or never end)."""
+    c, n = [int(x) for x in num_points], [int(x) for x in targets]
+    if len(c) != len(n):
+        raise ValueError("%d targets for %d clouds" % (len(n), len(c)))
+    for i, (ci, ni) in enumerate(zip(c, n)):
+        if ni < ci:
+            raise ValueError("cloud %d: the target %d is below its %d points" % (i, ni, ci))
+        if ni > ci and (ci <= k or ci < 10):
+            raise ValueError("cloud %d: %d points cannot grow with k = %d: it needs more than k and at least 10 points"
+                             % (i, ci, k))
+    rounds = [c]
+    while any(ci < ni for ci, ni in zip(c, n)):
+        c = [ci + min(ni - ci, ci // 10) for ci, ni in zip(c, n)]
+        rounds.append(c)
+    return rounds
+
+
+def upsample_points(points, n, k=16, normals=None, features=None, first_idx=None, num_points=None) -> Upsampled:
+    """Densify point clouds as the reference's ``upsample`` does (DSS/core/cloud.py:555-632; csrc/upsample.cu, the rules
+    are in include/dss_b200.h and DESIGN.md): in every round each cloud of ``c`` points gains ``min(n - c, c // 10)``
+    points, one next to each of its sparsest neighbourhoods.  For a point p and its ``k`` nearest other points q_j the
+    candidates are (q_j + 2 p) / 3; a point's sparsity is the largest over j of the distance from candidate j to its
+    nearest q; the points of largest sparsity (ties: the smaller index) each add their sparsest candidate.  With
+    ``normals`` a child's normal is normalize(2 n_p + n_q) of the unit normals, with ``features`` (colours or any D) its
+    feature is (f_q + 2 f_p) / 3.
+
+    ``points`` (P,3) float32 CUDA tensor, one cloud, or packed with ``first_idx`` / ``num_points`` (N,) int64 as for
+    ``knn_points_packed`` (gaps allowed); ``normals`` (P,3) / ``features`` (P,D) float32 in the same rows.  ``n`` an int
+    or N ints: the size of every cloud afterwards.  ``k`` in [3, 31].  The result is packed without gaps; each cloud
+    keeps its input rows first, in their order, and each round's points follow in the order of their parents' indices,
+    so an index never changes and ``parents`` stays valid.  Raises ValueError for a non-finite coordinate, a target
+    below a cloud's size, and a cloud that has to grow with at most ``k`` or fewer than 10 points.
+
+    Synchronises once, to read the sizes; then one library call (per round the K-NN and five kernels), the same bits on
+    every call.  No gradients."""
+    import numpy as np
+    dev = _lib.require_cuda(points, normals, features, first_idx, num_points)
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3)")
+    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 31:
+        raise ValueError("k must be an integer in [3, 31], got %r" % (k,))
+    k = int(k)
+    pts = _lib.as_f32(points.detach(), "points")
+    P = pts.shape[0]
+    nrm = None if normals is None else _lib.as_f32(normals.detach(), "normals")
+    if nrm is not None and tuple(nrm.shape) != (P, 3):
+        raise RuntimeError("normals must have shape (P, 3)")
+    ftr = None if features is None else _lib.as_f32(features.detach(), "features")
+    if ftr is not None and (ftr.dim() != 2 or ftr.shape[0] != P or ftr.shape[1] < 1):
+        raise RuntimeError("features must have shape (P, D)")
+    fi, npts = _packed_layout(pts, first_idx, num_points, dev)
+    N = int(npts.shape[0])
+    if N < 1:
+        raise ValueError("no clouds")
+    # the one synchronisation: every cloud's first row, size and count of non-finite rows
+    bad = torch.zeros((P + 1,), dtype=torch.int64, device=dev)
+    bad[1:] = torch.cumsum((~torch.isfinite(pts).all(1)).to(torch.int64), 0)
+    end = (fi + npts).clamp(0, P)
+    info = torch.stack([fi, npts, bad[end] - bad[fi.clamp(0, P)]]).cpu().numpy()
+    first_h, num_h = info[0], info[1]
+    if (num_h < 0).any() or (first_h < 0).any() or (first_h + num_h > P).any():
+        raise ValueError("first_idx / num_points leave the points")
+    if info[2].any():
+        raise ValueError("non-finite coordinates in cloud(s) %s" % np.flatnonzero(info[2]).tolist())
+    if torch.is_tensor(n):
+        n = n.tolist()
+    targets = [int(n)] * N if np.ndim(n) == 0 else [int(x) for x in n]
+    sched = upsample_schedule(num_h, targets, k)
+    rounds = len(sched) - 1
+    sizes = np.asarray(sched, dtype=np.int64)
+    out_num = sizes[-1]
+    out_first = np.concatenate([[0], np.cumsum(out_num)[:-1]]).astype(np.int64)
+    M = int(out_num.sum())
+    if M >= 2 ** 31 - 1:
+        raise ValueError("at most 2^31 - 2 points in all")
+    knn_num = np.where(sizes[1:] > sizes[:-1], sizes[:-1], 0)
+    src = np.concatenate([np.arange(f, f + c) for f, c in zip(first_h, num_h)] + [np.zeros(0, np.int64)])
+    dst = np.concatenate([np.arange(f, f + c) for f, c in zip(out_first, num_h)] + [np.zeros(0, np.int64)])
+    table = torch.from_numpy(np.concatenate([out_first, sizes.ravel(), knn_num.ravel(), src, dst])).to(dev)
+    o = torch.split(table, [N, sizes.size, knn_num.size, src.size, dst.size])
+    first_d, sizes_d, knn_d, src_d, dst_d = (t.contiguous() for t in o)
+    out_pts = torch.empty((M, 3), dtype=torch.float32, device=dev)
+    out_pts[dst_d] = pts[src_d]
+    out_nrm = out_ftr = None
+    if nrm is not None:
+        out_nrm = torch.empty((M, 3), dtype=torch.float32, device=dev)
+        out_nrm[dst_d] = nrm[src_d]
+    if ftr is not None:
+        out_ftr = torch.empty((M, ftr.shape[1]), dtype=torch.float32, device=dev)
+        out_ftr[dst_d] = ftr[src_d]
+    parents = torch.full((M, 2), -1, dtype=torch.int32, device=dev)
+    if rounds > 0:
+        _lib.call("dss_upsample_points", dev, out_pts, out_nrm, out_ftr, 0 if ftr is None else int(ftr.shape[1]),
+                  first_d, sizes_d, knn_d, N, M, rounds, k, parents)
+    return Upsampled(out_pts, out_nrm, out_ftr, first_d, sizes_d[rounds * N:], parents)
 
 
 class MeshRender(NamedTuple):

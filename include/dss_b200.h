@@ -248,6 +248,40 @@ DSS_API int dss_estimate_normals(dss_ctx *ctx, const float *points, const int64_
                                  const int64_t *num_points, int N, int64_t P, const int32_t *knn_idx, int k, int orient,
                                  float *normals, int32_t *root, int32_t *parent, void *stream);
 
+/* ---- outlier ratio -------------------------------------------------------------------------------------------------
+ * remove_outliers (DSS/core/cloud.py:363-378).  points, first_idx, num_points, knn_idx and k as for
+ * dss_estimate_normals, and the same float64 PCA.  Outputs, per row of every cloud: ratio (P,) f64 = l0 / ((l0 + l1) +
+ * l2) with l0 <= l1 <= l2 the covariance's eigenvalues, and keep (P,) uint8 = ratio < tolerance in float64.  A row with
+ * a -1 neighbour gets NaN, and so does a row whose neighbours all coincide (0 / 0); NaN is never kept.  Rows outside
+ * every range are not written.  One launch, one thread per row; no scratch, no host synchronisation: capturable. */
+DSS_API int dss_outlier_ratio(dss_ctx *ctx, const float *points, const int64_t *first_idx, const int64_t *num_points,
+                              int N, int64_t P, const int32_t *knn_idx, int k, double tolerance, double *ratio,
+                              uint8_t *keep, void *stream);
+
+/* ---- upsampling ----------------------------------------------------------------------------------------------------
+ * upsample (DSS/core/cloud.py:555-632), in rounds on preallocated packed buffers.  Cloud n owns rows [first_idx[n],
+ * first_idx[n] + sizes[rounds][n]) of points (M,3), and of normals (M,3) and features (M,D) when not NULL; these ranges
+ * must tile [0, M).  On entry each cloud holds its sizes[0][n] input rows at the start of its range.  sizes
+ * (rounds + 1, N) int64 is the schedule: round r grows cloud n from c = sizes[r][n] to sizes[r + 1][n] = c + m, with
+ * m = min(n_n - c, c / 10) (the caller computes it once; a cloud that grows has more than k points).  knn_num
+ * (rounds, N) int64 is c where m > 0 and 0 elsewhere.  3 <= k <= 31.  In each round, for every cloud that grows:
+ *  - the neighbours q_0 .. q_{k-1} of row i are its dss_knn_points row at K = k + 1, r = -1, less its own index (less
+ *    the last entry when its own index is not in the row: more than k duplicates of smaller index);
+ *  - in float32, rounded after every operation, without contraction: candidates c_j = (q_j + 2 p_i) / 3 per coordinate;
+ *    s_j = min over all k neighbours q_l of sqrt((dx dx + dy dy) + dz dz), d = c_j - q_l; s_i = max_j s_j, attained
+ *    first at j*;
+ *  - the m rows of largest s_i, ties to the smaller index, are the parents; parent i writes, in increasing order of i,
+ *    to the rows that follow the cloud's c current rows: the point c_{j*}, the normal normalize(2 normalize(n_i) +
+ *    normalize(n_{j*})) (normalize(v) = v / sqrt((x x + y y) + z z), same rounding), the feature (f_{j*} + 2 f_i) / 3
+ *    per channel, and parents (M,2) int32 = (i, j*) in local indices.
+ * Rows already written never change; parents of the input rows are left as the caller set them.  On the device
+ * (DESIGN.md): per round one K-NN call, one sparsity thread per row (k^2 distances), an 8-pass MSB-first radix select of
+ * (bits(s), ~i), flags, an exclusive scan and a write kernel.  Deterministic, no host synchronisation.  Scratch from the
+ * context: 8 (k + 1) + 20 bytes per row and 8 KB per cloud.  M < 2^31 - 1. */
+DSS_API int dss_upsample_points(dss_ctx *ctx, float *points, float *normals, float *features, int D,
+                                const int64_t *first_idx, const int64_t *sizes, const int64_t *knn_num, int N, int64_t M,
+                                int rounds, int k, int32_t *parents, void *stream);
+
 /* ---- surface regularisers of the training step (SURVEY.md section 8(f) row 2) -----------------------------------
  * Replaces the torch bodies of ProjectionLoss (kind 0) and RepulsionLoss (kind 1) (DSS/training/losses.py:282-497) on
  * packed clouds (points, normals (P,3); first_idx, num_points as for dss_knn_points).  knn_dists (P, K-1+self_col) f32
