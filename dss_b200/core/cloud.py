@@ -11,7 +11,8 @@ from typing import List, Optional, Sequence, Tuple
 
 import torch
 
-__all__ = ["PointClouds3D", "PointCloudsFilters", "upsample", "remove_outliers"]
+__all__ = ["PointClouds3D", "PointCloudsFilters", "upsample", "remove_outliers", "denoise_normals",
+           "project_to_latent_surface"]
 
 
 def _as_list(x, name):
@@ -181,6 +182,17 @@ class PointClouds3D:
         split = lambda t: None if t is None else list(t.split(sizes))
         return PointClouds3D(split(up.points), split(up.normals), split(up.features))
 
+    def project_to_latent_surface(self, neighborhood_size: int = 31, max_proj_iters: int = 10, max_est_iter: int = 5):
+        """A copy with every point moved onto the RIMLS surface of its cloud by :func:`dss_b200.ops.project_to_surface`,
+        the normals and features carried unchanged.  The clouds need normals and must be on a CUDA device."""
+        from ..ops import project_to_surface
+        if self._normals is None:
+            raise ValueError("projecting onto the surface needs normals (see PointClouds3D.estimate_normals)")
+        out = project_to_surface(self.points_packed(), self.normals_packed(), neighborhood_size, max_proj_iters,
+                                 max_est_iter, self.cloud_to_packed_first_idx(), self.num_points_per_cloud())
+        sizes = self.num_points_per_cloud().tolist()
+        return PointClouds3D(list(out.points.split(sizes)), self.normals_list(), self.features_list())
+
 
 class PointCloudsFilters:
     """Named per-point boolean masks, padded (N, P_max) (DSS/core/cloud.py:285-360): ``activation`` selects
@@ -261,6 +273,45 @@ def remove_outliers(pointclouds, neighborhood_size=16, tolerance=0.05):
     sel = lambda lst: None if lst is None else [t[m] for t, m in zip(lst, masks)]
     return PointClouds3D(sel(pointclouds.points_list()), sel(normals), sel(features))
 
+
+def _padded_layout(points, normals, num_points):
+    if points.dim() != 3 or points.shape[2] != 3 or tuple(normals.shape) != tuple(points.shape):
+        raise ValueError("points and normals must be padded (N, P, 3)")
+    N, P = points.shape[0], points.shape[1]
+    dev = points.device
+    if num_points is None:
+        num_points = torch.full((N,), P, dtype=torch.int64, device=dev)
+    first = torch.arange(N, dtype=torch.int64, device=dev) * P
+    return N, P, first, num_points.to(device=dev, dtype=torch.int64)
+
+
+def denoise_normals(points, normals, num_points=None, sharpness_sigma=30, knn_result=None, neighborhood_size=16):
+    """The reference's ``denoise_normals`` (DSS/core/cloud.py:515-553) on :func:`dss_b200.ops.denoise_normals`: padded
+    ``points`` and ``normals`` (N, P, 3) with ``num_points`` (N,) (default: all P) -> the denoised unit normals (N, P, 3);
+    rows past a cloud's size are returned as given.  Each cloud uses its own size and bounding box, where the
+    reference uses the padded size and the whole batch's box; a row whose weights are all zero keeps its own normal,
+    where the reference returns zero.  ``knn_result`` must be None: the neighbourhoods are computed on the device."""
+    from ..ops import denoise_normals as _denoise
+    if knn_result is not None:
+        raise ValueError("knn_result is not supported: the neighbourhoods are computed on the device")
+    N, P, first, num = _padded_layout(points, normals, num_points)
+    out = _denoise(points.reshape(N * P, 3), normals.reshape(N * P, 3), neighborhood_size, float(sharpness_sigma),
+                   first, num)
+    return out.view_as(normals)
+
+
+def project_to_latent_surface(points, normals, sharpness_angle=60, neighborhood_size=31, max_proj_iters=10,
+                              max_est_iter=5):
+    """The reference's ``project_to_latent_surface`` (DSS/core/cloud.py:442-513, RIMLS) on
+    :func:`dss_b200.ops.project_to_surface`: padded ``points`` and ``normals`` (N, P, 3), every cloud of P points ->
+    the projected points (N, P, 3).  The surface is fitted to the input samples throughout, where the reference reads
+    the neighbours from the points it is moving; ``points`` is not modified, where the reference overwrites it.
+    ``sharpness_angle`` is accepted and unused, as in the reference."""
+    from ..ops import project_to_surface
+    N, P, first, num = _padded_layout(points, normals, None)
+    out = project_to_surface(points.reshape(N * P, 3), normals.reshape(N * P, 3), neighborhood_size, max_proj_iters,
+                             max_est_iter, first, num)
+    return out.points.view(N, P, 3)
 
 # ---- duck typing for foreign cloud containers --------------------------------------------------------------------
 # The reference hands pytorch3d ``Pointclouds`` (or its own ``PointClouds3D`` subclass) to the renderer; the filter's

@@ -182,4 +182,14 @@ int colour_backward_fixed(dss_ctx *ctx, const int32_t *idx, const float *weights
                           int64_t num_pixels, int K, float *grad_colours, int64_t P, int64_t pixels_per_view,
                           cudaStream_t st);
 
+// The k nearest *other* points of local row i from its dss_knn_points row nb at K = k + 1: the row less entry
+// knn_own_entry(nb, k, i), which is i's own index, or the last entry when i is not in the row (more than k duplicates
+// of smaller index).  Neighbour s of the k is nb[knn_other(s, own)].  Upsampling and the RIMLS kernels share this rule.
+__device__ __forceinline__ int knn_own_entry(const int32_t *nb, int k, int32_t i) {
+    for (int s = 0; s <= k; ++s)
+        if (nb[s] == i) return s;
+    return k;
+}
+__device__ __forceinline__ int knn_other(int s, int own) { return s < own ? s : s + 1; }
+
 }  // namespace dss

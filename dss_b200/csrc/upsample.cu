@@ -77,14 +77,9 @@ __global__ void __launch_bounds__(UPS_THREADS) ups_sparsity_kernel(const __grid_
         const int64_t row = f_ + i;
         const int32_t *nb = a.knn_idx + row * (k + 1);
         // the K-NN row less the row's own index, or less its last entry when the index is not in it
-        int own = k;
-        for (int s = 0; s <= k; ++s)
-            if (nb[s] == (int32_t)i) {
-                own = s;
-                break;
-            }
+        const int own = knn_own_entry(nb, k, (int32_t)i);
         for (int s = 0; s < k; ++s) {
-            const int64_t q = f_ + nb[s < own ? s : s + 1];
+            const int64_t q = f_ + nb[knn_other(s, own)];
             sq[(0 * k + s) * T + t] = a.points[q * 3];
             sq[(1 * k + s) * T + t] = a.points[q * 3 + 1];
             sq[(2 * k + s) * T + t] = a.points[q * 3 + 2];
@@ -105,7 +100,7 @@ __global__ void __launch_bounds__(UPS_THREADS) ups_sparsity_kernel(const __grid_
         }
         // s >= 0, so its bit pattern orders like its value
         a.key[row] = ((unsigned long long)__float_as_uint(best) << 32) | (0xffffffffu - (uint32_t)i);
-        a.jstar[row] = nb[jb < own ? jb : jb + 1];
+        a.jstar[row] = nb[knn_other(jb, own)];
     }
 }
 

@@ -14,6 +14,7 @@ give them, the shininess and the per-point ellipse parameters are constants (com
 rasterizer.py:606-608, 562-565).
 """
 import ctypes as C
+import math
 from typing import NamedTuple, Optional
 
 import torch
@@ -23,7 +24,7 @@ from . import _lib
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
            "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "PointNormals",
            "estimate_normals", "Outliers", "outlier_ratio", "Upsampled", "upsample_schedule", "upsample_points",
-           "MeshRender", "render_mesh", "chamfer_distance",
+           "denoise_normals", "Projected", "project_to_surface", "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
            "ImageMetrics", "image_metrics", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
 
@@ -704,6 +705,120 @@ def upsample_points(points, n, k=16, normals=None, features=None, first_idx=None
         _lib.call("dss_upsample_points", dev, out_pts, out_nrm, out_ftr, 0 if ftr is None else int(ftr.shape[1]),
                   first_d, sizes_d, knn_d, N, M, rounds, k, parents)
     return Upsampled(out_pts, out_nrm, out_ftr, first_d, sizes_d[rounds * N:], parents)
+
+
+def _rimls_radius(diag, count, k, scale):
+    """The neighbourhood radius of one cloud of the RIMLS calls, in float64: ``min(scale * avg * k, 0.2)`` with
+    ``avg = sqrt(diag / count)`` (0 for an empty cloud)"""
+    if count <= 0:
+        return 0.0
+    return min(scale * math.sqrt(diag / count) * k, 0.2)
+
+
+def _rimls_setup(points, normals, k, first_idx, num_points, scale):
+    """Checks and the one host synchronisation of denoise_normals / project_to_surface: (pts, nrm, first_idx,
+    num_points, knn_idx (P, k + 1), radius (N,) float64) on the device"""
+    import numpy as np
+    from .frnn_grid import knn_points_packed
+    dev = _lib.require_cuda(points, normals, first_idx, num_points)
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3)")
+    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 31:
+        raise ValueError("k must be an integer in [3, 31], got %r" % (k,))
+    k = int(k)
+    pts = _lib.as_f32(points.detach(), "points")
+    nrm = _lib.as_f32(normals.detach(), "normals")
+    P = pts.shape[0]
+    if tuple(nrm.shape) != (P, 3):
+        raise RuntimeError("normals must have shape (P, 3)")
+    if P >= 2 ** 31 - 1:
+        raise ValueError("at most 2^31 - 2 points")
+    fi, npts = _packed_layout(pts, first_idx, num_points, dev)
+    N = int(npts.shape[0])
+    if N < 1:
+        raise ValueError("no clouds")
+    # the cloud of every row (id + 1, 0 in the gaps), then in one read-back: every cloud's first row, size, count of
+    # rows with a non-finite point or normal, and bounding box
+    ids = torch.arange(1, N + 1, dtype=torch.int64, device=dev)
+    mark = torch.zeros((P + 1,), dtype=torch.int64, device=dev)
+    mark.index_add_(0, fi.clamp(0, P), ids)
+    mark.index_add_(0, (fi + npts).clamp(0, P), -ids)
+    cloud = torch.cumsum(mark[:P], 0).clamp(0, N)
+    bad = ~(torch.isfinite(pts).all(1) & torch.isfinite(nrm).all(1))
+    nbad = torch.zeros((N + 1,), dtype=torch.float64, device=dev).index_add_(0, cloud, bad.double())
+    idx3 = cloud[:, None].expand(P, 3)
+    lo = torch.full((N + 1, 3), float("inf"), device=dev).scatter_reduce(0, idx3, pts, "amin")
+    hi = torch.full((N + 1, 3), -float("inf"), device=dev).scatter_reduce(0, idx3, pts, "amax")
+    info = torch.cat([fi.double()[:, None], npts.double()[:, None], nbad[1:, None], lo[1:].double(), hi[1:].double()],
+                     1).cpu().numpy()
+    first_h, num_h = info[:, 0].astype(np.int64), info[:, 1].astype(np.int64)
+    if (num_h < 0).any() or (first_h < 0).any() or (first_h + num_h > P).any():
+        raise ValueError("first_idx / num_points leave the points")
+    order = np.lexsort((num_h, first_h))
+    if (first_h[order][1:] < (first_h + num_h)[order][:-1]).any():
+        raise ValueError("the clouds' ranges overlap")
+    if info[:, 2].any():
+        raise ValueError("non-finite points or normals in cloud(s) %s" % np.flatnonzero(info[:, 2]).tolist())
+    radius = []
+    for n in range(N):
+        d = info[n, 6:9] - info[n, 3:6]
+        diag = math.sqrt((float(d[0]) * float(d[0]) + float(d[1]) * float(d[1])) + float(d[2]) * float(d[2])) \
+            if num_h[n] > 0 else 0.0
+        radius.append(_rimls_radius(diag, int(num_h[n]), k, scale))
+    radius = torch.tensor(radius, dtype=torch.float64, device=dev)
+    idx = knn_points_packed(pts, fi, npts, k + 1, -1.0)[1] if P > 0 else None
+    return pts, nrm, fi, npts, idx, radius
+
+
+def denoise_normals(points, normals, k=16, sharpness_sigma=30.0, first_idx=None, num_points=None):
+    """Smooth the normals of point clouds as the reference's ``denoise_normals`` does (DSS/core/cloud.py:515-553;
+    csrc/rimls.cu, the rules are in include/dss_b200.h and DESIGN.md): each row's unit normal becomes
+    ``normalize(sum_j w_j n_j / sum_j w_j)`` over its ``k`` nearest other points of its cloud within ``r = min(4 avg k,
+    0.2)``, ``avg = sqrt(diag / c)`` of the cloud's bounding-box diagonal and size, with ``w_j = exp(-d_j^2 c / 2)
+    exp(-((1 - n_i.n_j) / sharpness_sigma)^2)``, zero beyond ``d_j^2 > 32 / c``.  A row whose weights are all zero keeps
+    its own unit normal.
+
+    ``points``, ``normals`` (P,3) float32 CUDA tensors, one cloud, or packed with ``first_idx`` / ``num_points`` (N,)
+    int64 as for ``knn_points_packed`` (gaps allowed).  ``k`` in [3, 31].  Float64 throughout, rounded once to float32.
+    Raises ValueError for non-finite points or normals.  Synchronises once, to read the clouds' bounding boxes; then
+    the K-NN and one launch.  Returns the (P,3) float32 normals; rows outside every cloud are copied from ``normals``."""
+    pts, nrm, fi, npts, idx, radius = _rimls_setup(points, normals, k, first_idx, num_points, 4.0)
+    out = nrm.clone()
+    if pts.shape[0] > 0:
+        _lib.call("dss_denoise_normals", pts.device, pts, nrm, fi, npts, int(npts.shape[0]), pts.shape[0], idx, int(k),
+                  radius, float(sharpness_sigma), out)
+    return out
+
+
+class Projected(NamedTuple):
+    points: torch.Tensor              # (P,3) float32, the projected positions
+    iterations: torch.Tensor          # (P,) int32, the outer iterations that moved each row
+
+
+def project_to_surface(points, normals, k=31, max_proj_iters=10, max_est_iters=5, first_idx=None,
+                       num_points=None) -> Projected:
+    """Move every point onto the RIMLS surface (robust implicit moving least squares) of its cloud's samples, as the
+    reference's ``project_to_latent_surface`` does (DSS/core/cloud.py:442-513; csrc/rimls.cu, the rules are in
+    include/dss_b200.h and DESIGN.md), with the samples -- the input points and their unit normals -- fixed for the
+    whole call.  Each row fits the surface to its ``k`` nearest other points within ``r = min(16 avg k, 0.2)``, in at
+    most ``max_est_iters`` robust reweighting steps, moves along ``-f grad f``, and repeats up to ``max_proj_iters``
+    times while it moved farther than 5e-4.  A row without a neighbour at a positive distance within ``r`` stays.
+
+    ``points``, ``normals`` (P,3) float32 CUDA tensors, one cloud, or packed with ``first_idx`` / ``num_points`` (N,)
+    int64 as for ``knn_points_packed`` (gaps allowed).  ``k`` in [3, 31].  Float64 throughout, rounded once to float32;
+    the inputs are not modified and the normals are not updated.  Raises ValueError for non-finite points or normals.
+    Synchronises once, to read the clouds' bounding boxes; then the K-NN and one launch, the same bits on every call.
+    Rows outside every cloud are copied from ``points``.  No gradients."""
+    for name, v in (("max_proj_iters", max_proj_iters), ("max_est_iters", max_est_iters)):
+        if isinstance(v, bool) or int(v) != v or v < 0:
+            raise ValueError("%s must be a non-negative integer, got %r" % (name, v))
+    pts, nrm, fi, npts, idx, radius = _rimls_setup(points, normals, k, first_idx, num_points, 16.0)
+    out = pts.clone()
+    iterations = torch.zeros((pts.shape[0],), dtype=torch.int32, device=pts.device)
+    if pts.shape[0] > 0:
+        _lib.call("dss_project_to_surface", pts.device, pts, nrm, fi, npts, int(npts.shape[0]), pts.shape[0], idx,
+                  int(k), radius, int(max_proj_iters), int(max_est_iters), out, iterations)
+    return Projected(out, iterations)
 
 
 class MeshRender(NamedTuple):

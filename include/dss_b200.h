@@ -282,6 +282,38 @@ DSS_API int dss_upsample_points(dss_ctx *ctx, float *points, float *normals, flo
                                 const int64_t *first_idx, const int64_t *sizes, const int64_t *knn_num, int N, int64_t M,
                                 int rounds, int k, int32_t *parents, void *stream);
 
+/* ---- RIMLS projection and normal denoising -------------------------------------------------------------------------
+ * project_to_latent_surface and denoise_normals (DSS/core/cloud.py:442-553).  points, normals (P,3) f32; first_idx,
+ * num_points (N,) as for dss_knn_points (gaps allowed); knn_idx (P, k + 1) the dss_knn_points rows at K = k + 1,
+ * r = -1; 3 <= k <= 31; radius (N,) f64 the per-cloud r_n.  All arithmetic is float64; each output is rounded once to
+ * float32.  For row i of cloud n, with c_n = num_points[n]:
+ *  - neighbours: the K-NN row less i's own index (less the last entry when i is not in it), then less the entries
+ *    with squared distance d2_j = |p_i - q_j|^2 above r_n^2; dropped and -1 entries contribute nothing;
+ *  - unit normals: normalize(v) = v / max(|v|, 1e-12) (F.normalize: zero stays zero);
+ *  - every sum over the neighbours is the xor butterfly over 32 lanes (lane j holds neighbour j, the others 0):
+ *    the values v_0 .. v_31 become v_l + v_{l+16} for l < 16, then v_l + v_{l+8} for l < 8, ..., down to one;
+ *  - eps_denom(s) = sign(s) max(|s|, 1e-17), zero counted as positive.
+ * dss_denoise_normals (the caller's r_n = min(4 avg_n k, 0.2)): w_j = exp(-d2_j c_n / 2) exp(-((1 - n_i.n_j) /
+ * sigma)^2), zero where d2_j > 16 / (c_n / 2); out = normalize(sum w_j n_j / eps_denom(sum w_j)), or n_i when every
+ * w_j is zero.
+ * dss_project_to_surface (the caller's r_n = min(16 avg_n k, 0.2)): the samples q_j, n_j are the input's for the
+ * whole call.  inv = 1 / (16 d2min), d2min the smallest d2_j > 0; a row without one is written unchanged.  Then, from
+ * x = p_i, for t < max_proj_iters while the row is active: fx_j = (x - q_j).n_j; alpha_j = 1, f = 0, g = 0; for
+ * s < max_est_iters: when s >= 1, alpha'_j = exp(-(|n_j - g| / 0.5)^2) exp(-(fx_j - f)^2 inv / 4), and if
+ * max_j |alpha'_j - alpha_j| < 1e-4 the loop stops keeping f and g, otherwise alpha = alpha'; then phi_j =
+ * exp(-|x - q_j|^2 inv), w_j = phi_j alpha_j, gw_j = 2 (x - q_j) (inv phi_j) w_j, f = sum fx_j w_j / eps_denom(sum
+ * w_j), g = (sum gw_j fx_j - f sum gw_j + sum w_j n_j) / eps_denom(sum w_j).  x <- x - f g; the row stays active
+ * while |f g| > 5e-4.  out_points gets x, iterations (P,) int32 the number of outer iterations with f g != 0.
+ * Rows outside every range are not written.  One launch each, one warp per row; no scratch, no host
+ * synchronisation: capturable, and the same bits on every call. */
+DSS_API int dss_denoise_normals(dss_ctx *ctx, const float *points, const float *normals, const int64_t *first_idx,
+                                const int64_t *num_points, int N, int64_t P, const int32_t *knn_idx, int k,
+                                const double *radius, double sharpness_sigma, float *out_normals, void *stream);
+DSS_API int dss_project_to_surface(dss_ctx *ctx, const float *points, const float *normals, const int64_t *first_idx,
+                                   const int64_t *num_points, int N, int64_t P, const int32_t *knn_idx, int k,
+                                   const double *radius, int max_proj_iters, int max_est_iters, float *out_points,
+                                   int32_t *iterations, void *stream);
+
 /* ---- surface regularisers of the training step (SURVEY.md section 8(f) row 2) -----------------------------------
  * Replaces the torch bodies of ProjectionLoss (kind 0) and RepulsionLoss (kind 1) (DSS/training/losses.py:282-497) on
  * packed clouds (points, normals (P,3); first_idx, num_points as for dss_knn_points).  knn_dists (P, K-1+self_col) f32
