@@ -812,7 +812,7 @@ __global__ void __launch_bounds__(256) light_partials_kernel(const __grid_consta
             const V3 v = normalize3(sub3(cam, p), vlen);
             V3 diff = v3(0.f, 0.f, 0.f), spec = v3(0.f, 0.f, 0.f), g_nh = v3(0.f, 0.f, 0.f), g_v = v3(0.f, 0.f, 0.f);
             const LightTerm t = shade_light<true>(sL, g.light_type, g.shininess, p, nh, v, alb, gc, diff, spec, g_nh, g_v);
-            const V3 gvec = normalize3_bwd(t.d, t.dlen, t.g_d);
+            const V3 gvec = normalize3_bwd(t.d, t.dlen, t.draw, t.g_d);
             const V3 ga = v3(gc.x * alb.x, gc.y * alb.y, gc.z * alb.z);
             acc[0] += (double)gvec.x;
             acc[1] += (double)gvec.y;

@@ -20,14 +20,21 @@ __device__ __forceinline__ V3 add3(V3 a, V3 b) { return v3(a.x + b.x, a.y + b.y,
 __device__ __forceinline__ V3 sub3(V3 a, V3 b) { return v3(a.x - b.x, a.y - b.y, a.z - b.z); }
 __device__ __forceinline__ V3 mul3(V3 a, float s) { return v3(a.x * s, a.y * s, a.z * s); }
 __device__ __forceinline__ void store3(float *p, V3 a) { p[0] = a.x, p[1] = a.y, p[2] = a.z; }
-// F.normalize(x, p=2, dim=-1, eps=1e-6): x / max(|x|, eps); returns the (clamped) norm through `len`
-__device__ __forceinline__ V3 normalize3(V3 a, float &len) {
-    len = fmaxf(sqrtf(dot3(a, a)), 1e-6f);
+// F.normalize(x, p=2, dim=-1, eps=1e-6): x / max(|x|, eps); returns the clamped norm through `len` and, for the
+// backward, the unclamped one through `raw`
+__device__ __forceinline__ V3 normalize3(V3 a, float &len, float &raw) {
+    raw = sqrtf(dot3(a, a));
+    len = fmaxf(raw, 1e-6f);
     return mul3(a, 1.0f / len);
 }
-// gradient of y = normalize(x) given dL/dy (for |x| > eps; below it the map is linear: g / eps)
-__device__ __forceinline__ V3 normalize3_bwd(V3 y, float len, V3 gy) {
-    if (len <= 1e-6f) return mul3(gy, 1.0f / len);
+__device__ __forceinline__ V3 normalize3(V3 a, float &len) {
+    float raw;
+    return normalize3(a, len, raw);
+}
+// gradient of y = normalize(x) given dL/dy: the backward of x / clamp_min(|x|, eps), which passes the gradient through
+// the norm where |x| >= eps, at equality too (float32 F.normalize); only below eps is the map linear: g / eps
+__device__ __forceinline__ V3 normalize3_bwd(V3 y, float len, float raw, V3 gy) {
+    if (raw < 1e-6f) return mul3(gy, 1.0f / len);
     return mul3(sub3(gy, mul3(y, dot3(y, gy))), 1.0f / len);
 }
 
@@ -38,6 +45,7 @@ __device__ __forceinline__ V3 normalize3_bwd(V3 y, float len, V3 gy) {
 struct LightTerm {
     V3 d;          // normalised light direction (direction, or location - p)
     float dlen;    // clamped norm of the un-normalised one
+    float draw;    // its unclamped norm
     float lam;     // relu(n.d): factor of the diffuse colour
     float pw;      // (relu(v.r) [n.d > 0])^shininess: factor of the specular colour
     V3 g_d;        // BACKWARD: d L / d d
@@ -47,7 +55,7 @@ __device__ __forceinline__ LightTerm shade_light(const float *L, int light_type,
                                                  V3 alb, V3 gc, V3 &diff, V3 &spec, V3 &g_nh, V3 &g_v) {
     LightTerm t;
     const V3 draw = light_type ? sub3(v3(L[0], L[1], L[2]), p) : v3(L[0], L[1], L[2]);
-    t.d = normalize3(draw, t.dlen);
+    t.d = normalize3(draw, t.dlen, t.draw);
     const V3 d = t.d;
     const V3 cd = v3(L[3], L[4], L[5]), cs = v3(L[6], L[7], L[8]);
     const float cosang = dot3(nh, d);
@@ -88,20 +96,20 @@ template <bool BACKWARD, bool CAM_GRAD = false>
 __device__ __forceinline__ V3 shade_point(const float *sL, int n_lights, int light_type, float shininess, V3 amb, V3 p,
                                           V3 nrm, V3 alb, V3 cam, V3 gc, V3 &g_alb, V3 &g_nrm, V3 &g_pos,
                                           V3 *g_cam = nullptr) {
-    float nlen, vlen;
-    const V3 nh = normalize3(nrm, nlen);
-    const V3 v = normalize3(sub3(cam, p), vlen);
+    float nlen, vlen, nraw, vraw;
+    const V3 nh = normalize3(nrm, nlen, nraw);
+    const V3 v = normalize3(sub3(cam, p), vlen, vraw);
     V3 diff = v3(0.f, 0.f, 0.f), spec = v3(0.f, 0.f, 0.f);
     V3 g_nh = v3(0.f, 0.f, 0.f), g_v = v3(0.f, 0.f, 0.f);
     for (int l = 0; l < n_lights; ++l) {
         const LightTerm t = shade_light<BACKWARD>(sL + l * 9, light_type, shininess, p, nh, v, alb, gc, diff, spec, g_nh,
                                                   g_v);
-        if (BACKWARD && light_type) g_pos = sub3(g_pos, normalize3_bwd(t.d, t.dlen, t.g_d));   // d = normalize(loc - p)
+        if (BACKWARD && light_type) g_pos = sub3(g_pos, normalize3_bwd(t.d, t.dlen, t.draw, t.g_d));   // d = normalize(loc - p)
     }
     if (BACKWARD) {
         g_alb = add3(g_alb, v3(gc.x * (amb.x + diff.x), gc.y * (amb.y + diff.y), gc.z * (amb.z + diff.z)));
-        g_nrm = add3(g_nrm, normalize3_bwd(nh, nlen, g_nh));
-        const V3 g_cam_v = normalize3_bwd(v, vlen, g_v);                 // v = normalize(cam - p)
+        g_nrm = add3(g_nrm, normalize3_bwd(nh, nlen, nraw, g_nh));
+        const V3 g_cam_v = normalize3_bwd(v, vlen, vraw, g_v);           // v = normalize(cam - p)
         g_pos = sub3(g_pos, g_cam_v);
         if (CAM_GRAD) *g_cam = add3(*g_cam, g_cam_v);
     }
