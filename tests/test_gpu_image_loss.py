@@ -103,6 +103,12 @@ def reference(rgba, img, mask, lr=1.0, ls=1.0, ups=None):
 
 def compare(name, rgba, img, mask, lr=1.0, ls=1.0, ups=None, nan_ok=False):
     losses, grad = fused(rgba, img, mask, lr, ls, ups)
+    check(name, losses, grad, rgba, img, mask, lr, ls, ups, nan_ok)
+    return losses, grad
+
+
+def check(name, losses, grad, rgba, img, mask, lr=1.0, ls=1.0, ups=None, nan_ok=False):
+    """the three loss scalars and the RGBA gradient of a fused loss against `reference`, within the docstring's bounds"""
     rlosses, rgrad, iou_mag, mags = reference(rgba, img, mask, lr, ls, ups)
     worst = WORST.setdefault(name, [0.0, 0.0, 0.0])
     # gradient: NaN at the same places, the rest within the bound
@@ -130,7 +136,6 @@ def compare(name, rgba, img, mask, lr=1.0, ls=1.0, ups=None, nan_ok=False):
         assert e <= bound, (name, k, float(got), float(want), bound)
         worst[2] = max(worst[2], e / bound if bound > 0 else 0.0)
     print("%s: worst error / bound  rgb grad %.3f  alpha grad %.3f  losses %.3f" % (name, *worst))
-    return losses, grad
 
 
 # ---- 1. random images, every size --------------------------------------------------------------------------------
