@@ -20,7 +20,8 @@ import torch
 import torch.distributed as dist
 
 __all__ = ["shard_views", "assign_views", "view_costs_from_cameras", "GradSync", "pack_point_grads",
-           "unpack_point_grads", "allreduce_point_grads", "allreduce_visibility"]
+           "unpack_point_grads", "allreduce_point_grads", "allreduce_visibility", "replicas_differ", "check_replicas",
+           "agree_any"]
 
 
 def shard_views(n_views: int, world_size: int, rank: int) -> Tuple[int, int]:
@@ -168,3 +169,36 @@ def allreduce_visibility(visible: torch.Tensor, group=None):
     v = visible.to(torch.uint8)
     dist.all_reduce(v, op=dist.ReduceOp.MAX, group=group)
     return v.to(visible.dtype)
+
+
+def replicas_differ(tensors: Sequence[torch.Tensor], group=None) -> bool:
+    """True when the ranks' ``tensors`` (float32, any shapes, the same on every rank) are not the same bits on every
+    rank; every rank gets the same answer.  The float32 bit patterns, viewed as int32, and their complements go through
+    ONE all-reduce(MAX): max(~x) = ~min(x), so an element differs somewhere exactly when its max and min differ.  Bits,
+    not values: a 1-ulp difference, +0.0 against -0.0 and NaNs of other payloads all count.  Ends in a host
+    synchronisation (the answer is a Python bool); False without a group of more than one rank."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return False
+    bits = torch.cat([t.detach().reshape(-1).view(torch.int32) for t in tensors])
+    both = torch.cat([bits, ~bits])
+    dist.all_reduce(both, op=dist.ReduceOp.MAX, group=group)
+    n = bits.numel()
+    return bool((both[:n] != ~both[n:]).any())
+
+
+def check_replicas(named: Sequence[Tuple[str, torch.Tensor]], group=None):
+    """Raise RuntimeError on every rank when :func:`replicas_differ` finds the ``(name, tensor)`` pairs differ between
+    the ranks: replicas of a data-parallel model that drifted apart would otherwise train on silently."""
+    if replicas_differ([t for _, t in named], group):
+        raise RuntimeError("the ranks' replicas differ: %s are not the same bits on every rank"
+                           % ", ".join(name for name, _ in named))
+
+
+def agree_any(flag: bool, group=None) -> bool:
+    """True on every rank when ``flag`` is true on any rank: one all-reduce(MAX) of a host int32 over ``group``, which
+    must take CPU tensors (gloo).  It waits for the other ranks but adds no device synchronisation."""
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return bool(flag)
+    t = torch.tensor([1 if flag else 0], dtype=torch.int32)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
+    return bool(t.item())

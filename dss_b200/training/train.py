@@ -2,6 +2,7 @@
 trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trained cloud.
 
     python -m dss_b200.training.train --config CFG.yml [--exit-after S] [--max-it N]
+    torchrun --nproc-per-node G -m dss_b200.training.train --config CFG.yml [...] [--dist-backend nccl|gloo]
 
 - data: ``MVRData(data.data_dir)``, which is also the validation set.  Every epoch draws ``len(data)`` view indices
   with replacement from uniform weights (``WeightedSubsetRandomSampler``: ``torch.multinomial`` on the loop's own
@@ -28,34 +29,73 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   included: a resumed run computes what an uninterrupted one does.  (The reference starts a new epoch.)
 - ``--exit-after S`` saves ``model.pt`` and exits with status 3 once S seconds have passed (checked after every
   iteration; a negative S never exits); ``--max-it N`` saves ``model.pt`` and exits 0 after iteration N - 1.
+
+Several GPUs (``WORLD_SIZE`` > 1 in the environment, as torchrun sets it with ``RANK``, ``LOCAL_RANK``,
+``LOCAL_WORLD_SIZE``, ``MASTER_ADDR`` and ``MASTER_PORT``; ranks started by hand with the same variables work alike):
+every rank joins the group through ``init_method="env://"`` and runs the view-sharded step, an eager
+``TrainStep(..., grad_sync=GradSync())`` (``dss_b200.parallel``).  Without ``WORLD_SIZE``, or with 1, the loop above
+runs unchanged.
+- devices: ``--dist-backend nccl`` (the default) puts rank r on ``cuda:LOCAL_RANK`` and refuses, on every rank before
+  joining the group, a ``LOCAL_WORLD_SIZE`` larger than the number of visible GPUs; ``gloo`` puts it on
+  ``cuda:(LOCAL_RANK % device_count)``, for G ranks sharing one GPU.  The group has a timeout of
+  :data:`DIST_TIMEOUT`, so a rank that dies turns the others' next collective into an error, and every exit destroys it.
+- ``training.batch_size`` is the batch of one iteration over ALL the ranks, so G ranks solve the problem one GPU
+  solves with the same config, to the summation order of the render gradients and the image-loss sums.  Every rank draws
+  the same epoch order from ``training.seed`` and takes the same batch; :func:`deal_batch` deals its views by
+  ``assign_views`` over costs from the host camera matrices, and each rank stages and uploads only its own (a rank
+  dealt none runs the step's zero-view path).  Every rank keeps its own Adam, ``MultiStepLR`` and schedules: their
+  gradients are the same bits, so the replicas stay the same and no parameters are broadcast.
+- rank 0 alone writes the log, ``metrics.jsonl``, ``config.yaml``, the checkpoints and ``val/best.ply``, loads the
+  ground truth and validates; the other ranks print only errors.  The checks that can fail on the data or the config
+  run on every rank before the first collective, so a bad configuration fails every rank with the one-GPU message.
+- before every iteration that may write a checkpoint (``checkpoint_every``, ``backup_every``, ``validate_every``, the
+  time limit and the end) the ranks check that their points, normals and colours are the same bits
+  (``parallel.check_replicas``) and all raise if not; rank 0 logs "Replica check".
+- ``--exit-after``: the ranks agree on leaving after an iteration with one host all-reduce over a gloo group
+  (``parallel.agree_any``; no device synchronisation), and all exit with status 3 after rank 0 saved ``model.pt``: no
+  rank returns before rank 0's save is done, on any normal exit (one more host all-reduce).  torchrun reports a
+  worker's non-zero exit as a failure of the job and stops the other workers; the status 3 is that of every rank's
+  process.  Every checkpoint is written to ``<name>.tmp`` and moved over ``<name>``, so a killed writer leaves the
+  previous checkpoint whole.
+- every rank loads ``training.resume_from``; the checkpoint does not depend on G, so a run resumes on another number
+  of GPUs (mid-epoch included), and on the same number continues bit for bit.
 """
 import argparse
+import errno
 import json
 import math
 import os
 import sys
 import time
+from datetime import timedelta
 
+import numpy as np
 import torch
+import torch.distributed as dist
 import torch.nn.functional as F
 import yaml
 
 from ..core.camera import camera_matrices
 from ..core.cloud import PointClouds3D
 from ..ops import chamfer_distance, evaluate_2d
+from ..parallel import GradSync, agree_any, assign_views, check_replicas, view_costs_from_cameras
 from ..utils.create_mvr_data import ico_sphere, sample_points_from_mesh
 from ..utils.dataset import MVRData
 from ..utils.evaluate import p2f_stats
 from ..utils.io import read_mesh, save_ply
 from .config import (EVAL_SAMPLINGS, IMAGE_METRICS, check_config, load_config, selection_metric, splat_params,
                      step_settings)
-from .step import GraphedTrainStep
+from .step import GraphedTrainStep, TrainStep
 
 __all__ = ["radii_backward_scaler", "compound_lambda_proj", "initial_cloud", "make_optimizer", "make_lr_scheduler",
-           "ground_truth_cloud", "load_data", "Trainer", "main"]
+           "ground_truth_cloud", "check_ground_truth", "load_data", "dist_env", "rank_device", "deal_batch", "Trainer",
+           "main"]
 
 EXIT_TIME_LIMIT = 3        # train_mvr.py:221-227
 EVAL_SEED = 0              # the fixed draw of the ground-truth samples
+# a collective waits this long for the other ranks before it fails: longer than rank 0's validation of a large cloud,
+# while the others wait at their next collective
+DIST_TIMEOUT = timedelta(minutes=15)
 
 
 def radii_backward_scaler(init, steps, it):
@@ -108,8 +148,7 @@ def ground_truth_cloud(data, data_dir, n_eval_points, device, sampling="uniform"
     drawn once from a fixed seed, and with "poisson_disk" the reference's ``get_pointclouds(num_points=n_eval_points)``:
     geodesic Poisson-disk samples of that mesh (:meth:`MVRData.get_pointclouds`).  Only those compare with the
     reference's own chamfer values."""
-    if sampling not in EVAL_SAMPLINGS:
-        raise ValueError("training.eval_sampling must be one of %s, got %r" % (", ".join(EVAL_SAMPLINGS), sampling))
+    check_ground_truth(data, data_dir, n_eval_points, sampling)
     stored = data.get_pointclouds()
     n = int(n_eval_points)
     if n <= 0 or n == stored.points_packed().shape[0]:
@@ -123,6 +162,23 @@ def ground_truth_cloud(data, data_dir, n_eval_points, device, sampling="uniform"
                                    n, generator=g)
 
 
+def check_ground_truth(data, data_dir, n_eval_points, sampling="uniform"):
+    """the errors :func:`ground_truth_cloud` would raise on these arguments, without loading or sampling anything: an
+    unknown ``sampling``, and a missing ``<data_dir>/mesh.obj`` when the samples are drawn from it.  (Every rank of a
+    sharded run checks this at start, while only rank 0 loads the ground truth.)"""
+    if sampling not in EVAL_SAMPLINGS:
+        raise ValueError("training.eval_sampling must be one of %s, got %r" % (", ".join(EVAL_SAMPLINGS), sampling))
+    n = int(n_eval_points)
+    if n <= 0 or n == len(data.data_dict["points"]):
+        return
+    if sampling == "poisson_disk":
+        data.sampled_mesh(n)
+        return
+    mesh = os.path.join(data_dir, "mesh.obj")
+    if not os.path.isfile(mesh):
+        raise FileNotFoundError(errno.ENOENT, os.strerror(errno.ENOENT), mesh)      # what reading it would raise
+
+
 def load_data(cfg):
     """the configuration's ``MVRData`` (its ``data`` block), which must have images and masks"""
     dc = cfg["data"]
@@ -133,40 +189,96 @@ def load_data(cfg):
     return data
 
 
-class _Log:
-    """lines to ``<out>/<logfile>`` (and stdout), JSON records to ``<out>/metrics.jsonl``"""
+def dist_env(environ=None):
+    """``{"rank", "world", "local_rank", "local_world"}`` from the variables torchrun sets (``RANK``, ``WORLD_SIZE``,
+    ``LOCAL_RANK``, ``LOCAL_WORLD_SIZE``; the local ones default to the global), or None when ``WORLD_SIZE`` is unset or
+    1: the single-GPU loop."""
+    env = os.environ if environ is None else environ
+    world = int(env.get("WORLD_SIZE", "1") or 1)
+    if world <= 1:
+        return None
+    rank = int(env["RANK"])
+    return {"rank": rank, "world": world, "local_rank": int(env.get("LOCAL_RANK", rank)),
+            "local_world": int(env.get("LOCAL_WORLD_SIZE", world))}
 
-    def __init__(self, out_dir, logfile):
-        self.text = open(os.path.join(out_dir, logfile), "a")
-        self.metrics = open(os.path.join(out_dir, "metrics.jsonl"), "a")
+
+def rank_device(backend, local_rank, local_world, n_gpus):
+    """The device of a rank: ``cuda:local_rank`` over nccl, which needs a GPU per local rank (a RuntimeError
+    otherwise, raised before the rank joins the group, so that every rank fails alike and none waits);
+    ``cuda:(local_rank % n_gpus)`` over gloo, so that several ranks can share a GPU."""
+    if n_gpus < 1:
+        raise RuntimeError("the training loop needs a CUDA device (sm_90a); rank %d sees none" % local_rank)
+    if backend == "nccl":
+        if local_world > n_gpus:
+            raise RuntimeError("--dist-backend nccl runs one rank per GPU, but %d local ranks share %d visible GPU%s; "
+                               "start at most %d, or use --dist-backend gloo to share GPUs"
+                               % (local_world, n_gpus, "" if n_gpus == 1 else "s", n_gpus))
+        return torch.device("cuda", local_rank)
+    if backend == "gloo":
+        return torch.device("cuda", local_rank % n_gpus)
+    raise ValueError("--dist-backend must be nccl or gloo, got %r" % (backend,))
+
+
+def deal_batch(camera_mat, idx, world):
+    """The views of batch ``idx`` (indices into the data, repeats allowed) dealt to ``world`` ranks:
+    ``assign_views(view_costs_from_cameras(camera_mat[idx]), world)``, a list per rank of the data indices it renders.
+    Every position of ``idx`` goes to exactly one rank; a rank gets none when ``len(idx) < world``.  ``camera_mat``: the
+    data's (V,4,4) host world-to-view matrices, so dealing needs no device round trip, and every rank deals alike."""
+    idx = [int(i) for i in idx]
+    mats = torch.from_numpy(np.asarray(camera_mat, dtype=np.float32)[np.asarray(idx, dtype=np.int64)].reshape(-1, 4, 4))
+    return [[idx[j] for j in part] for part in assign_views(view_costs_from_cameras(mats).tolist(), world)]
+
+
+class _Log:
+    """lines to ``<out>/<logfile>`` (and stdout), JSON records to ``<out>/metrics.jsonl``; ``quiet``: neither (the
+    ranks other than 0)"""
+
+    def __init__(self, out_dir, logfile, quiet=False):
+        self.quiet = quiet
+        if not quiet:
+            self.text = open(os.path.join(out_dir, logfile), "a")
+            self.metrics = open(os.path.join(out_dir, "metrics.jsonl"), "a")
 
     def info(self, msg):
+        if self.quiet:
+            return
         line = "%s %s" % (time.strftime("%Y-%m-%d %H:%M:%S"), msg)
         print(line, flush=True)
         self.text.write(line + "\n")
         self.text.flush()
 
     def record(self, rec):
+        if self.quiet:
+            return
         self.metrics.write(json.dumps(rec) + "\n")
         self.metrics.flush()
 
     def close(self):
-        self.text.close()
-        self.metrics.close()
+        if not self.quiet:
+            self.text.close()
+            self.metrics.close()
 
 
 class Trainer:
     """The loop's state and one iteration at a time (see the module docstring).  ``Trainer(cfg).run(exit_after,
-    max_it)`` returns the process exit status."""
+    max_it)`` returns the process exit status.  ``grad_sync``: a ``GradSync`` of world size G > 1 makes this rank one
+    of G that shard every batch's views (the process group initialised, ``device`` this rank's GPU)."""
 
-    def __init__(self, cfg, device="cuda"):
+    def __init__(self, cfg, device="cuda", grad_sync=None):
         self.cfg = cfg
         self.dev = torch.device(device)
+        self.sync = grad_sync if grad_sync is not None and grad_sync.world_size > 1 else None
+        self.world = 1 if self.sync is None else self.sync.world_size
+        self.rank = 0 if self.sync is None else dist.get_rank(self.sync.group)
+        self.lead = self.rank == 0
+        self.host_group = None          # the gloo group of the exit agreement, made by run() when it needs one
+        self._checked_it = None         # the iteration the replica guard last ran at
         tr, dc = cfg["training"], cfg["data"]
         self.out_dir = os.path.join(str(tr["out_dir"]), str(cfg["name"]))
         self.val_dir = os.path.join(self.out_dir, "val")
-        os.makedirs(self.val_dir, exist_ok=True)
-        self.log = _Log(self.out_dir, tr["logfile"])
+        if self.lead:
+            os.makedirs(self.val_dir, exist_ok=True)
+        self.log = _Log(self.out_dir, tr["logfile"], quiet=not self.lead)
         # ---- data: images in host memory, cameras and lights of every view on the device
         self.data = load_data(cfg)
         V = len(self.data)
@@ -178,8 +290,9 @@ class Trainer:
             mesh_path = os.path.join(dc["data_dir"], "mesh.obj")
             if not os.path.isfile(mesh_path):
                 raise ValueError("model_selection_metric p2f_avg measures against %s, which does not exist" % mesh_path)
-            verts, faces = read_mesh(mesh_path)
-            self.mesh = (torch.from_numpy(verts).float().to(self.dev), torch.from_numpy(faces).to(self.dev))
+            if self.lead:
+                verts, faces = read_mesh(mesh_path)
+                self.mesh = (torch.from_numpy(verts).float().to(self.dev), torch.from_numpy(faces).to(self.dev))
         self.light_cls, self.light_props = lights
         cams = self.data.get_cameras()
         proj, _ = camera_matrices(cams)
@@ -197,6 +310,8 @@ class Trainer:
                 raise ValueError("model_selection_metric %s measures against the data's cloud, but %s has no %s; "
                                  "select by iou or psnr to train without one"
                                  % (self.metric, os.path.join(dc["data_dir"], dc["data_dict"]), " / ".join(missing)))
+            check_ground_truth(self.data, dc["data_dir"], tr["n_eval_points"], tr.get("eval_sampling", "uniform"))
+        if self.metric not in IMAGE_METRICS and self.lead:
             self.gt = ground_truth_cloud(self.data, dc["data_dir"], tr["n_eval_points"], self.dev,
                                          tr.get("eval_sampling", "uniform"))
         # ---- state: fresh, then whatever the checkpoint holds
@@ -222,11 +337,13 @@ class Trainer:
             self.lambda_dr_proj = float(ckpt["schedule"]["lambda_dr_proj"])
             self.params = self.params._replace(radii_backward_scaler=float(ckpt["schedule"]["radii_backward_scaler"]))
             self.log.info("resumed from %s at it=%d, epoch %d" % (ckpt_path, self.it, self.epoch_it))
-        with open(os.path.join(self.out_dir, "config.yaml"), "w") as f:
-            yaml.safe_dump(cfg, f, sort_keys=False)
+        if self.lead:
+            with open(os.path.join(self.out_dir, "config.yaml"), "w") as f:
+                yaml.safe_dump(cfg, f, sort_keys=False)
         # the step is captured on any batch of the right shape: the capture's warm-up steps leave the cloud unchanged,
-        # and every iteration loads its own batch first
-        self._build(points, normals, colours, self._batch(list(range(self.batch_size))), ckpt)
+        # and every iteration loads its own batch first (the sharded step is eager and takes none)
+        self._build(points, normals, colours,
+                    self._batch(list(range(self.batch_size))) if self.sync is None else None, ckpt)
 
     # ---- pieces ------------------------------------------------------------------------------------------------------
     def _batch(self, idx):
@@ -244,7 +361,10 @@ class Trainer:
     def _build(self, points, normals, colours, batch, ckpt):
         s = dict(self.settings)
         learn, s["lambda_dr_proj"] = s.pop("learn"), self.lambda_dr_proj
-        self.step = GraphedTrainStep(points, normals, colours, self.params, *batch, learn=learn, **s)
+        if self.sync is None:
+            self.step = GraphedTrainStep(points, normals, colours, self.params, *batch, learn=learn, **s)
+        else:
+            self.step = TrainStep(points, normals, colours, self.params, learn=learn, grad_sync=self.sync, **s)
         self.opt = make_optimizer({"points": self.step.points, "normals": self.step.normals,
                                    "colours": self.step.colours})
         self.lr_sched = make_lr_scheduler(self.opt, self.cfg)
@@ -287,9 +407,27 @@ class Trainer:
             _, ev["p2f_avg"], ev["p2f_std"] = p2f_stats(points, self.mesh)
         return ev
 
+    def _validate(self, metric):
+        """validation and model selection (rank 0): the log line, and on improvement ``model_best.pt`` and
+        ``val/best.ply``"""
+        ev = self.evaluate()
+        self.log.info("Validation metric (%s): %.4g  (%s)" % (metric, ev[metric], json.dumps(ev)))
+        if self.sign * (ev[metric] - self.best) > 0:
+            self.best = ev[metric]
+            self.log.info("New best model (loss %.4g)" % self.best)
+            self.save("model_best.pt")
+            points, normals = self.cloud()
+            save_ply(os.path.join(self.val_dir, "best.ply"), points.cpu().numpy(), normals=normals.cpu().numpy())
+
     def save(self, name):
+        """``<out>/name``, replaced whole (rank 0 alone writes; the other ranks return)"""
+        if not self.lead:
+            return
         s = self.step
         P0 = s.points.shape[0]
+        # written next to the target and moved over it: a process killed mid-write leaves the previous file whole
+        path = os.path.join(self.out_dir, name)
+        tmp = path + ".tmp"
         torch.save({
             "model": {"points": s.points.detach()[None].clone(), "normals": s.normals.detach()[None].clone(),
                       "colors": s.colours.detach()[None].clone(),
@@ -299,7 +437,40 @@ class Trainer:
             "schedule": {"radii_backward_scaler": self.params.radii_backward_scaler,
                          "lambda_dr_proj": self.lambda_dr_proj},
             "sampler": self.gen.get_state(), "epoch_order": list(self.order), "epoch_pos": self.pos,
-        }, os.path.join(self.out_dir, name))
+        }, tmp)
+        os.replace(tmp, path)
+
+    def check_replicas(self):
+        """the replica guard of a sharded run, before an iteration's checkpoints: every rank raises unless the ranks'
+        points, normals and colours are the same bits (one all-reduce, one host synchronisation).  Once per
+        iteration; nothing on one GPU."""
+        if self.sync is None or self._checked_it == self.it:
+            return
+        s = self.step
+        check_replicas((("points", s.points), ("normals", s.normals), ("colours", s.colours)), self.sync.group)
+        self._checked_it = self.it
+        self.log.info("Replica check: the %d ranks hold the same points, normals and colours" % self.world)
+
+    def _out_of_time(self, exit_after, t0):
+        """whether to leave after this iteration; a sharded run's ranks agree (any rank's clock decides for all)"""
+        if exit_after is None or exit_after < 0:
+            return False
+        over = time.time() - t0 >= exit_after
+        if self.sync is None:
+            return over
+        return agree_any(over, self._host_group())
+
+    def _host_group(self):
+        """the gloo group of the host-side agreements, made on first use (by every rank at the same point)"""
+        if self.host_group is None:
+            self.host_group = dist.new_group(backend="gloo", timeout=DIST_TIMEOUT)
+        return self.host_group
+
+    def _leave_together(self):
+        """on a sharded run's exit, after rank 0's last save: no rank returns before rank 0 has written, since a
+        launcher that sees one worker exit non-zero (torchrun, on the time limit's status 3) stops the others"""
+        if self.sync is not None:
+            agree_any(False, self._host_group())
 
     # ---- the loop ----------------------------------------------------------------------------------------------------
     def run(self, exit_after=600.0, max_it=None):
@@ -322,13 +493,16 @@ class Trainer:
                 self.pos += bs
                 self.it += 1
                 self._schedule()
-                self.step.load(*self._batch(idx))
-                if self.step.stale():
-                    self.step.capture()
-                loss = self.step.replay()
+                if self.sync is None:
+                    self.step.load(*self._batch(idx))
+                    if self.step.stale():
+                        self.step.capture()
+                    loss = self.step.replay()
+                else:
+                    loss = self.step(*self._batch(deal_batch(self.data.camera_mat, idx, self.world)[self.rank]))
                 self.opt.step()
                 it = self.it
-                if print_every > 0 and it % print_every == 0:
+                if self.lead and print_every > 0 and it % print_every == 0:
                     vals = {k: float(v) for k, v in loss.items()}
                     self.log.info("[Epoch %02d] it=%03d, loss=%.4f, time=%.4f " % (self.epoch_it, it, vals["loss"],
                                                                                    time.time() - t0b)
@@ -336,26 +510,26 @@ class Trainer:
                     self.log.record(dict(it=it, epoch=self.epoch_it, time=time.time() - t0, **vals))
                     t0b = time.time()
                 if it > 0 and checkpoint_every > 0 and it % checkpoint_every == 0:
+                    self.check_replicas()
                     self.log.info("Saving checkpoint")
                     self.save("model.pt")
                 if it > 0 and backup_every > 0 and it % backup_every == 0:
+                    self.check_replicas()
                     self.log.info("Backup checkpoint")
                     self.save("model_%d.pt" % it)
                 if it > 0 and validate_every > 0 and it % validate_every == 0:
-                    ev = self.evaluate()
-                    self.log.info("Validation metric (%s): %.4g  (%s)" % (metric, ev[metric], json.dumps(ev)))
-                    if self.sign * (ev[metric] - self.best) > 0:
-                        self.best = ev[metric]
-                        self.log.info("New best model (loss %.4g)" % self.best)
-                        self.save("model_best.pt")
-                        points, normals = self.cloud()
-                        save_ply(os.path.join(self.val_dir, "best.ply"), points.cpu().numpy(),
-                                 normals=normals.cpu().numpy())
-                if exit_after is not None and exit_after >= 0 and time.time() - t0 >= exit_after:
+                    self.check_replicas()             # before rank 0 may write model_best.pt
+                    if self.lead:
+                        self._validate(metric)
+                if self._out_of_time(exit_after, t0):
+                    self.check_replicas()
                     self.log.info("Time limit reached. Exiting.")
                     self.save("model.pt")
+                    self._leave_together()
                     return EXIT_TIME_LIMIT
+            self.check_replicas()
             self.save("model.pt")
+            self._leave_together()
             return 0
         finally:
             self.log.close()
@@ -367,11 +541,25 @@ def main(argv=None):
     p.add_argument("--exit-after", type=float, default=600,
                    help="save model.pt and exit with status 3 after this many seconds (negative: never)")
     p.add_argument("--max-it", type=int, default=None, help="save model.pt and exit 0 after this many iterations")
+    p.add_argument("--dist-backend", choices=("nccl", "gloo"), default="nccl",
+                   help="under torchrun (WORLD_SIZE > 1): nccl, one GPU per rank, or gloo, ranks sharing GPUs")
     args = p.parse_args(argv)
-    if not torch.cuda.is_available():
-        raise RuntimeError("the training loop needs a CUDA device (sm_90a)")
+    env = dist_env()
+    if env is None:
+        if not torch.cuda.is_available():
+            raise RuntimeError("the training loop needs a CUDA device (sm_90a)")
+        cfg = load_config(args.config)
+        return Trainer(cfg).run(exit_after=args.exit_after, max_it=args.max_it)
+    # refused here, before the group is joined, a bad device count fails every rank at once
+    dev = rank_device(args.dist_backend, env["local_rank"], env["local_world"], torch.cuda.device_count())
     cfg = load_config(args.config)
-    return Trainer(cfg).run(exit_after=args.exit_after, max_it=args.max_it)
+    torch.cuda.set_device(dev)
+    dist.init_process_group(args.dist_backend, init_method="env://", rank=env["rank"], world_size=env["world"],
+                            timeout=DIST_TIMEOUT)
+    try:
+        return Trainer(cfg, dev, grad_sync=GradSync()).run(exit_after=args.exit_after, max_it=args.max_it)
+    finally:
+        dist.destroy_process_group()
 
 
 if __name__ == "__main__":

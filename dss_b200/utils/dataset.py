@@ -92,14 +92,20 @@ class MVRData:
 
     def pinned_batch(self, indices):
         """Views `indices` stacked in PINNED host memory, ready for one non-blocking copy per tensor:
-        {"camera_mat": (B,4,4) [, "img.rgb": (B,3,H,W), "img.mask": (B,1,H,W)]} (what a training step uploads)."""
+        {"camera_mat": (B,4,4) [, "img.rgb": (B,3,H,W), "img.mask": (B,1,H,W)]} (what a training step uploads).
+        An empty ``indices`` gives B = 0 tensors of the same trailing shapes and dtypes (a rank of a view-sharded
+        step may be dealt no views)."""
         idx = [int(i) % len(self) for i in indices]
         pin = lambda t: t.pin_memory() if torch.cuda.is_available() else t
-        out = {"camera_mat": pin(torch.from_numpy(np.stack([self.camera_mat[i] for i in idx])))}
-        if self.images is not None:
-            out["img.rgb"] = pin(torch.stack([torch.as_tensor(self.images[i]) for i in idx]))
-        if self.masks is not None:
-            out["img.mask"] = pin(torch.stack([torch.as_tensor(self.masks[i]) for i in idx]))
+        out = {"camera_mat": pin(torch.from_numpy(self.camera_mat[np.asarray(idx, dtype=np.int64)]))}
+        for key, arr in (("img.rgb", self.images), ("img.mask", self.masks)):
+            if arr is None:
+                continue
+            if idx:
+                out[key] = pin(torch.stack([torch.as_tensor(arr[i]) for i in idx]))
+            else:
+                first = torch.as_tensor(arr[0])
+                out[key] = pin(first.new_empty((0,) + tuple(first.shape)))
         return out
 
     def __getitem__(self, idx):
@@ -145,10 +151,7 @@ class MVRData:
             return PointClouds3D([points], [t("normals")], [colors])
         n = int(num_points)
         if n not in self._poisson_disk:
-            mesh = None if self.data_dir is None else os.path.join(self.data_dir, "mesh.obj")
-            if mesh is None or not os.path.isfile(mesh):
-                raise ValueError("get_pointclouds(%d) samples the data's mesh.obj, which %s" % (
-                    n, "a data_dict file has not" if mesh is None else "does not exist: %s" % mesh))
+            mesh = self.sampled_mesh(n)
             from ..ops import sample_points_poisson_disk
             from .io import read_mesh
             verts, faces = read_mesh(mesh)
@@ -158,6 +161,15 @@ class MVRData:
             self._poisson_disk[n] = (s.points.cpu(), s.normals.cpu())
         p, nrm = self._poisson_disk[n]
         return PointClouds3D([p.clone()], [nrm.clone()], [torch.ones_like(p)])
+
+    def sampled_mesh(self, num_points):
+        """the path of ``<data_dir>/mesh.obj``, which ``get_pointclouds(num_points)`` samples; ValueError when it is
+        missing (checked without sampling, so that a caller can refuse early)"""
+        mesh = None if self.data_dir is None else os.path.join(self.data_dir, "mesh.obj")
+        if mesh is None or not os.path.isfile(mesh):
+            raise ValueError("get_pointclouds(%d) samples the data's mesh.obj, which %s" % (
+                int(num_points), "a data_dict file has not" if mesh is None else "does not exist: %s" % mesh))
+        return mesh
 
     def get_cameras(self, camera_mat=None, **camera_params):
         """``FoVPerspectiveCameras`` with R, T taken from ``camera_mat`` ((n,4,4) or (4,4); default: all images)

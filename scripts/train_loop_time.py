@@ -1,17 +1,24 @@
 """Time the training loop's pieces: ops.chamfer_distance (csrc/chamfer.cu) at 8000 ground-truth points against 5 000,
 100 000 and 1 000 000 model points with normals, next to a torch brute force (torch.cdist in chunks on the GPU), and the
-loop of dss_b200.training.train at configs/dss.yml's settings (5000 points, 8 views per batch, 512^2) next to bare
-GraphedTrainStep.replay() on the same batches.
+loop of dss_b200.training.train at configs/dss.yml's settings (by default 5000 points, 8 views per batch, 512^2) next to
+bare GraphedTrainStep.replay() on the same batches.
 
-    python scripts/train_loop_time.py [--iters 20] [--loop-its 200] [--out results.json]
+    python scripts/train_loop_time.py [--iters 20] [--loop-its 200] [--points 5000] [--batch 8] [--ranks G]
+                                      [--out results.json]
 
 CUDA events around each chamfer call, median after warm-up.  The loop's rate is taken between two of its own logged
-records (each ends in a host synchronisation), after the capture and a warm-up.  Prints one JSON line with the card name
-and its power limit."""
+records (each ends in a host synchronisation), after the capture and a warm-up.  ``--ranks G`` > 1 runs the loop as G
+NCCL ranks, one process and one GPU each, started with torchrun's variables (the view-sharded eager step; no bare
+replays), and reports rank 0's rate; a G larger than the number of visible GPUs is refused.  The data has
+max(64, batch) views.  Prints one JSON line with the card name and its power limit."""
 import argparse
 import json
 import os
 import shutil
+import signal
+import socket
+import subprocess
+import sys
 import tempfile
 import time
 
@@ -55,7 +62,45 @@ def chamfer_times(dev, warmup, iters):
     return out
 
 
-def loop_times(dev, loop_its, tmp):
+def _run_ranks(cfg_path, ranks, max_it, tmp, timeout=3600):
+    """the loop as ``ranks`` NCCL ranks, one GPU each, as torchrun starts them, each in its own session with its
+    output in a file under ``tmp``.  When a rank fails or the time runs out every rank still running is killed, so
+    none is left waiting at a collective; raises then."""
+    s = socket.socket()
+    s.bind(("127.0.0.1", 0))
+    port = s.getsockname()[1]
+    s.close()
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    procs, logs = [], []
+    for r in range(ranks):
+        env = dict(os.environ, RANK=str(r), LOCAL_RANK=str(r), WORLD_SIZE=str(ranks), LOCAL_WORLD_SIZE=str(ranks),
+                   MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+        env["PYTHONPATH"] = root + os.pathsep + env.get("PYTHONPATH", "")
+        logs.append(open(os.path.join(tmp, "rank%d.log" % r), "w+"))
+        procs.append(subprocess.Popen([sys.executable, "-m", "dss_b200.training.train", "--config", cfg_path,
+                                       "--exit-after", "-1", "--max-it", str(max_it), "--dist-backend", "nccl"],
+                                      cwd=root, env=env, stdout=logs[-1], stderr=subprocess.STDOUT,
+                                      start_new_session=True))
+    deadline = time.time() + timeout
+    try:
+        while any(p.poll() is None for p in procs):
+            if any(p.poll() not in (None, 0) for p in procs) or time.time() > deadline:
+                break
+            time.sleep(0.2)
+    finally:
+        for p in procs:
+            if p.poll() is None:
+                os.killpg(p.pid, signal.SIGKILL)
+                p.wait()
+    for r, (p, log) in enumerate(zip(procs, logs)):
+        log.seek(0)
+        out = log.read()
+        log.close()
+        if p.returncode != 0:
+            raise RuntimeError("rank %d exited with %d:\n%s" % (r, p.returncode, out))
+
+
+def loop_times(dev, loop_its, tmp, points=5000, batch=8, ranks=1):
     from dss_b200.training.config import load_config
     from dss_b200.training.train import Trainer
     from dss_b200.utils.create_mvr_data import main as create
@@ -63,31 +108,40 @@ def loop_times(dev, loop_its, tmp):
     from tests.test_mesh_data import torus
     verts, faces = torus(nu=192, nv=96)
     save_obj(os.path.join(tmp, "torus.obj"), verts.numpy(), faces.numpy())
+    n_views = max(64, batch)
     data_dir = create(["--points", os.path.join(tmp, "torus.obj"), "--output", os.path.join(tmp, "data"),
-                       "--num_cameras", "64", "--image-size", "512", "--tri_color_light", "--point_lights"])[0]
+                       "--num_cameras", str(n_views), "--image-size", "512", "--tri_color_light", "--point_lights"])[0]
     cfg_path = os.path.join(tmp, "dss.yml")
     warm = 40
     with open(cfg_path, "w") as f:
         yaml.safe_dump({
             "name": "time", "data": {"data_dir": data_dir},
-            "model": {"model_kwargs": {"n_points_per_cloud": 5000, "learn_colors": False}},
+            "model": {"model_kwargs": {"n_points_per_cloud": points, "learn_colors": False}},
             "renderer": {"raster_params": {"Vrk_invariant": True, "Vrk_isotropic": False, "clip_pts_grad": 0.05,
                                            "cutoff_threshold": 1.0, "depth_merging_threshold": 0.05,
                                            "image_size": 512, "points_per_pixel": 5, "radii_backward_scaler": 5}},
-            "training": {"out_dir": os.path.join(tmp, "out"), "batch_size": 8, "lambda_dr_proj": 0.01,
+            "training": {"out_dir": os.path.join(tmp, "out"), "batch_size": batch, "lambda_dr_proj": 0.01,
                          "lambda_dr_repel": 0.0, "steps_dss_backward_radii": 200, "print_every": warm,
                          "validate_every": 0, "checkpoint_every": 0}}, f)
-    t = Trainer(load_config(cfg_path))
-    t.run(exit_after=-1, max_it=warm + loop_its + 1)
-    with open(os.path.join(t.out_dir, "metrics.jsonl")) as f:
+    cfg = load_config(cfg_path)
+    t = None
+    if ranks == 1:
+        t = Trainer(cfg)
+        t.run(exit_after=-1, max_it=warm + loop_its + 1)
+    else:
+        _run_ranks(cfg_path, ranks, warm + loop_its + 1, tmp)
+    with open(os.path.join(cfg["training"]["out_dir"], "time", "metrics.jsonl")) as f:
         recs = [json.loads(line) for line in f]
     first = next(r for r in recs if r["it"] >= warm)
     last = recs[-1]
-    res = {"loop_it_per_s": (last["it"] - first["it"]) / (last["time"] - first["time"]),
+    res = {"ranks": ranks, "loop_points": points, "loop_batch": batch,
+           "loop_it_per_s": (last["it"] - first["it"]) / (last["time"] - first["time"]),
            "loop_its_timed": last["it"] - first["it"]}
+    if t is None:
+        return res
     # bare replays of the same step on batches already on the device
     step = t.step
-    batches = [t._batch(t.order[i:i + 8]) for i in range(0, 64, 8)]
+    batches = [t._batch(t.order[i:i + batch]) for i in range(0, n_views - batch + 1, batch)]
     torch.cuda.synchronize()
     for b in batches:
         step.load(*b)
@@ -102,7 +156,7 @@ def loop_times(dev, loop_its, tmp):
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     ev = t.evaluate()
-    res["validation_ms_5000_vs_8000"] = (time.perf_counter() - t0) * 1e3
+    res["validation_ms_%d_vs_8000" % points] = (time.perf_counter() - t0) * 1e3
     res["chamfer_point_at_end"] = ev["chamfer_point"]
     return res
 
@@ -112,13 +166,20 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--loop-its", type=int, default=200)
+    ap.add_argument("--points", type=int, default=5000, help="the loop's cloud size")
+    ap.add_argument("--batch", type=int, default=8, help="the loop's views per batch (over all the ranks)")
+    ap.add_argument("--ranks", type=int, default=1, help="run the loop as this many NCCL ranks, one GPU each")
     ap.add_argument("--out", default=None)
     opt = ap.parse_args()
+    have = torch.cuda.device_count()
+    if opt.ranks < 1 or opt.ranks > have:
+        raise SystemExit("--ranks %d: the loop runs one rank per GPU and %d GPU%s visible"
+                         % (opt.ranks, have, " is" if have == 1 else "s are"))
     dev = torch.device("cuda:0")
     res = chamfer_times(dev, opt.warmup, opt.iters)
     tmp = tempfile.mkdtemp(prefix="dss_loop_time_")
     try:
-        res.update(loop_times(dev, opt.loop_its, tmp))
+        res.update(loop_times(dev, opt.loop_its, tmp, opt.points, opt.batch, opt.ranks))
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
     gpu = card()
