@@ -94,6 +94,8 @@ _SIGNATURES = {
     "dss_denoise_normals": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int64, vp, C.c_int, vp, C.c_double, vp, vp]),
     "dss_project_to_surface": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int64, vp, C.c_int, vp, C.c_int, C.c_int,
                                          vp, vp, vp]),
+    "dss_l0_smooth": (C.c_int, [vp, vp, C.c_int, C.POINTER(C.c_int64), C.c_int, C.c_int, C.c_int, C.c_int, C.c_double,
+                                vp, vp]),
     "dss_surface_regulariser": (C.c_int, [vp, C.c_int, vp, vp, vp, vp, C.c_int, C.c_int64, vp, vp, C.c_int, C.c_int,
                                           vp, vp, vp, vp, C.c_float, C.c_float, vp, vp, vp]),
     "dss_image_loss_forward": (C.c_int, [vp, vp, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,

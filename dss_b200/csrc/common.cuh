@@ -94,6 +94,7 @@ enum BufId {
     BUF_IMAGE_METRICS,  // per-block fp64 partial sums of the image metrics, and the finish's block counter
     BUF_NORMALS,      // normal estimation: unoriented normals, the spanning forest's state, the Euler tours and flags
     BUF_UPSAMPLE,     // upsampling: the round's K-NN rows, select keys, chosen neighbours, flags and their scan, histograms
+    BUF_L0,           // L0 smoothing: the rows' complex transforms, twiddles, float64 input and estimate planes, keep flags
     NUM_BUFS
 };
 

@@ -24,7 +24,7 @@ from . import _lib
 __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_points", "preprocess_points",
            "point_filters", "point_filters_no_views", "set_point_filters", "local_frames", "PointNormals",
            "estimate_normals", "Outliers", "outlier_ratio", "Upsampled", "upsample_schedule", "upsample_points",
-           "denoise_normals", "Projected", "project_to_surface", "MeshRender", "render_mesh", "chamfer_distance",
+           "denoise_normals", "Projected", "project_to_surface", "l0_smooth", "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
            "ImageMetrics", "image_metrics", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
 
@@ -819,6 +819,62 @@ def project_to_surface(points, normals, k=31, max_proj_iters=10, max_est_iters=5
         _lib.call("dss_project_to_surface", pts.device, pts, nrm, fi, npts, int(npts.shape[0]), pts.shape[0], idx,
                   int(k), radius, int(max_proj_iters), int(max_est_iters), out, iterations)
     return Projected(out, iterations)
+
+
+L0_MAX_SIZE = 2048   # DSS_L0_MAX_SIZE
+
+
+def _five_smooth(n):
+    for p in (2, 3, 5):
+        while n % p == 0:
+            n //= p
+    return n == 1
+
+
+def l0_size_error(n):
+    """None when ``n`` is an image side ``l0_smooth`` accepts (2 .. 2048, no prime factor above 5), otherwise the
+    message of its ValueError, which names the nearest accepted side (the smaller one on a tie)"""
+    if 2 <= n <= L0_MAX_SIZE and _five_smooth(n):
+        return None
+    near = min((m for m in range(2, L0_MAX_SIZE + 1) if _five_smooth(m)), key=lambda m: (abs(m - n), m))
+    return ("l0_smooth takes image sides in [2, %d] with no prime factor above 5; %d is not one (nearest: %d)"
+            % (L0_MAX_SIZE, n, near))
+
+
+def l0_smooth(images, lmd=0.05):
+    """L0 gradient-minimisation smoothing (Xu et al. 2011), as the reference's ``L0Smooth(images, lmd)`` computes it
+    per image (DSS/misc/imageFilters.py:133-180; csrc/l0_smooth.cu, the rules are in include/dss_b200.h and DESIGN.md):
+    20 rounds, beta = 0.1 doubling to 52428.8; each round zeroes the periodic forward differences (hp, vp) of the
+    estimate where sum_c(hp^2 + vp^2) < lmd / beta and solves S = ifft2(fft2(I + beta div) / (1 + beta D)) on periodic
+    boundaries.  Edges whose contrast survives the threshold stay sharp; everything between them flattens.
+
+    ``images`` (N, H, W, C) float32 or float64 CUDA tensor, any strides, C in {1, 3}; H and W in [2, 2048] with no prime
+    factor above 5 (ValueError otherwise, naming the nearest accepted size).  ``lmd`` >= 0; 0 returns the input.
+    Float64 throughout on the device; returns a new contiguous tensor of the input's dtype.  One library call, no host
+    synchronisation, the same bits on every call: capturable.  No gradients."""
+    if not torch.is_tensor(images):
+        raise TypeError("images must be a tensor")
+    if images.dim() != 4:
+        raise ValueError("images must have shape (N, H, W, C), got %d dimensions" % images.dim())
+    N, H, W, Cn = (int(v) for v in images.shape)
+    if Cn not in (1, 3):
+        raise ValueError("images must have C = 1 or 3 channels, got %d" % Cn)
+    if images.dtype not in (torch.float32, torch.float64):
+        raise TypeError("images must be float32 or float64, got %s" % images.dtype)
+    dev = _lib.require_cuda(images)
+    for n in (H, W):
+        msg = l0_size_error(n)
+        if msg is not None:
+            raise ValueError(msg)
+    lmd = float(lmd)
+    if not (math.isfinite(lmd) and lmd >= 0.0):
+        raise ValueError("lmd must be finite and >= 0, got %r" % lmd)
+    img = images.detach()
+    out = torch.empty((N, H, W, Cn), dtype=img.dtype, device=dev)
+    if N > 0:
+        strides = (C.c_int64 * 4)(*img.stride())
+        _lib.call("dss_l0_smooth", dev, img, int(img.dtype == torch.float64), strides, N, H, W, Cn, lmd, out)
+    return out
 
 
 class MeshRender(NamedTuple):

@@ -314,6 +314,26 @@ DSS_API int dss_project_to_surface(dss_ctx *ctx, const float *points, const floa
                                    const double *radius, int max_proj_iters, int max_est_iters, float *out_points,
                                    int32_t *iterations, void *stream);
 
+/* ---- L0 image smoothing ------------------------------------------------------------------------------------------
+ * L0Smooth (DSS/misc/imageFilters.py:133-180; Xu et al. 2011) of N images (N, H, W, C), C in {1, 3}, read at the
+ * element strides strides[0..3] (host array, >= 0) as float32 (f64 == 0) or float64 (f64 != 0); out (N, H, W, C)
+ * contiguous, same dtype.  2 <= H, W <= DSS_L0_MAX_SIZE, each with no prime factor above 5; lmd finite, >= 0.  Float64
+ * throughout, whatever the dtype; a float32 result is rounded once.  Per image, S = I, beta = 0.1, rounds while
+ * beta <= 1e5 (20 rounds), beta doubling after each:
+ *  - hp, vp: periodic forward differences of S along x and y;
+ *  - (hp, vp) = 0 at the pixels where sum_c(hp^2 + vp^2) < lmd / beta, the channels summed in order, each operation
+ *    rounded on its own (NaN is kept);
+ *  - hv = (hp(x-1, y) - hp(x, y)) + (vp(x, y-1) - vp(x, y)), periodic;
+ *  - S = real(ifft2(fft2(I + beta hv) / (1 + beta D))) per channel, D(u, v) = (2 - 2 cos 2 pi u / W) + (2 - 2 cos 2 pi
+ *    v / H): the reference's |fft2(dx)|^2 + |fft2(dy)|^2 in closed form.
+ * On the device (DESIGN.md): per round a shrink pass, a row FFT whose load forms I + beta hv, a column pass (FFT,
+ * spectral division, inverse FFT) and an inverse row FFT whose store takes the real part; the FFTs are mixed-radix
+ * (4, 2, 3, 5) Stockham transforms in shared memory.  Deterministic (no atomics), no host synchronisation or
+ * allocation: capturable.  Scratch from the context: 32 bytes per value, 1 byte per pixel and 16 (H + W) bytes. */
+#define DSS_L0_MAX_SIZE 2048
+DSS_API int dss_l0_smooth(dss_ctx *ctx, const void *images, int f64, const int64_t *strides, int N, int H, int W, int C,
+                          double lmd, void *out, void *stream);
+
 /* ---- surface regularisers of the training step (SURVEY.md section 8(f) row 2) -----------------------------------
  * Replaces the torch bodies of ProjectionLoss (kind 0) and RepulsionLoss (kind 1) (DSS/training/losses.py:282-497) on
  * packed clouds (points, normals (P,3); first_idx, num_points as for dss_knn_points).  knn_dists (P, K-1+self_col) f32
