@@ -16,9 +16,8 @@ __all__ = ["splat_points", "_splat_points_naive", "_rasterize_coarse", "_rasteri
 
 
 def _check_packed(points, ellipse_params, cutoff_thres, radii, first_idx, num_points):
-    # rasterize_points.h:483-488
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3), got %s" % (tuple(points.shape),))
+    """rasterize_points.h:483-488 -> (points, first_idx, num_points) of _lib.packed_cloud"""
+    points, first_idx, num_points = _lib.packed_cloud(points, first_idx, num_points)
     P = points.shape[0]
     if radii is not None and tuple(radii.shape) != (P, 2):
         raise RuntimeError("radii must have shape (%d, 2), got %s" % (P, tuple(radii.shape)))
@@ -26,10 +25,7 @@ def _check_packed(points, ellipse_params, cutoff_thres, radii, first_idx, num_po
         raise RuntimeError("ellipse_params must have shape (%d, 3), got %s" % (P, tuple(ellipse_params.shape)))
     if cutoff_thres is not None and tuple(cutoff_thres.shape) != (P,):
         raise RuntimeError("cutoff_thres must have shape (%d,), got %s" % (P, tuple(cutoff_thres.shape)))
-    if first_idx.shape != num_points.shape or first_idx.dim() != 1:
-        raise RuntimeError("cloud_to_packed_first_idx and num_points_per_cloud must both have shape (N,)")
-    if first_idx.dtype != torch.int64 or num_points.dtype != torch.int64:
-        raise RuntimeError("cloud_to_packed_first_idx / num_points_per_cloud must be int64")
+    return points, first_idx, num_points
 
 
 def splat_points(points, ellipse_params, cutoff_thres, radii, cloud_to_packed_first_idx,
@@ -43,17 +39,15 @@ def splat_points(points, ellipse_params, cutoff_thres, radii, cloud_to_packed_fi
     ``num_bins >= 22`` error (rasterize_points.cu:462-468) cannot occur."""
     dev = _lib.require_cuda(points, ellipse_params, cutoff_thres, radii, cloud_to_packed_first_idx,
                             num_points_per_cloud)
-    _check_packed(points, ellipse_params, cutoff_thres, radii, cloud_to_packed_first_idx, num_points_per_cloud)
+    points, fi, npts = _check_packed(points, ellipse_params, cutoff_thres, radii, cloud_to_packed_first_idx,
+                                     num_points_per_cloud)
     K, S = int(points_per_pixel), int(image_size)
     if K > _lib.MAX_POINTS_PER_PIXEL:
         raise RuntimeError("Must have points_per_pixel <= %d" % _lib.MAX_POINTS_PER_PIXEL)
-    N, P = num_points_per_cloud.shape[0], points.shape[0]
-    points = _lib.as_f32(points.detach(), "points")
+    N, P = npts.shape[0], points.shape[0]
     ellipse_params = _lib.as_f32(ellipse_params.detach(), "ellipse_params")
     cutoff_thres = _lib.as_f32(cutoff_thres.detach(), "cutoff_thres")
     radii = _lib.as_f32(radii.detach(), "radii")
-    fi = cloud_to_packed_first_idx.contiguous()
-    npts = num_points_per_cloud.contiguous()
     idx = torch.empty((N, S, S, K), dtype=torch.int32, device=dev)
     zbuf = torch.empty((N, S, S, K), dtype=torch.float32, device=dev)
     qvalue = torch.empty((N, S, S, K), dtype=torch.float32, device=dev)
@@ -74,15 +68,13 @@ def _splat_points_naive(points, ellipse_params, cutoff_thres, radii, cloud_to_pa
 def _rasterize_coarse_csr(points, radii, cloud_to_packed_first_idx, num_points_per_cloud, image_size, bin_size):
     """Bin membership as CSR: ``(bin_offsets int32 (N*B*B+1,), bin_ids int32 (total,))``."""
     dev = _lib.require_cuda(points, radii, cloud_to_packed_first_idx, num_points_per_cloud)
-    _check_packed(points, None, None, radii, cloud_to_packed_first_idx, num_points_per_cloud)
+    points, fi, npts = _check_packed(points, None, None, radii, cloud_to_packed_first_idx, num_points_per_cloud)
     S, bs = int(image_size), int(bin_size)
     if bs <= 0:
         raise RuntimeError("bin_size must be positive")
-    N, P = num_points_per_cloud.shape[0], points.shape[0]
+    N, P = npts.shape[0], points.shape[0]
     B = 1 + (S - 1) // bs
-    points = _lib.as_f32(points.detach(), "points")
     radii = _lib.as_f32(radii.detach(), "radii")
-    fi, npts = cloud_to_packed_first_idx.contiguous(), num_points_per_cloud.contiguous()
     off = torch.empty(N * B * B + 1, dtype=torch.int32, device=dev)
     cap = max(2 * P, 1024)
     for first in (True, False):
@@ -140,16 +132,14 @@ def _splat_points_occ_backward(points, radii, grad_occ, cloud_to_packed_first_id
     backward (rectangular window ``radii * radii_s``, every renderable point): -> ``(P,2)``.  ``depth_merging_thres`` is
     accepted and unused, as in the reference kernel.  The training path uses the fast variant (rasterizer.py:816)."""
     dev = _lib.require_cuda(points, radii, grad_occ, cloud_to_packed_first_idx, num_points_per_cloud)
-    _check_packed(points, None, None, radii, cloud_to_packed_first_idx, num_points_per_cloud)
+    points, fi, npts = _check_packed(points, None, None, radii, cloud_to_packed_first_idx, num_points_per_cloud)
     if grad_occ.dim() != 3 or grad_occ.shape[1] != grad_occ.shape[2]:
         raise RuntimeError("grad_occ must have shape (N, S, S)")
     N, S, P = grad_occ.shape[0], grad_occ.shape[1], points.shape[0]
-    points = _lib.as_f32(points.detach(), "points")
     radii = _lib.as_f32(radii.detach(), "radii")
     grad_occ = _lib.as_f32(grad_occ.detach(), "grad_occ")
     out = torch.empty((P, 2), dtype=torch.float32, device=dev)
-    _lib.call("dss_occ_backward_slow", dev, points, radii, grad_occ, 1, 0, cloud_to_packed_first_idx.contiguous(),
-              num_points_per_cloud.contiguous(), N, P, S, float(radii_s), out)
+    _lib.call("dss_occ_backward_slow", dev, points, radii, grad_occ, 1, 0, fi, npts, N, P, S, float(radii_s), out)
     return out
 
 
@@ -177,15 +167,14 @@ def occ_backward(points, radii, visible, rs, grad_occ, cloud_to_packed_first_idx
     """Occupancy gather on unsorted packed points with an explicit visibility mask -> ``(P,2)``."""
     dev = _lib.require_cuda(points, radii, visible, rs, grad_occ)
     N, S = grad_occ.shape[0], grad_occ.shape[1]
+    points, fi, npts = _lib.packed_cloud(points, cloud_to_packed_first_idx, num_points_per_cloud, N)
     P = points.shape[0]
-    points = _lib.as_f32(points.detach(), "points")
     radii = _lib.as_f32(radii.detach(), "radii")
     grad_occ = _lib.as_f32(grad_occ.detach(), "grad_occ")
     rs = _lib.as_f32(rs.detach(), "rs")
     visible = visible.to(torch.uint8).contiguous()
     out = torch.empty((P, 2), dtype=torch.float32, device=dev)
-    _lib.call("dss_occ_backward", dev, points, radii, visible, rs, grad_occ, 1, 0,
-              cloud_to_packed_first_idx.contiguous(), num_points_per_cloud.contiguous(), N, P, S, out)
+    _lib.call("dss_occ_backward", dev, points, radii, visible, rs, grad_occ, 1, 0, fi, npts, N, P, S, out)
     return out
 
 
@@ -203,12 +192,12 @@ def visibility_from_idx(idx, P):
 
 def search_radius(radii, visible, cloud_to_packed_first_idx, num_points_per_cloud, radii_s):
     """(N,) f32: ``radii_s * lower_median(radii of the view's visible points)`` (rasterizer.py:888)."""
-    dev = _lib.require_cuda(radii, visible)
-    N = num_points_per_cloud.shape[0]
+    dev = _lib.require_cuda(radii, visible, cloud_to_packed_first_idx, num_points_per_cloud)
+    fi, npts = _lib.cloud_offsets(cloud_to_packed_first_idx, num_points_per_cloud)
+    N = npts.shape[0]
     rs = torch.empty(N, dtype=torch.float32, device=dev)
     radii = _lib.as_f32(radii.detach(), "radii")
-    _lib.call("dss_search_radius", dev, radii, visible.contiguous(), cloud_to_packed_first_idx.contiguous(),
-              num_points_per_cloud.contiguous(), N, radii.shape[0], float(radii_s), rs)
+    _lib.call("dss_search_radius", dev, radii, visible.contiguous(), fi, npts, N, radii.shape[0], float(radii_s), rs)
     return rs
 
 

@@ -284,3 +284,40 @@ def require_cuda(*tensors):
         elif t.device != dev:
             raise RuntimeError("all tensors must be on the same device (%s vs %s)" % (dev, t.device))
     return dev
+
+
+def cloud_offsets(first_idx, num_points, n_clouds=None):
+    """Contiguous ``(first_idx, num_points)`` of the packed layout (cloud n owns rows [first_idx[n], first_idx[n] +
+    num_points[n])), both required: int64 tensors of shape (N,), N = ``n_clouds`` or the length of ``first_idx``.  The
+    kernels read both as int64[N] and index rows with them, so this runs before any launch; their values stay on the
+    device (reading them back would synchronise the host)."""
+    if first_idx is None or num_points is None:
+        raise RuntimeError("packed clouds need cloud_to_packed_first_idx and num_points_per_cloud")
+    N = n_clouds if n_clouds is not None else (first_idx.shape[0] if first_idx.dim() else 0)
+    for name, t in (("cloud_to_packed_first_idx", first_idx), ("num_points_per_cloud", num_points)):
+        if t.dtype != torch.int64 or tuple(t.shape) != (N,):
+            raise RuntimeError("%s must be an int64 tensor of shape (%d,), got %s %s" % (name, N, t.dtype, tuple(t.shape)))
+    return first_idx.contiguous(), num_points.contiguous()
+
+
+def packed_cloud(points, first_idx=None, num_points=None, n_clouds=None):
+    """``(points, first_idx, num_points)`` of a cloud argument as the kernels take it: ``points`` (P,3) float32 on a
+    CUDA device, returned detached and contiguous, with the offsets of :func:`cloud_offsets` on the same device; with
+    neither offset given, one cloud of all P rows."""
+    require_cuda(points, first_idx, num_points)
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise RuntimeError("points must have shape (P, 3), got %s" % (tuple(points.shape),))
+    if (first_idx is None) != (num_points is None):
+        raise RuntimeError("pass both first_idx and num_points, or neither")
+    pts = as_f32(points.detach(), "points")
+    if first_idx is None:
+        first_idx = torch.zeros((1,), dtype=torch.int64, device=pts.device)
+        num_points = torch.full((1,), pts.shape[0], dtype=torch.int64, device=pts.device)
+    return (pts,) + cloud_offsets(first_idx, num_points, n_clouds)
+
+
+def check_k(k, lo, hi):
+    """``int(k)`` for a neighbourhood size in [lo, hi]; ValueError for anything else, a bool or a fraction included"""
+    if isinstance(k, bool) or int(k) != k or not lo <= k <= hi:
+        raise ValueError("k must be an integer in [%d, %d], got %r" % (lo, hi, k))
+    return int(k)

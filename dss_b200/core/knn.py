@@ -15,8 +15,4 @@ def knn_sq_dists(points: torch.Tensor, K: int = 7, radius: float = 0.2) -> torch
     included, distance 0).  Neighbours farther than ``radius`` (when radius > 0) are reported as -1 like frnn
     does for missing neighbours (frnn.py:176-301); the callers take ``max`` over the row, so -1 never wins
     as long as one neighbour exists."""
-    P = points.shape[0]
-    first = torch.zeros(1, dtype=torch.int64, device=points.device)
-    num = torch.full((1,), P, dtype=torch.int64, device=points.device)
-    d, _ = knn_points_packed(points, first, num, K, radius if radius is not None else -1.0, return_idx=False)
-    return d
+    return knn_points_packed(points, None, None, K, radius if radius is not None else -1.0, return_idx=False)[0]

@@ -42,26 +42,26 @@ def counting_sort_cuda(points, lengths, grid_cell, grid_idx, grid_off, sorted_po
 
 def knn_points_packed(points, first_idx, num_points, K, r=-1.0, queries=None, query_first_idx=None, query_num=None,
                       return_idx=True):
-    """Packed form: ``points`` (P,3) f32, cloud n owns rows [first_idx[n], first_idx[n] + num_points[n]).  The ranges
-    may leave gaps between them (padded storage passed as packed: first_idx = n * Pmax, num_points = lengths) but must
-    not overlap; rows outside every query range are left unwritten.  Returns ``(sq_dists (Pq,K) f32 ascending, idxs
-    (Pq,K) int32 local to the cloud or None)``, -1 padded.  Rows of points or queries with a NaN or infinite coordinate
-    are all -1, and such points are nobody's neighbour."""
+    """Packed form: ``points`` (P,3) f32, cloud n owns rows [first_idx[n], first_idx[n] + num_points[n]) (both None: one
+    cloud).  The ranges may leave gaps between them (padded storage passed as packed: first_idx = n * Pmax, num_points =
+    lengths) but must not overlap; rows outside every query range are left unwritten.  ``queries`` (Pq,3) f32 take the
+    points' offsets unless both ``query_first_idx`` and ``query_num`` are given.  Returns ``(sq_dists (Pq,K) f32
+    ascending, idxs (Pq,K) int32 local to the cloud or None)``, -1 padded.  Rows of points or queries with a NaN or
+    infinite coordinate are all -1, and such points are nobody's neighbour."""
     dev = _lib.require_cuda(points, first_idx, num_points, queries, query_first_idx, query_num)
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3)")
+    pts, first_idx, num_points = _lib.packed_cloud(points, first_idx, num_points)
     if not (1 <= int(K) <= 32):
         raise RuntimeError("K must be in [1, 32]")
-    pts = _lib.as_f32(points.detach(), "points")
-    q = pts if queries is None else _lib.as_f32(queries.detach(), "queries")
-    qf = first_idx if query_first_idx is None else query_first_idx
-    qn = num_points if query_num is None else query_num
-    Pq, P, N = q.shape[0], pts.shape[0], num_points.shape[0]
+    P, N = pts.shape[0], num_points.shape[0]
+    query_args = (None, None, None)
+    if queries is not None:
+        if query_first_idx is None and query_num is None:
+            query_first_idx, query_num = first_idx, num_points
+        query_args = _lib.packed_cloud(queries, query_first_idx, query_num, N)
+    Pq = P if queries is None else query_args[0].shape[0]
     d = torch.empty((Pq, K), dtype=torch.float32, device=dev)
     i = torch.empty((Pq, K), dtype=torch.int32, device=dev) if return_idx else None
-    query_args = (None, None, None) if queries is None else (q, qf.contiguous(), qn.contiguous())
-    _lib.call("dss_knn_points", dev, *query_args, pts, first_idx.contiguous(), num_points.contiguous(), N, Pq, P,
-              int(K), float(r), d, i)
+    _lib.call("dss_knn_points", dev, *query_args, pts, first_idx, num_points, N, Pq, P, int(K), float(r), d, i)
     return d, i
 
 

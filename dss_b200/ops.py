@@ -113,23 +113,16 @@ def _fill_common(a, points, normals, colours, proj, view, h, first_idx, num_poin
 
 
 def _layout(points, proj, first_idx, num_points, shared):
+    """(N, P0, P, first_idx, num_points) of a render call; a shared cloud reads no offsets (None)"""
     N = proj.shape[0]
     if shared:
         if N > _lib.MAX_SHARED_VIEWS:   # the backward's chain kernel holds the view matrices in shared memory
             raise RuntimeError("a shared cloud takes at most %d views per call, got %d" % (_lib.MAX_SHARED_VIEWS, N))
         P0 = points.shape[0]
-        return N, P0, N * P0
-    if first_idx is None or num_points is None:
-        raise RuntimeError("packed clouds need cloud_to_packed_first_idx and num_points_per_cloud")
+        return N, P0, N * P0, None, None
+    # packed rows that no view's range covers get zero gradients, see backward
     P = points.shape[0]
-    # the kernels read both arrays as int64[N] and index the packed arrays with them: check before any launch
-    # (their VALUES stay on the device -- reading them back would put a host sync into every forward; rows that no
-    #  range covers get zero gradients, see backward)
-    for name, t in (("cloud_to_packed_first_idx", first_idx), ("num_points_per_cloud", num_points)):
-        if t.dtype != torch.int64 or tuple(t.shape) != (N,):
-            raise RuntimeError("%s must be an int64 tensor of shape (%d,), got %s %s"
-                               % (name, N, t.dtype, tuple(t.shape)))
-    return N, P, P   # P0 is only an upper bound on the points of one view in packed mode
+    return (N, P, P) + _lib.cloud_offsets(first_idx, num_points, N)   # P0 only bounds one view's points when packed
 
 
 def _splat_shape(h, frames, rows, N, P):
@@ -162,7 +155,7 @@ class _RenderFunction(torch.autograd.Function):
         colours_c = _lib.as_f32(colours.detach(), "colours")
         proj_c = _lib.as_f32(proj.detach(), "proj")
         view_c = _lib.as_f32(view.detach(), "view")
-        N, P0, P = _layout(points_c, proj_c, first_idx, num_points, shared)
+        N, P0, P, fi, npts = _layout(points_c, proj_c, first_idx, num_points, shared)
         h_c, frames_c = _splat_shape(h, frames, P0 if shared else P, N, P)
         if shading is not None:
             if tuple(colours_c.shape) != (P0, 3):
@@ -195,8 +188,6 @@ class _RenderFunction(torch.autograd.Function):
         cell_counts = torch.empty((N * OB * OB * 1024,), dtype=torch.int32, device=dev)
         zbuf = torch.empty((N, S, S, K), **f32) if want_frags else None
         qvalue = torch.empty((N, S, S, K), **f32) if want_frags else None
-        fi = first_idx.contiguous() if first_idx is not None else None
-        npts = num_points.contiguous() if num_points is not None else None
         a = _lib.RenderArgs()
         _fill_common(a, points_c, normals_c, colours_c, proj_c, view_c, h_c, fi, npts, shared, N, P0, P, prm)
         a.frames = _lib.ptr(frames_c)
@@ -451,13 +442,11 @@ def preprocess_points(points, normals, proj, view, h, params: SplatParams, first
     dev = _lib.require_cuda(points, normals, proj, view, h, first_idx, num_points, frames)
     points_c, normals_c = _lib.as_f32(points.detach(), "points"), _lib.as_f32(normals.detach(), "normals")
     proj_c, view_c = _lib.as_f32(proj.detach(), "proj"), _lib.as_f32(view.detach(), "view")
-    N, P0, P = _layout(points_c, proj_c, first_idx, num_points, shared_cloud)
+    N, P0, P, fi, npts = _layout(points_c, proj_c, first_idx, num_points, shared_cloud)
     h_c, frames_c = _splat_shape(h, frames, P0 if shared_cloud else P, N, P)
     f32 = dict(dtype=torch.float32, device=dev)
     ndc, ell = torch.empty((P, 3), **f32), torch.empty((P, 3), **f32)
     radii, scaler = torch.empty((P, 2), **f32), torch.empty((P,), **f32)
-    fi = first_idx.contiguous() if first_idx is not None else None
-    npts = num_points.contiguous() if num_points is not None else None
     a = _lib.RenderArgs()
     _fill_common(a, points_c, normals_c, None, proj_c, view_c, h_c, fi, npts, shared_cloud, N, P0, P, params)
     a.frames = _lib.ptr(frames_c)
@@ -482,25 +471,16 @@ def local_frames(points, first_idx=None, num_points=None):
     single cloud of at most 8 points raises ValueError as the reference does (mathHelper.py:57-61), packed clouds are
     not checked on the host.  No gradients (the reference computes the frames under no_grad)."""
     from .frnn_grid import knn_points_packed
-    dev = _lib.require_cuda(points, first_idx, num_points)
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3)")
-    if (first_idx is None) != (num_points is None):
-        raise RuntimeError("pass both first_idx and num_points, or neither")
-    pts = _lib.as_f32(points.detach(), "points")
+    single = first_idx is None and num_points is None
+    pts, fi, npts = _lib.packed_cloud(points, first_idx, num_points)
     P = pts.shape[0]
-    single = first_idx is None
-    if single:
-        if P <= LOCAL_FRAME_K:
-            raise ValueError("the anisotropic kernel needs clouds of more than %d points (the neighbourhood size), "
-                             "got %d" % (LOCAL_FRAME_K, P))
-        first_idx = torch.zeros((1,), dtype=torch.int64, device=dev)
-        num_points = torch.full((1,), P, dtype=torch.int64, device=dev)
-    fi, npts = first_idx.contiguous(), num_points.contiguous()
+    if single and P <= LOCAL_FRAME_K:
+        raise ValueError("the anisotropic kernel needs clouds of more than %d points (the neighbourhood size), "
+                         "got %d" % (LOCAL_FRAME_K, P))
     _, idx = knn_points_packed(pts, fi, npts, LOCAL_FRAME_K, -1.0)
-    frames = torch.empty((P, 8), dtype=torch.float32, device=dev)
-    _lib.call("dss_local_frames", dev, pts, None if single else fi, None if single else npts, int(npts.shape[0]), P,
-              idx, frames)
+    frames = torch.empty((P, 8), dtype=torch.float32, device=pts.device)
+    _lib.call("dss_local_frames", pts.device, pts, None if single else fi, None if single else npts,
+              int(npts.shape[0]), P, idx, frames)
     return frames
 
 
@@ -525,22 +505,11 @@ def estimate_normals(points, k=20, orient=True, first_idx=None, num_points=None)
     NaN normal and root = parent = -1.  Two library calls (the K-NN and the estimate), no host synchronisation, the same
     bits on every call.  No gradients."""
     from .frnn_grid import knn_points_packed
-    dev = _lib.require_cuda(points, first_idx, num_points)
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3)")
-    if (first_idx is None) != (num_points is None):
-        raise RuntimeError("pass both first_idx and num_points, or neither")
-    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 32:
-        raise ValueError("k must be an integer in [3, 32], got %r" % (k,))
-    k = int(k)
-    pts = _lib.as_f32(points.detach(), "points")
-    P = pts.shape[0]
+    pts, fi, npts = _lib.packed_cloud(points, first_idx, num_points)
+    k = _lib.check_k(k, 3, 32)
+    dev, P = pts.device, pts.shape[0]
     if P >= 2 ** 30:
         raise ValueError("at most 2^30 - 1 points")
-    if first_idx is None:
-        first_idx = torch.zeros((1,), dtype=torch.int64, device=dev)
-        num_points = torch.full((1,), P, dtype=torch.int64, device=dev)
-    fi, npts = first_idx.contiguous(), num_points.contiguous()
     normals = torch.empty((P, 3), dtype=torch.float32, device=dev)
     root = torch.full((P,), -1, dtype=torch.int32, device=dev)
     parent = torch.full((P,), -1, dtype=torch.int32, device=dev)
@@ -550,15 +519,6 @@ def estimate_normals(points, k=20, orient=True, first_idx=None, num_points=None)
     _lib.call("dss_estimate_normals", dev, pts, fi, npts, int(npts.shape[0]), P, idx, k, int(bool(orient)), normals,
               root, parent)
     return PointNormals(normals, root, parent)
-
-
-def _packed_layout(pts, first_idx, num_points, dev):
-    if (first_idx is None) != (num_points is None):
-        raise RuntimeError("pass both first_idx and num_points, or neither")
-    if first_idx is None:
-        first_idx = torch.zeros((1,), dtype=torch.int64, device=dev)
-        num_points = torch.full((1,), pts.shape[0], dtype=torch.int64, device=dev)
-    return first_idx.contiguous(), num_points.contiguous()
 
 
 class Outliers(NamedTuple):
@@ -577,17 +537,11 @@ def outlier_ratio(points, k=16, tolerance=0.05, first_idx=None, num_points=None)
     a row whose neighbours all coincide (0 / 0), get ratio NaN and are not kept.  Two library calls (the K-NN and the
     ratio), no host synchronisation, so the call can be captured in a CUDA graph; the same bits on every call."""
     from .frnn_grid import knn_points_packed
-    dev = _lib.require_cuda(points, first_idx, num_points)
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3)")
-    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 32:
-        raise ValueError("k must be an integer in [3, 32], got %r" % (k,))
-    k = int(k)
-    pts = _lib.as_f32(points.detach(), "points")
-    P = pts.shape[0]
+    pts, fi, npts = _lib.packed_cloud(points, first_idx, num_points)
+    k = _lib.check_k(k, 3, 32)
+    dev, P = pts.device, pts.shape[0]
     if P >= 2 ** 30:
         raise ValueError("at most 2^30 - 1 points")
-    fi, npts = _packed_layout(pts, first_idx, num_points, dev)
     keep = torch.zeros((P,), dtype=torch.bool, device=dev)
     ratio = torch.full((P,), float("nan"), dtype=torch.float64, device=dev)
     if P == 0:
@@ -627,6 +581,21 @@ def upsample_schedule(num_points, targets, k=16):
     return rounds
 
 
+def _read_clouds(fi, npts, P, *per_cloud):
+    """The one host synchronisation of upsample_points and _rimls_setup: every cloud's first row and size (int64) and
+    the per-cloud values ``per_cloud``, (N,) or (N,c) each, as the columns of one (N, c...) float64 array, in one copy.
+    ValueError when a cloud's range leaves the P rows."""
+    import numpy as np
+    N = fi.shape[0]
+    # clamped to [-1, P + 1], which float64 holds exactly and where a range past the rows stays past them
+    offsets = (fi.clamp(-1, P + 1), npts.clamp(-1, P + 1))
+    info = torch.cat([t.double().reshape(N, -1) for t in offsets + per_cloud], 1).cpu().numpy()
+    first, num = info[:, 0].astype(np.int64), info[:, 1].astype(np.int64)
+    if (first < 0).any() or (num < 0).any() or (first > P - num).any():
+        raise ValueError("first_idx / num_points leave the points")
+    return first, num, info[:, 2:]
+
+
 def upsample_points(points, n, k=16, normals=None, features=None, first_idx=None, num_points=None) -> Upsampled:
     """Densify point clouds as the reference's ``upsample`` does (DSS/core/cloud.py:555-632; csrc/upsample.cu, the rules
     are in include/dss_b200.h and DESIGN.md): in every round each cloud of ``c`` points gains ``min(n - c, c // 10)``
@@ -646,13 +615,9 @@ def upsample_points(points, n, k=16, normals=None, features=None, first_idx=None
     Synchronises once, to read the sizes; then one library call (per round the K-NN and five kernels), the same bits on
     every call.  No gradients."""
     import numpy as np
-    dev = _lib.require_cuda(points, normals, features, first_idx, num_points)
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3)")
-    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 31:
-        raise ValueError("k must be an integer in [3, 31], got %r" % (k,))
-    k = int(k)
-    pts = _lib.as_f32(points.detach(), "points")
+    dev = _lib.require_cuda(points, normals, features)
+    pts, fi, npts = _lib.packed_cloud(points, first_idx, num_points)
+    k = _lib.check_k(k, 3, 31)
     P = pts.shape[0]
     nrm = None if normals is None else _lib.as_f32(normals.detach(), "normals")
     if nrm is not None and tuple(nrm.shape) != (P, 3):
@@ -660,20 +625,15 @@ def upsample_points(points, n, k=16, normals=None, features=None, first_idx=None
     ftr = None if features is None else _lib.as_f32(features.detach(), "features")
     if ftr is not None and (ftr.dim() != 2 or ftr.shape[0] != P or ftr.shape[1] < 1):
         raise RuntimeError("features must have shape (P, D)")
-    fi, npts = _packed_layout(pts, first_idx, num_points, dev)
     N = int(npts.shape[0])
     if N < 1:
         raise ValueError("no clouds")
     # the one synchronisation: every cloud's first row, size and count of non-finite rows
     bad = torch.zeros((P + 1,), dtype=torch.int64, device=dev)
     bad[1:] = torch.cumsum((~torch.isfinite(pts).all(1)).to(torch.int64), 0)
-    end = (fi + npts).clamp(0, P)
-    info = torch.stack([fi, npts, bad[end] - bad[fi.clamp(0, P)]]).cpu().numpy()
-    first_h, num_h = info[0], info[1]
-    if (num_h < 0).any() or (first_h < 0).any() or (first_h + num_h > P).any():
-        raise ValueError("first_idx / num_points leave the points")
-    if info[2].any():
-        raise ValueError("non-finite coordinates in cloud(s) %s" % np.flatnonzero(info[2]).tolist())
+    first_h, num_h, info = _read_clouds(fi, npts, P, bad[(fi + npts).clamp(0, P)] - bad[fi.clamp(0, P)])
+    if info[:, 0].any():
+        raise ValueError("non-finite coordinates in cloud(s) %s" % np.flatnonzero(info[:, 0]).tolist())
     if torch.is_tensor(n):
         n = n.tolist()
     targets = [int(n)] * N if np.ndim(n) == 0 else [int(x) for x in n]
@@ -720,20 +680,15 @@ def _rimls_setup(points, normals, k, first_idx, num_points, scale):
     num_points, knn_idx (P, k + 1), radius (N,) float64) on the device"""
     import numpy as np
     from .frnn_grid import knn_points_packed
-    dev = _lib.require_cuda(points, normals, first_idx, num_points)
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise RuntimeError("points must have shape (P, 3)")
-    if isinstance(k, bool) or int(k) != k or not 3 <= k <= 31:
-        raise ValueError("k must be an integer in [3, 31], got %r" % (k,))
-    k = int(k)
-    pts = _lib.as_f32(points.detach(), "points")
+    dev = _lib.require_cuda(points, normals)
+    pts, fi, npts = _lib.packed_cloud(points, first_idx, num_points)
+    k = _lib.check_k(k, 3, 31)
     nrm = _lib.as_f32(normals.detach(), "normals")
     P = pts.shape[0]
     if tuple(nrm.shape) != (P, 3):
         raise RuntimeError("normals must have shape (P, 3)")
     if P >= 2 ** 31 - 1:
         raise ValueError("at most 2^31 - 2 points")
-    fi, npts = _packed_layout(pts, first_idx, num_points, dev)
     N = int(npts.shape[0])
     if N < 1:
         raise ValueError("no clouds")
@@ -749,19 +704,15 @@ def _rimls_setup(points, normals, k, first_idx, num_points, scale):
     idx3 = cloud[:, None].expand(P, 3)
     lo = torch.full((N + 1, 3), float("inf"), device=dev).scatter_reduce(0, idx3, pts, "amin")
     hi = torch.full((N + 1, 3), -float("inf"), device=dev).scatter_reduce(0, idx3, pts, "amax")
-    info = torch.cat([fi.double()[:, None], npts.double()[:, None], nbad[1:, None], lo[1:].double(), hi[1:].double()],
-                     1).cpu().numpy()
-    first_h, num_h = info[:, 0].astype(np.int64), info[:, 1].astype(np.int64)
-    if (num_h < 0).any() or (first_h < 0).any() or (first_h + num_h > P).any():
-        raise ValueError("first_idx / num_points leave the points")
+    first_h, num_h, info = _read_clouds(fi, npts, P, nbad[1:], lo[1:], hi[1:])
     order = np.lexsort((num_h, first_h))
     if (first_h[order][1:] < (first_h + num_h)[order][:-1]).any():
         raise ValueError("the clouds' ranges overlap")
-    if info[:, 2].any():
-        raise ValueError("non-finite points or normals in cloud(s) %s" % np.flatnonzero(info[:, 2]).tolist())
+    if info[:, 0].any():
+        raise ValueError("non-finite points or normals in cloud(s) %s" % np.flatnonzero(info[:, 0]).tolist())
     radius = []
     for n in range(N):
-        d = info[n, 6:9] - info[n, 3:6]
+        d = info[n, 4:7] - info[n, 1:4]
         diag = math.sqrt((float(d[0]) * float(d[0]) + float(d[1]) * float(d[1])) + float(d[2]) * float(d[2])) \
             if num_h[n] > 0 else 0.0
         radius.append(_rimls_radius(diag, int(num_h[n]), k, scale))
@@ -936,8 +887,8 @@ def _chamfer_input(points, lengths, normals, name):
     own normals; a padded (N,P,3) tensor is passed as packed with gaps (cloud n owns rows [n P, n P + lengths[n]))."""
     if hasattr(points, "points_packed"):
         pts, nrm = points.points_packed(), points.normals_packed()
-        first, num = points.cloud_to_packed_first_idx(), points.num_points_per_cloud()
         N = len(points)
+        first, num = _lib.cloud_offsets(points.cloud_to_packed_first_idx(), points.num_points_per_cloud(), N)
     else:
         if not torch.is_tensor(points) or points.dim() != 3 or points.shape[2] != 3:
             raise ValueError("%s must be a PointClouds3D or a padded (N, P, 3) tensor" % name)

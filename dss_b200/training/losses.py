@@ -161,9 +161,7 @@ def surface_regulariser(kind, points, normals, first_idx, num_points, knn_dists,
         raise RuntimeError("points and normals must both have shape (P, 3)")
     if points.dtype != torch.float32 or normals.dtype != torch.float32:
         raise RuntimeError("points and normals must be float32")
-    if first_idx.dim() != 1 or first_idx.shape != num_points.shape or first_idx.dtype != torch.int64 \
-            or num_points.dtype != torch.int64:
-        raise RuntimeError("first_idx and num_points must be int64 of shape (N,)")
+    first_idx, num_points = _lib.cloud_offsets(first_idx, num_points)
     P = points.shape[0]
     if knn_dists.dim() != 2 or knn_dists.shape[0] != P or knn_idx.shape != knn_dists.shape:
         raise RuntimeError("knn_dists and knn_idx must both have shape (P, W) with P = %d" % P)
@@ -183,8 +181,8 @@ def surface_regulariser(kind, points, normals, first_idx, num_points, knn_dists,
         if m is not None and (m.shape != (P,) or m.dtype not in (torch.bool, torch.uint8)):
             raise RuntimeError("%s must be a (P,) bool tensor" % name)
         masks.append(None if m is None else m.contiguous())
-    return _SurfaceRegulariser.apply(points.contiguous(), normals.detach().contiguous(), first_idx.contiguous(),
-                                     num_points.contiguous(), knn_dists, knn_idx, K, int(bool(self_col)),
+    return _SurfaceRegulariser.apply(points.contiguous(), normals.detach().contiguous(), first_idx, num_points,
+                                     knn_dists, knn_idx, K, int(bool(self_col)),
                                      None if knn_points is None else knn_points.detach(),
                                      None if neighbour_points is None else neighbour_points.detach(), masks[0],
                                      masks[1], _KINDS[kind], sharpness_sigma, filter_scale)
