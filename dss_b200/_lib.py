@@ -107,6 +107,7 @@ _SIGNATURES = {
     "dss_image_loss_finish": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, vp, vp, vp, vp]),
     "dss_image_metrics": (C.c_int, [vp, vp, C.c_int, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                     vp, vp, vp]),
+    "dss_gather_views": (C.c_int, [vp, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp]),
     "dss_point_filters": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp, C.c_int, C.POINTER(C.c_int64),
                                     C.c_int, C.c_int, vp, vp, vp]),
     "dss_point_filters_gated": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp, C.c_int,

@@ -26,7 +26,7 @@ __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_poi
            "estimate_normals", "Outliers", "outlier_ratio", "Upsampled", "upsample_schedule", "upsample_points",
            "denoise_normals", "Projected", "project_to_surface", "l0_smooth", "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
-           "ImageMetrics", "image_metrics", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
+           "ImageMetrics", "image_metrics", "gather_views", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
 
 
 class SplatParams(NamedTuple):
@@ -1165,6 +1165,32 @@ def image_metrics(pred_rgba, gt_rgb, gt_mask) -> ImageMetrics:
     return ImageMetrics(means[0], means[1], per_view)
 
 
+def gather_views(store, idx, img, mask):
+    """Views ``idx`` of a device-resident view store into the training step's ground truth (csrc/views.cu; the rules
+    are in include/dss_b200.h).  ``store`` (V,H,W,4) contiguous, r, g, b, mask per pixel: uint8 (rgb u / 255 as
+    correctly rounded float32 division, mask u != 0) or float32 (copied bit for bit).  ``idx`` (B,) int64 on the
+    store's device, every value in [0, V): NOT checked here (that would read the indices back); the caller checks them
+    on the host before it uploads them.  ``img`` (B,H,W,3) and ``mask`` (B,H,W) float32 contiguous outputs, written in
+    place and returned.  One launch on the current stream, no allocation, no host synchronisation: capturable."""
+    dev = _lib.require_cuda(store, idx, img, mask)
+    if store.dtype not in (torch.uint8, torch.float32) or store.dim() != 4 or store.shape[3] != 4 \
+            or not store.is_contiguous():
+        raise RuntimeError("store must be a contiguous (V, H, W, 4) uint8 or float32 tensor, got %s %s"
+                           % (store.dtype, tuple(store.shape)))
+    V, H, W = store.shape[:3]
+    if idx.dtype != torch.int64 or idx.dim() != 1:
+        raise RuntimeError("idx must be an int64 tensor of shape (B,), got %s %s" % (idx.dtype, tuple(idx.shape)))
+    B = idx.shape[0]
+    for name, t, shape in (("img", img, (B, H, W, 3)), ("mask", mask, (B, H, W))):
+        if t.dtype != torch.float32 or tuple(t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError("%s must be a contiguous float32 tensor of shape %s, got %s %s"
+                               % (name, shape, t.dtype, tuple(t.shape)))
+    if B > 65535:
+        raise ValueError("gather_views takes at most 65535 views at a time, got %d" % B)
+    _lib.call("dss_gather_views", dev, store, int(store.dtype == torch.float32), V, H, W, idx, B, img, mask)
+    return img, mask
+
+
 def shared_cloud_splats(points, n_views, Vrk_invariant=True, Vrk_isotropic=True, frnn_radius=0.2):
     """``(h, frames)`` for :func:`render_points` of ``n_views`` views of ONE shared cloud, as the training step sizes its
     splats: the spacing rule of ``SurfaceSplatting._compute_h`` (one h per view with ``Vrk_invariant``, one per point
@@ -1183,22 +1209,27 @@ def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotr
     from .core.camera import camera_matrices
     from .core.lighting import pack_lights
     from .core.texture import camera_centres
+    from .utils.dataset import DeviceViews
     dev = _lib.require_cuda(points, normals, colours)
-    lp = data.light_props(dev)
-    if lp is None:
-        raise ValueError("the data has no lights_%d entries: the views are shaded with the data's lights")
-    light_cls, props = lp
     # the training loop's matrices and light rows, bit for bit: all the views' projections, then the batch's
-    proj_all = camera_matrices(data.get_cameras())[0].to(dev)
-    view_all = torch.from_numpy(data.camera_mat[:len(data)]).to(dev)
+    if isinstance(data, DeviceViews):
+        lights_of = None if data.light_cls is None else data.lights
+        proj_all, view_all = data.proj, data.camera_mat
+    else:
+        lp = data.light_props(dev)
+        lights_of = None if lp is None else \
+            (lambda idx: lp[0](**{k: v.index_select(0, idx) for k, v in lp[1].items()}, device=dev))
+        proj_all = camera_matrices(data.get_cameras())[0].to(dev)
+        view_all = torch.from_numpy(data.camera_mat[:len(data)]).to(dev)
+    if lights_of is None:
+        raise ValueError("the data has no lights_%d entries: the views are shaded with the data's lights")
     p, c = points.detach(), colours.detach()
     n = torch.nn.functional.normalize(normals.detach(), dim=-1)
     h1, frames = shared_cloud_splats(p, 1, Vrk_invariant, Vrk_isotropic, frnn_radius)
 
     def render(params, views):
         idx = torch.as_tensor(list(views), dtype=torch.int64, device=dev)
-        lights = light_cls(**{k: v.index_select(0, idx) for k, v in props.items()}, device=dev)
-        rows, ambient, kind = pack_lights(lights)
+        rows, ambient, kind = pack_lights(lights_of(idx))
         view = view_all.index_select(0, idx)
         with torch.no_grad():
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), kind, float(shininess))
@@ -1211,24 +1242,30 @@ def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotr
 def render_data_views(points, normals, colours, data, params: SplatParams, views, Vrk_invariant=True,
                       Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0):
     """(len(views), S, S, 4) renders, S = ``params.image_size``, of one shared cloud from the cameras of ``data``'s
-    views ``views`` (an ``MVRData``: its ``get_cameras()`` projections and ``camera_mat`` view matrices) with fused
-    shading by each view's own lights (``data.light_props``), as the training step renders a batch: unit normals, the
-    splats of :func:`shared_cloud_splats`, ``colours`` the albedo.  Forward only."""
+    views ``views`` (an ``MVRData``: its ``get_cameras()`` projections and ``camera_mat`` view matrices, or the same
+    held by a ``DeviceViews``) with fused shading by each view's own lights (``data.light_props``), as the training
+    step renders a batch: unit normals, the splats of :func:`shared_cloud_splats`, ``colours`` the albedo.  Forward
+    only."""
     return _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius,
                                shininess)(params, views)
 
 
 def evaluate_2d(points, normals, colours, data, params: SplatParams, image_size, batch=1, Vrk_invariant=True,
                 Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0):
-    """The reference's ``Trainer.evaluate_2d`` for a point cloud: every view of ``data`` (an ``MVRData`` with images
-    and masks) rendered at ``image_size`` x ``image_size`` with the splat renderer, ``batch`` views at a time
-    (:func:`render_data_views` with ``params`` at that size), scored by :func:`image_metrics` against the view's
-    ground truth.  Returns ``{"iou", "psnr"}`` (float64 device scalars, the means over all the views) and
-    ``"per_view"`` (V,5) float64 rows (I, U, E, iou, psnr).  Renders and ground truth of one batch at a time are on the
-    device; uses no random numbers and none of a training step's buffers."""
-    if data.images is None or data.masks is None:
-        raise ValueError("evaluate_2d needs the data's images and masks")
+    """The reference's ``Trainer.evaluate_2d`` for a point cloud: every view of ``data`` rendered at ``image_size`` x
+    ``image_size`` with the splat renderer, ``batch`` views at a time (:func:`render_data_views` with ``params`` at
+    that size), scored by :func:`image_metrics` against the view's ground truth.  ``data``: a ``DeviceViews`` (the
+    training loop passes its own, so a validation uploads nothing) or an ``MVRData`` with images and masks, whose
+    ``device_views`` this builds first.  The ground truth of each batch is gathered from the views' store
+    (:func:`gather_views`).  Returns ``{"iou", "psnr"}`` (float64 device scalars, the means over all the views) and
+    ``"per_view"`` (V,5) float64 rows (I, U, E, iou, psnr).  Uses no random numbers and none of a training step's
+    buffers."""
+    from .utils.dataset import DeviceViews
     dev = _lib.require_cuda(points, normals, colours)
+    if not isinstance(data, DeviceViews):
+        if data.images is None or data.masks is None:
+            raise ValueError("evaluate_2d needs the data's images and masks")
+        data = data.device_views(dev)
     prm = params._replace(image_size=int(image_size))
     V, B = len(data), max(1, int(batch))
     render = _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius, shininess)
@@ -1236,8 +1273,7 @@ def evaluate_2d(points, normals, colours, data, params: SplatParams, image_size,
     for i in range(0, V, B):
         views = list(range(i, min(i + B, V)))
         image = render(prm, views)
-        rgb = torch.stack([torch.as_tensor(data.images[v]) for v in views]).to(dev).permute(0, 2, 3, 1)
-        mask = torch.stack([torch.as_tensor(data.masks[v]) for v in views]).to(dev)
+        rgb, mask = data.gather(data.upload(views))
         rows.append(image_metrics(image, rgb, mask).per_view)
     per_view = torch.cat(rows)
     means = per_view[:, 3:].mean(0)

@@ -209,11 +209,14 @@ class GraphedTrainStep(TrainStep, GraphedStep):
     the forward's tile-list capacity is frozen into the capture: replays stay correct when the lists outgrow it, and
     :meth:`stale` tells when a new capture (:meth:`capture`) would be faster.  The capture holds the library's scratch
     buffers; when a library call outside the step has reallocated them (the library's scratch total changed), the next
-    ``replay()`` captures again too."""
+    ``replay()`` captures again too.
+
+    :meth:`from_views` builds the step on views resident on the device instead: the capture gathers each batch itself,
+    and ``load_views(idx)`` takes the place of ``load``."""
     _OUTPUTS = ("loss", "image", "visibility", "inmask")
 
     def __init__(self, points, normals, colours, params: SplatParams, img, mask_img, proj, view, lights, warmup=3,
-                 **settings):
+                 _views=None, **settings):
         sync = settings.get("grad_sync")
         if sync is not None and sync.world_size > 1:
             raise NotImplementedError("GraphedTrainStep runs on one GPU; a view-sharded step runs eagerly: "
@@ -225,15 +228,66 @@ class GraphedTrainStep(TrainStep, GraphedStep):
         self.img, self.mask_img = img.detach().clone(), mask_img.detach().clone()
         self.proj, self.view = proj.detach().float().contiguous().clone(), view.detach().float().contiguous().clone()
         self.lights, self.ambient = rows.detach().clone(), ambient.detach().clone()
+        # from_views: the device views and the static (B,) index the capture gathers the batch with
+        self._views, self._index = _views if _views is not None else (None, None)
         self._warmup = max(1, int(warmup))
         self._leaves = (self.points, self.normals, self.colours)
         self.capture()
 
+    @classmethod
+    def from_views(cls, points, normals, colours, params: SplatParams, views, idx, warmup=3, **settings):
+        """The step on views resident on the device (``views``: a ``DeviceViews``), first on views ``idx`` (a host
+        list).  The capture begins with the batch: the gather of the images and masks into ``step.img`` /
+        ``step.mask_img`` and the selection of ``step.proj``, ``step.view`` and the light rows, all from one static
+        (B,) device index; ``load_views(idx)`` sets that index and ``replay()`` runs the whole iteration::
+
+            step = GraphedTrainStep.from_views(points, normals, colours, params, views, order[:B])
+            for idx in batches:
+                step.load_views(idx)
+                step.replay()
+                optimizer.step()
+
+        The batch is the one ``load(*views.batch(idx))`` would copy in, bit for bit.  ``load()`` refuses such a step:
+        the capture's gather would overwrite what it copied."""
+        if views.light_cls is None:
+            raise ValueError("the training step shades every view with its lights, and the views have none")
+        index = views.upload(idx)
+        return cls(points, normals, colours, params, *views.batch_at(index), warmup=warmup, _views=(views, index),
+                   **settings)
+
+    def _gather(self):
+        """the batch of the static index into the static inputs: the start of a from_views capture"""
+        views, index = self._views, self._index
+        views.gather(index, self.img, self.mask_img)
+        torch.index_select(views.proj, 0, index, out=self.proj)
+        torch.index_select(views.camera_mat, 0, index, out=self.view)
+        # pack_lights on the batch's light properties, as the step packs the lights it is handed: the ambient colour is
+        # summed over the lights per batch, in the order torch's reduction takes for the batch's shape
+        rows, ambient, _ = pack_lights(views.lights(index))
+        self.lights.copy_(rows)
+        self.ambient.copy_(ambient)
+
     def _eager(self):
+        if self._views is not None:
+            self._gather()
         return self._run(self.img, self.mask_img, self.proj, self.view, self.lights, self.ambient, self._light_type)
+
+    def load_views(self, idx):
+        """the next batch of a :meth:`from_views` step: the host list ``idx`` (as many views as the capture's, checked
+        by ``DeviceViews.check`` before anything is copied) into the static index, without blocking, from a fresh
+        pinned tensor"""
+        if self._views is None:
+            raise RuntimeError("load_views() needs a step made by GraphedTrainStep.from_views; use load()")
+        idx = self._views.check(idx)
+        if len(idx) != self._index.shape[0]:
+            raise ValueError("load_views() takes the capture's %d views, got %d" % (self._index.shape[0], len(idx)))
+        self._index.copy_(torch.tensor(idx, dtype=torch.int64).pin_memory(), non_blocking=True)
 
     def load(self, img, mask_img, proj, view, lights):
         """copy the next batch into the static inputs (no synchronisation)"""
+        if self._views is not None:
+            raise RuntimeError("this step gathers its batch from device views inside the capture, which would "
+                               "overwrite a loaded batch: use load_views(idx)")
         self._check_batch(img, mask_img, proj, view)
         rows, ambient, kind = pack_lights(lights)
         if kind != self._light_type or rows.shape != self.lights.shape or ambient.shape != self.ambient.shape:

@@ -6,9 +6,10 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
 
 - data: ``MVRData(data.data_dir)``, which is also the validation set.  Every epoch draws ``len(data)`` view indices
   with replacement from uniform weights (``WeightedSubsetRandomSampler``: ``torch.multinomial`` on the loop's own
-  generator) and cuts them into batches of ``training.batch_size`` views, the last partial batch dropped.  A batch is
-  staged in pinned memory (``MVRData.pinned_batch``) and uploaded without blocking; its lights are the per-image
-  ``lights_%d`` entries.
+  generator) and cuts them into batches of ``training.batch_size`` views, the last partial batch dropped.  Every view's
+  image, mask, cameras and lights (the per-image ``lights_%d`` entries) are uploaded once, at start, into a
+  ``DeviceViews`` store (``MVRData.device_views``: 4 bytes per pixel for 8-bit data); the captured step gathers each
+  batch from it (``GraphedTrainStep.from_views``), so an iteration uploads nothing but its (B,) view indices.
 - model: ``model.model_kwargs.n_points_per_cloud`` area-weighted samples of ``ico_sphere(4)`` scaled by 0.5 with their
   face normals and albedo ones (config.py:177-183), drawn from ``training.seed``.
 - optimizer: Adam, betas (0.5, 0.9), one group per learnt tensor: normals lr 0.01, points lr 0.01, colours lr 1.0
@@ -42,8 +43,9 @@ runs unchanged.
 - ``training.batch_size`` is the batch of one iteration over ALL the ranks, so G ranks solve the problem one GPU
   solves with the same config, to the summation order of the render gradients and the image-loss sums.  Every rank draws
   the same epoch order from ``training.seed`` and takes the same batch; :func:`deal_batch` deals its views by
-  ``assign_views`` over costs from the host camera matrices, and each rank stages and uploads only its own (a rank
-  dealt none runs the step's zero-view path).  Every rank keeps its own Adam, ``MultiStepLR`` and schedules: their
+  ``assign_views`` over costs from the host camera matrices, and each rank gathers its own from its copy of the device
+  views (``DeviceViews.batch``; every rank holds them all, as the views dealt to a rank change from batch to batch; a
+  rank dealt none runs the step's zero-view path).  Every rank keeps its own Adam, ``MultiStepLR`` and schedules: their
   gradients are the same bits, so the replicas stay the same and no parameters are broadcast.
 - rank 0 alone writes the log, ``metrics.jsonl``, ``config.yaml``, the checkpoints and ``val/best.ply``, loads the
   ground truth and validates; the other ranks print only errors.  The checks that can fail on the data or the config
@@ -75,7 +77,6 @@ import torch.distributed as dist
 import torch.nn.functional as F
 import yaml
 
-from ..core.camera import camera_matrices
 from ..core.cloud import PointClouds3D
 from ..ops import chamfer_distance, evaluate_2d
 from ..parallel import GradSync, agree_any, assign_views, check_replicas, view_costs_from_cameras
@@ -279,11 +280,14 @@ class Trainer:
         if self.lead:
             os.makedirs(self.val_dir, exist_ok=True)
         self.log = _Log(self.out_dir, tr["logfile"], quiet=not self.lead)
-        # ---- data: images in host memory, cameras and lights of every view on the device
+        # ---- data: every view's image, mask, cameras and lights on the device, uploaded once
         self.data = load_data(cfg)
         V = len(self.data)
-        lights = self.data.light_props(self.dev)
-        check_config(cfg, self.data.resolution, lights is not None)
+        self.views = self.data.device_views(self.dev)
+        self.log.info("Views on the device: %d of %dx%d, %s store, %.1f MB"
+                      % (V, self.views.H, self.views.W, str(self.views.store.dtype).replace("torch.", ""),
+                         self.views.nbytes / 1e6))
+        check_config(cfg, self.data.resolution, self.views.light_cls is not None)
         self.metric = selection_metric(cfg)
         self.mesh = None
         if self.metric == "p2f_avg":
@@ -293,10 +297,7 @@ class Trainer:
             if self.lead:
                 verts, faces = read_mesh(mesh_path)
                 self.mesh = (torch.from_numpy(verts).float().to(self.dev), torch.from_numpy(faces).to(self.dev))
-        self.light_cls, self.light_props = lights
         cams = self.data.get_cameras()
-        proj, _ = camera_matrices(cams)
-        self.proj_all = proj.to(self.dev)
         self.params = splat_params(cfg, cams.znear, cams.zfar)
         self.settings = step_settings(cfg)
         self.batch_size = int(tr["batch_size"])
@@ -340,29 +341,17 @@ class Trainer:
         if self.lead:
             with open(os.path.join(self.out_dir, "config.yaml"), "w") as f:
                 yaml.safe_dump(cfg, f, sort_keys=False)
-        # the step is captured on any batch of the right shape: the capture's warm-up steps leave the cloud unchanged,
-        # and every iteration loads its own batch first (the sharded step is eager and takes none)
-        self._build(points, normals, colours,
-                    self._batch(list(range(self.batch_size))) if self.sync is None else None, ckpt)
+        self._build(points, normals, colours, ckpt)
 
     # ---- pieces ------------------------------------------------------------------------------------------------------
-    def _batch(self, idx):
-        """the views ``idx`` on the device, uploaded from pinned memory without blocking"""
-        b = self.data.pinned_batch(idx)
-        idx_dev = torch.tensor(idx, dtype=torch.int64).pin_memory().to(self.dev, non_blocking=True)
-        img = b["img.rgb"].to(self.dev, non_blocking=True).permute(0, 2, 3, 1)
-        mask = b["img.mask"].to(self.dev, non_blocking=True)[:, 0]
-        view = b["camera_mat"].to(self.dev, non_blocking=True)
-        proj = self.proj_all.index_select(0, idx_dev)
-        lights = self.light_cls(**{k: v.index_select(0, idx_dev) for k, v in self.light_props.items()},
-                                device=self.dev)
-        return img, mask, proj, view, lights
-
-    def _build(self, points, normals, colours, batch, ckpt):
+    def _build(self, points, normals, colours, ckpt):
         s = dict(self.settings)
         learn, s["lambda_dr_proj"] = s.pop("learn"), self.lambda_dr_proj
         if self.sync is None:
-            self.step = GraphedTrainStep(points, normals, colours, self.params, *batch, learn=learn, **s)
+            # captured on any batch of the right shape: the capture's warm-up steps leave the cloud unchanged, and every
+            # iteration loads its own view indices first (the sharded step is eager)
+            self.step = GraphedTrainStep.from_views(points, normals, colours, self.params, self.views,
+                                                    list(range(self.batch_size)), learn=learn, **s)
         else:
             self.step = TrainStep(points, normals, colours, self.params, learn=learn, grad_sync=self.sync, **s)
         self.opt = make_optimizer({"points": self.step.points, "normals": self.step.normals,
@@ -395,7 +384,7 @@ class Trainer:
         ``batch_size`` views at a time, scored by :func:`~dss_b200.ops.evaluate_2d`."""
         if self.metric in IMAGE_METRICS:
             st = self.step
-            ev = evaluate_2d(st.points, st.normals, st.colours, self.data, self.params,
+            ev = evaluate_2d(st.points, st.normals, st.colours, self.views, self.params,
                              max(1, self.data.resolution[0] // 4), self.batch_size, st.Vrk_invariant, st.Vrk_isotropic,
                              st.frnn_radius, st.shininess)
             return {"iou": float(ev["iou"]), "psnr": float(ev["psnr"])}
@@ -494,12 +483,12 @@ class Trainer:
                 self.it += 1
                 self._schedule()
                 if self.sync is None:
-                    self.step.load(*self._batch(idx))
+                    self.step.load_views(idx)
                     if self.step.stale():
                         self.step.capture()
                     loss = self.step.replay()
                 else:
-                    loss = self.step(*self._batch(deal_batch(self.data.camera_mat, idx, self.world)[self.rank]))
+                    loss = self.step(*self.views.batch(deal_batch(self.data.camera_mat, idx, self.world)[self.rank]))
                 self.opt.step()
                 it = self.it
                 if self.lead and print_every > 0 and it % print_every == 0:

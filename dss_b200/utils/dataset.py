@@ -2,8 +2,9 @@
 scripts/create_mvr_data_from_mesh.py:170-255): the cloud in object coordinates and one 4x4 world-to-view matrix per
 image, plus the ground-truth image and mask files next to it (dataset.py:36-101: every file of ``<data_dir>/image`` /
 ``<data_dir>/mask`` with the configured extension, sorted; rgb -> (3,H,W) float32 in [0,1], mask -> (1,H,W) float 0/1),
-read with PIL (the reference uses imageio, which this image lacks).  ``pinned_batch`` stages a batch of views in pinned
-host memory for the step's host->device copy.  Dense depth maps (OpenEXR) are not read.  Host-side and cold."""
+read with PIL (the reference uses imageio, which this image lacks).  ``device_views`` uploads every view once into a
+:class:`DeviceViews` store that the training loop gathers its batches from; ``pinned_batch`` stages a batch of views in
+pinned host memory for a host->device copy.  Dense depth maps (OpenEXR) are not read."""
 import os
 
 import numpy as np
@@ -12,7 +13,7 @@ import torch
 from ..core.camera import FoVPerspectiveCameras
 from ..core.cloud import PointClouds3D
 
-__all__ = ["MVRData", "decompose_to_R_and_t"]
+__all__ = ["MVRData", "DeviceViews", "decompose_to_R_and_t"]
 
 
 def decompose_to_R_and_t(transform_mat, row_major=True):
@@ -108,6 +109,10 @@ class MVRData:
                 out[key] = pin(first.new_empty((0,) + tuple(first.shape)))
         return out
 
+    def device_views(self, device) -> "DeviceViews":
+        """every view's image, mask, cameras and lights on ``device``, uploaded once (:class:`DeviceViews`)"""
+        return DeviceViews(self, device)
+
     def __getitem__(self, idx):
         idx = idx % len(self)
         out = {"camera_mat": self.camera_mat[idx].copy()}
@@ -185,3 +190,125 @@ class MVRData:
             m = m[None]
         R, T = decompose_to_R_and_t(m)
         return FoVPerspectiveCameras(R=R.contiguous(), T=T.contiguous(), **params)
+
+
+# float32 k / 255 for every byte k, correctly rounded: what load_all_images gives for an 8-bit value k
+_BYTE_VALUES = np.arange(256, dtype=np.float32) / np.float32(255.0)
+
+
+def _as_bytes(rgb, mask):
+    """``(k, m)``: the bytes of one view, rgb (H,W,3) and mask (H,W) uint8, when every rgb value is bitwise some
+    float32 k / 255 and every mask value +0 or 1; None otherwise"""
+    if not np.isfinite(rgb).all():
+        return None
+    k = np.clip(np.rint(rgb * np.float32(255.0)), 0, 255).astype(np.uint8)
+    if not np.array_equal(_BYTE_VALUES[k].view(np.uint32), rgb.view(np.uint32)):
+        return None
+    bits = mask.view(np.uint32)
+    if not ((bits == 0) | (bits == np.float32(1.0).view(np.uint32))).all():
+        return None
+    return k.transpose(1, 2, 0), (bits != 0).astype(np.uint8)
+
+
+class DeviceViews:
+    """The views of an ``MVRData`` resident on one device, uploaded once, for the training loop and the validation
+    (``MVRData.device_views(device)``).  V = ``len(data)`` views of H x W pixels:
+
+    - ``store`` (V,H,W,4): r, g, b and mask per pixel.  uint8 when every rgb value is some float32 k / 255 and every
+      mask value 0 or 1 (a data directory's 8-bit PNGs always are: 4 bytes per pixel), else float32 with the values'
+      bits (images and masks passed to ``MVRData`` by hand, fractional masks included).  Never rounded.
+    - ``camera_mat`` (V,4,4): the world-to-view matrices; ``proj`` (V,4,4): ``camera_matrices(data.get_cameras())``.
+    - ``light_cls`` and ``light_props`` (``{property: (V,L,3)}``), as ``data.light_props`` gives them, or None when
+      the data has no lights; :meth:`lights` selects views' lights from them.
+    - ``nbytes``: the device bytes held.
+
+    :meth:`batch` gives the training step's arguments for a list of views, the same bits as uploading
+    ``data.pinned_batch``; ``ops.gather_views`` fills the images and masks from the store."""
+
+    def __init__(self, data, device):
+        from ..core.camera import camera_matrices
+        if data.images is None or data.masks is None:
+            raise ValueError("device_views needs the data's images and masks")
+        self.device = torch.device(device)
+        V = len(data)
+        self.H, self.W = data.resolution
+        rgb = [torch.as_tensor(data.images[i]).numpy() for i in range(V)]
+        mask = [torch.as_tensor(data.masks[i]).numpy() for i in range(V)]
+        for i in range(V):
+            if rgb[i].dtype != np.float32 or rgb[i].shape != (3, self.H, self.W):
+                raise TypeError("image %d must be a float32 (3, %d, %d) array, got %s %s"
+                                % (i, self.H, self.W, rgb[i].dtype, rgb[i].shape))
+            if mask[i].shape != (1, self.H, self.W):
+                raise ValueError("mask %d must have shape (1, %d, %d), got %s" % (i, self.H, self.W, mask[i].shape))
+            mask[i] = mask[i].astype(np.float32)[0]
+        as_bytes = []
+        for r, m in zip(rgb, mask):
+            b = _as_bytes(r, m)
+            if b is None:
+                as_bytes = None
+                break
+            as_bytes.append(b)
+        host = np.empty((V, self.H, self.W, 4), dtype=np.uint8 if as_bytes is not None else np.float32)
+        for i in range(V):
+            k, m = as_bytes[i] if as_bytes is not None else (rgb[i].transpose(1, 2, 0), mask[i])
+            host[i, ..., :3], host[i, ..., 3] = k, m
+        self.store = torch.from_numpy(host).to(self.device)
+        self.camera_mat = torch.from_numpy(data.camera_mat[:V]).to(self.device)
+        self.proj = camera_matrices(data.get_cameras())[0].to(self.device)
+        lights = data.light_props(self.device)
+        self.light_cls, self.light_props = (None, None) if lights is None else lights
+        held = [self.store, self.camera_mat, self.proj] + list((self.light_props or {}).values())
+        self.nbytes = sum(t.numel() * t.element_size() for t in held)
+
+    def __len__(self):
+        return self.store.shape[0]
+
+    def check(self, idx):
+        """the host list ``idx`` as view indices in [0, V): integers in [-V, V), taken % V as ``pinned_batch`` takes
+        them; IndexError for any other value (the gather does not check its device indices)"""
+        V = len(self)
+        out = []
+        for i in idx:
+            j = int(i)
+            if j != i or not -V <= j < V:
+                raise IndexError("view index %r out of range for %d views" % (i, V))
+            out.append(j % V)
+        return out
+
+    def upload(self, idx):
+        """``idx`` (checked by :meth:`check`) as a (B,) int64 tensor on the device, copied without blocking from a
+        fresh pinned tensor (the caching host allocator keeps it until the copy has run)"""
+        t = torch.tensor(self.check(idx), dtype=torch.int64)
+        if self.device.type == "cuda":
+            t = t.pin_memory()
+        return t.to(self.device, non_blocking=True)
+
+    def gather(self, idx_dev, img=None, mask=None):
+        """``(img (B,H,W,3), mask (B,H,W))`` float32 of the device indices ``idx_dev`` (``ops.gather_views``), into
+        ``img`` / ``mask`` when given"""
+        from ..ops import gather_views
+        B = idx_dev.shape[0]
+        if img is None:
+            img = torch.empty((B, self.H, self.W, 3), dtype=torch.float32, device=self.device)
+        if mask is None:
+            mask = torch.empty((B, self.H, self.W), dtype=torch.float32, device=self.device)
+        return gather_views(self.store, idx_dev, img, mask)
+
+    def lights(self, idx_dev):
+        """the lights of the device indices ``idx_dev``: ``light_cls`` with every property's rows ``idx_dev`` (what the
+        training loop built from ``data.light_props``), or None without lights"""
+        if self.light_cls is None:
+            return None
+        return self.light_cls(**{k: v.index_select(0, idx_dev) for k, v in self.light_props.items()},
+                              device=self.device)
+
+    def batch_at(self, idx_dev):
+        """``(img, mask, proj, view, lights)`` of the device indices ``idx_dev``: the training step's arguments"""
+        img, mask = self.gather(idx_dev)
+        return (img, mask, self.proj.index_select(0, idx_dev), self.camera_mat.index_select(0, idx_dev),
+                self.lights(idx_dev))
+
+    def batch(self, idx):
+        """``(img (B,H,W,3), mask (B,H,W), proj (B,4,4), view (B,4,4), lights)`` on the device for the host list
+        ``idx`` (checked before anything is uploaded); an empty ``idx`` gives batch-0 tensors"""
+        return self.batch_at(self.upload(idx))

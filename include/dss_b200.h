@@ -413,6 +413,17 @@ DSS_API int dss_image_metrics(dss_ctx *ctx, const float *pred, int s, const floa
                               const void *mask, int mask_kind, int V, int H, int W, double *per_view, double *means,
                               void *stream);
 
+/* ---- training views resident on the device ----------------------------------------------------------------------
+ * Gathers views idx[0..B) of a store (n_store, H, W, 4) contiguous, r, g, b, mask per pixel, uint8 (store_f32 == 0,
+ * 4-byte aligned) or float32 (store_f32 == 1, 16-byte aligned), into img (B, H, W, 3) and mask (B, H, W), float32,
+ * contiguous, 4-byte aligned.  uint8: rgb = __fdiv_rn((float)u, 255.f) (what numpy's correctly rounded float32 u / 255.0
+ * gives), mask = u != 0 ? 1.f : 0.f; float32: the values' bits unchanged.  idx: B int64 on the device; PRECONDITION:
+ * every idx[b] lies in [0, n_store) (not checked: the caller validates the indices before it uploads them).  Repeats
+ * are allowed.  0 <= B <= 65535; B == 0 launches nothing.  64-bit offsets throughout.  One launch on the caller's
+ * stream, no allocation, no host synchronisation: capturable. */
+DSS_API int dss_gather_views(dss_ctx *ctx, const void *store, int store_f32, int64_t n_store, int H, int W,
+                             const int64_t *idx, int B, float *img, float *mask, void *stream);
+
 /* ---- point filters of the training step -------------------------------------------------------------------------
  * Model.forward's visibility and inmask filters (DSS/models/point_modeling.py:172-173, 188-212) of one SHARED cloud of
  * P0 points seen by N cameras (shared_cloud must be 1: packed clouds return DSS_E_INVALID), from the forward's records

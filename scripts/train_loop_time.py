@@ -1,16 +1,23 @@
 """Time the training loop's pieces: ops.chamfer_distance (csrc/chamfer.cu) at 8000 ground-truth points against 5 000,
 100 000 and 1 000 000 model points with normals, next to a torch brute force (torch.cdist in chunks on the GPU), and the
-loop of dss_b200.training.train at configs/dss.yml's settings (by default 5000 points, 8 views per batch, 512^2) next to
-bare GraphedTrainStep.replay() on the same batches.
+loop of dss_b200.training.train at configs/dss.yml's settings (512^2 views) at each size of ``--points`` / ``--batch``
+(by default 5 000 points with 8 views per batch, and 1 000 000 with 64), next to three arms on the same batches, in the
+same process, each over ``--loop-its`` iterations:
 
-    python scripts/train_loop_time.py [--iters 20] [--loop-its 200] [--points 5000] [--batch 8] [--ranks G]
-                                      [--out results.json]
+  replay    -- bare GraphedTrainStep.replay() of a batch already loaded;
+  staged    -- MVRData.pinned_batch, the non-blocking upload, load() and replay(): the loop before its views were
+               resident on the device;
+  resident  -- load_views() and replay() of the loop's own step (GraphedTrainStep.from_views): what the loop does.
 
-CUDA events around each chamfer call, median after warm-up.  The loop's rate is taken between two of its own logged
-records (each ends in a host synchronisation), after the capture and a warm-up.  ``--ranks G`` > 1 runs the loop as G
-NCCL ranks, one process and one GPU each, started with torchrun's variables (the view-sharded eager step; no bare
-replays), and reports rank 0's rate; a G larger than the number of visible GPUs is refused.  The data has
-max(64, batch) views.  Prints one JSON line with the card name and its power limit."""
+    python scripts/train_loop_time.py [--iters 20] [--loop-its 200] [--points 5000 1000000] [--batch 8 64]
+                                      [--ranks G] [--no-chamfer] [--out results.json]
+
+CUDA events around each chamfer call, median after warm-up.  The arms are host wall-clock rates between two device
+synchronisations.  The loop's rate is taken between two of its own logged records (each ends in a host
+synchronisation), after the capture and a warm-up.  ``--ranks G`` > 1 runs the loop as G NCCL ranks, one process and
+one GPU each, started with torchrun's variables (the view-sharded eager step; no arms), and reports rank 0's rate; a G
+larger than the number of visible GPUs is refused.  The data has max(64, batch) views.  Prints one JSON line with the
+card name and its power limit."""
 import argparse
 import json
 import os
@@ -139,20 +146,7 @@ def loop_times(dev, loop_its, tmp, points=5000, batch=8, ranks=1):
            "loop_its_timed": last["it"] - first["it"]}
     if t is None:
         return res
-    # bare replays of the same step on batches already on the device
-    step = t.step
-    batches = [t._batch(t.order[i:i + batch]) for i in range(0, n_views - batch + 1, batch)]
-    torch.cuda.synchronize()
-    for b in batches:
-        step.load(*b)
-        step.replay()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for i in range(loop_its):
-        step.load(*batches[i % len(batches)])
-        step.replay()
-    torch.cuda.synchronize()
-    res["replay_it_per_s"] = loop_its / (time.perf_counter() - t0)
+    res.update(arm_rates(t, n_views, batch, loop_its))
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     ev = t.evaluate()
@@ -161,27 +155,77 @@ def loop_times(dev, loop_its, tmp, points=5000, batch=8, ranks=1):
     return res
 
 
+def staged_batch(data, dev, proj_all, light_props, idx):
+    """the views ``idx`` as the loop staged them before they were resident: pinned, uploaded without blocking"""
+    b = data.pinned_batch(idx)
+    idx_dev = torch.tensor(idx, dtype=torch.int64).pin_memory().to(dev, non_blocking=True)
+    img = b["img.rgb"].to(dev, non_blocking=True).permute(0, 2, 3, 1)
+    mask = b["img.mask"].to(dev, non_blocking=True)[:, 0]
+    view = b["camera_mat"].to(dev, non_blocking=True)
+    light_cls, props = light_props
+    lights = light_cls(**{k: v.index_select(0, idx_dev) for k, v in props.items()}, device=dev)
+    return img, mask, proj_all.index_select(0, idx_dev), view, lights
+
+
+def arm_rates(t, n_views, batch, loop_its):
+    """it/s of the three arms on the same batches (the loop's last epoch order, cut into batches)"""
+    from dss_b200.core.camera import camera_matrices
+    from dss_b200.training.step import GraphedTrainStep
+    dev, data, resident = t.dev, t.data, t.step
+    proj_all = camera_matrices(data.get_cameras())[0].to(dev)
+    light_props = data.light_props(dev)
+    batches = [t.order[i:i + batch] for i in range(0, n_views - batch + 1, batch)]
+    stage = lambda idx: staged_batch(data, dev, proj_all, light_props, idx)
+    s = dict(t.settings)
+    learn, s["lambda_dr_proj"] = s.pop("learn"), t.lambda_dr_proj
+    staged = GraphedTrainStep(resident.points.detach(), resident.normals.detach(), resident.colours.detach(), t.params,
+                              *stage(batches[0]), learn=learn, **s)
+    arms = {
+        "replay": lambda idx: staged.replay(),
+        "staged": lambda idx: (staged.load(*stage(idx)), staged.replay()),
+        "resident": lambda idx: (resident.load_views(idx), resident.replay()),
+    }
+    out = {}
+    for name, fn in arms.items():
+        for idx in batches[:3]:
+            fn(idx)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for i in range(loop_its):
+            fn(batches[i % len(batches)])
+        torch.cuda.synchronize()
+        out["%s_it_per_s" % name] = loop_its / (time.perf_counter() - t0)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--loop-its", type=int, default=200)
-    ap.add_argument("--points", type=int, default=5000, help="the loop's cloud size")
-    ap.add_argument("--batch", type=int, default=8, help="the loop's views per batch (over all the ranks)")
+    ap.add_argument("--points", type=int, nargs="+", default=[5000, 1000000], help="the loop's cloud sizes")
+    ap.add_argument("--batch", type=int, nargs="+", default=[8, 64],
+                    help="the loop's views per batch (over all the ranks), one per --points")
     ap.add_argument("--ranks", type=int, default=1, help="run the loop as this many NCCL ranks, one GPU each")
+    ap.add_argument("--no-chamfer", action="store_true", help="time the loop alone")
     ap.add_argument("--out", default=None)
     opt = ap.parse_args()
     have = torch.cuda.device_count()
     if opt.ranks < 1 or opt.ranks > have:
         raise SystemExit("--ranks %d: the loop runs one rank per GPU and %d GPU%s visible"
                          % (opt.ranks, have, " is" if have == 1 else "s are"))
+    if len(opt.points) != len(opt.batch):
+        raise SystemExit("--points and --batch take one value per loop size")
     dev = torch.device("cuda:0")
-    res = chamfer_times(dev, opt.warmup, opt.iters)
-    tmp = tempfile.mkdtemp(prefix="dss_loop_time_")
-    try:
-        res.update(loop_times(dev, opt.loop_its, tmp, opt.points, opt.batch, opt.ranks))
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
+    res = {} if opt.no_chamfer else chamfer_times(dev, opt.warmup, opt.iters)
+    res["loops"] = []
+    for points, batch in zip(opt.points, opt.batch):
+        tmp = tempfile.mkdtemp(prefix="dss_loop_time_")
+        try:
+            res["loops"].append(loop_times(dev, opt.loop_its, tmp, points, batch, opt.ranks))
+        finally:
+            shutil.rmtree(tmp, ignore_errors=True)
+        torch.cuda.empty_cache()
     gpu = card()
     res["card"], res["power_limit"] = gpu["name"], gpu["power_limit"]
     print(json.dumps(res))
