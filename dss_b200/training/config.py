@@ -9,8 +9,9 @@ import warnings
 
 import yaml
 
-__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "step_settings", "splat_params",
-           "EVAL_SAMPLINGS", "SELECTION_METRICS", "IMAGE_METRICS", "selection_metric"]
+__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "cloud_size",
+           "check_cloud_size", "GROW_K", "step_settings", "splat_params", "EVAL_SAMPLINGS", "SELECTION_METRICS",
+           "IMAGE_METRICS", "selection_metric"]
 
 EVAL_SAMPLINGS = ("uniform", "poisson_disk")
 
@@ -41,8 +42,13 @@ DEFAULTS = {
         "resume_from": "model.pt", "model_selection_metric": "chamfer_point", "model_selection_mode": "minimize",
         "n_eval_points": 8000, "steps_dss_backward_radii": 100, "steps_proj": -1, "gamma_proj": 5,
         "eval_sampling": "uniform",
+        "grow_milestones": [], "grow_points": [],
     },
 }
+
+# the neighbourhood size of the loop's growth events (ops.upsample_points' default): a cloud that grows needs more
+# than GROW_K and at least 10 points
+GROW_K = 16
 
 # Keys of the reference's configurations that change nothing in its point-model training with data lights (the
 # renderer classes it instantiates are the ones this loop runs, `learning_rate` is overridden by the per-group rates,
@@ -129,6 +135,66 @@ def check_config(cfg, resolution, has_lights):
                          % (S, None if resolution is None else tuple(resolution)))
     if not has_lights:
         raise ValueError("the data directory has no lights_%d entries: the loop shades with the data's lights")
+    check_growth(cfg)
+
+
+def _is_int(x):
+    return isinstance(x, int) and not isinstance(x, bool)
+
+
+def check_growth(cfg):
+    """Refuse a growth schedule the loop cannot follow: ``training.grow_milestones`` (the iterations at whose start the
+    cloud grows) and ``training.grow_points`` (its size from that iteration on) must be lists of one length, the
+    milestones strictly increasing integers >= 1, the sizes strictly increasing integers above
+    ``model.model_kwargs.n_points_per_cloud``, and that initial cloud one ``ops.upsample_points`` can grow with k =
+    :data:`GROW_K` (more than k and at least 10 points)."""
+    from ..ops import upsample_schedule
+    tr = cfg["training"]
+    ms, ns = tr.get("grow_milestones", []), tr.get("grow_points", [])
+    if not isinstance(ms, (list, tuple)) or not isinstance(ns, (list, tuple)):
+        raise ValueError("training.grow_milestones and training.grow_points must be lists, got %r and %r" % (ms, ns))
+    if len(ms) != len(ns):
+        raise ValueError("training.grow_milestones has %d entries and training.grow_points %d: they must pair up"
+                         % (len(ms), len(ns)))
+    if not ms:
+        return
+    if not all(_is_int(m) for m in ms) or ms[0] < 1 or any(b <= a for a, b in zip(ms, ms[1:])):
+        raise ValueError("training.grow_milestones must be strictly increasing integers >= 1, got %r" % (list(ms),))
+    n0 = cfg["model"]["model_kwargs"]["n_points_per_cloud"]
+    if not all(_is_int(n) for n in ns) or any(b <= a for a, b in zip(ns, ns[1:])):
+        raise ValueError("training.grow_points must be strictly increasing integers, got %r" % (list(ns),))
+    if ns[0] <= n0:
+        raise ValueError("training.grow_points must start above model.model_kwargs.n_points_per_cloud (%d), got %r"
+                         % (n0, list(ns)))
+    try:
+        upsample_schedule([n0], [ns[0]], GROW_K)
+    except ValueError as e:
+        raise ValueError("training.grow_points: the initial cloud of n_points_per_cloud = %d points cannot grow (%s)"
+                         % (n0, e)) from None
+
+
+def cloud_size(cfg, it):
+    """The cloud's size during (and after) iteration ``it`` under the growth schedule: the ``grow_points`` entry of the
+    last milestone <= ``it``, or ``n_points_per_cloud`` before the first (``it`` = -1: the initial cloud)."""
+    tr = cfg["training"]
+    n = int(cfg["model"]["model_kwargs"]["n_points_per_cloud"])
+    for m, size in zip(tr.get("grow_milestones", []), tr.get("grow_points", [])):
+        if int(m) <= it:
+            n = int(size)
+    return n
+
+
+def check_cloud_size(cfg, it, n_points):
+    """Refuse a checkpoint of ``n_points`` points saved after iteration ``it`` when a growth schedule is configured and
+    gives another size at ``it`` (say, the schedule or ``n_points_per_cloud`` was edited since).  Without a schedule the
+    checkpoint's cloud is taken at whatever size it has, as it always was."""
+    if not cfg["training"].get("grow_milestones"):
+        return
+    want = cloud_size(cfg, it)
+    if int(n_points) != want:
+        raise ValueError("the checkpoint holds %d points after it=%d, but model.model_kwargs.n_points_per_cloud with "
+                         "training.grow_milestones / grow_points gives %d there: the configuration changed since it "
+                         "was written" % (n_points, it, want))
 
 
 IMAGE_METRICS = ("iou", "psnr")

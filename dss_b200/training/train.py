@@ -26,6 +26,12 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   the validation is the reference's ``evaluate_2d`` instead (see :meth:`Trainer.evaluate`): it needs only the images,
   masks, cameras and lights, so data without a ground-truth cloud (``points`` / ``normals``) or mesh trains;
   ``model.pt`` every ``checkpoint_every``, ``model_%d.pt`` every ``backup_every``.
+- growth (``training.grow_milestones`` / ``grow_points``, empty by default): at the start of iteration
+  ``grow_milestones[i]``, before the schedules and the batch, the cloud grows to ``grow_points[i]`` points
+  (:meth:`Trainer.grow`): its rows and their Adam moments stay, the new rows and their moments come from one
+  ``upsample_points`` call, and the step is built anew with Adam and ``MultiStepLR`` continuing from their state.
+  A checkpoint holds the cloud at its size; a resumed run grows at the milestones still ahead, and refuses a
+  checkpoint whose size is not the one the schedule gives at its ``it``.
 - ``training.resume_from`` (in ``<out>``) is loaded when it exists, and the run continues where it stopped, mid-epoch
   included: a resumed run computes what an uninterrupted one does.  (The reference starts a new epoch.)
 - ``--exit-after S`` saves ``model.pt`` and exits with status 3 once S seconds have passed (checked after every
@@ -61,6 +67,8 @@ runs unchanged.
   previous checkpoint whole.
 - every rank loads ``training.resume_from``; the checkpoint does not depend on G, so a run resumes on another number
   of GPUs (mid-epoch included), and on the same number continues bit for bit.
+- every rank grows its replica at a milestone with the same deterministic call, builds a new eager step, and the
+  ranks check right after it that their points, normals, colours and Adam moments are the same bits.
 """
 import argparse
 import errno
@@ -78,14 +86,14 @@ import torch.nn.functional as F
 import yaml
 
 from ..core.cloud import PointClouds3D
-from ..ops import chamfer_distance, evaluate_2d
+from ..ops import chamfer_distance, evaluate_2d, upsample_points
 from ..parallel import GradSync, agree_any, assign_views, check_replicas, view_costs_from_cameras
 from ..utils.create_mvr_data import ico_sphere, sample_points_from_mesh
 from ..utils.dataset import MVRData
 from ..utils.evaluate import p2f_stats
 from ..utils.io import read_mesh, save_ply
-from .config import (EVAL_SAMPLINGS, IMAGE_METRICS, check_config, load_config, selection_metric, splat_params,
-                     step_settings)
+from .config import (EVAL_SAMPLINGS, GROW_K, IMAGE_METRICS, check_cloud_size, check_config, load_config,
+                     selection_metric, splat_params, step_settings)
 from .step import GraphedTrainStep, TrainStep
 
 __all__ = ["radii_backward_scaler", "compound_lambda_proj", "initial_cloud", "make_optimizer", "make_lr_scheduler",
@@ -337,14 +345,19 @@ class Trainer:
             self.order, self.pos = ckpt["epoch_order"], int(ckpt["epoch_pos"])
             self.lambda_dr_proj = float(ckpt["schedule"]["lambda_dr_proj"])
             self.params = self.params._replace(radii_backward_scaler=float(ckpt["schedule"]["radii_backward_scaler"]))
+            check_cloud_size(cfg, self.it, points.shape[0])
             self.log.info("resumed from %s at it=%d, epoch %d" % (ckpt_path, self.it, self.epoch_it))
+        # the growth schedule: {iteration: the cloud's size from its start on}
+        self.grow_at = {int(m): int(n) for m, n in zip(tr.get("grow_milestones", []), tr.get("grow_points", []))}
         if self.lead:
             with open(os.path.join(self.out_dir, "config.yaml"), "w") as f:
                 yaml.safe_dump(cfg, f, sort_keys=False)
-        self._build(points, normals, colours, ckpt)
+        self._build(points, normals, colours, None if ckpt is None else (ckpt["optimizer"], ckpt["lr_scheduler"]))
 
     # ---- pieces ------------------------------------------------------------------------------------------------------
-    def _build(self, points, normals, colours, ckpt):
+    def _build(self, points, normals, colours, state=None):
+        """the step on this cloud, its Adam and ``MultiStepLR``; ``state``: (optimizer, lr scheduler) state dicts to
+        continue from (a checkpoint's, or those of a growth event)"""
         s = dict(self.settings)
         learn, s["lambda_dr_proj"] = s.pop("learn"), self.lambda_dr_proj
         if self.sync is None:
@@ -357,9 +370,41 @@ class Trainer:
         self.opt = make_optimizer({"points": self.step.points, "normals": self.step.normals,
                                    "colours": self.step.colours})
         self.lr_sched = make_lr_scheduler(self.opt, self.cfg)
-        if ckpt is not None:
-            self.opt.load_state_dict(ckpt["optimizer"])
-            self.lr_sched.load_state_dict(ckpt["lr_scheduler"])
+        if state is not None:
+            self.opt.load_state_dict(state[0])
+            self.lr_sched.load_state_dict(state[1])
+
+    def grow(self, n):
+        """The growth event: the cloud grows from P to ``n`` points, at the start of a milestone's iteration.  The P
+        rows of the points, normals and colours and of Adam's moments stay as they are; the new rows are those of one
+        ``upsample_points(points, n, k=GROW_K)`` call that is given the unit normals and, as features, the colours and
+        the moments of every learnt tensor side by side, so that a child's moments follow the ``(f_q + 2 f_p) / 3``
+        rule of its colour (a child with zero moments would take a first step of about 1.6 lr in every coordinate:
+        Adam's step count, and with it the bias correction, is shared by the whole tensor).  The step is built anew on
+        the grown cloud (the old one and its graph dropped first), and Adam and ``MultiStepLR`` continue from the old
+        ones' state: step counts, betas and the current learning rates.  Deterministic, so replicas stay replicas."""
+        s, opt = self.step, self.opt
+        P = s.points.shape[0]
+        t0 = time.perf_counter()
+        old = {"points": s.points.detach(), "normals": s.normals.detach(), "colours": s.colours.detach()}
+        sd = opt.state_dict()
+        keys = [(i, k) for i in sorted(sd["state"]) for k in ("exp_avg", "exp_avg_sq")]
+        moments = [sd["state"][i][k] for i, k in keys]
+        up = upsample_points(old["points"], n, k=GROW_K, normals=F.normalize(old["normals"], dim=-1),
+                             features=torch.cat([old["colours"]] + moments, 1))
+        grown = lambda rows, new: torch.cat([rows, new[P:]])
+        points, normals = grown(old["points"], up.points), grown(old["normals"], up.normals)
+        cols = torch.split(up.features, 3, 1)
+        colours = grown(old["colours"], cols[0])
+        state = {i: dict(st) for i, st in sd["state"].items()}
+        for (i, k), m, col in zip(keys, moments, cols[1:]):
+            state[i][k] = grown(m, col)
+        sched = self.lr_sched.state_dict()
+        self.step = self.opt = self.lr_sched = s = opt = up = None     # the old step and its graph go first
+        self._build(points, normals, colours, (dict(sd, state=state), sched))
+        torch.cuda.synchronize(self.dev)
+        self.log.info("Grew the cloud at it=%d: %d -> %d points (%.1f ms: upsample and new step)"
+                      % (self.it, P, n, 1e3 * (time.perf_counter() - t0)))
 
     def _schedule(self):
         """TrainerScheduler.step (trainer.py:227) before the step; a changed setting makes the next replay capture"""
@@ -429,16 +474,23 @@ class Trainer:
         }, tmp)
         os.replace(tmp, path)
 
-    def check_replicas(self):
+    def check_replicas(self, event=False):
         """the replica guard of a sharded run, before an iteration's checkpoints: every rank raises unless the ranks'
         points, normals and colours are the same bits (one all-reduce, one host synchronisation).  Once per
-        iteration; nothing on one GPU."""
-        if self.sync is None or self._checked_it == self.it:
+        iteration; nothing on one GPU.  ``event``: the check right after a growth event, before the iteration's step,
+        which also covers Adam's moments and leaves the guard of the iteration's checkpoints to run."""
+        if self.sync is None or (not event and self._checked_it == self.it):
             return
         s = self.step
-        check_replicas((("points", s.points), ("normals", s.normals), ("colours", s.colours)), self.sync.group)
-        self._checked_it = self.it
-        self.log.info("Replica check: the %d ranks hold the same points, normals and colours" % self.world)
+        named = [("points", s.points), ("normals", s.normals), ("colours", s.colours)]
+        if event:
+            named += [("Adam's %s of the %s" % (k, n), self.opt.state[t][k]) for n, t in named
+                      if t in self.opt.state for k in ("exp_avg", "exp_avg_sq")]
+        check_replicas(named, self.sync.group)
+        if not event:
+            self._checked_it = self.it
+        self.log.info("Replica check: the %d ranks hold the same points, normals and colours%s"
+                      % (self.world, " and Adam moments" if event else ""))
 
     def _out_of_time(self, exit_after, t0):
         """whether to leave after this iteration; a sharded run's ranks agree (any rank's clock decides for all)"""
@@ -481,6 +533,9 @@ class Trainer:
                 idx = self.order[self.pos:self.pos + bs]
                 self.pos += bs
                 self.it += 1
+                if self.it in self.grow_at:
+                    self.grow(self.grow_at[self.it])
+                    self.check_replicas(event=True)
                 self._schedule()
                 if self.sync is None:
                     self.step.load_views(idx)
