@@ -26,7 +26,8 @@ __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_poi
            "estimate_normals", "Outliers", "outlier_ratio", "Upsampled", "upsample_schedule", "upsample_points",
            "denoise_normals", "Projected", "project_to_surface", "l0_smooth", "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
-           "ImageMetrics", "image_metrics", "gather_views", "shared_cloud_splats", "render_data_views", "evaluate_2d"]
+           "ImageMetrics", "image_metrics", "gather_views", "shared_cloud_splats", "render_data_views", "evaluate_2d",
+           "Coverage", "accumulate_coverage", "point_coverage"]
 
 
 class SplatParams(NamedTuple):
@@ -355,6 +356,27 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
 
 
+def _shared_render_masks(out: RenderOutput, mask_img):
+    """``(device, P0, head)`` of a shared-cloud render and its N masks, checked: ``head`` the leading C-ABI arguments
+    (records, visible, shared_cloud, N, P0, mask, mask_kind, mask_strides, H, W) of dss_point_filters and
+    dss_point_coverage"""
+    N = out.image.shape[0]
+    P = out.records.shape[0]
+    if out.image.dim() != 4 or tuple(out.records.shape[1:]) != (8,) or P % N or tuple(out.visible.shape) != (P,):
+        raise RuntimeError("out must be the RenderOutput of a shared cloud: records (N*P0, 8) and visible (N*P0,)")
+    if mask_img.dim() == 4 and mask_img.shape[1] == 1:
+        mask_img = mask_img[:, 0]
+    if mask_img.dim() != 3 or mask_img.shape[0] != N or mask_img.shape[1] < 1 or mask_img.shape[2] < 1:
+        raise RuntimeError("mask_img must have shape (%d, H, W) or (%d, 1, H, W), got %s" % (N, N, tuple(mask_img.shape)))
+    if mask_img.dtype not in (torch.float32, torch.uint8, torch.bool):
+        raise TypeError("mask_img must be float32, uint8 or bool, got %s" % mask_img.dtype)
+    dev = _lib.require_cuda(out.records, out.visible, mask_img)
+    P0 = P // N
+    strides = (C.c_int64 * 3)(*mask_img.stride())
+    return dev, P0, (out.records, out.visible, 1, N, P0, mask_img, int(mask_img.dtype != torch.float32), strides,
+                     int(mask_img.shape[1]), int(mask_img.shape[2]))
+
+
 def point_filters(out: RenderOutput, mask_img, group=None):
     """The visibility and inmask point filters of the reference's ``Model.forward`` (point_modeling.py:172-173,
     188-212) for the SHARED cloud that ``render_points`` drew in ``out``: ``visibility`` = visible in any view,
@@ -369,21 +391,7 @@ def point_filters(out: RenderOutput, mask_img, group=None):
     filters are then those of all the views, the same on every rank (exact: ORs of bytes).  Two launches and two
     all-reduces (MAX) of P0 bytes: this rank's visibility, ORed over the ranks, gates ``dss_point_filters_gated``,
     whose inmask is ORed over the ranks in turn.  A rank without views calls :func:`point_filters_no_views`."""
-    N = out.image.shape[0]
-    P = out.records.shape[0]
-    if out.image.dim() != 4 or tuple(out.records.shape[1:]) != (8,) or P % N or tuple(out.visible.shape) != (P,):
-        raise RuntimeError("out must be the RenderOutput of a shared cloud: records (N*P0, 8) and visible (N*P0,)")
-    if mask_img.dim() == 4 and mask_img.shape[1] == 1:
-        mask_img = mask_img[:, 0]
-    if mask_img.dim() != 3 or mask_img.shape[0] != N or mask_img.shape[1] < 1 or mask_img.shape[2] < 1:
-        raise RuntimeError("mask_img must have shape (%d, H, W) or (%d, 1, H, W), got %s" % (N, N, tuple(mask_img.shape)))
-    if mask_img.dtype not in (torch.float32, torch.uint8, torch.bool):
-        raise TypeError("mask_img must be float32, uint8 or bool, got %s" % mask_img.dtype)
-    dev = _lib.require_cuda(out.records, out.visible, mask_img)
-    P0 = P // N
-    strides = (C.c_int64 * 3)(*mask_img.stride())
-    head = (out.records, out.visible, 1, N, P0, mask_img, int(mask_img.dtype != torch.float32), strides,
-            int(mask_img.shape[1]), int(mask_img.shape[2]))
+    dev, P0, head = _shared_render_masks(out, mask_img)
     if group is None:
         visibility = torch.empty((P0,), dtype=torch.bool, device=dev)
         inmask = torch.empty((P0,), dtype=torch.bool, device=dev)
@@ -415,6 +423,30 @@ def set_point_filters(points_filter, out: RenderOutput, mask_img):
     visibility, inmask = point_filters(out, mask_img)
     points_filter.set_filter(visibility=visibility[None], inmask=inmask[None])
     return points_filter
+
+
+class Coverage(NamedTuple):
+    seen: torch.Tensor       # (P0,) int32: the views in which the point is in some pixel's K-list
+    outside: torch.Tensor    # (P0,) int32: the views in which it is kept, in the frame and over background
+
+
+def accumulate_coverage(out: RenderOutput, mask_img, seen, outside):
+    """Add the view coverage of the SHARED cloud that ``render_points`` drew in ``out`` to the (P0,) int32 counters
+    ``seen`` and ``outside`` (csrc/prune.cu; the rule is in include/dss_b200.h): ``seen[i]`` += the number of views in
+    which point i is in some pixel's K-list (``out.visible``), ``outside[i]`` += the number of views in which the
+    preprocess kept it (record z > 0), it projects inside the frame (finite x, y with ``|x|, |y| <= 1``) and the
+    ``mask_img`` sample there, the one :func:`point_filters` takes, is zero.  Not gated on visibility: a visual-hull
+    test.  ``mask_img`` as :func:`point_filters` takes it.  One launch, no host synchronisation, deterministic:
+    capturable.  Returns ``Coverage(seen, outside)``."""
+    dev, P0, head = _shared_render_masks(out, mask_img)
+    for name, t in (("seen", seen), ("outside", outside)):
+        if not isinstance(t, torch.Tensor) or t.dtype != torch.int32 or tuple(t.shape) != (P0,) \
+                or not t.is_contiguous() or t.device != dev:
+            raise RuntimeError("%s must be a contiguous int32 tensor of shape (%d,) on %s, got %s" % (
+                name, P0, dev, "%s %s on %s" % (t.dtype, tuple(t.shape), t.device) if isinstance(t, torch.Tensor)
+                else type(t).__name__))
+    _lib.call("dss_point_coverage", dev, *head, seen, outside)
+    return Coverage(seen, outside)
 
 
 def make_shading(lights, view_matrices, shininess=64.0) -> Shading:
@@ -1204,8 +1236,8 @@ def shared_cloud_splats(points, n_views, Vrk_invariant=True, Vrk_isotropic=True,
 
 
 def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius, shininess):
-    """render(params, views) -> the renders of :func:`render_data_views`, with what does not depend on the views (the
-    cloud's splat sizes, all the views' cameras and lights on the device) computed once"""
+    """render(params, views) -> the ``RenderOutput`` whose image :func:`render_data_views` returns, with what does not
+    depend on the views (the cloud's splat sizes, all the views' cameras and lights on the device) computed once"""
     from .core.camera import camera_matrices
     from .core.lighting import pack_lights
     from .core.texture import camera_centres
@@ -1235,7 +1267,7 @@ def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotr
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), kind, float(shininess))
             return render_points(p, n, c, proj_all.index_select(0, idx), view,
                                  None if h1 is None else h1.repeat(idx.shape[0]), params, shading=shading,
-                                 deterministic=True, frames=frames).image
+                                 deterministic=True, frames=frames)
     return render
 
 
@@ -1247,7 +1279,7 @@ def render_data_views(points, normals, colours, data, params: SplatParams, views
     step renders a batch: unit normals, the splats of :func:`shared_cloud_splats`, ``colours`` the albedo.  Forward
     only."""
     return _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius,
-                               shininess)(params, views)
+                               shininess)(params, views).image
 
 
 def evaluate_2d(points, normals, colours, data, params: SplatParams, image_size, batch=1, Vrk_invariant=True,
@@ -1272,9 +1304,40 @@ def evaluate_2d(points, normals, colours, data, params: SplatParams, image_size,
     rows = []
     for i in range(0, V, B):
         views = list(range(i, min(i + B, V)))
-        image = render(prm, views)
+        image = render(prm, views).image
         rgb, mask = data.gather(data.upload(views))
         rows.append(image_metrics(image, rgb, mask).per_view)
     per_view = torch.cat(rows)
     means = per_view[:, 3:].mean(0)
     return {"iou": means[0], "psnr": means[1], "per_view": per_view}
+
+
+def point_coverage(points, normals, data, params: SplatParams, batch=1, views=None, Vrk_invariant=True,
+                   Vrk_isotropic=True, frnn_radius=0.2) -> Coverage:
+    """The view coverage of one shared cloud over views of ``data``: :func:`accumulate_coverage` of the renders of
+    ``views`` (default all of ``data``'s views), ``batch`` at a time, each against its ground-truth masks, gathered from
+    the views' store (:func:`gather_views`).  The renders are :func:`render_data_views`' at ``params`` (unit normals,
+    the splats of :func:`shared_cloud_splats`); a point's K-list membership in a view depends on that view alone, so the
+    counts do not depend on ``batch``.  ``data``: a ``DeviceViews`` or an ``MVRData`` with images and masks, whose
+    ``device_views`` this builds first.  Returns ``Coverage(seen, outside)``, (P0,) int32 counts of views."""
+    from .utils.dataset import DeviceViews
+    dev = _lib.require_cuda(points, normals)
+    if not isinstance(data, DeviceViews):
+        if data.images is None or data.masks is None:
+            raise ValueError("point_coverage needs the data's images and masks")
+        data = data.device_views(dev)
+    views = list(range(len(data))) if views is None else list(views)
+    B = max(1, int(batch))
+    P0 = points.shape[0]
+    cov = Coverage(torch.zeros((P0,), dtype=torch.int32, device=dev), torch.zeros((P0,), dtype=torch.int32, device=dev))
+    if not views:
+        return cov
+    # the albedo and the shininess change the shading alone, not which points a view keeps or draws
+    render = _data_view_renderer(points, normals, torch.ones_like(points), data, Vrk_invariant, Vrk_isotropic,
+                                 frnn_radius, 64.0)
+    for i in range(0, len(views), B):
+        part = views[i:i + B]
+        out = render(params, part)
+        _, mask = data.gather(data.upload(part))
+        accumulate_coverage(out, mask, *cov)
+    return cov

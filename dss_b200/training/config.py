@@ -9,8 +9,8 @@ import warnings
 
 import yaml
 
-__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "cloud_size",
-           "check_cloud_size", "GROW_K", "step_settings", "splat_params", "EVAL_SAMPLINGS", "SELECTION_METRICS",
+__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "check_pruning",
+           "cloud_size", "check_cloud_size", "GROW_K", "step_settings", "splat_params", "EVAL_SAMPLINGS", "SELECTION_METRICS",
            "IMAGE_METRICS", "selection_metric"]
 
 EVAL_SAMPLINGS = ("uniform", "poisson_disk")
@@ -43,11 +43,12 @@ DEFAULTS = {
         "n_eval_points": 8000, "steps_dss_backward_radii": 100, "steps_proj": -1, "gamma_proj": 5,
         "eval_sampling": "uniform",
         "grow_milestones": [], "grow_points": [],
+        "prune_milestones": [], "prune_min_views": 1, "prune_max_outside": 0,
     },
 }
 
 # the neighbourhood size of the loop's growth events (ops.upsample_points' default): a cloud that grows needs more
-# than GROW_K and at least 10 points
+# than GROW_K and at least 10 points, so a prune never leaves GROW_K or fewer
 GROW_K = 16
 
 # Keys of the reference's configurations that change nothing in its point-model training with data lights (the
@@ -136,6 +137,7 @@ def check_config(cfg, resolution, has_lights):
     if not has_lights:
         raise ValueError("the data directory has no lights_%d entries: the loop shades with the data's lights")
     check_growth(cfg)
+    check_pruning(cfg)
 
 
 def _is_int(x):
@@ -173,6 +175,27 @@ def check_growth(cfg):
                          % (n0, e)) from None
 
 
+def check_pruning(cfg):
+    """Refuse a pruning schedule the loop cannot follow: ``training.prune_milestones`` (the iterations at whose start
+    the cloud is pruned) must be a list of strictly increasing integers >= 1, ``training.prune_min_views`` (keep a point
+    seen in at least this many views; 0: no such test) an integer >= 0, ``training.prune_max_outside`` (keep a point
+    over background in at most this many views; None: no such test) an integer >= 0 or None, and milestones need one
+    of the two tests on."""
+    tr = cfg["training"]
+    ms = tr.get("prune_milestones", [])
+    k, j = tr.get("prune_min_views", 1), tr.get("prune_max_outside", 0)
+    if not isinstance(ms, (list, tuple)) or not all(_is_int(m) for m in ms) or (ms and ms[0] < 1) \
+            or any(b <= a for a, b in zip(ms, ms[1:])):
+        raise ValueError("training.prune_milestones must be a list of strictly increasing integers >= 1, got %r" % (ms,))
+    if not _is_int(k) or k < 0:
+        raise ValueError("training.prune_min_views must be an integer >= 0 (0: no such test), got %r" % (k,))
+    if j is not None and (not _is_int(j) or j < 0):
+        raise ValueError("training.prune_max_outside must be an integer >= 0 or null (no such test), got %r" % (j,))
+    if ms and k == 0 and j is None:
+        raise ValueError("training.prune_milestones is set, but prune_min_views 0 and prune_max_outside null turn both "
+                         "of its tests off")
+
+
 def cloud_size(cfg, it):
     """The cloud's size during (and after) iteration ``it`` under the growth schedule: the ``grow_points`` entry of the
     last milestone <= ``it``, or ``n_points_per_cloud`` before the first (``it`` = -1: the initial cloud)."""
@@ -185,16 +208,26 @@ def cloud_size(cfg, it):
 
 
 def check_cloud_size(cfg, it, n_points):
-    """Refuse a checkpoint of ``n_points`` points saved after iteration ``it`` when a growth schedule is configured and
-    gives another size at ``it`` (say, the schedule or ``n_points_per_cloud`` was edited since).  Without a schedule the
-    checkpoint's cloud is taken at whatever size it has, as it always was."""
-    if not cfg["training"].get("grow_milestones"):
+    """Refuse a checkpoint of ``n_points`` points saved after iteration ``it`` that the growth and pruning schedules
+    cannot give there (say, a schedule or ``n_points_per_cloud`` was edited since).  Without either schedule the
+    checkpoint's cloud is taken at whatever size it has, as it always was.  With pruning, where the last event at or
+    before ``it`` is a prune (a growth on the same iteration comes after it), the size may be anything from
+    ``GROW_K + 1`` to :func:`cloud_size`'s, or that size itself (a prune that removed nothing or would have left too
+    few); everywhere else it must be :func:`cloud_size`'s."""
+    tr = cfg["training"]
+    if not tr.get("grow_milestones") and not tr.get("prune_milestones"):
         return
     want = cloud_size(cfg, it)
-    if int(n_points) != want:
-        raise ValueError("the checkpoint holds %d points after it=%d, but model.model_kwargs.n_points_per_cloud with "
-                         "training.grow_milestones / grow_points gives %d there: the configuration changed since it "
-                         "was written" % (n_points, it, want))
+    n = int(n_points)
+    last_prune = max((int(m) for m in tr.get("prune_milestones", []) if int(m) <= it), default=None)
+    last_grow = max((int(m) for m in tr.get("grow_milestones", []) if int(m) <= it), default=None)
+    pruned = last_prune is not None and (last_grow is None or last_prune > last_grow)
+    if n == want or (pruned and GROW_K < n < want):
+        return
+    raise ValueError("the checkpoint holds %d points after it=%d, but model.model_kwargs.n_points_per_cloud with "
+                     "training.grow_milestones / grow_points%s gives %s there: the configuration changed since it "
+                     "was written" % (n, it, " and prune_milestones" if tr.get("prune_milestones") else "",
+                                      "%d to %d" % (GROW_K + 1, want) if pruned else want))
 
 
 IMAGE_METRICS = ("iou", "psnr")

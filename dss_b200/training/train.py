@@ -32,6 +32,12 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   ``upsample_points`` call, and the step is built anew with Adam and ``MultiStepLR`` continuing from their state.
   A checkpoint holds the cloud at its size; a resumed run grows at the milestones still ahead, and refuses a
   checkpoint whose size is not the one the schedule gives at its ``it``.
+- pruning (``training.prune_milestones``, empty by default, with ``prune_min_views`` 1 and ``prune_max_outside`` 0):
+  at the start of iteration ``prune_milestones[i]``, before a growth on the same iteration, the cloud keeps the points
+  seen in at least ``prune_min_views`` views and over background in at most ``prune_max_outside`` (:meth:`Trainer.prune`,
+  from ``ops.point_coverage`` over every view); the kept rows and their Adam moments stay in order and the step is
+  built anew as after a growth.  A cloud with nothing to remove, or that would keep ``GROW_K`` points or fewer, is left
+  as it is.  A checkpoint saved after a prune may hold any size from ``GROW_K + 1`` to the schedule's.
 - ``training.resume_from`` (in ``<out>``) is loaded when it exists, and the run continues where it stopped, mid-epoch
   included: a resumed run computes what an uninterrupted one does.  (The reference starts a new epoch.)
 - ``--exit-after S`` saves ``model.pt`` and exits with status 3 once S seconds have passed (checked after every
@@ -68,7 +74,9 @@ runs unchanged.
 - every rank loads ``training.resume_from``; the checkpoint does not depend on G, so a run resumes on another number
   of GPUs (mid-epoch included), and on the same number continues bit for bit.
 - every rank grows its replica at a milestone with the same deterministic call, builds a new eager step, and the
-  ranks check right after it that their points, normals, colours and Adam moments are the same bits.
+  ranks check right after it that their points, normals, colours and Adam moments are the same bits.  A prune covers
+  views ``rank, rank + G, ...`` on each rank and sums the int32 counts over the ranks (exact, in any order), so every
+  rank keeps the same points, and the same check follows.
 """
 import argparse
 import errno
@@ -86,7 +94,7 @@ import torch.nn.functional as F
 import yaml
 
 from ..core.cloud import PointClouds3D
-from ..ops import chamfer_distance, evaluate_2d, upsample_points
+from ..ops import chamfer_distance, evaluate_2d, point_coverage, upsample_points
 from ..parallel import GradSync, agree_any, assign_views, check_replicas, view_costs_from_cameras
 from ..utils.create_mvr_data import ico_sphere, sample_points_from_mesh
 from ..utils.dataset import MVRData
@@ -349,6 +357,11 @@ class Trainer:
             self.log.info("resumed from %s at it=%d, epoch %d" % (ckpt_path, self.it, self.epoch_it))
         # the growth schedule: {iteration: the cloud's size from its start on}
         self.grow_at = {int(m): int(n) for m, n in zip(tr.get("grow_milestones", []), tr.get("grow_points", []))}
+        self.prune_at = set(int(m) for m in tr.get("prune_milestones", []))
+        self.prune_min_views, self.prune_max_outside = int(tr.get("prune_min_views", 1)), tr.get("prune_max_outside", 0)
+        if self.prune_at and self.prune_min_views > V:
+            raise ValueError("training.prune_min_views %d is above the data's %d views: a prune would remove every point"
+                             % (self.prune_min_views, V))
         if self.lead:
             with open(os.path.join(self.out_dir, "config.yaml"), "w") as f:
                 yaml.safe_dump(cfg, f, sort_keys=False)
@@ -374,6 +387,24 @@ class Trainer:
             self.opt.load_state_dict(state[0])
             self.lr_sched.load_state_dict(state[1])
 
+    def _cloud_state(self):
+        """the cloud's (points, normals, colours), detached, Adam's state dict, and the (state index, moment) keys of
+        the moments of every learnt tensor"""
+        s, sd = self.step, self.opt.state_dict()
+        keys = [(i, k) for i in sorted(sd["state"]) for k in ("exp_avg", "exp_avg_sq")]
+        return (s.points.detach(), s.normals.detach(), s.colours.detach()), sd, keys
+
+    def _rebuild(self, points, normals, colours, sd, moments):
+        """the step built anew on a changed cloud, after an event: Adam continues from ``sd`` with the moments
+        ``moments`` ({(state index, moment): rows}), and ``MultiStepLR`` from its state: step counts, betas and the
+        current learning rates"""
+        state = {i: dict(st) for i, st in sd["state"].items()}
+        for (i, k), m in moments.items():
+            state[i][k] = m
+        sched = self.lr_sched.state_dict()
+        self.step = self.opt = self.lr_sched = None     # the old step and its graph go first
+        self._build(points, normals, colours, (dict(sd, state=state), sched))
+
     def grow(self, n):
         """The growth event: the cloud grows from P to ``n`` points, at the start of a milestone's iteration.  The P
         rows of the points, normals and colours and of Adam's moments stay as they are; the new rows are those of one
@@ -383,28 +414,57 @@ class Trainer:
         Adam's step count, and with it the bias correction, is shared by the whole tensor).  The step is built anew on
         the grown cloud (the old one and its graph dropped first), and Adam and ``MultiStepLR`` continue from the old
         ones' state: step counts, betas and the current learning rates.  Deterministic, so replicas stay replicas."""
-        s, opt = self.step, self.opt
-        P = s.points.shape[0]
         t0 = time.perf_counter()
-        old = {"points": s.points.detach(), "normals": s.normals.detach(), "colours": s.colours.detach()}
-        sd = opt.state_dict()
-        keys = [(i, k) for i in sorted(sd["state"]) for k in ("exp_avg", "exp_avg_sq")]
+        (points, normals, colours), sd, keys = self._cloud_state()
+        P = points.shape[0]
         moments = [sd["state"][i][k] for i, k in keys]
-        up = upsample_points(old["points"], n, k=GROW_K, normals=F.normalize(old["normals"], dim=-1),
-                             features=torch.cat([old["colours"]] + moments, 1))
+        up = upsample_points(points, n, k=GROW_K, normals=F.normalize(normals, dim=-1),
+                             features=torch.cat([colours] + moments, 1))
         grown = lambda rows, new: torch.cat([rows, new[P:]])
-        points, normals = grown(old["points"], up.points), grown(old["normals"], up.normals)
         cols = torch.split(up.features, 3, 1)
-        colours = grown(old["colours"], cols[0])
-        state = {i: dict(st) for i, st in sd["state"].items()}
-        for (i, k), m, col in zip(keys, moments, cols[1:]):
-            state[i][k] = grown(m, col)
-        sched = self.lr_sched.state_dict()
-        self.step = self.opt = self.lr_sched = s = opt = up = None     # the old step and its graph go first
-        self._build(points, normals, colours, (dict(sd, state=state), sched))
+        self._rebuild(grown(points, up.points), grown(normals, up.normals), grown(colours, cols[0]), sd,
+                      {key: grown(m, col) for key, m, col in zip(keys, moments, cols[1:])})
         torch.cuda.synchronize(self.dev)
         self.log.info("Grew the cloud at it=%d: %d -> %d points (%.1f ms: upsample and new step)"
                       % (self.it, P, n, 1e3 * (time.perf_counter() - t0)))
+
+    def prune(self):
+        """The prune event, at the start of a milestone's iteration (before a growth on the same one): the view coverage
+        of the cloud (:func:`~dss_b200.ops.point_coverage` over all the data's views, ``batch_size`` at a time, with the
+        step's current splat settings; on G ranks each covers views ``rank, rank + G, ...`` and the int32 counts are
+        summed over the ranks, exactly), and the points kept where ``seen >= prune_min_views`` and ``outside <=
+        prune_max_outside`` (a test off: 0, null).  The kept rows of the points, normals, colours and Adam's moments stay
+        in their order, and the step is built anew as after a growth.  The cloud is left as it is when every point
+        passes, or when GROW_K or fewer would remain (so that a later growth can run)."""
+        t0 = time.perf_counter()
+        (points, normals, colours), sd, keys = self._cloud_state()
+        P, st = points.shape[0], self.step
+        cov = point_coverage(points, normals, self.views, self.params, self.batch_size,
+                             range(self.rank, len(self.views), self.world), st.Vrk_invariant, st.Vrk_isotropic,
+                             st.frnn_radius)
+        st = None
+        if self.sync is not None:
+            for c in cov:
+                dist.all_reduce(c, op=dist.ReduceOp.SUM, group=self.sync.group)
+        k, j = self.prune_min_views, self.prune_max_outside
+        few = cov.seen < k
+        over = cov.outside > j if j is not None else torch.zeros_like(few)
+        keep = ~(few | over)
+        n, n_few, n_over = torch.stack([keep.sum(), few.sum(), over.sum()]).tolist()
+        why = ", ".join(([] if k == 0 else ["%d seen in fewer than %d views" % (n_few, k)])
+                        + ([] if j is None else ["%d outside the masks in more than %d views" % (n_over, j)]))
+        if n == P or n <= GROW_K:
+            self.log.info("Kept the cloud at it=%d: %s (%s)" % (
+                self.it, "every point passes" if n == P else "pruning would leave %d points, %d or fewer" % (n, GROW_K),
+                why))
+            return
+        idx = keep.nonzero()[:, 0]
+        rows = lambda t: t.index_select(0, idx)
+        self._rebuild(rows(points), rows(normals), rows(colours), sd,
+                      {(i, m): rows(sd["state"][i][m]) for i, m in keys})
+        torch.cuda.synchronize(self.dev)
+        self.log.info("Pruned the cloud at it=%d: %d -> %d points (%s; %.1f ms)"
+                      % (self.it, P, n, why, 1e3 * (time.perf_counter() - t0)))
 
     def _schedule(self):
         """TrainerScheduler.step (trainer.py:227) before the step; a changed setting makes the next replay capture"""
@@ -533,8 +593,11 @@ class Trainer:
                 idx = self.order[self.pos:self.pos + bs]
                 self.pos += bs
                 self.it += 1
+                if self.it in self.prune_at:
+                    self.prune()                      # first: a growth on the same iteration seeds no strays
                 if self.it in self.grow_at:
                     self.grow(self.grow_at[self.it])
+                if self.it in self.prune_at or self.it in self.grow_at:
                     self.check_replicas(event=True)
                 self._schedule()
                 if self.sync is None:

@@ -446,6 +446,20 @@ DSS_API int dss_point_filters_gated(dss_ctx *ctx, const float *records, const ui
                                     int H, int W, const uint8_t *visibility_gate, uint8_t *visibility,
                                     uint8_t *inmask, void *stream);
 
+/* ---- per-point view coverage (pruning the cloud) ------------------------------------------------------------------
+ * From one dss_render_forward of a SHARED cloud of P0 points seen by N cameras (shared_cloud must be 1: packed clouds
+ * return DSS_E_INVALID) -- its records (N*P0, 8) f32, 16-byte aligned, and visible (N*P0,) bytes -- and the N
+ * ground-truth masks, passed as dss_point_filters takes them, ADDS to the int32 (P0,) counters:
+ *   seen[i]    += sum_n [visible[n*P0 + i] != 0],
+ *   outside[i] += sum_n [z > 0 && |x| <= 1 && |y| <= 1 && sample_n(clamp(-x, -1, 1), clamp(-y, -1, 1)) == 0],
+ * x, y, z the record of (view n, point i) and sample_n dss_point_filters' mask sample.  z > 0: the preprocess kept the
+ * point in view n (its depth range and backface test); a non-finite x or y fails |x|, |y| <= 1.  outside is not gated
+ * on visibility: a hidden point over background counts, an off-frame or depth-filtered one does not.
+ * One launch, one thread per point; deterministic; no atomics, no scratch, no host synchronisation: capturable. */
+DSS_API int dss_point_coverage(dss_ctx *ctx, const float *records, const uint8_t *visible, int shared_cloud, int N,
+                               int64_t P0, const void *mask, int mask_kind, const int64_t *mask_strides, int H, int W,
+                               int32_t *seen, int32_t *outside, void *stream);
+
 /* ---- fused renderer path (what bench.py times) ----------------------------------------------
  * One call per direction for SurfaceSplattingRenderer.forward / its autograd backward
  * (DSS/core/renderer.py:36-82, DSS/core/rasterizer.py:584-664,749-977).  All pointers device. */
