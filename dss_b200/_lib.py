@@ -114,6 +114,8 @@ _SIGNATURES = {
                                           C.POINTER(C.c_int64), C.c_int, C.c_int, vp, vp, vp, vp]),
     "dss_point_coverage": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int64, vp, C.c_int, C.POINTER(C.c_int64),
                                      C.c_int, C.c_int, vp, vp, vp]),
+    "dss_pose_forward": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp]),
+    "dss_pose_backward": (C.c_int, [vp, vp, vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]),
     "dss_rasterize_mesh": (C.c_int, [vp, vp, C.c_int64, vp, C.c_int64, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                      C.c_int, C.c_float, vp, vp, vp, vp, vp, vp, vp]),
     "dss_chamfer": (C.c_int, [vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int64, C.c_int, vp, vp]),

@@ -27,7 +27,7 @@ __all__ = ["SplatParams", "Shading", "make_shading", "RenderOutput", "render_poi
            "denoise_normals", "Projected", "project_to_surface", "l0_smooth", "MeshRender", "render_mesh", "chamfer_distance",
            "PointMeshDistance", "point_mesh_distance", "PoissonMesh", "poisson_reconstruction", "marching_tetrahedra",
            "ImageMetrics", "image_metrics", "gather_views", "shared_cloud_splats", "render_data_views", "evaluate_2d",
-           "Coverage", "accumulate_coverage", "point_coverage"]
+           "Coverage", "accumulate_coverage", "point_coverage", "check_rigid_cameras", "pose_cameras"]
 
 
 class SplatParams(NamedTuple):
@@ -1221,6 +1221,75 @@ def gather_views(store, idx, img, mask):
         raise ValueError("gather_views takes at most 65535 views at a time, got %d" % B)
     _lib.call("dss_gather_views", dev, store, int(store.dtype == torch.float32), V, H, W, idx, B, img, mask)
     return img, mask
+
+
+RIGID_TOLERANCE = 1e-4     # max |R R^T - I| and |last column - (0, 0, 0, 1)| of a camera the pose map takes
+
+
+def check_rigid_cameras(view0, tol=RIGID_TOLERANCE):
+    """Refuse with ValueError world-to-view matrices ``view0`` (V,4,4), row-vector convention, that the pose map cannot
+    invert as rigid motions: a 3x3 block R with ``max |R R^T - I| > tol`` or ``det R <= 0``, or a last column further
+    than ``tol`` from (0, 0, 0, 1).  Reads the matrices to the host: a set-up check, once per set of cameras."""
+    m = torch.as_tensor(view0).detach().to("cpu", torch.float64)
+    if m.dim() != 3 or tuple(m.shape[1:]) != (4, 4):
+        raise ValueError("camera matrices must be (V, 4, 4), got %s" % (tuple(m.shape),))
+    R = m[:, :3, :3]
+    ortho = (R @ R.transpose(1, 2) - torch.eye(3, dtype=torch.float64)).abs().amax((1, 2))
+    col = (m[:, :, 3] - torch.tensor([0.0, 0.0, 0.0, 1.0], dtype=torch.float64)).abs().amax(1)
+    bad = (ortho > tol) | (col > tol) | (torch.linalg.det(R) <= 0) | ~torch.isfinite(m).all(2).all(1)
+    if bool(bad.any()):
+        v = int(bad.nonzero()[0, 0])
+        raise ValueError("camera %d is not a rigid world-to-view transform within %g (max |R R^T - I| = %.3g, det R = "
+                         "%.6g, last column %s): the pose refinement takes rotations and translations only"
+                         % (v, tol, float(ortho[v]), float(torch.linalg.det(R[v])), m[v, :, 3].tolist()))
+
+
+class _PoseCameras(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, poses, idx, view0, proj0):
+        dev = poses.device
+        V, B = poses.shape[0], idx.shape[0]
+        view = torch.empty((B, 4, 4), dtype=torch.float32, device=dev)
+        proj = torch.empty((B, 4, 4), dtype=torch.float32, device=dev)
+        p = poses.detach()
+        _lib.call("dss_pose_forward", dev, p, idx, V, B, view0, proj0, view, proj)
+        ctx.set_materialize_grads(False)
+        ctx.save_for_backward(p, idx, view0, proj0)
+        return view, proj
+
+    @staticmethod
+    def backward(ctx, grad_view, grad_proj):
+        p, idx, view0, proj0 = ctx.saved_tensors
+        g = lambda t, name: None if t is None else _lib.as_f32(t, name)
+        grad = torch.empty_like(p)
+        _lib.call("dss_pose_backward", p.device, p, idx, p.shape[0], idx.shape[0], view0, proj0,
+                  g(grad_view, "grad_view"), g(grad_proj, "grad_proj"), grad)
+        return grad, None, None, None
+
+
+def pose_cameras(poses, idx, view0, proj0):
+    """The refined cameras of a batch of views (csrc/poses.cu; the map is in include/dss_b200.h): ``poses`` (V,6)
+    float32, one correction (rotation vector, translation) per view applied in the camera frame; ``idx`` (B,) int64 the
+    batch's views (repeats allowed), every value in [0, V): NOT checked here (that would read them back; out of range
+    gives NaN cameras); ``view0`` / ``proj0`` (V,4,4) float32 the views' world-to-view and full projection matrices,
+    whose 3x3 view blocks must be rotations (:func:`check_rigid_cameras`, which the callers run once at set-up).
+    Returns ``(view, proj)`` (B,4,4): ``view0[idx] E`` and ``view0[idx] E view0[idx]^-1 proj0[idx]``, ``view0`` /
+    ``proj0`` bit for bit where a pose is zero.  Differentiable in ``poses`` only; the backward writes every row of the
+    (V,6) gradient, summing repeated views in batch order, the same bits on every run.  One launch each way, no scratch,
+    no host synchronisation: capturable."""
+    _lib.require_cuda(poses, idx, view0, proj0)
+    if poses.dtype != torch.float32 or poses.dim() != 2 or poses.shape[1] != 6 or poses.shape[0] < 1:
+        raise RuntimeError("poses must be a float32 (V, 6) tensor with V >= 1, got %s %s"
+                           % (poses.dtype, tuple(poses.shape)))
+    V = poses.shape[0]
+    if idx.dtype != torch.int64 or idx.dim() != 1:
+        raise RuntimeError("idx must be an int64 tensor of shape (B,), got %s %s" % (idx.dtype, tuple(idx.shape)))
+    for name, t in (("view0", view0), ("proj0", proj0)):
+        if t.dtype != torch.float32 or tuple(t.shape) != (V, 4, 4):
+            raise RuntimeError("%s must be a float32 tensor of shape (%d, 4, 4), got %s %s"
+                               % (name, V, t.dtype, tuple(t.shape)))
+    return _PoseCameras.apply(poses.contiguous(), idx.contiguous(), view0.detach().contiguous(),
+                              proj0.detach().contiguous())
 
 
 def shared_cloud_splats(points, n_views, Vrk_invariant=True, Vrk_isotropic=True, frnn_radius=0.2):

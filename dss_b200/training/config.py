@@ -9,7 +9,7 @@ import warnings
 
 import yaml
 
-__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "check_pruning",
+__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "check_pruning", "check_cameras",
            "cloud_size", "check_cloud_size", "GROW_K", "step_settings", "splat_params", "EVAL_SAMPLINGS", "SELECTION_METRICS",
            "IMAGE_METRICS", "selection_metric"]
 
@@ -33,7 +33,7 @@ DEFAULTS = {
     },
     "model": {"type": "point",
               "model_kwargs": {"learn_points": True, "learn_normals": True, "learn_colors": False,
-                               "n_points_per_cloud": 8000}},
+                               "n_points_per_cloud": 8000, "learn_cameras": False}},
     "training": {
         "out_dir": "exp", "seed": 0,
         "lambda_dr_rgb": 1.0, "lambda_dr_silhouette": 1.0, "lambda_dr_proj": 0.1, "lambda_dr_repel": 0.1,
@@ -44,6 +44,7 @@ DEFAULTS = {
         "eval_sampling": "uniform",
         "grow_milestones": [], "grow_points": [],
         "prune_milestones": [], "prune_min_views": 1, "prune_max_outside": 0,
+        "lr_cameras": 1e-4, "cameras_from_it": 300,
     },
 }
 
@@ -138,6 +139,7 @@ def check_config(cfg, resolution, has_lights):
         raise ValueError("the data directory has no lights_%d entries: the loop shades with the data's lights")
     check_growth(cfg)
     check_pruning(cfg)
+    check_cameras(cfg)
 
 
 def _is_int(x):
@@ -194,6 +196,21 @@ def check_pruning(cfg):
     if ms and k == 0 and j is None:
         raise ValueError("training.prune_milestones is set, but prune_min_views 0 and prune_max_outside null turn both "
                          "of its tests off")
+
+
+def check_cameras(cfg):
+    """Refuse camera refinement settings the loop cannot follow: ``model.model_kwargs.learn_cameras`` must be a bool,
+    ``training.lr_cameras`` (the Adam learning rate of the pose corrections) a finite number > 0 and
+    ``training.cameras_from_it`` (the first iteration whose step learns them) an integer >= 0."""
+    tr = cfg["training"]
+    on = cfg["model"]["model_kwargs"].get("learn_cameras", False)
+    lr, start = tr.get("lr_cameras", 1e-4), tr.get("cameras_from_it", 300)
+    if not isinstance(on, bool):
+        raise ValueError("model.model_kwargs.learn_cameras must be true or false, got %r" % (on,))
+    if isinstance(lr, bool) or not isinstance(lr, (int, float)) or not 0 < lr < float("inf"):
+        raise ValueError("training.lr_cameras must be a number > 0, got %r" % (lr,))
+    if not _is_int(start) or start < 0:
+        raise ValueError("training.cameras_from_it must be an integer >= 0, got %r" % (start,))
 
 
 def cloud_size(cfg, it):

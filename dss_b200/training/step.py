@@ -34,8 +34,8 @@ from ..core.cloud import PointClouds3D, PointCloudsFilters
 from ..core.lighting import pack_lights
 from ..core.texture import camera_centres
 from ..graph import GraphedStep
-from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, point_filters, point_filters_no_views, render_points,
-                   shared_cloud_splats)
+from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, point_filters, point_filters_no_views, pose_cameras,
+                   render_points, shared_cloud_splats)
 from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
 
 __all__ = ["TrainStep", "GraphedTrainStep"]
@@ -64,13 +64,22 @@ class TrainStep:
     ``Vrk_invariant`` / ``Vrk_isotropic`` select the splat shape as in the rasterizer settings: one h per view, one h
     per point, or, with both False (``configs/default.yaml``), anisotropic splats from the local frames of every point's
     8 nearest neighbours (``local_frames``, computed every step from the current points; a view-sharded step computes
-    them on every rank from the same cloud, no collective).  The anisotropic kernel needs P0 > 8."""
+    them on every rank from the same cloud, no collective).  The anisotropic kernel needs P0 > 8.
+
+    ``poses`` (V,6) float32 with ``views`` (the ``DeviceViews`` of the data, whose cameras must be rigid): the step also
+    learns one camera correction per view (``ops.pose_cameras``) on its own leaf ``step.poses``, a copy of ``poses``.
+    ``step(..., idx=idx)`` then renders with the refined cameras of the batch's views ``idx`` ((B,) int64 on the
+    device, the views ``proj`` / ``view`` are the unrefined cameras of), which receive the render's and the shading
+    camera centres' gradients, and ``step.poses.grad`` holds the (V,6) gradient after the step.  View-sharded, every
+    rank's gradient rows of its own views are summed over the ranks with one all-reduce of 6 V floats (a rank without
+    views adds zeros), so every rank holds the same gradient.  At zero poses the step computes the loss, image,
+    filters and cloud gradients of the step without ``poses``."""
 
     def __init__(self, points, normals, colours, params: SplatParams, *, learn=("points", "normals"),
                  Vrk_invariant=True, Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0, lambda_dr_rgb=1.0,
                  lambda_dr_silhouette=1.0, lambda_dr_proj=0.01, lambda_dr_repel=0.0, knn_k=12, filter_scale=2.0,
-                 sharpness_sigma=0.75, grad_sync=None):
-        dev = _lib.require_cuda(points, normals, colours)
+                 sharpness_sigma=0.75, grad_sync=None, poses=None, views=None):
+        dev = _lib.require_cuda(points, normals, colours, poses)
         for name, t in (("points", points), ("normals", normals), ("colours", colours)):
             if t.dtype != torch.float32 or t.dim() != 2 or tuple(t.shape) != (points.shape[0], 3):
                 raise RuntimeError("%s must be a float32 (P0, 3) tensor, got %s %s" % (name, t.dtype, tuple(t.shape)))
@@ -97,12 +106,23 @@ class TrainStep:
         # that a capture cannot take
         self._num = torch.full((1,), points.shape[0], dtype=torch.int64, device=dev)
         self.loss = self.image = self.visibility = self.inmask = None
+        self.poses = self._cameras = None
+        if poses is not None:
+            if views is None:
+                raise ValueError("learning camera poses needs the views' cameras: pass views=DeviceViews")
+            V = len(views)
+            if poses.dtype != torch.float32 or tuple(poses.shape) != (V, 6):
+                raise RuntimeError("poses must be a float32 (%d, 6) tensor, one row per view, got %s %s"
+                                   % (V, poses.dtype, tuple(poses.shape)))
+            views.check_rigid()
+            self.poses = poses.detach().clone().requires_grad_(True)
+            self._cameras = (views.camera_mat, views.proj)
 
     def settings(self):
         """every host-side value the step bakes into its launches"""
         return (tuple(self.params), self.Vrk_invariant, self.Vrk_isotropic, self.frnn_radius, self.shininess,
                 self.lambda_dr_rgb, self.lambda_dr_silhouette, self.lambda_dr_proj, self.lambda_dr_repel, self.knn_k,
-                self.filter_scale, self.sharpness_sigma)
+                self.filter_scale, self.sharpness_sigma, self.poses is not None)
 
     def _check_batch(self, img, mask_img, proj, view):
         _lib.require_cuda(self.points, img, mask_img, proj, view)
@@ -116,17 +136,25 @@ class TrainStep:
         if tuple(img.shape) != (N, S, S, 3):
             raise RuntimeError("img must have shape (N, S, S, 3) = %s, got %s" % ((N, S, S, 3), tuple(img.shape)))
 
-    def __call__(self, img, mask_img, proj, view, lights):
+    def __call__(self, img, mask_img, proj, view, lights, idx=None):
         self._check_batch(img, mask_img, proj, view)
+        if self.poses is not None:
+            if idx is None or idx.dtype != torch.int64 or tuple(idx.shape) != (proj.shape[0],) \
+                    or idx.device != self.device:
+                raise RuntimeError("a step that learns poses takes the batch's views: idx, an int64 tensor of shape "
+                                   "(%d,) on %s" % (proj.shape[0], self.device))
         if self._sync is not None and proj.shape[0] == 0:
-            return self._run(img, mask_img, proj, view, None, None, None)
+            return self._run(img, mask_img, proj, view, None, None, None, idx)
         rows, ambient, kind = pack_lights(lights)
-        return self._run(img, mask_img, proj, view, rows.detach(), ambient.detach(), kind)
+        return self._run(img, mask_img, proj, view, rows.detach(), ambient.detach(), kind, idx)
 
-    def _run(self, img, mask_img, proj, view, rows, ambient, light_type):
-        for t in (self.points, self.normals, self.colours):
-            t.grad = None
+    def _run(self, img, mask_img, proj, view, rows, ambient, light_type, idx=None):
+        for t in (self.points, self.normals, self.colours, self.poses):
+            if t is not None:
+                t.grad = None
         N, dev = proj.shape[0], self.device
+        if self.poses is not None and N > 0:
+            view, proj = pose_cameras(self.poses, idx, *self._cameras)
         normals = F.normalize(self.normals, dim=-1)
         if N == 0:
             # a rank of a view-sharded step without views: the collectives of the others, with zero contributions
@@ -162,6 +190,11 @@ class TrainStep:
         if rendered is not None:
             total = total + rendered
         total.backward()
+        if self.poses is not None:
+            if self.poses.grad is None:       # a rank without views
+                self.poses.grad = torch.zeros_like(self.poses)
+            if self._sync is not None:
+                dist.all_reduce(self.poses.grad, op=dist.ReduceOp.SUM, group=self._group)
         self.loss = {"loss": total.detach(), "loss_dr_rgb": loss["loss_dr_rgb"].detach(),
                      "loss_dr_silhouette": loss["loss_dr_silhouette"].detach(),
                      "loss_dr_proj": reg["loss_dr_proj"].detach(), "loss_dr_repel": reg["loss_dr_repel"].detach()}
@@ -212,7 +245,8 @@ class GraphedTrainStep(TrainStep, GraphedStep):
     ``replay()`` captures again too.
 
     :meth:`from_views` builds the step on views resident on the device instead: the capture gathers each batch itself,
-    and ``load_views(idx)`` takes the place of ``load``."""
+    and ``load_views(idx)`` takes the place of ``load``.  Only such a step learns camera poses (``poses=``): the capture
+    runs the pose map on the gathered index, and ``step.poses`` is one more leaf."""
     _OUTPUTS = ("loss", "image", "visibility", "inmask")
 
     def __init__(self, points, normals, colours, params: SplatParams, img, mask_img, proj, view, lights, warmup=3,
@@ -221,7 +255,10 @@ class GraphedTrainStep(TrainStep, GraphedStep):
         if sync is not None and sync.world_size > 1:
             raise NotImplementedError("GraphedTrainStep runs on one GPU; a view-sharded step runs eagerly: "
                                       "TrainStep(..., grad_sync=...)")
-        super().__init__(points, normals, colours, params, **settings)
+        if settings.get("poses") is not None and _views is None:
+            raise ValueError("a graphed step learns camera poses on device views: GraphedTrainStep.from_views(..., "
+                             "poses=...)")
+        super().__init__(points, normals, colours, params, views=None if _views is None else _views[0], **settings)
         self._check_batch(img, mask_img, proj, view)
         rows, ambient, self._light_type = pack_lights(lights)
         # static inputs (clone keeps a permuted view's strides)
@@ -231,7 +268,7 @@ class GraphedTrainStep(TrainStep, GraphedStep):
         # from_views: the device views and the static (B,) index the capture gathers the batch with
         self._views, self._index = _views if _views is not None else (None, None)
         self._warmup = max(1, int(warmup))
-        self._leaves = (self.points, self.normals, self.colours)
+        self._leaves = (self.points, self.normals, self.colours) + ((self.poses,) if self.poses is not None else ())
         self.capture()
 
     @classmethod
@@ -270,7 +307,8 @@ class GraphedTrainStep(TrainStep, GraphedStep):
     def _eager(self):
         if self._views is not None:
             self._gather()
-        return self._run(self.img, self.mask_img, self.proj, self.view, self.lights, self.ambient, self._light_type)
+        return self._run(self.img, self.mask_img, self.proj, self.view, self.lights, self.ambient, self._light_type,
+                         self._index)
 
     def load_views(self, idx):
         """the next batch of a :meth:`from_views` step: the host list ``idx`` (as many views as the capture's, checked

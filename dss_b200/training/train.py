@@ -38,6 +38,13 @@ trainer.py:73-238) on :class:`GraphedTrainStep`, from a data directory to a trai
   from ``ops.point_coverage`` over every view); the kept rows and their Adam moments stay in order and the step is
   built anew as after a growth.  A cloud with nothing to remove, or that would keep ``GROW_K`` points or fewer, is left
   as it is.  A checkpoint saved after a prune may hold any size from ``GROW_K + 1`` to the schedule's.
+- camera refinement (``model.model_kwargs.learn_cameras``, off by default): one pose correction per view
+  (``ops.pose_cameras``), learnt from iteration ``training.cameras_from_it`` on (before it the step is built without
+  them, as when refinement is off, and at it the step is built anew with them) by one more Adam group, betas (0.5, 0.9)
+  and ``training.lr_cameras``, stepped by the same ``MultiStepLR``.  Growth and pruning leave the poses and their Adam
+  moments as they are.  Validation and pruning see the refined cameras (``DeviceViews.with_poses``), the log line adds
+  the mean and maximum correction angle (degrees) and translation, and checkpoints hold ``"cameras": {"poses"}``; a
+  checkpoint without them resumes at zero poses with a fresh Adam group.
 - ``training.resume_from`` (in ``<out>``) is loaded when it exists, and the run continues where it stopped, mid-epoch
   included: a resumed run computes what an uninterrupted one does.  (The reference starts a new epoch.)
 - ``--exit-after S`` saves ``model.pt`` and exits with status 3 once S seconds have passed (checked after every
@@ -106,9 +113,10 @@ from .step import GraphedTrainStep, TrainStep
 
 __all__ = ["radii_backward_scaler", "compound_lambda_proj", "initial_cloud", "make_optimizer", "make_lr_scheduler",
            "ground_truth_cloud", "check_ground_truth", "load_data", "dist_env", "rank_device", "deal_batch", "Trainer",
-           "main"]
+           "pose_stats", "main"]
 
 EXIT_TIME_LIMIT = 3        # train_mvr.py:221-227
+CAMERA_GROUP = "cameras"   # the name of the pose corrections' Adam group
 EVAL_SEED = 0              # the fixed draw of the ground-truth samples
 # a collective waits this long for the other ranks before it fails: longer than rank 0's validation of a large cloud,
 # while the others wait at their next collective
@@ -142,14 +150,25 @@ def initial_cloud(n_points, seed=0, device="cuda"):
     return points.contiguous(), normals.contiguous(), torch.ones_like(points)
 
 
-def make_optimizer(tensors):
+def make_optimizer(tensors, poses=None, lr_cameras=None):
     """train_mvr.py:83-95: Adam, betas (0.5, 0.9), groups in the reference's order for the tensors that require grad:
-    normals lr 0.01, points lr 0.01, colours lr 1.0.  ``tensors``: {"points", "normals", "colours"}."""
+    normals lr 0.01, points lr 0.01, colours lr 1.0.  ``tensors``: {"points", "normals", "colours"}.  ``poses``: the
+    (V,6) camera corrections, one more group last, named ``"cameras"``, with lr ``lr_cameras``."""
     groups = [{"params": [tensors[name]], "lr": lr, "betas": (0.5, 0.9)}
               for name, lr in (("normals", 0.01), ("points", 0.01), ("colours", 1.0)) if tensors[name].requires_grad]
     if not groups:
         raise ValueError("nothing to learn: model.model_kwargs sets every learn_* false")
+    if poses is not None:
+        groups.append({"params": [poses], "lr": float(lr_cameras), "betas": (0.5, 0.9), "name": CAMERA_GROUP})
     return torch.optim.Adam(groups, lr=0.01, betas=(0.5, 0.9))
+
+
+def pose_stats(poses):
+    """(4,) float32 on the poses' device: the mean and maximum rotation angle (degrees) and translation norm of the
+    (V,6) corrections"""
+    with torch.no_grad():
+        ang, tr = torch.rad2deg(poses[:, :3].norm(dim=1)), poses[:, 3:].norm(dim=1)
+        return torch.stack([ang.mean(), ang.amax(), tr.mean(), tr.amax()]).double()
 
 
 def make_lr_scheduler(optimizer, cfg):
@@ -340,6 +359,11 @@ class Trainer:
         self.best = -self.sign * math.inf
         self.radii_init = self.params.radii_backward_scaler
         self.lambda_dr_proj = self.settings["lambda_dr_proj"]
+        self.learn_cameras = bool(cfg["model"]["model_kwargs"].get("learn_cameras", False))
+        self.lr_cameras, self.cameras_from_it = float(tr.get("lr_cameras", 1e-4)), int(tr.get("cameras_from_it", 300))
+        if self.learn_cameras:
+            self.views.check_rigid()
+        self.poses = None
         ckpt_path = os.path.join(self.out_dir, str(tr["resume_from"]))
         # loaded to the host: the optimizer moves its state to the parameters' device, the sampler state stays there
         ckpt = torch.load(ckpt_path, map_location="cpu", weights_only=False) if os.path.exists(ckpt_path) else None
@@ -355,6 +379,27 @@ class Trainer:
             self.params = self.params._replace(radii_backward_scaler=float(ckpt["schedule"]["radii_backward_scaler"]))
             check_cloud_size(cfg, self.it, points.shape[0])
             self.log.info("resumed from %s at it=%d, epoch %d" % (ckpt_path, self.it, self.epoch_it))
+        state = None if ckpt is None else (ckpt["optimizer"], ckpt["lr_scheduler"])
+        has_poses = ckpt is not None and "cameras" in ckpt
+        if ckpt is not None and not self.learn_cameras and any(
+                g.get("name") == CAMERA_GROUP for g in ckpt["optimizer"]["param_groups"]):
+            raise ValueError("the checkpoint %s learnt camera poses: resume it with model.model_kwargs.learn_cameras: "
+                             "true" % ckpt_path)
+        poses = None
+        if self.learn_cameras:
+            poses = torch.zeros((V, 6), dtype=torch.float32, device=self.dev)
+            if has_poses:
+                p = ckpt["cameras"]["poses"]
+                if tuple(p.shape) != (V, 6):
+                    raise ValueError("the checkpoint %s holds camera poses of shape %s, but the data has %d views"
+                                     % (ckpt_path, tuple(p.shape), V))
+                poses = p.to(self.dev, torch.float32)
+            elif state is not None:
+                # a checkpoint without poses: they start at zero with a fresh Adam group, appended after the cloud's
+                state = (dict(state[0], param_groups=list(state[0]["param_groups"]) + [None]),
+                         dict(state[1], base_lrs=list(state[1]["base_lrs"]) + [self.lr_cameras],
+                              _last_lr=list(state[1]["_last_lr"]) + [self.lr_cameras]))
+                self.log.info("the checkpoint holds no camera poses: they start at zero")
         # the growth schedule: {iteration: the cloud's size from its start on}
         self.grow_at = {int(m): int(n) for m, n in zip(tr.get("grow_milestones", []), tr.get("grow_points", []))}
         self.prune_at = set(int(m) for m in tr.get("prune_milestones", []))
@@ -365,33 +410,49 @@ class Trainer:
         if self.lead:
             with open(os.path.join(self.out_dir, "config.yaml"), "w") as f:
                 yaml.safe_dump(cfg, f, sort_keys=False)
-        self._build(points, normals, colours, None if ckpt is None else (ckpt["optimizer"], ckpt["lr_scheduler"]))
+        self._build(points, normals, colours, poses, self._cameras_due(self.it + 1), state)
 
     # ---- pieces ------------------------------------------------------------------------------------------------------
-    def _build(self, points, normals, colours, state=None):
-        """the step on this cloud, its Adam and ``MultiStepLR``; ``state``: (optimizer, lr scheduler) state dicts to
-        continue from (a checkpoint's, or those of a growth event)"""
+    def _cameras_due(self, it):
+        """whether the step of iteration ``it`` learns the camera poses"""
+        return self.learn_cameras and it >= self.cameras_from_it
+
+    def _build(self, points, normals, colours, poses=None, cameras=False, state=None):
+        """the step on this cloud, its Adam and ``MultiStepLR``; ``poses``: the (V,6) camera corrections when they are
+        learnt, and ``cameras`` whether this step learns them (the step then holds the leaf, otherwise the trainer
+        does, so that the Adam group stays); ``state``: (optimizer, lr scheduler) state dicts to continue from (a
+        checkpoint's, or those of an event), where a pose group of None stands for a fresh one"""
         s = dict(self.settings)
         learn, s["lambda_dr_proj"] = s.pop("learn"), self.lambda_dr_proj
+        if cameras:
+            s["poses"] = poses
         if self.sync is None:
             # captured on any batch of the right shape: the capture's warm-up steps leave the cloud unchanged, and every
             # iteration loads its own view indices first (the sharded step is eager)
             self.step = GraphedTrainStep.from_views(points, normals, colours, self.params, self.views,
                                                     list(range(self.batch_size)), learn=learn, **s)
         else:
-            self.step = TrainStep(points, normals, colours, self.params, learn=learn, grad_sync=self.sync, **s)
+            self.step = TrainStep(points, normals, colours, self.params, learn=learn, grad_sync=self.sync,
+                                  views=self.views if cameras else None, **s)
+        self.poses = self.step.poses if cameras else (
+            None if poses is None else poses.detach().clone().requires_grad_(True))
         self.opt = make_optimizer({"points": self.step.points, "normals": self.step.normals,
-                                   "colours": self.step.colours})
+                                   "colours": self.step.colours}, self.poses, self.lr_cameras)
         self.lr_sched = make_lr_scheduler(self.opt, self.cfg)
         if state is not None:
+            groups = state[0]["param_groups"]
+            if groups and groups[-1] is None:
+                fresh = self.opt.state_dict()["param_groups"][-1]
+                state = (dict(state[0], param_groups=groups[:-1] + [fresh]), state[1])
             self.opt.load_state_dict(state[0])
             self.lr_sched.load_state_dict(state[1])
 
     def _cloud_state(self):
         """the cloud's (points, normals, colours), detached, Adam's state dict, and the (state index, moment) keys of
-        the moments of every learnt tensor"""
+        the moments of every learnt tensor of the cloud (not of the camera poses, which no cloud event changes)"""
         s, sd = self.step, self.opt.state_dict()
-        keys = [(i, k) for i in sorted(sd["state"]) for k in ("exp_avg", "exp_avg_sq")]
+        cloud = {i for g in sd["param_groups"] if g.get("name") != CAMERA_GROUP for i in g["params"]}
+        keys = [(i, k) for i in sorted(sd["state"]) if i in cloud for k in ("exp_avg", "exp_avg_sq")]
         return (s.points.detach(), s.normals.detach(), s.colours.detach()), sd, keys
 
     def _rebuild(self, points, normals, colours, sd, moments):
@@ -402,8 +463,20 @@ class Trainer:
         for (i, k), m in moments.items():
             state[i][k] = m
         sched = self.lr_sched.state_dict()
+        poses = None if self.poses is None else self.poses.detach()
         self.step = self.opt = self.lr_sched = None     # the old step and its graph go first
-        self._build(points, normals, colours, (dict(sd, state=state), sched))
+        self._build(points, normals, colours, poses, self._cameras_due(self.it), (dict(sd, state=state), sched))
+
+    def start_cameras(self):
+        """the step built anew with the camera poses learnt (at ``cameras_from_it``): the cloud, the poses and Adam's
+        state as they are"""
+        (points, normals, colours), sd, _ = self._cloud_state()
+        self._rebuild(points, normals, colours, sd, {})
+        self.log.info("Learning the camera poses from it=%d" % self.it)
+
+    def views_now(self):
+        """the data's device views with the current camera corrections (the views themselves when none are learnt)"""
+        return self.views if self.poses is None else self.views.with_poses(self.poses)
 
     def grow(self, n):
         """The growth event: the cloud grows from P to ``n`` points, at the start of a milestone's iteration.  The P
@@ -439,7 +512,7 @@ class Trainer:
         t0 = time.perf_counter()
         (points, normals, colours), sd, keys = self._cloud_state()
         P, st = points.shape[0], self.step
-        cov = point_coverage(points, normals, self.views, self.params, self.batch_size,
+        cov = point_coverage(points, normals, self.views_now(), self.params, self.batch_size,
                              range(self.rank, len(self.views), self.world), st.Vrk_invariant, st.Vrk_isotropic,
                              st.frnn_radius)
         st = None
@@ -489,7 +562,7 @@ class Trainer:
         ``batch_size`` views at a time, scored by :func:`~dss_b200.ops.evaluate_2d`."""
         if self.metric in IMAGE_METRICS:
             st = self.step
-            ev = evaluate_2d(st.points, st.normals, st.colours, self.views, self.params,
+            ev = evaluate_2d(st.points, st.normals, st.colours, self.views_now(), self.params,
                              max(1, self.data.resolution[0] // 4), self.batch_size, st.Vrk_invariant, st.Vrk_isotropic,
                              st.frnn_radius, st.shininess)
             return {"iou": float(ev["iou"]), "psnr": float(ev["psnr"])}
@@ -531,6 +604,7 @@ class Trainer:
             "schedule": {"radii_backward_scaler": self.params.radii_backward_scaler,
                          "lambda_dr_proj": self.lambda_dr_proj},
             "sampler": self.gen.get_state(), "epoch_order": list(self.order), "epoch_pos": self.pos,
+            **({} if self.poses is None else {"cameras": {"poses": self.poses.detach().clone()}}),
         }, tmp)
         os.replace(tmp, path)
 
@@ -543,14 +617,17 @@ class Trainer:
             return
         s = self.step
         named = [("points", s.points), ("normals", s.normals), ("colours", s.colours)]
+        if self.poses is not None:
+            named.append(("camera poses", self.poses))
         if event:
             named += [("Adam's %s of the %s" % (k, n), self.opt.state[t][k]) for n, t in named
                       if t in self.opt.state for k in ("exp_avg", "exp_avg_sq")]
         check_replicas(named, self.sync.group)
         if not event:
             self._checked_it = self.it
-        self.log.info("Replica check: the %d ranks hold the same points, normals and colours%s"
-                      % (self.world, " and Adam moments" if event else ""))
+        self.log.info("Replica check: the %d ranks hold the same points, normals%s and colours%s"
+                      % (self.world, ", camera poses" if self.poses is not None else "",
+                         " and Adam moments" if event else ""))
 
     def _out_of_time(self, exit_after, t0):
         """whether to leave after this iteration; a sharded run's ranks agree (any rank's clock decides for all)"""
@@ -597,6 +674,8 @@ class Trainer:
                     self.prune()                      # first: a growth on the same iteration seeds no strays
                 if self.it in self.grow_at:
                     self.grow(self.grow_at[self.it])
+                if self.learn_cameras and self.step.poses is None and self._cameras_due(self.it):
+                    self.start_cameras()
                 if self.it in self.prune_at or self.it in self.grow_at:
                     self.check_replicas(event=True)
                 self._schedule()
@@ -606,11 +685,15 @@ class Trainer:
                         self.step.capture()
                     loss = self.step.replay()
                 else:
-                    loss = self.step(*self.views.batch(deal_batch(self.data.camera_mat, idx, self.world)[self.rank]))
+                    mine = self.views.upload(deal_batch(self.data.camera_mat, idx, self.world)[self.rank])
+                    loss = self.step(*self.views.batch_at(mine), idx=mine if self.step.poses is not None else None)
                 self.opt.step()
                 it = self.it
                 if self.lead and print_every > 0 and it % print_every == 0:
-                    vals = {k: float(v) for k, v in loss.items()}
+                    names = list(loss) + ([] if self.poses is None else
+                                          ["cam_rot_mean", "cam_rot_max", "cam_trans_mean", "cam_trans_max"])
+                    cam = [] if self.poses is None else list(pose_stats(self.poses))
+                    vals = dict(zip(names, torch.stack([v.double() for v in loss.values()] + cam).tolist()))
                     self.log.info("[Epoch %02d] it=%03d, loss=%.4f, time=%.4f " % (self.epoch_it, it, vals["loss"],
                                                                                    time.time() - t0b)
                                   + " ".join("%s=%.4g" % kv for kv in vals.items() if kv[0] != "loss"))

@@ -158,10 +158,35 @@ def normalize_mesh(verts):
     return verts / verts.norm(dim=1).max()
 
 
+def perturb_cameras(camera_mat, degrees, frac, seed=0):
+    """``camera_mat`` (V,4,4) world-to-view matrices (row-vector convention) with every pose perturbed in its camera
+    frame, as the pose refinement corrects it (``view E``, E = [[R, 0], [t, 1]]): R a rotation of exactly ``degrees``
+    about a uniformly random axis and t a uniformly random direction of length ``frac`` times the camera's distance to
+    the origin, which is then how far the camera centre moves.  Drawn from ``numpy.random.default_rng(seed)``,
+    computed in float64; returns float32 (V,4,4)."""
+    m = np.asarray(camera_mat, dtype=np.float64)
+    V = m.shape[0]
+    rng = np.random.default_rng(int(seed))
+    unit = lambda x: x / np.linalg.norm(x, axis=1, keepdims=True)
+    axis, direction = unit(rng.standard_normal((V, 3))), unit(rng.standard_normal((V, 3)))
+    centres = -np.einsum("vj,vij->vi", m[:, 3, :3], m[:, :3, :3])          # c R + t = 0
+    th = np.deg2rad(float(degrees))
+    out = m.copy()
+    for v in range(V):
+        k = axis[v]
+        K = np.array([[0.0, -k[2], k[1]], [k[2], 0.0, -k[0]], [-k[1], k[0], 0.0]])
+        E = np.eye(4)
+        E[:3, :3] = np.eye(3) + np.sin(th) * K + (1.0 - np.cos(th)) * (K @ K)
+        E[3, :3] = float(frac) * np.linalg.norm(centres[v]) * direction[v]
+        out[v] = m[v] @ E
+    return out.astype(np.float32)
+
+
 def write_mvr_data(output_dir, verts, faces, images, masks, camera_mat, lights, points, normals, point_lights,
-                   camera_params):
+                   camera_params, camera_mat_true=None):
     """Write the data directory from renders already made (host arrays): images (N,S,S,4) float in [0,1]-ish, masks
-    (N,S,S) bool, camera_mat (N,4,4), lights a list of N ``light_value_dict`` dicts, points / normals (P,3).  Returns
+    (N,S,S) bool, camera_mat (N,4,4), lights a list of N ``light_value_dict`` dicts, points / normals (P,3), and
+    ``camera_mat_true`` (N,4,4), the cameras the images were rendered from when ``camera_mat`` is not.  Returns
     ``output_dir``."""
     from PIL import Image
     rgb_dir, mask_dir = os.path.join(output_dir, "image"), os.path.join(output_dir, "mask")
@@ -178,6 +203,8 @@ def write_mvr_data(output_dir, verts, faces, images, masks, camera_mat, lights, 
     data = {"cameras_type": CAMERAS_TYPE, "cameras_params": dict(camera_params), "lights_type": LIGHTS_TYPE[bool(point_lights)],
             "points": points, "normals": np.asarray(normals, dtype=np.float32),
             "colors": np.ones_like(points, dtype=np.float32), "camera_mat": np.asarray(camera_mat, dtype=np.float32)}
+    if camera_mat_true is not None:
+        data["camera_mat_true"] = np.asarray(camera_mat_true, dtype=np.float32)
     for i, d in enumerate(lights):
         data["lights_%d" % i] = d
     np.savez(os.path.join(output_dir, "data_dict.npz"), **data)
@@ -186,8 +213,10 @@ def write_mvr_data(output_dir, verts, faces, images, masks, camera_mat, lights, 
 
 def create_mvr_data(mesh_path, output, num_cameras=120, image_size=512, tri_color_light=False, point_lights=False,
                     has_specular=False, min_dist=1.2, max_dist=2.2, znear=0.1, seed=0, num_points=20000,
-                    device="cuda", views_per_call=32):
-    """Render one mesh into ``<output>/<name>_variational_light/`` (see the module docstring).  Returns the directory."""
+                    device="cuda", views_per_call=32, camera_noise=None):
+    """Render one mesh into ``<output>/<name>_variational_light/`` (see the module docstring).  ``camera_noise``:
+    ``(degrees, frac)``, the data's ``camera_mat`` are then those of :func:`perturb_cameras` (seeded with ``seed``) and
+    ``camera_mat_true`` the cameras the images are rendered from.  Returns the directory."""
     from ..ops import make_shading, render_mesh
     dev = torch.device(device)
     name = os.path.splitext(os.path.basename(mesh_path))[0]
@@ -221,9 +250,12 @@ def create_mvr_data(mesh_path, output, num_cameras=120, image_size=512, tri_colo
         masks.append((r.pix_to_face >= 0).cpu())
     gd = torch.Generator(device=dev).manual_seed(int(seed))
     points, normals = sample_points_from_mesh(vd, fd, num_points, generator=gd)
+    cams_out, cams_true = view.numpy(), None
+    if camera_noise is not None:
+        cams_out, cams_true = perturb_cameras(view.numpy(), camera_noise[0], camera_noise[1], seed), view.numpy()
     return write_mvr_data(out_dir, verts.numpy(), faces_np, torch.cat(images).numpy(), torch.cat(masks).numpy(),
-                          view.numpy(), [light_value_dict(l) for l in lights], points.cpu().numpy(),
-                          normals.cpu().numpy(), point_lights, camera_params)
+                          cams_out, [light_value_dict(l) for l in lights], points.cpu().numpy(),
+                          normals.cpu().numpy(), point_lights, camera_params, cams_true)
 
 
 def main(argv=None):
@@ -239,13 +271,18 @@ def main(argv=None):
     p.add_argument("--max_dist", type=float, default=2.2)
     p.add_argument("--znear", type=float, default=0.1)
     p.add_argument("--seed", type=int, default=0)
+    p.add_argument("--camera-noise", type=float, nargs=2, metavar=("DEG", "FRAC"), default=None,
+                   help="store every camera perturbed by a random rotation of DEG degrees and a translation of FRAC "
+                        "times its distance to the origin (the exact ones as camera_mat_true)")
     opt = p.parse_args(argv)
+    if opt.camera_noise is not None and (opt.camera_noise[0] < 0 or opt.camera_noise[1] < 0):
+        p.error("--camera-noise takes DEG >= 0 and FRAC >= 0")
     paths = sorted({q for pat in opt.points for q in (glob.glob(pat) or [pat])})
     out = []
     for path in paths:
         out.append(create_mvr_data(path, opt.output, opt.num_cameras, opt.image_size, opt.tri_color_light,
                                    opt.point_lights, opt.has_specular, opt.min_dist, opt.max_dist, opt.znear,
-                                   opt.seed))
+                                   opt.seed, camera_noise=opt.camera_noise))
         print(out[-1])
     return out
 

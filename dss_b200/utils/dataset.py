@@ -5,6 +5,7 @@ image, plus the ground-truth image and mask files next to it (dataset.py:36-101:
 read with PIL (the reference uses imageio, which this image lacks).  ``device_views`` uploads every view once into a
 :class:`DeviceViews` store that the training loop gathers its batches from; ``pinned_batch`` stages a batch of views in
 pinned host memory for a host->device copy.  Dense depth maps (OpenEXR) are not read."""
+import copy
 import os
 
 import numpy as np
@@ -312,3 +313,26 @@ class DeviceViews:
         """``(img (B,H,W,3), mask (B,H,W), proj (B,4,4), view (B,4,4), lights)`` on the device for the host list
         ``idx`` (checked before anything is uploaded); an empty ``idx`` gives batch-0 tensors"""
         return self.batch_at(self.upload(idx))
+
+    def check_rigid(self):
+        """refuse with ValueError cameras the pose refinement cannot take (``ops.check_rigid_cameras``); checked once"""
+        if not getattr(self, "_rigid", False):
+            from ..ops import check_rigid_cameras
+            check_rigid_cameras(self.camera_mat)
+            self._rigid = True
+
+    def with_poses(self, poses):
+        """These views with every camera refined by ``poses`` (V,6), one correction per view (``ops.pose_cameras``):
+        a ``DeviceViews`` sharing this one's store and lights, whose ``camera_mat`` and ``proj`` are the refined
+        matrices of all V views (no gradient), so that ``evaluate_2d``, ``point_coverage`` and ``render_data_views``
+        see the refined cameras.  Zero poses give this one's matrices bit for bit."""
+        from ..ops import pose_cameras
+        self.check_rigid()
+        V = len(self)
+        if tuple(poses.shape) != (V, 6):
+            raise ValueError("poses must have shape (%d, 6), got %s" % (V, tuple(poses.shape)))
+        out = copy.copy(self)
+        with torch.no_grad():
+            idx = torch.arange(V, dtype=torch.int64, device=self.device)
+            out.camera_mat, out.proj = pose_cameras(poses.detach(), idx, self.camera_mat, self.proj)
+        return out

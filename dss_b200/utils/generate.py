@@ -12,7 +12,9 @@ default, or ``--model``), keeps the points whose ``points_activation`` is set, n
   - with ``--images`` (:func:`generate_images`): ``images/%04d.png``, the renders of the data's first
     ``generation.vis_n_outputs`` views at the data's resolution S, clipped to [0, 1] (``generate_images``,
     point_modeling.py:335-348), and ``image_metrics.json``, the ``evaluate_2d`` metrics of every view at S // 4 (the
-    training loop's validation size) and at S.
+    training loop's validation size) and at S.  When the checkpoint holds camera poses (a run with
+    ``model.model_kwargs.learn_cameras``), the views are rendered and scored with the refined cameras, and
+    ``cameras.npz`` holds their ``camera_mat`` (V,4,4) float32, in ``data_dict.npz``'s layout.
 The ``generation`` block is read over ``configs/default.yaml``'s values (:data:`GENERATION_DEFAULTS`)."""
 import argparse
 import copy
@@ -22,7 +24,8 @@ import warnings
 
 import torch
 
-__all__ = ["GENERATION_DEFAULTS", "generation_settings", "load_cloud", "generate", "generate_images", "main"]
+__all__ = ["GENERATION_DEFAULTS", "generation_settings", "load_cloud", "load_poses", "generate", "generate_images",
+           "main"]
 
 # configs/default.yaml's generation block (refinement_step and points_batch_size have no effect on a point model's
 # export; batch_size is the number of views --images renders at once, vis_n_outputs how many it writes)
@@ -52,6 +55,13 @@ def load_cloud(path, device):
     return points.float().contiguous(), normals.float().contiguous(), colours.float().contiguous()
 
 
+def load_poses(path, device):
+    """the (V,6) camera poses of a ``Trainer.save`` checkpoint on ``device``, or None when it holds none"""
+    ckpt = torch.load(path, map_location=device, weights_only=False)
+    cams = ckpt.get("cameras")
+    return None if cams is None else cams["poses"].float().contiguous()
+
+
 def generate(cfg, depth=8, model=None, images=False):
     """write pointcloud.ply and mesh.<ext> (and, with ``images``, what :func:`generate_images` writes); returns (cloud
     path, mesh path, number of points, PoissonMesh)"""
@@ -75,17 +85,19 @@ def generate(cfg, depth=8, model=None, images=False):
     else:
         save_obj(mesh_path, mesh.verts.cpu().numpy(), mesh.faces.cpu().numpy())
     if images:
-        generate_images(cfg, points, normals, colours, gen_dir)
+        generate_images(cfg, points, normals, colours, gen_dir, load_poses(path, points.device))
     return cloud_path, mesh_path, points.shape[0], mesh
 
 
-def generate_images(cfg, points, normals, colours, gen_dir):
+def generate_images(cfg, points, normals, colours, gen_dir, poses=None):
     """``<gen_dir>/images/%04d.png`` (RGBA, ``uint8(255 c)`` of c clipped to [0, 1]) for the first ``vis_n_outputs``
     views of the configuration's data at its resolution S, rendered as the training step renders them, and
     ``<gen_dir>/image_metrics.json``: for s = S // 4 and s = S, ``iou`` and ``psnr`` (the reference's names: 1 - IoU
     and the squared RGB error summed over the channels, per pixel) and ``psnr_db`` = -10 log10(psnr / 3), the PSNR in
     dB of the per-channel mean squared error of images in [0, 1] (null when the error is 0), per view and as their means
-    over the views.  Returns (the PNG paths, the JSON path)."""
+    over the views.  ``poses``: (V,6) camera corrections of the data's views; the views are then rendered and scored
+    with the refined cameras (``DeviceViews.with_poses``), whose world-to-view matrices go to ``<gen_dir>/cameras.npz``
+    as ``camera_mat`` (V,4,4) float32.  Returns (the PNG paths, the JSON path)."""
     import json
     import math
 
@@ -103,6 +115,12 @@ def generate_images(cfg, points, normals, colours, gen_dir):
     st = step_settings(cfg)
     flags = (st["Vrk_invariant"], st["Vrk_isotropic"])
     V, B = len(data), max(1, int(g["batch_size"]))
+    if poses is not None:
+        if tuple(poses.shape) != (V, 6):
+            raise ValueError("the checkpoint holds camera poses of shape %s, but the data has %d views"
+                             % (tuple(poses.shape), V))
+        data = data.device_views(points.device).with_poses(poses)
+        np.savez(os.path.join(gen_dir, "cameras.npz"), camera_mat=data.camera_mat.cpu().numpy())
     img_dir = os.path.join(gen_dir, "images")
     os.makedirs(img_dir, exist_ok=True)
     pngs = []

@@ -782,6 +782,24 @@ DSS_API int dss_sample_mesh_poisson_disk(dss_ctx *ctx, const float *verts, int64
 DSS_API int dss_poisson_disk_stats(dss_ctx *ctx, int *probes, double *radii, int64_t *counts, int *rounds,
                                    float *stage_ms);
 
+/* ---- camera pose corrections ------------------------------------------------------------------------------------
+ * V per-view corrections xi_v = (w, t), poses (V,6) f32: a rotation vector w and a translation t applied in the camera
+ * frame.  Row-vector convention: E = [[R(w), 0], [t, 1]] with R(w) = I + s [w]x + c [w]x^2 (s = sin th / th, c = (1 -
+ * cos th) / th^2, th = |w|: scipy's Rotation.from_rotvec(w).as_matrix()), and for batch entry b of view v = idx[b]
+ *   view[b] = view0[v] + view0[v] D,   proj[b] = proj0[v] + view0[v] D K,   D = E - I,   K = view0[v]^-1 proj0[v],
+ * view0[v]^-1 the rigid inverse [[R^T, 0], [-t R^T, 1]] (the caller checks that view0's 3x3 blocks are rotations).  D
+ * is formed directly, so xi = 0 gives view0 and proj0 bit for bit.  Computed in float64, each output element rounded
+ * once.  idx (B,) int64 device, each in [0, V) (the call does not read them on the host; an index out of range gives
+ * NaN matrices); view0 / proj0 (V,4,4), view / proj (B,4,4) f32 contiguous.  No scratch, no host synchronisation. */
+DSS_API int dss_pose_forward(dss_ctx *ctx, const float *poses, const int64_t *idx, int V, int B, const float *view0,
+                             const float *proj0, float *view, float *proj, void *stream);
+/* The backward: grad_poses (V,6), every row written, from grad_view / grad_proj (B,4,4) f32 (either may be NULL: zero).
+ * Row v sums the batch entries with idx[b] == v in batch order in float64, then applies the chain rule once; rows of
+ * views outside the batch are +0.  One thread per row, no atomics: the same bits on every run. */
+DSS_API int dss_pose_backward(dss_ctx *ctx, const float *poses, const int64_t *idx, int V, int B, const float *view0,
+                              const float *proj0, const float *grad_view, const float *grad_proj, float *grad_poses,
+                              void *stream);
+
 #ifdef __cplusplus
 }
 #endif
