@@ -50,6 +50,7 @@ class RenderArgs(C.Structure):
         ("cell_counts", vp),
         ("frames", vp),
         ("deterministic_colours", C.c_int32),
+        ("depth", vp), ("grad_depth", vp),
     ]
 
 
@@ -105,6 +106,13 @@ _SIGNATURES = {
     "dss_image_loss_partial": (C.c_int, [vp, vp, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                          C.c_double, C.c_double, vp, vp]),
     "dss_image_loss_finish": (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, vp, vp, vp, vp]),
+    "dss_depth_loss_forward": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                         C.c_double, vp, vp, vp]),
+    "dss_depth_loss_partial": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                         vp, vp]),
+    "dss_depth_loss_finish": (C.c_int, [vp, vp, C.c_double, vp, vp]),
+    "dss_depth_loss_backward": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float,
+                                          C.c_double, vp, vp, vp, vp]),
     "dss_image_metrics": (C.c_int, [vp, vp, C.c_int, vp, C.POINTER(C.c_int64), vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                     vp, vp, vp]),
     "dss_gather_views": (C.c_int, [vp, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp]),

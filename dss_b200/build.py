@@ -17,7 +17,7 @@ SOURCES = ["ctx.cu", "binning.cu", "raster_fwd.cu", "backward.cu", "occ_backward
            "regularisers.cu", "image_loss.cu", "point_filter.cu", "local_frames.cu", "mesh_raster.cu", "chamfer.cu",
            "mesh_distance.cu", "poisson.cu", "mesh_sample.cu", "image_metrics.cu", "normals.cu", "upsample.cu",
            "rimls.cu", "l0_smooth.cu", "views.cu", "prune.cu",
-           "poses.cu"]
+           "poses.cu", "depth.cu"]
 HEADERS = ["binning.cuh", "common.cuh", "kernels.cuh", "mask_sample.cuh", "shading.cuh", "sym3_eigen.cuh", os.path.join("..", "..", "include", "dss_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]   # H100 (Hopper)

@@ -95,14 +95,6 @@ colour_backward_kernel(const int32_t *__restrict__ idx, const float *__restrict_
 // integer once: the error of a record is at most (its terms / 2) * G * pixels_per_view * 2^-62, about 2^-45 G per term at
 // 512^2.  The finish writes sum * 2^-e.  A non-finite term is added to the float output with float atomics instead:
 // its NaN or infinity does not depend on the order, and the finish leaves such entries as they are.
-__device__ __forceinline__ int colour_fixed_exp(const int *gmax, int64_t pixels_per_view) {
-    int x;
-    frexp((double)__int_as_float(*gmax) * (double)pixels_per_view, &x);
-    return 62 - x;
-}
-
-__device__ __forceinline__ int finite_abs_bits(float v) { return isfinite(v) ? __float_as_int(fabsf(v)) : 0; }
-
 __global__ void __launch_bounds__(256)
 colour_gmax_kernel(const float4 *__restrict__ grad_image, int64_t num_pixels, int *__restrict__ gmax) {
     int m = 0;

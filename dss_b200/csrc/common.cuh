@@ -95,6 +95,8 @@ enum BufId {
     BUF_NORMALS,      // normal estimation: unoriented normals, the spanning forest's state, the Euler tours and flags
     BUF_UPSAMPLE,     // upsampling: the round's K-NN rows, select keys, chosen neighbours, flags and their scan, histograms
     BUF_L0,           // L0 smoothing: the rows' complex transforms, twiddles, float64 input and estimate planes, keep flags
+    BUF_DEPTH_FIXED,  // depth backward: per-record 64-bit fixed-point sums and the call's scale
+    BUF_DEPTH_LOSS,   // per-block fp64 partial sums of the depth loss
     NUM_BUFS
 };
 
@@ -104,7 +106,7 @@ namespace dss {
 enum Stage {
     ST_PACK = 0, ST_PREPROCESS, ST_BIN_COUNT, ST_SCAN, ST_BIN_SCATTER, ST_RASTER_FWD, ST_VISIBILITY,
     ST_SEARCH_RADIUS, ST_OCC_BWD, ST_COLOUR_BWD, ST_ZBUF_BWD, ST_CHAIN, ST_GRID, ST_OCC_BIN, ST_KNN,
-    ST_CAMERA_BWD, ST_LIGHT_BWD, NUM_STAGES
+    ST_CAMERA_BWD, ST_LIGHT_BWD, ST_DEPTH_FWD, ST_DEPTH_BWD, NUM_STAGES
 };
 struct ProfPending {
     cudaEvent_t a, b;

@@ -102,7 +102,7 @@ static void prof_collect(dss_ctx *ctx) {
 static const char *k_stage_names[NUM_STAGES] = {
     "pack_records", "preprocess", "bin_count", "scan", "bin_scatter", "raster_forward", "visibility",
     "search_radius", "occ_backward", "colour_backward", "zbuf_backward", "chain_world", "grid_2d", "occ_bin", "knn",
-    "camera_backward", "light_backward"};
+    "camera_backward", "light_backward", "depth_forward", "depth_backward"};
 
 // ---------------------------------------------------------------------------------------------
 // Exclusive scan, single pass with decoupled look-back.  Replaces external/prefix_sum

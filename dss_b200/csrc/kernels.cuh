@@ -182,6 +182,22 @@ int colour_backward_fixed(dss_ctx *ctx, const int32_t *idx, const float *weights
                           int64_t num_pixels, int K, float *grad_colours, int64_t P, int64_t pixels_per_view,
                           cudaStream_t st);
 
+// Scale 2^e of a 64-bit fixed-point sum whose terms are at most G in magnitude, at most pixels_per_view of them per
+// sum (gmax: the int bits of G): every sum stays below 2^62 in magnitude (see colour_backward_fixed in backward.cu)
+__device__ __forceinline__ int colour_fixed_exp(const int *gmax, int64_t pixels_per_view) {
+    int x;
+    frexp((double)__int_as_float(*gmax) * (double)pixels_per_view, &x);
+    return 62 - x;
+}
+
+__device__ __forceinline__ int finite_abs_bits(float v) { return isfinite(v) ? __float_as_int(fabsf(v)) : 0; }
+
+// depth.cu: the blend's depth map D = sum_k w_k z_k (N,S,S) from the forward's idx, weights and records ...
+int depth_forward(dss_ctx *ctx, const dss_render_args *g, const float4 *rec, cudaStream_t st);
+// ... and its record gradient gz[s] += sum g_D w_k over the pixels whose list holds s, the weights held constant,
+// summed in 64-bit fixed point (the same bits on every run)
+int depth_backward(dss_ctx *ctx, const dss_render_args *g, float *gz, cudaStream_t st);
+
 // The k nearest *other* points of local row i from its dss_knn_points row nb at K = k + 1: the row less entry
 // knn_own_entry(nb, k, i), which is i's own index, or the last entry when i is not in the row (more than k duplicates
 // of smaller index).  Neighbour s of the k is nb[knn_other(s, own)].  Upsampling and the RIMLS kernels share this rule.

@@ -914,8 +914,10 @@ int dss_render_forward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
     a.visible = g->visible;
     a.cell_counts = cell_counts;
     a.zrange = zrange;   // already filled by the preprocess or its pre-pass
-    return bin_and_raster(ctx, a, g->shared_cloud ? nullptr : g->first_idx, g->num_points, g->P0, st,
-                          count_here ? &counted : nullptr);
+    rc = bin_and_raster(ctx, a, g->shared_cloud ? nullptr : g->first_idx, g->num_points, g->P0, st,
+                        count_here ? &counted : nullptr);
+    if (rc || !g->depth) return rc;
+    return depth_forward(ctx, g, rec, st);
 }
 
 int dss_colour_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
@@ -966,10 +968,11 @@ int dss_render_backward(dss_ctx *ctx, const dss_render_args *g, void *stream) {
         DSS_CUDA_TRY(cudaMemcpyAsync(g->search_radius, rs, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if ((rc = side.join())) return rc;
     float *gz = nullptr;
-    if (g->grad_zbuf) {
+    if (g->grad_zbuf || g->grad_depth) {
         if ((rc = ctx_get(ctx, BUF_MISC, (size_t)P, &gz))) return rc;
         DSS_CUDA_TRY(cudaMemsetAsync(gz, 0, (size_t)P * sizeof(float), st));
-        if ((rc = zbuf_backward(ctx, g->idx, g->grad_zbuf, npix, K, gz, 1, st))) return rc;
+        if (g->grad_zbuf && (rc = zbuf_backward(ctx, g->idx, g->grad_zbuf, npix, K, gz, 1, st))) return rc;
+        if (g->grad_depth && (rc = depth_backward(ctx, g, gz, st))) return rc;
     }
     const float2 *grad_xy = reinterpret_cast<const float2 *>(gxy);
     // the shading's position gradient exists only when this call ran the colour half

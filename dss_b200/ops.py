@@ -62,6 +62,7 @@ class RenderOutput(NamedTuple):
     visible: torch.Tensor    # (P,) uint8
     records: torch.Tensor    # (P,8) {x,y,z,rx, ry,a,b,c}
     scaler: torch.Tensor     # (P,)
+    depth: Optional[torch.Tensor] = None   # (N,S,S) sum_k w_k z_k, with depth=True
 
 
 def _fill_shading(a, sh, albedo):
@@ -148,7 +149,7 @@ class _RenderFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, normals, colours, proj, view, h, first_idx, num_points, shared, prm, want_frags,
                 grad_sync=None, shading=None, cam_centres=None, lights=None, ambient=None, frames=None,
-                deterministic=False):
+                deterministic=False, want_depth=False):
         # cam_centres, lights and ambient are the shading's tensors, passed on their own so that autograd tracks them
         dev = _lib.require_cuda(points, normals, colours, proj, view, h, first_idx, num_points, frames)
         points_c = _lib.as_f32(points.detach(), "points")
@@ -189,6 +190,7 @@ class _RenderFunction(torch.autograd.Function):
         cell_counts = torch.empty((N * OB * OB * 1024,), dtype=torch.int32, device=dev)
         zbuf = torch.empty((N, S, S, K), **f32) if want_frags else None
         qvalue = torch.empty((N, S, S, K), **f32) if want_frags else None
+        depth = torch.empty((N, S, S), **f32) if want_depth else None
         a = _lib.RenderArgs()
         _fill_common(a, points_c, normals_c, colours_c, proj_c, view_c, h_c, fi, npts, shared, N, P0, P, prm)
         a.frames = _lib.ptr(frames_c)
@@ -201,6 +203,7 @@ class _RenderFunction(torch.autograd.Function):
         a.records, a.scaler, a.image, a.idx = _lib.ptr(records), _lib.ptr(scaler), _lib.ptr(image), _lib.ptr(idx)
         a.weights, a.visible, a.zbuf, a.qvalue = _lib.ptr(weights), _lib.ptr(visible), _lib.ptr(zbuf), _lib.ptr(qvalue)
         a.cell_counts = _lib.ptr(cell_counts)
+        a.depth = _lib.ptr(depth)
         _lib.call("dss_render_forward", dev, C.byref(a))
         # no zero-filled gradients for the outputs nobody differentiates (idx, weights, records ... would cost five
         # fill kernels over ~400 MB per backward); backward() handles None
@@ -210,24 +213,29 @@ class _RenderFunction(torch.autograd.Function):
         ctx.deterministic = bool(deterministic)
         ctx.cell_counts = cell_counts
         ctx.meta = (shared, prm, N, P0, P, want_frags, shared_col, grad_sync)
+        ctx.want_depth = bool(want_depth)
         outs = (image, idx, weights, visible, records, scaler)
+        tail = (depth,) if want_depth else ()
         if want_frags:
             ctx.mark_non_differentiable(idx, weights, visible, records, scaler, qvalue)
-            return outs + (zbuf, qvalue)
+            return outs + (zbuf, qvalue) + tail
         ctx.mark_non_differentiable(idx, weights, visible, records, scaler)
-        return outs
+        return outs + tail
 
     @staticmethod
     def backward(ctx, grad_image, *rest):
         points_c, proj_c, view_c, records, idx, weights, visible, fi, npts = ctx.saved_tensors
         shared, prm, N, P0, P, want_frags, shared_col, grad_sync = ctx.meta
         dev = points_c.device
-        grad_zbuf = rest[5] if (want_frags and len(rest) > 5) else None
+        grad_zbuf = rest[5] if want_frags else None
+        grad_depth = rest[-1] if ctx.want_depth else None
         if grad_image is None:
             grad_image = torch.zeros((N, prm.image_size, prm.image_size, 4), dtype=torch.float32, device=dev)
         grad_image = _lib.as_f32(grad_image, "grad_image")
         if grad_zbuf is not None:
             grad_zbuf = _lib.as_f32(grad_zbuf, "grad_zbuf")
+        if grad_depth is not None:
+            grad_depth = _lib.as_f32(grad_depth, "grad_depth")
         shade = ctx.shading
         # with fused shading the colour scatter fills a (P,3) scratch (d L / d shaded colour) that the shading backward
         # turns into d albedo / d normal / d position
@@ -241,6 +249,7 @@ class _RenderFunction(torch.autograd.Function):
         a.cell_counts = _lib.ptr(ctx.cell_counts)
         a.shared_colours = int(shared_col)
         a.grad_image, a.grad_zbuf = _lib.ptr(grad_image), _lib.ptr(grad_zbuf)
+        a.grad_depth = _lib.ptr(grad_depth)
         a.grad_colours, a.grad_points_world = _lib.ptr(grad_colours), _lib.ptr(grad_points)
         grad_albedo = grad_pshade = None
         if shade is not None:
@@ -312,7 +321,7 @@ class _RenderFunction(torch.autograd.Function):
                 light_backward()
             grad_sync.reduce_late(grad_points)
             grad_sync.join(dev)
-        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb, None, None)
+        cams = (grad_proj, grad_view) + (None,) * 8 + (grad_cam, grad_lights, grad_amb, None, None, None)
         if shade is not None:
             return (grad_points, grad_normals, grad_albedo) + cams
         return (grad_points, None, grad_colours) + cams
@@ -320,7 +329,7 @@ class _RenderFunction(torch.autograd.Function):
 
 def render_points(points, normals, colours, proj, view, h, params: SplatParams, first_idx=None, num_points=None,
                   shared_cloud=True, return_fragments=False, grad_sync=None, shading=None, frames=None,
-                  deterministic=False) -> RenderOutput:
+                  deterministic=False, depth=False) -> RenderOutput:
     """Render ``N`` views of an oriented point cloud to RGBA.
 
     points, normals : (P0,3) when ``shared_cloud`` (one cloud seen from N cameras) else packed (P,3)
@@ -346,14 +355,20 @@ def render_points(points, normals, colours, proj, view, h, params: SplatParams, 
     deterministic   : with ``shading``, the backward sums d L / d shaded in 64-bit fixed point, so that its gradients are
                       the same bits on every run (the training step asks for it: the loop's resume relies on it); off,
                       float atomics add those terms in arrival order, which is faster at large P
+    depth           : also return ``RenderOutput.depth``, the (N,S,S) depth of the blend D = sum_k w_k z_k over the
+                      pixel's K-list (``weights`` and the records' view depth z; 0 where the list is empty), one launch
+                      more.  Differentiable: its gradient reaches each listed record's view depth as sum g_D w_k -- the
+                      weights held constant, as the reference holds the blend weights -- summed in 64-bit fixed point
+                      (the same bits on every run), and from there the positions and, when they require grad, ``proj``
+                      and ``view``
     """
     outs = _RenderFunction.apply(points, normals, colours, proj, view, h, first_idx, num_points,
                                  bool(shared_cloud), params, bool(return_fragments), grad_sync, shading,
                                  *((shading.cam_centres, shading.lights, shading.ambient) if shading is not None
-                                   else (None, None, None)), frames, bool(deterministic))
+                                   else (None, None, None)), frames, bool(deterministic), bool(depth))
     image, idx, weights, visible, records, scaler = outs[:6]
     zbuf, qvalue = (outs[6], outs[7]) if return_fragments else (None, None)
-    return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler)
+    return RenderOutput(image, idx, zbuf, qvalue, weights, visible, records, scaler, outs[-1] if depth else None)
 
 
 def _shared_render_masks(out: RenderOutput, mask_img):
@@ -1305,8 +1320,8 @@ def shared_cloud_splats(points, n_views, Vrk_invariant=True, Vrk_isotropic=True,
 
 
 def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius, shininess):
-    """render(params, views) -> the ``RenderOutput`` whose image :func:`render_data_views` returns, with what does not
-    depend on the views (the cloud's splat sizes, all the views' cameras and lights on the device) computed once"""
+    """render(params, views, depth=False) -> the ``RenderOutput`` whose image :func:`render_data_views` returns (with
+    ``depth``, its depth map too), with what does not depend on the views (the cloud's splat sizes, all the views' cameras and lights on the device) computed once"""
     from .core.camera import camera_matrices
     from .core.lighting import pack_lights
     from .core.texture import camera_centres
@@ -1328,7 +1343,7 @@ def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotr
     n = torch.nn.functional.normalize(normals.detach(), dim=-1)
     h1, frames = shared_cloud_splats(p, 1, Vrk_invariant, Vrk_isotropic, frnn_radius)
 
-    def render(params, views):
+    def render(params, views, depth=False):
         idx = torch.as_tensor(list(views), dtype=torch.int64, device=dev)
         rows, ambient, kind = pack_lights(lights_of(idx))
         view = view_all.index_select(0, idx)
@@ -1336,19 +1351,20 @@ def _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotr
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), kind, float(shininess))
             return render_points(p, n, c, proj_all.index_select(0, idx), view,
                                  None if h1 is None else h1.repeat(idx.shape[0]), params, shading=shading,
-                                 deterministic=True, frames=frames)
+                                 deterministic=True, frames=frames, depth=depth)
     return render
 
 
 def render_data_views(points, normals, colours, data, params: SplatParams, views, Vrk_invariant=True,
-                      Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0):
+                      Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0, depth=False):
     """(len(views), S, S, 4) renders, S = ``params.image_size``, of one shared cloud from the cameras of ``data``'s
     views ``views`` (an ``MVRData``: its ``get_cameras()`` projections and ``camera_mat`` view matrices, or the same
     held by a ``DeviceViews``) with fused shading by each view's own lights (``data.light_props``), as the training
     step renders a batch: unit normals, the splats of :func:`shared_cloud_splats`, ``colours`` the albedo.  Forward
-    only."""
-    return _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius,
-                               shininess)(params, views).image
+    only.  With ``depth``: ``(images, depth maps (len(views), S, S))``, the depth of ``render_points(..., depth=True)``."""
+    out = _data_view_renderer(points, normals, colours, data, Vrk_invariant, Vrk_isotropic, frnn_radius,
+                              shininess)(params, views, depth=depth)
+    return (out.image, out.depth) if depth else out.image
 
 
 def evaluate_2d(points, normals, colours, data, params: SplatParams, image_size, batch=1, Vrk_invariant=True,

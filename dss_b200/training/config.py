@@ -9,7 +9,7 @@ import warnings
 
 import yaml
 
-__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "check_pruning", "check_cameras",
+__all__ = ["DEFAULTS", "load_config", "update_recursive", "check_config", "check_growth", "check_pruning", "check_cameras", "check_depth",
            "cloud_size", "check_cloud_size", "GROW_K", "step_settings", "splat_params", "EVAL_SAMPLINGS", "SELECTION_METRICS",
            "IMAGE_METRICS", "selection_metric"]
 
@@ -22,7 +22,7 @@ DEFAULTS = {
     "name": "demo",
     "data": {"type": "MVR", "data_dir": "example_data", "data_dict": "data_dict.npz", "img_folder": "image",
              "mask_folder": "mask", "img_extension": "png", "mask_extension": "png", "n_imgs": None,
-             "resolution": [512, 512]},
+             "resolution": [512, 512], "load_dense_depth": False, "depth_folder": "depth", "depth_extension": "exr"},
     "renderer": {
         "is_neural_texture": False,
         "lighting": "from_data",
@@ -45,6 +45,7 @@ DEFAULTS = {
         "grow_milestones": [], "grow_points": [],
         "prune_milestones": [], "prune_min_views": 1, "prune_max_outside": 0,
         "lr_cameras": 1e-4, "cameras_from_it": 300,
+        "lambda_dr_depth": 0.0,
     },
 }
 
@@ -58,7 +59,7 @@ GROW_K = 16
 # gamma_dss_backward_radii nor limit_dss_backward_radii, trainer.py:118-123): accepted without a warning.
 _NO_EFFECT = {
     "type", "test",
-    "data.img_extension_input", "data.depth_folder", "data.img_with_camera", "data.img_with_mask",
+    "data.img_extension_input", "data.img_with_camera", "data.img_with_mask",
     "renderer.renderer_type", "renderer.raster_type", "renderer.compositor_type", "renderer.composite_params",
     "training.batch_size_val", "training.n_workers", "training.patch_size", "training.learning_rate",
     "training.overwrite_visualization", "training.n_debug_points", "training.point_file", "training.n_training_points",
@@ -122,9 +123,10 @@ def load_config(path, default_path=None):
     return cfg
 
 
-def check_config(cfg, resolution, has_lights):
+def check_config(cfg, resolution, has_lights, has_depth=False):
     """Refuse what the loop cannot train: a neural texture, lighting other than the data's, an image size other than
-    the data's ``resolution`` (H, W), data without per-image lights."""
+    the data's ``resolution`` (H, W), data without per-image lights, a depth term without depth maps
+    (``has_depth``)."""
     r = cfg["renderer"]
     if r.get("is_neural_texture", False):
         raise NotImplementedError("renderer.is_neural_texture: true is not supported (NeuralTexture is out of scope); "
@@ -140,6 +142,20 @@ def check_config(cfg, resolution, has_lights):
     check_growth(cfg)
     check_pruning(cfg)
     check_cameras(cfg)
+    check_depth(cfg, has_depth)
+
+
+def check_depth(cfg, has_depth):
+    """Refuse depth settings the loop cannot follow: ``training.lambda_dr_depth`` must be a finite number >= 0,
+    ``data.load_dense_depth`` a bool, and a lambda > 0 needs the data's depth maps (``has_depth``)."""
+    lam, on = cfg["training"].get("lambda_dr_depth", 0.0), cfg["data"].get("load_dense_depth", False)
+    if isinstance(lam, bool) or not isinstance(lam, (int, float)) or not 0 <= lam < float("inf"):
+        raise ValueError("training.lambda_dr_depth must be a number >= 0, got %r" % (lam,))
+    if not isinstance(on, bool):
+        raise ValueError("data.load_dense_depth must be true or false, got %r" % (on,))
+    if lam > 0 and not has_depth:
+        raise ValueError("training.lambda_dr_depth %g needs dense depth maps: set data.load_dense_depth: true with the "
+                         "maps in <data_dir>/%s" % (lam, cfg["data"].get("depth_folder", "depth")))
 
 
 def _is_int(x):
@@ -279,4 +295,4 @@ def step_settings(cfg):
     return {"Vrk_invariant": bool(rp["Vrk_invariant"]), "Vrk_isotropic": bool(rp["Vrk_isotropic"]),
             "lambda_dr_rgb": float(tr["lambda_dr_rgb"]), "lambda_dr_silhouette": float(tr["lambda_dr_silhouette"]),
             "lambda_dr_proj": float(tr["lambda_dr_proj"]), "lambda_dr_repel": float(tr["lambda_dr_repel"]),
-            "learn": learn}
+            "lambda_dr_depth": float(tr.get("lambda_dr_depth", 0.0)), "learn": learn}

@@ -27,7 +27,8 @@ import torch.nn as nn
 from .. import _lib
 
 __all__ = ["BaseLoss", "L1Loss", "L2Loss", "SurfaceLoss", "ProjectionLoss", "RepulsionLoss", "KNN",
-           "surface_regulariser", "IouLoss", "image_loss", "image_loss_torch", "fused_image_loss_targets"]
+           "surface_regulariser", "IouLoss", "image_loss", "image_loss_torch", "fused_image_loss_targets",
+           "depth_loss", "depth_loss_torch"]
 
 
 class KNN(NamedTuple):
@@ -618,3 +619,119 @@ def image_loss(rgba, img, mask_img, lambda_rgb=1.0, lambda_silhouette=1.0, group
     loss, loss_rgb, loss_sil = _ImageLoss.apply(rgba_c, img, mask, lambda_rgb, lambda_silhouette, group)
     zero = torch.zeros((), dtype=torch.float32, device=rgba.device)
     return {"loss": loss, "loss_dr_rgb": loss_rgb, "loss_dr_silhouette": loss_sil, "loss_image_gradients": zero}
+
+
+def _depth_loss_inputs(depth, rgba, depth_gt, mask_img, min_views=1):
+    """shape and device checks shared by both routes; returns the mask as (N,H,W)"""
+    if depth.dim() != 3:
+        raise RuntimeError("depth must have shape (N, H, W), got %s" % (tuple(depth.shape),))
+    N, H, W = depth.shape
+    if N < min_views or H < 1 or W < 1:
+        raise RuntimeError("depth must hold at least one pixel, got %s" % (tuple(depth.shape),))
+    if tuple(rgba.shape) != (N, H, W, 4):
+        raise RuntimeError("rgba must have shape (N, H, W, 4) = %s, got %s" % ((N, H, W, 4), tuple(rgba.shape)))
+    if tuple(depth_gt.shape) != (N, H, W):
+        raise RuntimeError("depth_gt must have shape (N, H, W) = %s, got %s" % ((N, H, W), tuple(depth_gt.shape)))
+    if tuple(mask_img.shape) not in ((N, H, W), (N, 1, H, W)):
+        raise RuntimeError("mask_img must have shape (N, H, W) or (N, 1, H, W), got %s" % (tuple(mask_img.shape),))
+    if not (depth.device == rgba.device == depth_gt.device == mask_img.device):
+        raise RuntimeError("depth, rgba, depth_gt and mask_img must be on one device")
+    return mask_img.reshape(N, H, W)
+
+
+def _depth_valid(rgba, depth_gt, mask_img, znear, zfar):
+    return mask_img.bool() & rgba[..., 3].bool() & torch.isfinite(depth_gt) & (depth_gt > znear) & (depth_gt < zfar)
+
+
+def depth_loss_torch(depth, rgba, depth_gt, mask_img, lambda_depth=1.0, znear=1.0, zfar=100.0, group=None):
+    """:func:`depth_loss` in torch ops, any dtype and device, with host synchronisations; the float64 reference of the
+    tests.  ``group``: as for :func:`depth_loss`."""
+    mask_img = _depth_loss_inputs(depth, rgba, depth_gt, mask_img, min_views=0 if group is not None else 1)
+    valid = _depth_valid(rgba, depth_gt, mask_img, znear, zfar)
+    s = (depth - depth_gt).abs()[valid].sum()
+    M = valid.sum()
+    if group is not None:
+        import torch.distributed as dist
+        row = torch.stack([M.to(torch.float64), s.detach().to(torch.float64)])
+        dist.all_reduce(row, op=dist.ReduceOp.SUM, group=group)
+        M = float(row[0])
+        if M == 0:
+            return depth.new_zeros(())
+        local = s / M * lambda_depth
+        return (row[1] / M * lambda_depth).to(depth.dtype) + (local - local.detach())
+    if not M > 0 or not lambda_depth > 0:
+        return depth.new_zeros(())
+    return s / M * lambda_depth
+
+
+def _depth_loss_args(depth, rgba, depth_gt, mask, znear, zfar):
+    """the leading arguments of dss_depth_loss_forward, _partial and _backward"""
+    N, H, W = depth.shape
+    return (depth, rgba, depth_gt, mask, int(mask.dtype != torch.float32), N, H, W, float(znear), float(zfar))
+
+
+class _DepthLoss(torch.autograd.Function):
+    """dss_depth_loss_forward (the scalar and the total row) and dss_depth_loss_backward (d L / d depth, from the
+    upstream gradient on the device).  With a process group: dss_depth_loss_partial, the total row summed over the
+    ranks (one all-reduce of 2 doubles), dss_depth_loss_finish."""
+
+    @staticmethod
+    def forward(ctx, depth, rgba, depth_gt, mask, lambda_depth, znear, zfar, group=None):
+        dev = depth.device
+        totals = torch.empty((2,), dtype=torch.float64, device=dev)
+        loss = torch.empty((), dtype=torch.float32, device=dev)
+        args = _depth_loss_args(depth, rgba, depth_gt, mask, znear, zfar)
+        if group is None:
+            _lib.call("dss_depth_loss_forward", dev, *args, float(lambda_depth), totals, loss)
+        else:
+            import torch.distributed as dist
+            if depth.shape[0]:
+                _lib.call("dss_depth_loss_partial", dev, *args, totals)
+            else:
+                totals.zero_()
+            dist.all_reduce(totals, op=dist.ReduceOp.SUM, group=group)
+            _lib.call("dss_depth_loss_finish", dev, totals, float(lambda_depth), loss)
+        ctx.consts = (lambda_depth, znear, zfar)
+        ctx.save_for_backward(depth, rgba, depth_gt, mask, totals)
+        return loss
+
+    @staticmethod
+    def backward(ctx, g_loss):
+        depth, rgba, depth_gt, mask, totals = ctx.saved_tensors
+        lambda_depth, znear, zfar = ctx.consts
+        grad = torch.empty_like(depth, memory_format=torch.contiguous_format)
+        if depth.shape[0]:
+            _lib.call("dss_depth_loss_backward", depth.device, *_depth_loss_args(depth, rgba, depth_gt, mask, znear, zfar),
+                      float(lambda_depth), totals, g_loss.to(torch.float32).contiguous(), grad)
+        return grad, None, None, None, None, None, None, None
+
+
+def depth_loss(depth, rgba, depth_gt, mask_img, lambda_depth=1.0, znear=1.0, zfar=100.0, group=None):
+    """The dense depth term of the training step: ``lambda_depth * sum |depth - depth_gt| / M`` over the valid pixels
+    -- ground-truth mask set, render alpha non-zero (the RGB term's ``mask & alpha`` rule of :func:`image_loss`), and
+    ``depth_gt`` finite and strictly inside (``znear``, ``zfar``) -- M their count; 0 when M = 0 or ``lambda_depth`` is
+    not > 0.  Returns the device scalar ``loss_dr_depth``.
+
+    ``depth`` (N,H,W): the render's ``RenderOutput.depth``; ``rgba`` (N,H,W,4) the render's image (its alpha only gates
+    the pixels, it receives no gradient); ``depth_gt`` (N,H,W) view-space depth; ``mask_img`` (N,H,W) or (N,1,H,W).
+
+    float32 CUDA inputs (float32, uint8 or bool mask) take the fused route (csrc/depth.cu: two launches forward, one
+    backward, no host synchronisation, bit-reproducible), which differentiates ``depth``; every other dtype or device,
+    and targets that require grad, run :func:`depth_loss_torch`.
+
+    ``group``: a torch.distributed process group whose ranks each hold some of the views (a rank may hold none): M and
+    the sum of |depth - depth_gt| are summed over the ranks (one all-reduce of 2 doubles), the loss is the same on every
+    rank, and each rank's ``depth`` receives the gradient of its own views."""
+    mask = _depth_loss_inputs(depth, rgba, depth_gt, mask_img, min_views=0 if group is not None else 1)
+    fused = (depth.is_cuda and depth.dtype == rgba.dtype == depth_gt.dtype == torch.float32
+             and mask.dtype in (torch.float32, torch.uint8, torch.bool)
+             and not depth_gt.requires_grad and not mask.requires_grad)
+    if not fused:
+        return depth_loss_torch(depth, rgba, depth_gt, mask_img, lambda_depth, znear, zfar, group=group)
+    if not float(lambda_depth) > 0:
+        return torch.zeros((), dtype=torch.float32, device=depth.device)
+    rgba_c = rgba.detach().contiguous()
+    if rgba_c.data_ptr() % 16:
+        rgba_c = rgba_c.clone()
+    return _DepthLoss.apply(depth.contiguous(), rgba_c, depth_gt.contiguous(), mask.contiguous(), float(lambda_depth),
+                            float(znear), float(zfar), group)

@@ -36,7 +36,7 @@ from ..core.texture import camera_centres
 from ..graph import GraphedStep
 from ..ops import (LOCAL_FRAME_K, Shading, SplatParams, point_filters, point_filters_no_views, pose_cameras,
                    render_points, shared_cloud_splats)
-from .losses import ProjectionLoss, RepulsionLoss, fused_image_loss_targets, image_loss
+from .losses import ProjectionLoss, RepulsionLoss, depth_loss, fused_image_loss_targets, image_loss
 
 __all__ = ["TrainStep", "GraphedTrainStep"]
 
@@ -73,12 +73,19 @@ class TrainStep:
     camera centres' gradients, and ``step.poses.grad`` holds the (V,6) gradient after the step.  View-sharded, every
     rank's gradient rows of its own views are summed over the ranks with one all-reduce of 6 V floats (a rank without
     views adds zeros), so every rank holds the same gradient.  At zero poses the step computes the loss, image,
-    filters and cloud gradients of the step without ``poses``."""
+    filters and cloud gradients of the step without ``poses``.
+
+    ``lambda_dr_depth`` > 0 adds the dense depth term ``loss_dr_depth`` (``losses.depth_loss``) to the loss and to the
+    loss dict: the render's depth map (``render_points(..., depth=True)``) against the batch's ``depth`` (N,S,S) float32
+    view-space depth, passed as ``step(..., depth=depth)``, over the pixels inside the ground-truth mask and the render's
+    alpha whose depth is finite and inside (znear, zfar) of ``params``.  Its gradient reaches the points (and the poses)
+    through the render's view-depth gradient.  View-sharded, its two sums are all-reduced (2 doubles).  At 0 (the
+    default) the step reads no depth and computes what it computes without the term."""
 
     def __init__(self, points, normals, colours, params: SplatParams, *, learn=("points", "normals"),
                  Vrk_invariant=True, Vrk_isotropic=True, frnn_radius=0.2, shininess=64.0, lambda_dr_rgb=1.0,
                  lambda_dr_silhouette=1.0, lambda_dr_proj=0.01, lambda_dr_repel=0.0, knn_k=12, filter_scale=2.0,
-                 sharpness_sigma=0.75, grad_sync=None, poses=None, views=None):
+                 sharpness_sigma=0.75, grad_sync=None, poses=None, views=None, lambda_dr_depth=0.0):
         dev = _lib.require_cuda(points, normals, colours, poses)
         for name, t in (("points", points), ("normals", normals), ("colours", colours)):
             if t.dtype != torch.float32 or t.dim() != 2 or tuple(t.shape) != (points.shape[0], 3):
@@ -102,6 +109,9 @@ class TrainStep:
         self.lambda_dr_rgb, self.lambda_dr_silhouette = float(lambda_dr_rgb), float(lambda_dr_silhouette)
         self.lambda_dr_proj, self.lambda_dr_repel = float(lambda_dr_proj), float(lambda_dr_repel)
         self.knn_k, self.filter_scale, self.sharpness_sigma = int(knn_k), float(filter_scale), float(sharpness_sigma)
+        self.lambda_dr_depth = float(lambda_dr_depth)
+        if not 0.0 <= self.lambda_dr_depth < float("inf"):
+            raise ValueError("lambda_dr_depth must be a finite number >= 0, got %r" % (lambda_dr_depth,))
         # the cloud's point count as a device tensor made once: PointClouds3D would build it from a host list, a copy
         # that a capture cannot take
         self._num = torch.full((1,), points.shape[0], dtype=torch.int64, device=dev)
@@ -122,10 +132,10 @@ class TrainStep:
         """every host-side value the step bakes into its launches"""
         return (tuple(self.params), self.Vrk_invariant, self.Vrk_isotropic, self.frnn_radius, self.shininess,
                 self.lambda_dr_rgb, self.lambda_dr_silhouette, self.lambda_dr_proj, self.lambda_dr_repel, self.knn_k,
-                self.filter_scale, self.sharpness_sigma, self.poses is not None)
+                self.filter_scale, self.sharpness_sigma, self.poses is not None, self.lambda_dr_depth)
 
-    def _check_batch(self, img, mask_img, proj, view):
-        _lib.require_cuda(self.points, img, mask_img, proj, view)
+    def _check_batch(self, img, mask_img, proj, view, depth=None):
+        _lib.require_cuda(self.points, img, mask_img, proj, view, depth)
         if not fused_image_loss_targets(img, mask_img):
             raise TypeError("img must be float32 and mask_img float32, uint8 or bool, neither requiring grad; got %s "
                             "and %s" % (img.dtype, mask_img.dtype))
@@ -135,20 +145,25 @@ class TrainStep:
         S = int(self.params.image_size)
         if tuple(img.shape) != (N, S, S, 3):
             raise RuntimeError("img must have shape (N, S, S, 3) = %s, got %s" % ((N, S, S, 3), tuple(img.shape)))
+        if self.lambda_dr_depth > 0 and (depth is None or depth.dtype != torch.float32 or tuple(depth.shape) != (N, S, S)
+                                         or depth.requires_grad):
+            raise RuntimeError("a step with lambda_dr_depth > 0 takes the batch's depth maps: depth, a float32 tensor "
+                               "of shape %s not requiring grad, got %s" % ((N, S, S), None if depth is None else
+                                                                           "%s %s" % (depth.dtype, tuple(depth.shape))))
 
-    def __call__(self, img, mask_img, proj, view, lights, idx=None):
-        self._check_batch(img, mask_img, proj, view)
+    def __call__(self, img, mask_img, proj, view, lights, idx=None, depth=None):
+        self._check_batch(img, mask_img, proj, view, depth)
         if self.poses is not None:
             if idx is None or idx.dtype != torch.int64 or tuple(idx.shape) != (proj.shape[0],) \
                     or idx.device != self.device:
                 raise RuntimeError("a step that learns poses takes the batch's views: idx, an int64 tensor of shape "
                                    "(%d,) on %s" % (proj.shape[0], self.device))
         if self._sync is not None and proj.shape[0] == 0:
-            return self._run(img, mask_img, proj, view, None, None, None, idx)
+            return self._run(img, mask_img, proj, view, None, None, None, idx, depth)
         rows, ambient, kind = pack_lights(lights)
-        return self._run(img, mask_img, proj, view, rows.detach(), ambient.detach(), kind, idx)
+        return self._run(img, mask_img, proj, view, rows.detach(), ambient.detach(), kind, idx, depth)
 
-    def _run(self, img, mask_img, proj, view, rows, ambient, light_type, idx=None):
+    def _run(self, img, mask_img, proj, view, rows, ambient, light_type, idx=None, depth_gt=None):
         for t in (self.points, self.normals, self.colours, self.poses):
             if t is not None:
                 t.grad = None
@@ -156,11 +171,16 @@ class TrainStep:
         if self.poses is not None and N > 0:
             view, proj = pose_cameras(self.poses, idx, *self._cameras)
         normals = F.normalize(self.normals, dim=-1)
+        want_depth = self.lambda_dr_depth > 0
         if N == 0:
             # a rank of a view-sharded step without views: the collectives of the others, with zero contributions
             S = int(self.params.image_size)
             image = torch.zeros((0, S, S, 4), dtype=torch.float32, device=dev)
+            # (in the order of the branch below: collectives pair up by their order on the group)
             loss = image_loss(image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette, group=self._group)
+            if want_depth:
+                loss_depth = depth_loss(image[..., 0], image, depth_gt, mask_img, self.lambda_dr_depth,
+                                        self.params.znear, self.params.zfar, group=self._group)
             visibility, inmask = point_filters_no_views(self.points.shape[0], dev, self._group)
             rendered = _NoViews.apply(self.points, normals, self.colours, self._sync)
         else:
@@ -168,9 +188,12 @@ class TrainStep:
             shading = Shading(rows, ambient, camera_centres(view).contiguous(), light_type, self.shininess)
             out = render_points(self.points, normals, self.colours, proj, view, h, self.params, shading=shading,
                                 deterministic=True,
-                                grad_sync=self._sync, frames=frames)
+                                grad_sync=self._sync, frames=frames, depth=want_depth)
             loss = image_loss(out.image, img, mask_img, self.lambda_dr_rgb, self.lambda_dr_silhouette,
                               group=self._group)
+            if want_depth:
+                loss_depth = depth_loss(out.depth, out.image, depth_gt, mask_img, self.lambda_dr_depth,
+                                        self.params.znear, self.params.zfar, group=self._group)
             visibility, inmask = point_filters(out, mask_img, group=self._group)
             image, rendered = out.image, None
         cloud = PointClouds3D([self.points], [normals])
@@ -187,6 +210,8 @@ class TrainStep:
                 reg[key] = fn(cloud, rebuild_knn=True, points_filter=points_filter) * lam
         # trainer.py:313: loss = proj + repel + the image loss
         total = reg["loss_dr_proj"] + reg["loss_dr_repel"] + loss["loss"]
+        if want_depth:
+            total = total + loss_depth
         if rendered is not None:
             total = total + rendered
         total.backward()
@@ -198,6 +223,8 @@ class TrainStep:
         self.loss = {"loss": total.detach(), "loss_dr_rgb": loss["loss_dr_rgb"].detach(),
                      "loss_dr_silhouette": loss["loss_dr_silhouette"].detach(),
                      "loss_dr_proj": reg["loss_dr_proj"].detach(), "loss_dr_repel": reg["loss_dr_repel"].detach()}
+        if want_depth:
+            self.loss["loss_dr_depth"] = loss_depth.detach()
         self.image, self.visibility, self.inmask = image.detach(), visibility, inmask
         return self.loss
 
@@ -250,7 +277,7 @@ class GraphedTrainStep(TrainStep, GraphedStep):
     _OUTPUTS = ("loss", "image", "visibility", "inmask")
 
     def __init__(self, points, normals, colours, params: SplatParams, img, mask_img, proj, view, lights, warmup=3,
-                 _views=None, **settings):
+                 _views=None, depth=None, **settings):
         sync = settings.get("grad_sync")
         if sync is not None and sync.world_size > 1:
             raise NotImplementedError("GraphedTrainStep runs on one GPU; a view-sharded step runs eagerly: "
@@ -259,12 +286,13 @@ class GraphedTrainStep(TrainStep, GraphedStep):
             raise ValueError("a graphed step learns camera poses on device views: GraphedTrainStep.from_views(..., "
                              "poses=...)")
         super().__init__(points, normals, colours, params, views=None if _views is None else _views[0], **settings)
-        self._check_batch(img, mask_img, proj, view)
+        self._check_batch(img, mask_img, proj, view, depth)
         rows, ambient, self._light_type = pack_lights(lights)
         # static inputs (clone keeps a permuted view's strides)
         self.img, self.mask_img = img.detach().clone(), mask_img.detach().clone()
         self.proj, self.view = proj.detach().float().contiguous().clone(), view.detach().float().contiguous().clone()
         self.lights, self.ambient = rows.detach().clone(), ambient.detach().clone()
+        self.depth = depth.detach().clone() if self.lambda_dr_depth > 0 else None
         # from_views: the device views and the static (B,) index the capture gathers the batch with
         self._views, self._index = _views if _views is not None else (None, None)
         self._warmup = max(1, int(warmup))
@@ -289,8 +317,13 @@ class GraphedTrainStep(TrainStep, GraphedStep):
         if views.light_cls is None:
             raise ValueError("the training step shades every view with its lights, and the views have none")
         index = views.upload(idx)
+        depth = None
+        if float(settings.get("lambda_dr_depth", 0.0)) > 0:
+            if views.depth is None:
+                raise ValueError("lambda_dr_depth > 0 needs the views' depth maps (MVRData(..., load_dense_depth=True))")
+            depth = views.depth_at(index)
         return cls(points, normals, colours, params, *views.batch_at(index), warmup=warmup, _views=(views, index),
-                   **settings)
+                   depth=depth, **settings)
 
     def _gather(self):
         """the batch of the static index into the static inputs: the start of a from_views capture"""
@@ -298,6 +331,8 @@ class GraphedTrainStep(TrainStep, GraphedStep):
         views.gather(index, self.img, self.mask_img)
         torch.index_select(views.proj, 0, index, out=self.proj)
         torch.index_select(views.camera_mat, 0, index, out=self.view)
+        if self.depth is not None:
+            torch.index_select(views.depth, 0, index, out=self.depth)
         # pack_lights on the batch's light properties, as the step packs the lights it is handed: the ambient colour is
         # summed over the lights per batch, in the order torch's reduction takes for the batch's shape
         rows, ambient, _ = pack_lights(views.lights(index))
@@ -308,7 +343,7 @@ class GraphedTrainStep(TrainStep, GraphedStep):
         if self._views is not None:
             self._gather()
         return self._run(self.img, self.mask_img, self.proj, self.view, self.lights, self.ambient, self._light_type,
-                         self._index)
+                         self._index, self.depth)
 
     def load_views(self, idx):
         """the next batch of a :meth:`from_views` step: the host list ``idx`` (as many views as the capture's, checked
@@ -321,18 +356,19 @@ class GraphedTrainStep(TrainStep, GraphedStep):
             raise ValueError("load_views() takes the capture's %d views, got %d" % (self._index.shape[0], len(idx)))
         self._index.copy_(torch.tensor(idx, dtype=torch.int64).pin_memory(), non_blocking=True)
 
-    def load(self, img, mask_img, proj, view, lights):
-        """copy the next batch into the static inputs (no synchronisation)"""
+    def load(self, img, mask_img, proj, view, lights, depth=None):
+        """copy the next batch into the static inputs (no synchronisation); ``depth`` with ``lambda_dr_depth`` > 0"""
         if self._views is not None:
             raise RuntimeError("this step gathers its batch from device views inside the capture, which would "
                                "overwrite a loaded batch: use load_views(idx)")
-        self._check_batch(img, mask_img, proj, view)
+        self._check_batch(img, mask_img, proj, view, depth)
         rows, ambient, kind = pack_lights(lights)
         if kind != self._light_type or rows.shape != self.lights.shape or ambient.shape != self.ambient.shape:
             raise ValueError("the lights must keep the kind and shape of the capture: %s %s, got %s %s"
                              % (self._light_type, tuple(self.lights.shape), kind, tuple(rows.shape)))
-        for dst, src in ((self.img, img), (self.mask_img, mask_img), (self.proj, proj), (self.view, view),
-                         (self.lights, rows), (self.ambient, ambient)):
+        pairs = ((self.img, img), (self.mask_img, mask_img), (self.proj, proj), (self.view, view),
+                 (self.lights, rows), (self.ambient, ambient)) + (((self.depth, depth),) if self.depth is not None else ())
+        for dst, src in pairs:
             if dst.shape != src.shape or dst.dtype != src.dtype:
                 raise ValueError("load() takes a batch of the capture's shapes and dtypes: %s %s, got %s %s"
                                  % (tuple(dst.shape), dst.dtype, tuple(src.shape), src.dtype))

@@ -219,7 +219,9 @@ def load_data(cfg):
     """the configuration's ``MVRData`` (its ``data`` block), which must have images and masks"""
     dc = cfg["data"]
     data = MVRData(dc["data_dir"], data_dict=dc["data_dict"], n_imgs=dc["n_imgs"], img_folder=dc["img_folder"],
-                   mask_folder=dc["mask_folder"], img_extension=dc["img_extension"], mask_extension=dc["mask_extension"])
+                   mask_folder=dc["mask_folder"], img_extension=dc["img_extension"], mask_extension=dc["mask_extension"],
+                   load_dense_depth=bool(dc.get("load_dense_depth", False)), depth_folder=dc.get("depth_folder", "depth"),
+                   depth_extension=dc.get("depth_extension", "exr"))
     if data.images is None or data.masks is None:
         raise ValueError("%s has no images and masks" % dc["data_dir"])
     return data
@@ -322,7 +324,7 @@ class Trainer:
         self.log.info("Views on the device: %d of %dx%d, %s store, %.1f MB"
                       % (V, self.views.H, self.views.W, str(self.views.store.dtype).replace("torch.", ""),
                          self.views.nbytes / 1e6))
-        check_config(cfg, self.data.resolution, self.views.light_cls is not None)
+        check_config(cfg, self.data.resolution, self.views.light_cls is not None, self.views.depth is not None)
         self.metric = selection_metric(cfg)
         self.mesh = None
         if self.metric == "p2f_avg":
@@ -686,7 +688,8 @@ class Trainer:
                     loss = self.step.replay()
                 else:
                     mine = self.views.upload(deal_batch(self.data.camera_mat, idx, self.world)[self.rank])
-                    loss = self.step(*self.views.batch_at(mine), idx=mine if self.step.poses is not None else None)
+                    loss = self.step(*self.views.batch_at(mine), idx=mine if self.step.poses is not None else None,
+                                     depth=self.views.depth_at(mine) if self.step.lambda_dr_depth > 0 else None)
                 self.opt.step()
                 it = self.it
                 if self.lead and print_every > 0 and it % print_every == 0:

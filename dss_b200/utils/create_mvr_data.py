@@ -9,12 +9,14 @@ For every mesh it writes ``<output>/<name>_variational_light/``, the directory `
 - ``image/%06d.png``: RGBA, ``uint8(255 c)`` truncated as the reference's ``astype('uint8')``, c clamped to [0, 1]
   first (the reference's cast of values above 1 is undefined);
 - ``mask/%06d.png``: 8-bit 0 / 255 coverage;
+- ``depth/%06d.exr``: the view-space depth of the closest face (``render_mesh``'s z-buffer) where the mesh covers the
+  pixel and the cameras' ``zfar`` elsewhere, one float32 ``Y`` channel, ZIP compressed (``utils.io.write_exr``), as
+  the reference writes it (create_mvr_data_from_mesh.py:215-219, 240-242);
 - ``data_dict.npz``: ``points``, ``normals``, ``colors`` (ones) of 20 000 surface samples, ``camera_mat`` (V,4,4)
   row-vector world-to-view matrices, ``lights_%d`` per image, ``cameras_type``, ``cameras_params`` and ``lights_type``.
 
-The images are rendered on the GPU by ``render_mesh`` (flat shading, one light set per image).  Not written:
-``depth/*.exr`` (no OpenEXR writer here, nothing here reads it; ``render_mesh`` returns the depth) and the DVR-only
-``cameras.npz`` / ``pcl.npz``.  All randomness comes from ``--seed`` (a ``torch.Generator`` for the cameras, the
+The images are rendered on the GPU by ``render_mesh`` (flat shading, one light set per image).  Not written: the
+DVR-only ``cameras.npz`` / ``pcl.npz``.  All randomness comes from ``--seed`` (a ``torch.Generator`` for the cameras, the
 tri-colour light frames and the surface samples, a ``random.Random`` for the single-light draws); the reference's own
 random draws are not reproduced.
 """
@@ -30,7 +32,7 @@ import torch.nn.functional as F
 
 from ..core.camera import CameraSampler, FoVPerspectiveCameras, camera_matrices, look_at_rotation
 from ..core.lighting import DirectionalLights, PointLights
-from .io import read_mesh, save_obj
+from .io import read_mesh, save_obj, write_exr
 
 __all__ = ["get_tri_color_lights_for_view", "get_light_for_view", "light_value_dict", "sample_points_from_mesh",
            "ico_sphere", "normalize_mesh", "write_mvr_data", "create_mvr_data", "main"]
@@ -183,11 +185,11 @@ def perturb_cameras(camera_mat, degrees, frac, seed=0):
 
 
 def write_mvr_data(output_dir, verts, faces, images, masks, camera_mat, lights, points, normals, point_lights,
-                   camera_params, camera_mat_true=None):
+                   camera_params, camera_mat_true=None, depths=None):
     """Write the data directory from renders already made (host arrays): images (N,S,S,4) float in [0,1]-ish, masks
-    (N,S,S) bool, camera_mat (N,4,4), lights a list of N ``light_value_dict`` dicts, points / normals (P,3), and
-    ``camera_mat_true`` (N,4,4), the cameras the images were rendered from when ``camera_mat`` is not.  Returns
-    ``output_dir``."""
+    (N,S,S) bool, camera_mat (N,4,4), lights a list of N ``light_value_dict`` dicts, points / normals (P,3),
+    ``camera_mat_true`` (N,4,4), the cameras the images were rendered from when ``camera_mat`` is not, and ``depths``
+    (N,S,S) float32, the dense depth maps, written to ``depth/%06d.exr`` when given.  Returns ``output_dir``."""
     from PIL import Image
     rgb_dir, mask_dir = os.path.join(output_dir, "image"), os.path.join(output_dir, "mask")
     os.makedirs(rgb_dir, exist_ok=True)
@@ -199,6 +201,11 @@ def write_mvr_data(output_dir, verts, faces, images, masks, camera_mat, lights, 
         rgba = (np.clip(images[i], 0.0, 1.0) * np.float32(255.0)).astype(np.uint8)
         Image.fromarray(rgba).save(os.path.join(rgb_dir, "%06d.png" % i))
         Image.fromarray(masks[i].astype(np.uint8) * 255).save(os.path.join(mask_dir, "%06d.png" % i))
+    if depths is not None:
+        depth_dir = os.path.join(output_dir, "depth")
+        os.makedirs(depth_dir, exist_ok=True)
+        for i, d in enumerate(np.asarray(depths, dtype=np.float32)):
+            write_exr(os.path.join(depth_dir, "%06d.exr" % i), d)
     points = np.asarray(points, dtype=np.float32)
     data = {"cameras_type": CAMERAS_TYPE, "cameras_params": dict(camera_params), "lights_type": LIGHTS_TYPE[bool(point_lights)],
             "points": points, "normals": np.asarray(normals, dtype=np.float32),
@@ -240,7 +247,8 @@ def create_mvr_data(mesh_path, output, num_cameras=120, image_size=512, tri_colo
     all_cams = FoVPerspectiveCameras(R=sampler.R, T=sampler.T, **camera_params)
     proj, view = camera_matrices(all_cams)
     vd, fd = verts.to(dev), faces.to(dev)
-    images, masks = [], []
+    images, masks, depths = [], [], []
+    zfar = torch.tensor(all_cams.zfar, dtype=torch.float32, device=dev)
     for n0 in range(0, num_cameras, views_per_call):
         sl = slice(n0, min(n0 + views_per_call, num_cameras))
         view_n = view[sl].to(dev)
@@ -248,6 +256,7 @@ def create_mvr_data(mesh_path, output, num_cameras=120, image_size=512, tri_colo
         r = render_mesh(vd, fd, proj[sl].to(dev), view_n, image_size, shading=shading)
         images.append(r.image.cpu())
         masks.append((r.pix_to_face >= 0).cpu())
+        depths.append(torch.where(r.pix_to_face >= 0, r.zbuf, zfar).cpu())
     gd = torch.Generator(device=dev).manual_seed(int(seed))
     points, normals = sample_points_from_mesh(vd, fd, num_points, generator=gd)
     cams_out, cams_true = view.numpy(), None
@@ -255,7 +264,7 @@ def create_mvr_data(mesh_path, output, num_cameras=120, image_size=512, tri_colo
         cams_out, cams_true = perturb_cameras(view.numpy(), camera_noise[0], camera_noise[1], seed), view.numpy()
     return write_mvr_data(out_dir, verts.numpy(), faces_np, torch.cat(images).numpy(), torch.cat(masks).numpy(),
                           cams_out, [light_value_dict(l) for l in lights], points.cpu().numpy(),
-                          normals.cpu().numpy(), point_lights, camera_params, cams_true)
+                          normals.cpu().numpy(), point_lights, camera_params, cams_true, torch.cat(depths).numpy())
 
 
 def main(argv=None):

@@ -2,9 +2,11 @@
 scripts/create_mvr_data_from_mesh.py:170-255): the cloud in object coordinates and one 4x4 world-to-view matrix per
 image, plus the ground-truth image and mask files next to it (dataset.py:36-101: every file of ``<data_dir>/image`` /
 ``<data_dir>/mask`` with the configured extension, sorted; rgb -> (3,H,W) float32 in [0,1], mask -> (1,H,W) float 0/1),
-read with PIL (the reference uses imageio, which this image lacks).  ``device_views`` uploads every view once into a
+read with PIL (the reference uses imageio, which this image lacks).  With ``load_dense_depth`` the dense depth maps
+too (dataset.py:71-82, 204-209: every file of ``<data_dir>/<depth_folder>`` with ``depth_extension``, sorted; OpenEXR
+through ``utils.io.read_exr``) -> (1,H,W) float32.  ``device_views`` uploads every view once into a
 :class:`DeviceViews` store that the training loop gathers its batches from; ``pinned_batch`` stages a batch of views in
-pinned host memory for a host->device copy.  Dense depth maps (OpenEXR) are not read."""
+pinned host memory for a host->device copy."""
 import copy
 import os
 
@@ -30,11 +32,14 @@ def decompose_to_R_and_t(transform_mat, row_major=True):
 class MVRData:
     """points / normals / colors and per-image ``camera_mat`` of a ``data_dict.npz``.
 
-    ``data[i]`` -> ``{"camera_mat": (4,4) f32 [, "img.rgb": (3,H,W), "img.mask": (1,H,W)]}`` like
-    ``MVRDataset.__getitem__`` (dataset.py:171-211); images are only present when given to the constructor."""
+    ``data[i]`` -> ``{"camera_mat": (4,4) f32 [, "img.rgb": (3,H,W), "img.mask": (1,H,W), "img.depth": (1,H,W)]}``
+    like ``MVRDataset.__getitem__`` (dataset.py:171-211); images are only present when given to the constructor, depth
+    maps with ``load_dense_depth`` (or ``depths``, (H,W) arrays given by hand).  A count of depth maps other than the
+    number of views, or a depth map of a size other than the images', is refused."""
 
     def __init__(self, data_dir_or_file, data_dict="data_dict.npz", images=None, masks=None, n_imgs=None,
-                 img_folder="image", mask_folder="mask", img_extension="png", mask_extension="png", load_images=True):
+                 img_folder="image", mask_folder="mask", img_extension="png", mask_extension="png", load_images=True,
+                 load_dense_depth=False, depth_folder="depth", depth_extension="exr", depths=None):
         path = data_dir_or_file
         data_dir = None
         if os.path.isdir(path):
@@ -52,6 +57,16 @@ class MVRData:
                 images = self.load_all_images()
             if self.mask_files:
                 masks = self.load_all_masks()
+        if load_dense_depth and depths is None:
+            if data_dir is None:
+                raise ValueError("load_dense_depth reads <data_dir>/%s: pass the data directory" % depth_folder)
+            d = os.path.join(data_dir, depth_folder)
+            if not os.path.isdir(d):
+                raise ValueError("load_dense_depth: %s does not exist" % d)
+            self.depth_files = [os.path.join(d, f) for f in sorted(os.listdir(d))
+                                if os.path.splitext(f)[1].lower()[1:] == str(depth_extension).lower()]
+            from .io import read_exr
+            depths = [read_exr(f) for f in self.depth_files]
         self.data_dict = np.load(path, allow_pickle=True)
         if "camera_mat" not in self.data_dict:
             raise ValueError("data_dict must contain camera_mat!")
@@ -62,7 +77,16 @@ class MVRData:
             if arr is not None and len(arr) != len(self.camera_mat):
                 raise ValueError("Found unequal number of %s and camera matrices! (%d, %d)"
                                  % (name, len(arr), len(self.camera_mat)))
-        self.images, self.masks = images, masks
+        if depths is not None:
+            if len(depths) != len(self.camera_mat):
+                raise ValueError("Found invalid number of dense depth maps: %d for %d views"
+                                 % (len(depths), len(self.camera_mat)))
+            depths = [np.asarray(torch.as_tensor(d), dtype=np.float32).reshape(np.shape(d)[-2:]) for d in depths]
+            size = None if images is None else tuple(torch.as_tensor(images[0]).shape[1:])
+            for i, d in enumerate(depths):
+                if d.shape != (size or depths[0].shape):
+                    raise ValueError("depth map %d has size %s, but the images are %s" % (i, d.shape, size or depths[0].shape))
+        self.images, self.masks, self.depths = images, masks, depths
         self.data_dir = data_dir          # None when a data_dict file was given: no mesh.obj to sample
         self._poisson_disk = {}           # get_pointclouds(num_points) samples, per count
         self.n_imgs = len(self.camera_mat) if n_imgs is None else min(int(n_imgs), len(self.camera_mat))
@@ -121,6 +145,8 @@ class MVRData:
             out["img.rgb"] = self.images[idx]
         if self.masks is not None:
             out["img.mask"] = self.masks[idx]
+        if self.depths is not None:
+            out["img.depth"] = self.depths[idx][None]
         lights = self.data_dict["lights_%d" % idx] if ("lights_%d" % idx) in self.data_dict else None
         if lights is not None:
             props = lights.item() if hasattr(lights, "item") and lights.dtype == object else None
@@ -221,6 +247,7 @@ class DeviceViews:
     - ``camera_mat`` (V,4,4): the world-to-view matrices; ``proj`` (V,4,4): ``camera_matrices(data.get_cameras())``.
     - ``light_cls`` and ``light_props`` (``{property: (V,L,3)}``), as ``data.light_props`` gives them, or None when
       the data has no lights; :meth:`lights` selects views' lights from them.
+    - ``depth`` (V,H,W) float32: the data's dense depth maps, or None without them; :meth:`depth_at` selects views.
     - ``nbytes``: the device bytes held.
 
     :meth:`batch` gives the training step's arguments for a list of views, the same bits as uploading
@@ -258,7 +285,11 @@ class DeviceViews:
         self.proj = camera_matrices(data.get_cameras())[0].to(self.device)
         lights = data.light_props(self.device)
         self.light_cls, self.light_props = (None, None) if lights is None else lights
-        held = [self.store, self.camera_mat, self.proj] + list((self.light_props or {}).values())
+        self.depth = None
+        if data.depths is not None:
+            self.depth = torch.from_numpy(np.stack(data.depths[:V])).to(self.device)
+        held = [self.store, self.camera_mat, self.proj] + list((self.light_props or {}).values()) \
+            + ([self.depth] if self.depth is not None else [])
         self.nbytes = sum(t.numel() * t.element_size() for t in held)
 
     def __len__(self):
@@ -302,6 +333,12 @@ class DeviceViews:
             return None
         return self.light_cls(**{k: v.index_select(0, idx_dev) for k, v in self.light_props.items()},
                               device=self.device)
+
+    def depth_at(self, idx_dev):
+        """the (B,H,W) depth maps of the device indices ``idx_dev``; ValueError without depth maps"""
+        if self.depth is None:
+            raise ValueError("the views have no dense depth maps (MVRData(..., load_dense_depth=True))")
+        return self.depth.index_select(0, idx_dev)
 
     def batch_at(self, idx_dev):
         """``(img, mask, proj, view, lights)`` of the device indices ``idx_dev``: the training step's arguments"""

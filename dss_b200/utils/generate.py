@@ -97,7 +97,9 @@ def generate_images(cfg, points, normals, colours, gen_dir, poses=None):
     dB of the per-channel mean squared error of images in [0, 1] (null when the error is 0), per view and as their means
     over the views.  ``poses``: (V,6) camera corrections of the data's views; the views are then rendered and scored
     with the refined cameras (``DeviceViews.with_poses``), whose world-to-view matrices go to ``<gen_dir>/cameras.npz``
-    as ``camera_mat`` (V,4,4) float32.  Returns (the PNG paths, the JSON path)."""
+    as ``camera_mat`` (V,4,4) float32.  With the images, ``<gen_dir>/depth/%04d.exr``: their depth maps
+    (``render_points(..., depth=True)``: the blend's view-space depth, 0 where no splat covers the pixel), one float32
+    ``Y`` channel, ZIP compressed.  Returns (the PNG paths, the JSON path)."""
     import json
     import math
 
@@ -105,6 +107,7 @@ def generate_images(cfg, points, normals, colours, gen_dir, poses=None):
     from PIL import Image
 
     from ..ops import evaluate_2d, render_data_views
+    from .io import write_exr
     from ..training.config import splat_params, step_settings
     from ..training.train import load_data
     g = generation_settings(cfg)
@@ -121,16 +124,19 @@ def generate_images(cfg, points, normals, colours, gen_dir, poses=None):
                              % (tuple(poses.shape), V))
         data = data.device_views(points.device).with_poses(poses)
         np.savez(os.path.join(gen_dir, "cameras.npz"), camera_mat=data.camera_mat.cpu().numpy())
-    img_dir = os.path.join(gen_dir, "images")
+    img_dir, depth_dir = os.path.join(gen_dir, "images"), os.path.join(gen_dir, "depth")
     os.makedirs(img_dir, exist_ok=True)
+    os.makedirs(depth_dir, exist_ok=True)
     pngs = []
     n_out = min(max(0, int(g["vis_n_outputs"])), V)
     for i in range(0, n_out, B):
         views = list(range(i, min(i + B, n_out)))
-        rgba = render_data_views(points, normals, colours, data, params, views, *flags).clamp(0, 1).cpu().numpy()
-        for v, img in zip(views, rgba):
+        rgba, depth = render_data_views(points, normals, colours, data, params, views, *flags, depth=True)
+        rgba, depth = rgba.clamp(0, 1).cpu().numpy(), depth.cpu().numpy()
+        for v, img, d in zip(views, rgba, depth):
             pngs.append(os.path.join(img_dir, "%04d.png" % v))
             Image.fromarray((255 * img).astype(np.uint8)).save(pngs[-1])
+            write_exr(os.path.join(depth_dir, "%04d.exr" % v), d)
     db = lambda e: -10.0 * math.log10(e / 3.0) if e > 0 else None
     report = {"views": V, "resolution": S, "metrics": []}
     for s in (max(1, S // 4), S):

@@ -5,12 +5,18 @@
 by default) -- what ``Generator.generate_pointclouds`` exports (DSS/models/point_modeling.py:284-326) and what the
 example data ships (example_data/pointclouds/*.ply).  The reference goes through the ``plyfile`` package (absent here);
 the format is simple enough to read and write directly with numpy.  Host-side and cold: nothing here touches the GPU.
+
+``read_exr`` / ``write_exr``: the OpenEXR depth maps of the data directory (``depth/%06d.exr``, written by
+scripts/create_mvr_data_from_mesh.py:240-242 and read by DSS/utils/dataset.py:204-209 through imageio), also written
+directly: single-part scanline files with NONE, RLE, ZIPS or ZIP compression and HALF or FLOAT pixels.
 """
 import os
+import struct
+import zlib
 
 import numpy as np
 
-__all__ = ["read_ply", "save_ply", "read_mesh", "save_obj"]
+__all__ = ["read_ply", "save_ply", "read_mesh", "save_obj", "read_exr", "write_exr"]
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "i2", "int16": "i2",
               "ushort": "u2", "uint16": "u2", "int": "i4", "int32": "i4", "uint": "u4", "uint32": "u4",
@@ -312,3 +318,214 @@ def save_obj(path, verts, faces):
     with open(path, "w") as f:
         f.writelines("v %.9g %.9g %.9g\n" % tuple(float(x) for x in v) for v in verts)
         f.writelines("f %d %d %d\n" % tuple(int(i) + 1 for i in t) for t in faces)
+
+
+# ---- OpenEXR ---------------------------------------------------------------------------------------------------------
+_EXR_MAGIC = 20000630
+_EXR_COMPRESSIONS = ("NONE", "RLE", "ZIPS", "ZIP", "PIZ", "PXR24", "B44", "B44A", "DWAA", "DWAB")
+_EXR_LINES = {"NONE": 1, "RLE": 1, "ZIPS": 1, "ZIP": 16}     # scanlines per chunk of the compressions read here
+_EXR_PIXELS = {1: np.dtype("<f2"), 2: np.dtype("<f4")}       # HALF, FLOAT (UINT = 0 is not read)
+
+
+def _exr_unpredict(raw):
+    """undo the byte predictor and the even / odd split that RLE and ZIP apply before compressing"""
+    t = np.frombuffer(raw, np.uint8)
+    t = np.cumsum(t.astype(np.int64) - 128, dtype=np.int64) + 128   # t[i] = t[i-1] + d[i] - 128 (mod 256), t[0] as is
+    t = (t & 0xFF).astype(np.uint8)
+    out = np.empty_like(t)
+    half = (t.size + 1) // 2
+    out[0::2], out[1::2] = t[:half], t[half:]
+    return out.tobytes()
+
+
+def _exr_predict(raw):
+    t = np.frombuffer(raw, np.uint8)
+    half = (t.size + 1) // 2
+    s = np.empty_like(t)
+    s[:half], s[half:] = t[0::2], t[1::2]
+    d = s.astype(np.int64)
+    d[1:] = d[1:] - d[:-1] + 128
+    return (d & 0xFF).astype(np.uint8).tobytes()
+
+
+def _exr_rle_decode(data, size, path):
+    out = bytearray()
+    i, n = 0, len(data)
+    while i < n:
+        count = struct.unpack_from("<b", data, i)[0]
+        i += 1
+        if count < 0:
+            out += data[i:i - count]
+            i -= count
+        else:
+            out += data[i:i + 1] * (count + 1)
+            i += 1
+    if len(out) != size:
+        raise ValueError("%s: an RLE chunk decodes to %d bytes, expected %d" % (path, len(out), size))
+    return bytes(out)
+
+
+def _exr_rle_encode(raw):
+    out, i, n = bytearray(), 0, len(raw)
+    while i < n:
+        j = i + 1
+        while j < n and raw[j] == raw[i] and j - i < 128:
+            j += 1
+        if j - i >= 3:                              # a run: count - 1, then the byte
+            out += struct.pack("<b", j - i - 1) + raw[i:i + 1]
+            i = j
+            continue
+        j = i                                       # literal bytes up to the next run of three
+        while j < n and j - i < 127 and not (j + 2 < n and raw[j] == raw[j + 1] == raw[j + 2]):
+            j += 1
+        out += struct.pack("<b", -(j - i)) + raw[i:j]
+        i = j
+    return bytes(out)
+
+
+def _exr_header(f, path):
+    if struct.unpack("<i", f.read(4))[0] != _EXR_MAGIC:
+        raise ValueError("%s is not an OpenEXR file" % path)
+    version = struct.unpack("<i", f.read(4))[0]
+    if version & 0xFF != 2:
+        raise ValueError("%s: OpenEXR version %d is not read" % (path, version & 0xFF))
+    if version & 0x1A00:                            # tiled 0x200, non-image (deep) 0x800, multi-part 0x1000
+        raise ValueError("%s: only single-part scanline OpenEXR files are read (version flags 0x%x)"
+                         % (path, version & ~0xFF))
+    attrs = {}
+
+    def cstr():
+        b = bytearray()
+        while True:
+            c = f.read(1)
+            if not c:
+                raise ValueError("%s: truncated OpenEXR header" % path)
+            if c == b"\0":
+                return b.decode("latin-1")
+            b += c
+    while True:
+        name = cstr()
+        if not name:
+            break
+        typ = cstr()
+        size = struct.unpack("<i", f.read(4))[0]
+        attrs[name] = (typ, f.read(size))
+    for key in ("channels", "compression", "dataWindow"):
+        if key not in attrs:
+            raise ValueError("%s: the OpenEXR header has no %s" % (path, key))
+    return attrs
+
+
+def _exr_channels(blob, path):
+    chans, i = [], 0
+    while blob[i:i + 1] != b"\0":
+        end = blob.index(b"\0", i)
+        name = blob[i:end].decode("latin-1")
+        ptype, _, xs, ys = struct.unpack_from("<iB3xii", blob, end + 1)
+        if ptype not in _EXR_PIXELS:
+            raise ValueError("%s: channel %s has pixel type %d; HALF (1) and FLOAT (2) are read" % (path, name, ptype))
+        if xs != 1 or ys != 1:
+            raise ValueError("%s: channel %s is subsampled (%d, %d)" % (path, name, xs, ys))
+        chans.append((name, _EXR_PIXELS[ptype]))
+        i = end + 1 + 16
+    return chans
+
+
+def read_exr(path):
+    """The depth (or other single-channel) map of an OpenEXR file as an (H, W) float32 array: its only channel, or
+    ``Y``, else ``R``, of several.  Reads single-part scanline files with NONE, RLE, ZIPS or ZIP compression and HALF or
+    FLOAT pixels; ValueError for anything else, naming it (PIZ, the default of FreeImage's writer, among them)."""
+    with open(path, "rb") as f:
+        attrs = _exr_header(f, path)
+        comp_id = attrs["compression"][1][0]
+        comp = _EXR_COMPRESSIONS[comp_id] if comp_id < len(_EXR_COMPRESSIONS) else "compression %d" % comp_id
+        if comp not in _EXR_LINES:
+            raise ValueError("%s: %s compression is not read (NONE, RLE, ZIPS and ZIP are)" % (path, comp))
+        chans = _exr_channels(attrs["channels"][1], path)
+        names = [c[0] for c in chans]
+        if len(chans) == 1:
+            pick = 0
+        elif "Y" in names or "R" in names:
+            pick = names.index("Y" if "Y" in names else "R")
+        else:
+            raise ValueError("%s: no single, Y or R channel among %s" % (path, names))
+        x0, y0, x1, y1 = struct.unpack("<4i", attrs["dataWindow"][1])
+        W, H = x1 - x0 + 1, y1 - y0 + 1
+        if W < 1 or H < 1:
+            raise ValueError("%s: empty data window" % path)
+        lines = _EXR_LINES[comp]
+        chunks = (H + lines - 1) // lines
+        offsets = struct.unpack("<%dQ" % chunks, f.read(8 * chunks))
+        line_bytes = W * sum(dt.itemsize for _, dt in chans)
+        out = np.empty((H, W), np.float32)
+        for off in offsets:
+            f.seek(off)
+            y, size = struct.unpack("<ii", f.read(8))
+            data = f.read(size)
+            row = y - y0
+            n = min(lines, H - row)
+            if row < 0 or row >= H or len(data) != size:
+                raise ValueError("%s: bad chunk at offset %d" % (path, off))
+            raw_size = n * line_bytes
+            if size < raw_size:                     # else the chunk was stored uncompressed
+                if comp == "RLE":
+                    data = _exr_unpredict(_exr_rle_decode(data, raw_size, path))
+                else:
+                    data = _exr_unpredict(zlib.decompress(data))
+            if len(data) != raw_size:
+                raise ValueError("%s: a chunk holds %d bytes, expected %d" % (path, len(data), raw_size))
+            start = 0
+            for c, (_, dt) in enumerate(chans):
+                if c == pick:
+                    break
+                start += W * dt.itemsize
+            dt = chans[pick][1]
+            buf = np.frombuffer(data, np.uint8).reshape(n, line_bytes)[:, start:start + W * dt.itemsize]
+            out[row:row + n] = np.ascontiguousarray(buf).view(dt).reshape(n, W)
+    return out
+
+
+def write_exr(path, image, compression="ZIP", pixel_type="FLOAT"):
+    """Write an (H, W) map as a single-part scanline OpenEXR file with one ``Y`` channel: FLOAT pixels and ZIP
+    compression by default (``compression`` NONE, RLE, ZIPS or ZIP; ``pixel_type`` FLOAT or HALF)."""
+    img = np.asarray(image)
+    if img.ndim != 2 or img.shape[0] < 1 or img.shape[1] < 1:
+        raise ValueError("write_exr takes an (H, W) array, got shape %s" % (img.shape,))
+    comp, ptype = str(compression).upper(), str(pixel_type).upper()
+    if comp not in _EXR_LINES:
+        raise ValueError("write_exr writes NONE, RLE, ZIPS or ZIP compression, not %s" % compression)
+    if ptype not in ("FLOAT", "HALF"):
+        raise ValueError("write_exr writes FLOAT or HALF pixels, not %s" % pixel_type)
+    code = 2 if ptype == "FLOAT" else 1
+    pix = np.ascontiguousarray(img, dtype=_EXR_PIXELS[code])
+    H, W = pix.shape
+    attr = lambda name, typ, blob: name.encode() + b"\0" + typ.encode() + b"\0" + struct.pack("<i", len(blob)) + blob
+    header = struct.pack("<ii", _EXR_MAGIC, 2)
+    header += attr("channels", "chlist", b"Y\0" + struct.pack("<iB3xii", code, 0, 1, 1) + b"\0")
+    header += attr("compression", "compression", bytes([_EXR_COMPRESSIONS.index(comp)]))
+    header += attr("dataWindow", "box2i", struct.pack("<4i", 0, 0, W - 1, H - 1))
+    header += attr("displayWindow", "box2i", struct.pack("<4i", 0, 0, W - 1, H - 1))
+    header += attr("lineOrder", "lineOrder", b"\0")
+    header += attr("pixelAspectRatio", "float", struct.pack("<f", 1.0))
+    header += attr("screenWindowCenter", "v2f", struct.pack("<2f", 0.0, 0.0))
+    header += attr("screenWindowWidth", "float", struct.pack("<f", 1.0))
+    header += b"\0"
+    lines = _EXR_LINES[comp]
+    chunks = []
+    for y in range(0, H, lines):
+        raw = pix[y:y + lines].tobytes()
+        data = raw
+        if comp == "RLE":
+            data = _exr_rle_encode(_exr_predict(raw))
+        elif comp in ("ZIPS", "ZIP"):
+            data = zlib.compress(_exr_predict(raw))
+        if len(data) >= len(raw):                   # stored as is, as OpenEXR does
+            data = raw
+        chunks.append(struct.pack("<ii", y, len(data)) + data)
+    pos = len(header) + 8 * len(chunks)
+    offsets = []
+    for c in chunks:
+        offsets.append(pos)
+        pos += len(c)
+    with open(path, "wb") as f:
+        f.write(header + struct.pack("<%dQ" % len(offsets), *offsets) + b"".join(chunks))

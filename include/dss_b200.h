@@ -396,6 +396,30 @@ DSS_API int dss_image_loss_partial(dss_ctx *ctx, const float *pred, const float 
 DSS_API int dss_image_loss_finish(dss_ctx *ctx, const double *total_row, int H, int W, double lambda_rgb,
                                   double lambda_sil, float *loss, float *loss_rgb, float *loss_sil, void *stream);
 
+/* ---- depth loss ---------------------------------------------------------------------------------------------------
+ * The training step's dense depth term on the blend's depth map (dss_render_args.depth):
+ *   loss = lambda sum_valid |depth - gt| / M,  valid = mask != 0 (NaN counts as set) & alpha != 0 & gt finite &
+ *          znear < gt < zfar,  M = |valid|;  0 when M = 0
+ * depth, gt (N,H,W) f32 contiguous; pred (N,H,W,4) f32 rgba, 16-byte aligned (its alpha gates the pixel); mask
+ * (N,H,W) f32 (mask_kind 0) or bytes (1).  Forward (2 launches): totals (2,) f64 (M, sum |depth - gt|), kept for the
+ * backward, and the f32 scalar loss.  Backward (1 launch): grad_depth (N,H,W) f32, every element written:
+ * sign(depth - gt) lambda g / M on valid pixels, else 0 (sign(0) = sign(NaN) = 0), g the upstream gradient (a device
+ * f32 scalar).  Deterministic fixed-order fp64 sums, no host synchronisation.
+ * View-sharded: dss_depth_loss_partial (2 launches) writes the rank's totals only; the caller sums them over the ranks
+ * (2 doubles) and dss_depth_loss_finish (1 launch) writes the loss from the summed row; the backward then reads M from
+ * the summed row. */
+DSS_API int dss_depth_loss_forward(dss_ctx *ctx, const float *depth, const float *pred, const float *gt,
+                                   const void *mask, int mask_kind, int N, int H, int W, float znear, float zfar,
+                                   double lambda, double *totals, float *loss, void *stream);
+DSS_API int dss_depth_loss_partial(dss_ctx *ctx, const float *depth, const float *pred, const float *gt,
+                                   const void *mask, int mask_kind, int N, int H, int W, float znear, float zfar,
+                                   double *totals, void *stream);
+DSS_API int dss_depth_loss_finish(dss_ctx *ctx, const double *total_row, double lambda, float *loss, void *stream);
+DSS_API int dss_depth_loss_backward(dss_ctx *ctx, const float *depth, const float *pred, const float *gt,
+                                    const void *mask, int mask_kind, int N, int H, int W, float znear, float zfar,
+                                    double lambda, const double *totals, const float *grad_loss, float *grad_depth,
+                                    void *stream);
+
 /* ---- image-space validation metrics -----------------------------------------------------------------------------
  * Trainer.eval_step (DSS/training/trainer.py:173-212) on V renders of s x s pixels: the ground truth of H x W pixels is
  * resized to s x s as torch's F.interpolate(mode='bilinear', align_corners=False) without antialias does it, in float32
@@ -557,6 +581,14 @@ typedef struct dss_render_args {
     /* with `shade`: != 0 sums the colour scatter into d L / d shaded in 64-bit fixed point (the same bits on every run,
      * see dss_colour_backward); 0 adds it with float atomics (faster at large P).  The training step sets it. */
     int32_t deterministic_colours;
+    /* dense depth of the blend: (N,S,S) D = sum_k w_k z_k over the pixel's K-list in k order (the normalised weights
+     * of `weights`, the records' view depth z), 0 where the list is empty; written by dss_render_forward (one launch
+     * after the raster, which needs `weights`) when not NULL. */
+    float *depth;
+    /* backward: (N,S,S) d L / d depth or NULL.  Adds sum g_D w_k to the view-depth gradient of every record in the
+     * pixel's list, the weights held constant, summed in 64-bit fixed point (the same bits on every run); that gradient
+     * reaches the positions, `grad_ndc` and so the camera backward, as `grad_zbuf`'s does. */
+    const float *grad_depth;
 } dss_render_args;
 #define DSS_MAX_LIGHTS 8
 
